@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- predict_rank throughput of the B200-native hot path (BASELINE.json metric), one JSON line on stdout.
+"""bench.py -- predict_rank throughput of the H100 (sm_90a) hot path (BASELINE.json metric), one JSON line on stdout.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
 
 Workload (BASELINE.json north_star / SURVEY.md 8d, "C5 at 1M x 1M"): predict_rank top-10 over 1M users x 1M items,
 n_components = 128, indicator-regime sparse features (identity + 3 random tags per row, F = 1.2 R, ~4 nnz/row),
@@ -9,14 +9,17 @@ LinearRepresentationGraph x DotProductPredictionGraph, biased, n_tastes = 1.  Sy
 
 One step = one full pass of the hot path over the batch:
     K1 users -> split operand,  K1 items -> split operand,  2 x project_biases,  pack item meta,
-    K2+K3 fused tcgen05 score + top-k,  merge           [N > 1: item axis sharded, + 1 NCCL all-gather, merge]
+    K2+K3 fused wgmma score + top-k,    merge           [N > 1: item axis sharded, + 1 NCCL all-gather, merge]
 value  = U * I / step time with the CSR inputs and the weights already resident in HBM (CUDA events, max over ranks);
 e2e    = the same metric through TensorRec.predict_rank(user_features, item_features, k) with HOST scipy matrices
          (pinned): host->device copy of the CSR arrays and device->host read of the top-k inside the timed region;
-roofline: the fused kernel's algorithmic flops (2*U*I*d) / its CUDA-event time against the measured bf16 peak;
+roofline: the fused kernel's algorithmic flops (2*U*I*d) / its CUDA-event time against the dense fp16/bf16 peak;
 cpu_baseline: the oracle (numpy/scipy restatement of the reference's TF-CPU ops) on this box's host cores, on a
          bounded user sample of the same workload.
-`--impl reference` times that oracle alone (TensorFlow, the reference's only back-end, cannot be installed)."""
+`--impl reference` times that oracle alone (TensorFlow, the reference's only back-end, cannot be installed).
+`--dump-outputs DIR` writes the top-k of the last timed step (DIR/top_items.npy, DIR/top_scores.npy and the user rows
+they belong to, DIR/user_rows.npy; a fixed, seeded sample of rows when all of them would exceed 64 MB), so that two
+builds can be compared output for output on identical, seeded inputs."""
 import argparse
 import concurrent.futures
 import json
@@ -222,22 +225,36 @@ class ClockSampler(object):
                 'power_w_max': float(max(power)), 'samples': len(sm)}
 
 
-def ncu_traffic(kernel_key):
-    """DRAM bytes (read + write) of one launch of the dominant kernel at the bench workload, from the committed ncu
-    capture (profiles/ncu_traffic.json, written by scripts/ncu_summary.py runs); None if not captured."""
-    path = os.path.join(ROOT, 'profiles', 'ncu_traffic.json')
-    if os.path.exists(path):
-        return json.load(open(path)).get(kernel_key)
-    return None
-
-
 def measured_peaks():
     path = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(path):
         p = json.load(open(path))
         return {'hbm_gbs': p['hbm_gbs'], 'tflops_burst': p['bf16_tflops'],
                 'tflops_sustained': p.get('bf16_tflops_sustained', p['bf16_tflops']), 'source': 'measured'}
-    return {'hbm_gbs': 6650.0, 'tflops_burst': 1590.0, 'tflops_sustained': 1400.0, 'source': 'fallback'}
+    # NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense fp16/bf16 TFLOP/s; a card run at a lower power
+    # limit clocks lower under sustained load (`clocks` in the result line shows what it ran at)
+    return {'hbm_gbs': 3350.0, 'tflops_burst': 989.0, 'tflops_sustained': 989.0, 'source': 'H100 SXM data sheet'}
+
+
+H100_L2_MB = 50.0             # L2 of the H100 (SXM and PCIe)
+DUMP_MAX_BYTES = 60 << 20    # the three .npy files, headers included, stay below 64 MB
+
+
+def dump_outputs(out_dir, top, user_lo, suffix='', max_bytes=DUMP_MAX_BYTES):
+    """The top-k the timed path returned in its last step: items (float64: exact for int32 ids), scores (float32) and
+    the global user row of each line.  All rows when they fit max_bytes, else a fixed seeded sample of rows."""
+    import torch
+    n, k = int(top.items.shape[0]), int(top.items.shape[1])
+    per_row = k * (8 + 4) + 8
+    rows = np.arange(n, dtype=np.int64)
+    if n * per_row > max_bytes:
+        rows = np.sort(np.random.default_rng(20240611).choice(n, max_bytes // per_row, replace=False))
+    idx = torch.from_numpy(rows).to(top.items.device)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, 'top_items%s.npy' % suffix), top.items[idx].cpu().numpy().astype(np.float64))
+    np.save(os.path.join(out_dir, 'top_scores%s.npy' % suffix), top.scores[idx].cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, 'user_rows%s.npy' % suffix), (rows + user_lo).astype(np.float64))
+    log('[bench] wrote %d of %d top-k rows to %s' % (len(rows), n, out_dir))
 
 
 # ----------------------------------------------------------------------------------------------------- GPU arm
@@ -248,9 +265,9 @@ def workload_config(args):
     operands_mb = (args.users + args.items) * 2 * d_pad * 2 / 1e6
     tables_mb = (f_users + f_items) * args.d * 4 / 1e6
     return {'workload': workload_string(args),
-            'l2': 'split operands %.0f MB, weight tables %.0f MB against 126 MB of L2: %s'
-                  % (operands_mb, tables_mb, 'inputs exceed L2, no flush between steps needed'
-                     if min(operands_mb, tables_mb) > 126 else 'inputs FIT in L2 - a test size, not a bench line')}
+            'l2': 'split operands %.0f MB, weight tables %.0f MB against %.0f MB of L2: %s'
+                  % (operands_mb, tables_mb, H100_L2_MB, 'inputs exceed L2, no flush between steps needed'
+                     if min(operands_mb, tables_mb) > H100_L2_MB else 'inputs FIT in L2 - a test size, not a bench line')}
 
 
 def workload_string(args):
@@ -463,6 +480,9 @@ def run_b200(args):
         bad_ids = bad_ids[(bad_ids >= s_lo) & (bad_ids < s_hi)][:args.parity_fallback_rows]      # rows within the group
         fallback_ids = bad_ids.cpu().numpy() + g_lo                                               # global user ids
         fallback_items = out.items[bad_ids - s_lo].cpu().numpy()
+    if args.dump_outputs:
+        # every rank writes its own user slice; together they stay within the one budget
+        dump_outputs(args.dump_outputs, out, u_lo, '' if world == 1 else '_rank%d' % rank, DUMP_MAX_BYTES // world)
 
     # ---- e2e: the public API with host buffers ----------------------------------------------------------
     def pinned_csr(m):
@@ -554,9 +574,9 @@ def run_b200(args):
     result = {
         'metric': METRIC, 'value': value, 'unit': UNIT, 'n_gpus': world, 'steps': args.steps, 'warmup': args.warmup,
         'ms_per_step': ms_step, 'higher_is_better': True, 'scaling': 'strong', 'vs_baseline': None,
-        'dtype': ('f32 (1 fp16 tcgen05 filter pass with a certified bound + re-scoring of the survivors from the 22-bit '
+        'dtype': ('f32 (1 fp16 wgmma filter pass with a certified bound + re-scoring of the survivors from the 22-bit '
                   'split operands, fp32 accumulate)'
-                  if use_filter else 'f32 (3 x fp16 split-product tcgen05 passes, fp32 accumulate)'),
+                  if use_filter else 'f32 (3 x fp16 split-product wgmma passes, fp32 accumulate)'),
         'data': 'synthetic',
         'config': workload_config(args),
         'details': {'parallelism': ('item axis sharded x%d%s: 1 NCCL all-to-all of the per-shard top-k per item group, '
@@ -575,16 +595,13 @@ def run_b200(args):
         'roofline': {'kernel': ('score_filter_kernel (trk_score_filter_f16)' if use_filter
                                 else 'score_tc_kernel<topk> (trk_score_topk_f16x3)'), 'bound': 'tensor',
                      'achieved': achieved, 'peak': peak, 'unit': 'TFLOP/s', 'frac': achieved / peak,
-                     'traffic': ncu_traffic('score_filter_kernel@%dx%dx%d' % (n_users, n_local, d)) if use_filter
-                     else ncu_traffic('score_tc_kernel@%dx%dx%d' % (n_users, n_local, d)),
-                     'peak_source': peaks['source'] + ' bf16_tflops_sustained', 'ms_per_launch': fused_ms,
+                     'peak_source': peaks['source'] + ' fp16/bf16 dense', 'ms_per_launch': fused_ms,
                      'issued_tflops': (1 if use_filter else 3) * achieved,
                      'issued_frac': (1 if use_filter else 3) * achieved / peak, 'share_of_step': fused_ms / ms_step},
         'roofline_k1': {'kernel': 'csr_gather_reduce_kernel (users) + csr_project_biases_kernel', 'bound': 'hbm',
                         'achieved': k1_gbs, 'peak': peaks['hbm_gbs'], 'unit': 'GB/s', 'frac': k1_gbs / peaks['hbm_gbs'],
                         'ms_per_launch': k1u_ms, 'algorithmic_bytes': int(k1_survey_bytes),
-                        'bytes_with_scale_and_norm': int(k1_bytes),
-                        'traffic': ncu_traffic('csr_gather_reduce_kernel@%dx%d' % (n_users, d))},
+                        'bytes_with_scale_and_norm': int(k1_bytes)},
         'phases_ms': {'rank0': phase_table(phase_ms), 'max_over_ranks': phase_table(all_phase.max(axis=0)),
                       'mean_over_ranks': phase_table(all_phase.mean(axis=0)),
                       'unsharded_share_of_step': rest_ms / ms_step if world > 1 or n_shards > 1 else None},
@@ -608,8 +625,8 @@ def run_b200(args):
 
 
 def run_extras(args):
-    """Secondary workloads measured in the same default run (N = 1) so that they are driver-run too: each entry is the
-    JSON object the corresponding --workload prints."""
+    """Secondary workloads measured in the same default run (N = 1), with the run's --steps / --warmup: each entry is
+    the JSON object the corresponding --workload prints."""
     import copy
     extras = {}
     for name, fn, over in (('dense', run_dense, {'users': 65536, 'items': 100000, 'd': 64}),
@@ -618,7 +635,6 @@ def run_extras(args):
         a = copy.copy(args)
         for key, val in over.items():
             setattr(a, key, val)
-        a.steps, a.warmup = 3, 2
         try:
             extras[name] = fn(a, emit=False)
         except Exception as exc:      # a secondary line must not take the headline down
@@ -962,10 +978,14 @@ def main():
                     help='ranks per item group (default: all ranks = the item axis sharded over every GPU); a divisor of the '
                          'rank count gives the grid form: item_shards x (ranks / item_shards) user groups')
     ap.add_argument('--no-extra', action='store_true', help='skip the secondary workloads of the default run')
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help='write the top-k of the last timed step as DIR/<name>.npy (at most 64 MB, seeded row sample)')
     ap.add_argument('--n-sampled', type=int, default=64, help='--workload train: n_sampled_items')
     ap.add_argument('--train-dtype', default='bf16', choices=['bf16', 'f32'], help='--workload train: representations')
     ap.add_argument('--train-cpu-users', type=int, default=20000, help='--workload train: users of the CPU oracle sample')
     args = ap.parse_args()
+    if args.dump_outputs and (args.workload != 'topk' or args.impl != 'b200'):
+        ap.error('--dump-outputs writes the top-k of the flagship workload: it needs --workload topk --impl b200')
     if args.workload == 'dense':
         run_dense(args)
     elif args.workload == 'ranks':

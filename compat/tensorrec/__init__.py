@@ -1,7 +1,7 @@
 """`import tensorrec` for code written against jfkirk/tensorrec: every name resolves to tensorrec_b200.
 
 Put this directory on PYTHONPATH (next to the repository root) and the reference's own modules -- tensorrec.eval,
-tensorrec.util, tensorrec.loss_graphs, ... -- are the B200 implementations; `from tensorrec import TensorRec` works
+tensorrec.util, tensorrec.loss_graphs, ... -- are the H100 implementations; `from tensorrec import TensorRec` works
 unchanged."""
 import importlib
 import os

@@ -1,5 +1,5 @@
 /*
- * tensorrec_b200.h -- C ABI of the B200-native predict / predict_rank hot path of jfkirk/tensorrec.
+ * tensorrec_b200.h -- C ABI of the H100-native (sm_90a) predict / predict_rank hot path of jfkirk/tensorrec.
  *
  * The reference (pure Python over TensorFlow 1.x, commit 80690737) has no FFI of its own; the boundary a
  * maintainer would bind is the set of TF ops its graph evaluates on this path.  Each entry point below
@@ -124,7 +124,7 @@ int trk_rank_full(const float* scores, int32_t* ranks, int64_t n_users, int64_t 
 int trk_order_from_ranks(const int32_t* ranks, int64_t n, int32_t* order, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------
- * K2+K3 fused (tensor cores, sm_100a)  scores and per-user top-k without materialising [n_users, n_items]
+ * K2+K3 fused (tensor cores, sm_90a)   scores and per-user top-k without materialising [n_users, n_items]
  *
  * replaces the chain  tf.matmul (prediction_graphs.py:49-50)  ->  bias_prediction_dense
  * (recommendation_graphs.py:41)  ->  rank_predictions (recommendation_graphs.py:73-82) restricted to the
@@ -132,7 +132,7 @@ int trk_order_from_ranks(const int32_t* ranks, int64_t n, int32_t* order, void* 
  *
  * Operands are the split-fp16 layout produced by K1 (hi/lo halves, per-row power-of-two scale); the score is
  *   s[u,i] = (hi_u.hi_i + hi_u.lo_i + lo_u.hi_i) * scale_u * scale_i + user_bias[u] + item_bias[i]
- * accumulated in fp32 in tensor memory (three tcgen05.mma passes per k-block; relative error vs an fp32 dot
+ * accumulated in fp32 in registers (three groups of wgmma per k-block; relative error vs an fp32 dot
  * product <= 2^-21 of |u|.|i|, and exact for integer-valued representations).
  *
  * The item axis is cut into n_splits contiguous ranges (parallelism when n_users is small; shards when the

@@ -1,7 +1,7 @@
 """
 TEST INFRASTRUCTURE (see oracle/__init__.py).  numpy/scipy restatement of the reference ops on the
 predict / predict_rank path.  Every function cites the reference lines it follows
-(paths relative to /root/reference).  All arithmetic is float32, like the reference's TF graph
+(paths relative to the root of jfkirk/tensorrec @ 80690737).  All arithmetic is float32, like the reference's TF graph
 (tensorrec/input_utils.py:34 casts values to float32; every tf.Variable is float32).
 
 TensorFlow op semantics encoded here (TF is a third-party dependency of the reference, not vendored;

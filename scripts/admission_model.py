@@ -3,9 +3,9 @@ compactions a warp performs, as a function of the sweep length and of the thresh
 N(0, 1) (dot products of random d=128 rows in units of their standard deviation; the 2.25 m band is 0.037 of it), one
 warp = 32 rows sharing the instruction stream, buffer of 32 entries, compaction keeps <= 16, tile-end compaction above 26.
 
-    python scripts/admission_model.py > profiles/model_r2_admission.txt
+    python scripts/admission_model.py
 
-Rows 'shared k-th best after a prefix' model the next round's designs (DESIGN section 8): the item axis split over 8
+Rows 'shared k-th best after a prefix' model a shared-threshold design: the item axis split over 8
 shards, every shard sweeps a prefix of its items, the k-th best of the UNION of the shards' lists becomes the starting
 threshold of the rest of the sweep."""
 import sys

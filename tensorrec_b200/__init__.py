@@ -1,4 +1,4 @@
-"""tensorrec_b200 -- the predict / predict_rank hot path of jfkirk/tensorrec, B200-native (sm_100a), behind the
+"""tensorrec_b200 -- the predict / predict_rank hot path of jfkirk/tensorrec, H100-native (sm_90a), behind the
 reference's own TensorRec class and RepresentationGraph / PredictionGraph / LossGraph plugin surface.
 
 Export list mirrors tensorrec/__init__.py:1-14."""

@@ -1,4 +1,4 @@
-"""Builds libtensorrec_b200.so (the C-ABI library of include/tensorrec_b200.h) in-tree with nvcc for sm_100a.
+"""Builds libtensorrec_b200.so (the C-ABI library of include/tensorrec_b200.h) in-tree with nvcc for sm_90a (H100).
 
     python -m tensorrec_b200.csrc.build [--force] [--verbose]
 
@@ -19,7 +19,7 @@ HEADERS = [os.path.join(HERE, 'common.cuh'), os.path.join(ROOT, 'include', 'tens
 LIB_PATH = os.path.join(os.path.dirname(HERE), 'libtensorrec_b200.so')
 
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a',
+    '-gencode', 'arch=compute_90a,code=sm_90a',
     '-O3', '-std=c++17', '-lineinfo',
     '-Xcompiler', '-fPIC',
     '--expt-relaxed-constexpr',
@@ -53,7 +53,7 @@ def build(force=False, verbose=False):
                 print(' '.join(cmd), flush=True)
             subprocess.run(cmd, check=True)
     if force or _stale(LIB_PATH, objs):
-        cmd = [nvcc, '-shared', '-gencode', 'arch=compute_100a,code=sm_100a', '-o', LIB_PATH] + objs
+        cmd = [nvcc, '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', LIB_PATH] + objs
         if verbose:
             print(' '.join(cmd), flush=True)
         subprocess.run(cmd, check=True)

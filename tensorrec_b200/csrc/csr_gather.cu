@@ -12,12 +12,8 @@
 //   * a group of G lanes owns one row and every lane keeps CH float4 accumulators (d = 128: G = 8, CH = 4, so a warp
 //     works on four rows at once); kBatch x CH 16-byte gathers are in flight per lane, 32 warps per SM.  The launch
 //     bound (4 resident blocks) matters: without it ptxas budgets 32 registers, sinks every gather next to its FMAs and
-//     the kernel runs one memory latency per nonzero -- it then reacts to neither byte count nor L2 hints
-//     (profiles/probe_r1_k1_hints.txt);
+//     the kernel runs one memory latency per nonzero -- it then reacts to neither byte count nor L2 hints;
 //   * outputs are written with streaming stores (single use);
-//   (measured and not kept: L2 eviction-priority hints -- evict_last for re-referenced rows, evict_first for the
-//    once-read ones -- gain ~1.5 %: the 102 MB of randomly re-referenced tag rows of the indicator regime exceed what
-//    the two-partition L2 keeps next to 2 GB of streaming traffic, their hit rate stays ~37 %.)
 //   * accumulation is fp32 FMA in CSR storage order -> bit-identical from run to run, duplicates are summed;
 //   * the epilogue (row still in registers) optionally L2-normalises, writes fp32 and/or the split-fp16 operand
 //     (hi | lo, per-row power-of-two scale) that the tensor-core score kernel consumes.
@@ -32,8 +28,8 @@ constexpr int kNnzCap = 3072;  // staged (col,val) pairs per tile: 24 KB
 
 // Weight-row gathers are issued through `asm volatile` and their results pinned by empty volatile asm statements: with
 // plain __ldg the compiler sinks every load next to its FMAs to save registers (32 registers, one gather in flight per
-// lane: four serialised memory latencies per 4-entry row -- the kernel then ignores both byte count and L2 hints,
-// profiles/probe_r1_k1_hints.txt).  This keeps the loads of a batch together, ahead of the first FMA.
+// lane: four serialised memory latencies per 4-entry row -- the kernel then ignores both byte count and L2 hints).
+// This keeps the loads of a batch together, ahead of the first FMA.
 __device__ __forceinline__ float4 ldg_f4_nc(const float* ptr) {
   float4 v;
   asm volatile("ld.global.nc.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(ptr));
@@ -396,8 +392,8 @@ bool pick_shape(int d, int d_pad, bool want_split, bool aligned16, RowShape* s) 
     const int units = cover / 4;
     s->vec = true;
     // narrow groups, several 16-byte chunks per lane: a warp then works on 4 (or 2) rows at once, which amortises the
-    // per-row control instructions and puts kBatch x CH gathers in flight per lane (K1 at 1M rows x d128, 4 entries per
-    // row: 32 lanes x 1 chunk 0.52 ms, 16 x 2 0.44 ms, 8 x 4 0.42 ms; scripts/k1_probe.py)
+    // per-row control instructions and puts kBatch x CH gathers in flight per lane (scripts/k1_probe.py times the
+    // variants)
     if (units <= 8) { s->g = 8; s->ch = 1; }
     else if (units <= 16) { s->g = 8; s->ch = 2; }
     else if (units <= 32) { s->g = 8; s->ch = 4; }

@@ -1,4 +1,4 @@
-// K2+K3 fused, filter form: ONE tcgen05 pass over the fp16 "hi" halves produces approximate scores with a proven
+// K2+K3 fused, filter form: ONE wgmma pass over the fp16 "hi" halves produces approximate scores with a proven
 // error bound; per user row the kernel keeps every item that could still belong to the top-k (approximate score
 // within the bound of the running k-th best).  The few survivors are re-scored exactly in fp32 and ranked by
 // rescore_topk_kernel (rescore_topk.cu), which also verifies the bound and flags rows for the exact 3-pass kernel
@@ -7,13 +7,14 @@
 // rank_predictions (:73-82) restricted to rank <= k.
 //
 // CTA = 256 user rows (two 128-row blocks) x a sweep over 128-item tiles: every B tile fetched from L2 feeds two
-// accumulators.  The user rows live in TENSOR MEMORY (columns [0,128), written by the epilogue threads with
-// tcgen05.st) and are the A operand of tcgen05.mma straight from there; the remaining 384 columns hold a ring of
-// three 128-column accumulators.  Epilogue group g = warps 4+4g..7+4g drains the accumulators of user block g, one
-// thread per user row.
+// warpgroups.  Warp 0 streams the item tiles with TMA; consumer warpgroup g (warps 4+4g..7+4g) loads user block g
+// (hi half, TMA) into shared memory once per work unit, computes each tile's 128 x 128 accumulator in two 64-column
+// halves with m64n64k16 wgmma into registers, and passes it through a 32-column shared-memory staging tile so that the
+// admission code runs one thread per user row.  While one warpgroup filters, the other's wgmma keeps the tensor cores
+// busy.
 //
-// Why: the exact split-product kernel issues 3 tensor passes and its per-row sorted-list inserts serialise a warp
-// (profiles/r1_v2_fused_ncu.json: tensor pipe 37 %, top stall = insert loop).  Here
+// Why: the exact split-product kernel issues 3 tensor passes and its per-row sorted-list inserts serialise a warp.
+// Here
 //   * tensor work is 1 pass (2*U*I*d flops = the algorithmic count);
 //   * items are processed in descending-bias order (host side), so within a 128-item block the biases are almost equal
 //     and the admission test v_j = acc_j + bias_j / c > tau (c = user scale x GLOBAL item scale, both powers of two)
@@ -22,8 +23,7 @@
 //   * a passing column is APPENDED raw (accumulator, position) to the row's 32-entry buffer in shared memory; when
 //     some row's buffer passes half full the whole warp compacts it cooperatively: one entry per lane, raw entries
 //     resolved to (approximate score, item id), a 15-step bitonic sort through shuffles, keep everything >= (k-th best
-//     - 2.25m), tighten the threshold;
-//   * the epilogue warps never meet at a block or group barrier.
+//     - 2.25m), tighten the threshold.
 //
 // Error bound.  hi = fp16(x * 2^e) has relative error <= 2^-11 per element (absolute 2^-25 below the fp16 normal
 // range), so |approx - exact| <= (2^-10 + 2^-22) |u|.|i| <= m := kMarginFactor * |u|_2 * max_j |i_j|_2 with
@@ -38,22 +38,22 @@
 namespace trk {
 
 constexpr int kFBlockM = 128;
-constexpr int kFBlockN = 128;          // item tile; TMEM: 128 columns of A operand + 3 accumulators of 128 columns
-constexpr int kFAccSlots = 3;
-constexpr uint32_t kFTmemAccCol = 128;   // first accumulator column (columns [0, 128): user operand, 64 per block)
+constexpr int kFBlockN = 128;          // item tile
 constexpr int kFKBlock = 64;
-constexpr int kFUmmaK = 16;
+constexpr int kFMmaK = 16;
 constexpr int kFThreads = 384;
+constexpr int kFConsumerThreads = 128; // per consumer warpgroup (= user rows of its block)
+constexpr int kFStageStride = 33;      // fp32 per staged row (32 columns + 1: conflict-free row reads)
 constexpr uint32_t kFBTileBytes = kFBlockN * kFKBlock * 2;   // 16 KB
+constexpr uint32_t kFATileBytes = kFBlockM * kFKBlock * 2;   // 16 KB
+constexpr uint32_t kFAccStageBytes = kFBlockM * kFStageStride * 4u;   // per warpgroup
 constexpr int kFMaxStages = 10;
-constexpr uint32_t kFTmemCols = 512;
 constexpr int kBufEntries = 32;      // candidate buffer per (row, epilogue group)
 constexpr int kKeepMax = 16;         // entries kept by a compaction (>= k + slack); also the per-group output width
 constexpr int kFilterMaxK = 12;
 constexpr float kMarginFactor = 1.5f * 0.0009765625f;   // 1.5 * 2^-10
 constexpr float kBiasUlps = 4.0f * 1.1920929e-7f;        // 4 ulp(1): rounding of (dot + ub) + ib
 constexpr float kThetaMargins = 2.25f;                   // theta = a_k - 2.25 m  (> 2 m is what the proof needs)
-constexpr int kTileEndMaxTiles = 3072;   // sweeps of up to 393216 items per split run the tile-end compaction variant
 constexpr int kGiveUpOverflows = 8;   // a row whose compactions overflow this often is handed to the exact kernel
 
 struct FilterParams {
@@ -77,37 +77,30 @@ struct FilterParams {
   int32_t n_tiles;
   int32_t n_user_pairs;        // ceil(n_users / 256)
   int32_t item_id_offset;
-  int32_t tile_end_trigger;    // kTileEnd kernels: rows holding more entries than this are compacted at the END of a tile
-  int32_t debug_mode;          // timing experiments only (TRK_FILTER_DEBUG): 1 = drain TMEM without filtering, 2 = no drain,
-                               // 4 = nothing admitted, 6 = MMA only (no B stream, no drain), 7 = full kernel + clock readout
-                               // (9, "filter half of every tile's columns", was a build-time experiment: its run-time
-                               // loop bound cost 2.5 % at 1M items -- profiles/probe_r2_v18_filter_ab_full.txt)
+  int32_t tile_end_trigger;    // rows holding more entries than this are compacted at the END of a tile
   float* cand_score;           // [n_users, n_splits, kKeepMax] approximate scores (sentinel -inf)
   int32_t* cand_item;          // [n_users, n_splits, kKeepMax] global ids (sentinel INT32_MAX)
   float* row_theta;            // [n_users, n_splits] final admission threshold (certified by rescore_topk_kernel)
 };
 
 struct FilterLayout {
-  uint32_t b_off, buf_off, bar_off, total;
+  uint32_t a_off, b_off, buf_off, acc_off, bar_off, total;
 };
-__host__ __device__ inline FilterLayout filter_layout(int n_stages) {
+__host__ __device__ inline FilterLayout filter_layout(int n_kblocks, int n_stages) {
   FilterLayout L;
-  L.b_off = 0;
+  L.a_off = 0;                                                    // user blocks 0 and 1, n_kblocks tiles each
+  L.b_off = L.a_off + 2u * static_cast<uint32_t>(n_kblocks) * kFATileBytes;
   L.buf_off = L.b_off + static_cast<uint32_t>(n_stages) * kFBTileBytes;
-  L.bar_off = L.buf_off + 2u * kFBlockM * kBufEntries * 8u;       // 64 KB of candidate buffers
+  L.acc_off = L.buf_off + 2u * kFBlockM * kBufEntries * 8u;       // 64 KB of candidate buffers
+  L.bar_off = L.acc_off + 2u * kFAccStageBytes;
   L.total = L.bar_off + 512u;
   return L;
 }
 // The B ring is organised in TILE slots of n_kblocks k-blocks (16 KB each): one full / one empty barrier per item tile.
-// barriers (uint64): [0..1] a_full (per user block) [2..4] tmem_full [5..7] tmem_empty [8 .. 8+T) b_full
-// [8+T .. 8+2T) b_empty, T = n_stages / n_kblocks tile slots; TMEM base address (uint32) at byte 400 of the block.
-// Accumulators: (tile it, user block b) is number q = 2 it + b and lives in TMEM slot q % 3 (its n-th use, n = q / 3,
-// has barrier parity n & 1).  Epilogue group b drains the accumulators of user block b: while it works on one, the
-// MMA warp can fill the next of either block.
+// barriers (uint64): [0..1] a_full (per user block) [2 .. 2+T) b_full [2+T .. 2+2T) b_empty, T = n_stages / n_kblocks
+// tile slots.  b_empty counts the 8 consumer warps of every CTA that received the tile.
 // The item biases are NOT staged: the hot loop needs only the block maximum (one cached global load per tile,
-// prefetched a tile ahead) and the rare admission path reads the few biases it needs through L2.  (A two-slot
-// shared-memory ring fed by one bulk copy per tile put the copy's ~2 us latency on the critical path of every
-// second tile: TRK_FILTER_DEBUG=6 showed 112 cycles per MMA step against 64 for the bare instruction stream.)
+// prefetched a tile ahead) and the rare admission path reads the few biases it needs through L2.
 
 __device__ __forceinline__ void f_sts64(uint32_t addr, float s, int32_t id) {
   asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(__float_as_uint(s)), "r"(id) : "memory");
@@ -275,7 +268,6 @@ __device__ __forceinline__ void compact_rows(unsigned rows, uint32_t buf_row_add
 // (no per-score bias load, no per-score FFMA) and one vote; only when some lane's bound passes are the exact v_j
 // formed.  The hitting lanes then append their survivors (approximate score + original item id) and rows whose buffer
 // passed half full are compacted by the whole warp.
-// (Voting once per 32 columns instead measured 7-11 % SLOWER at 1M x 1M x d128; the 16-column granularity stays.)
 // maximum of 16 columns; g[q] = maximum of columns [4q, 4q + 4) (the slow path looks only into the groups that pass)
 __device__ __forceinline__ float acc_max_16(const uint32_t* acc, float (&g)[4]) {
 #pragma unroll
@@ -386,16 +378,13 @@ __device__ __forceinline__ void filter_32(const uint32_t* acc, int32_t pos_base,
 
 // ---- first tile of a work unit: a threshold to start from -----------------------------------------------------------
 // With tau = -inf every column of the first tile is admitted: 128 appends and 8 warp-cooperative compactions per row,
-// 32 rows of a warp one after the other (~50 us per 256-user unit; 2 % of a 1M-item sweep but 15 % of a 125K-item
-// shard, which is what held the 8-GPU run at 0.74 of the tensor peak per shard).  Instead every thread first reduces
-// its row of the first accumulator to 16 group maxima (8 columns each), sorts them in registers and takes the k-th
-// largest, A: k DIFFERENT columns have acc >= A, their biases are >= the block minimum, so the k-th best approximate
-// score of the tile is >= fma(A, c, ub) + bmin and theta may start 2.25 m below that.  The tile is then filtered as
-// usual: ~1.5 k admissions per row instead of 128, no compaction.  (Measured at the 125K-item shard: -1.3 ms of 35.
-// Scanning MORE tiles first -- 4 to 32 tiles reduced to a running top-16 of group maxima, then filtered in a second
-// pass -- gained nothing: profiles/probe_r2_filter_shard8_scan_prologue.txt.  The cost of the admission path is
-// proportional to the number of 32-column chunks in which ANY of a warp's 32 rows passes its bound, ~25 ns of SM time
-// each at either size, and the early tiles are few chunks whatever they admit.)
+// 32 rows of a warp one after the other -- a cost per work unit that weighs most on short sweeps (item shards).
+// Instead every thread first reduces its row of the first accumulator to 16 group maxima (8 columns each), sorts them
+// in registers and takes the k-th largest, A: k DIFFERENT columns have acc >= A, their biases are >= the block
+// minimum, so the k-th best approximate score of the tile is >= fma(A, c, ub) + bmin and theta may start 2.25 m below
+// that.  The tile is then filtered as usual: ~1.5 k admissions per row instead of 128, no compaction.  The cost of the
+// admission path is proportional to the number of 32-column chunks in which ANY of a warp's 32 rows passes its bound,
+// and the early tiles are few chunks whatever they admit.
 __device__ __forceinline__ float acc_max_8(const uint32_t* acc) {
   return fmaxf(fmaxf(fmaxf(__uint_as_float(acc[0]), __uint_as_float(acc[1])),
                      fmaxf(__uint_as_float(acc[2]), __uint_as_float(acc[3]))),
@@ -422,35 +411,61 @@ __device__ __forceinline__ void sort16_desc(float (&g)[16]) {
   }
 }
 
-__device__ long long g_filter_debug_clock[2];   // {SM cycles, ns} of CTA 0, written in the timing-experiment modes only
+// Writes columns [32 c, 32 c + 32) of the warpgroup's 128 x 64 accumulator half (acc[m] = rows [64 m, 64 m + 64)) to
+// the staging tile: afterwards thread `wt` finds its row's 32 raw accumulators at stage + wt * kFStageStride (valid
+// until the next call), row-per-thread from the wgmma register layout.  The admission code reads them from there.
+template <int c>
+__device__ __forceinline__ void stage_chunk(const float (&acc0)[32], const float (&acc1)[32], float* stage, int wt,
+                                            int group) {
+  named_barrier_sync(1 + group, kFConsumerThreads);   // the previous chunk's rows have been read
+#pragma unroll
+  for (int i = 16 * c; i < 16 * c + 16; ++i) {
+    const int row = wgmma_acc_row(wt, i), col = wgmma_acc_col(wt, i) - 32 * c;
+    stage[row * kFStageStride + col] = acc0[i];
+    stage[(64 + row) * kFStageStride + col] = acc1[i];
+  }
+  named_barrier_sync(1 + group, kFConsumerThreads);
+}
+
+// 128 user rows x 64 items (column half `h` of the tile in B slot `b_slot`), fp16 hi x hi, fp32 accumulate
+template <int kNKB>
+__device__ __forceinline__ void filter_mma_half(float (&acc0)[32], float (&acc1)[32], uint32_t a_base, uint32_t b_slot,
+                                                int h) {
+  wgmma_fence();
+#pragma unroll
+  for (int kb = 0; kb < kNKB; ++kb) {
+#pragma unroll
+    for (int ks = 0; ks < kFKBlock / kFMmaK; ++ks) {
+      const uint64_t db = wgmma_desc_k_major_sw128(b_slot + kb * kFBTileBytes + h * (kFBTileBytes / 2)) + 2u * ks;
+      const uint64_t da = wgmma_desc_k_major_sw128(a_base + kb * kFATileBytes) + 2u * ks;
+      const uint32_t accumulate = static_cast<uint32_t>(kb > 0 || ks > 0);
+      wgmma_m64n64k16_f16(acc0, da, db, accumulate);
+      wgmma_m64n64k16_f16(acc1, da + ((kFATileBytes / 2) >> 4), db, accumulate);   // rows 64..127: +8 KB
+    }
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+}
 
 // kNKB: k-blocks of 64 per row (d_pad / 64).  kCluster: 1, or 2 = clusters of two CTAs that work on two different
 // 256-user groups over the SAME item tiles: each CTA fetches half of every tile and TMA-multicasts it into both CTAs'
-// shared memory, so the L2 -> SM stream of the item operand (1 TB per launch at 1M x 1M x d128, the second largest
-// consumer after the MMAs) is halved.
-// kTileEnd: compile the tile-end compaction pass in (see the epilogue).  It pays for short sweeps, where the admission
-// path is a large share of the time, and costs at long ones -- mostly through what its second inlined copy of the
-// compaction does to the hot loop's code, so it is a template parameter and not a run-time switch
-// (profiles/probe_r2_v18_filter_ab_*.txt: 125K items 32.35 -> 31.7 ms with it, 1M items 205.6 -> 209.3 ms).
-template <int kNKB, int kCluster, bool kTileEnd>
+// shared memory, so the L2 -> SM stream of the item operand is halved.
+template <int kNKB, int kCluster>
 __global__ void __launch_bounds__(kFThreads, 1)
-score_filter_kernel(const __grid_constant__ CUtensorMap map_items, const FilterParams p) {
+score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_constant__ CUtensorMap map_items,
+                    const FilterParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const FilterLayout L = filter_layout(p.n_stages);
+  const FilterLayout L = filter_layout(kNKB, p.n_stages);
   const int n_slots = p.n_stages / kNKB;   // B tile slots
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
   uint64_t* a_full = bars + 0;        // [user block]
-  uint64_t* tmem_full = bars + 2;     // [accumulator slot]
-  uint64_t* tmem_empty = bars + 5;
-  uint64_t* b_full = bars + 8;
-  uint64_t* b_empty = bars + 8 + n_slots;
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(smem + L.bar_off + 400);
+  uint64_t* b_full = bars + 2;
+  uint64_t* b_empty = bars + 2 + n_slots;
   constexpr uint32_t kSlotBytes = kNKB * kFBTileBytes;
 
   const int warp = threadIdx.x / 32;
   const int lane = threadIdx.x % 32;
-  constexpr int n_kb = kNKB;
   // work unit = (group of kCluster user pairs, item split); CTA `crank` of the cluster takes pair kCluster * g + crank
   const uint32_t crank = kCluster == 2 ? cluster_ctarank() : 0u;
   const int n_groups = (p.n_user_pairs + kCluster - 1) / kCluster;
@@ -458,43 +473,35 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_items, const FilterP
   const int64_t w_first = blockIdx.x / kCluster, w_step = gridDim.x / kCluster;
   constexpr uint16_t kClusterMask = (1u << kCluster) - 1u;
 
-  if (warp == 0 && lane == 0) tma_prefetch_desc(&map_items);
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&map_items);
+    tma_prefetch_desc(&map_users);
+  }
   if (warp == 1 && lane == 0) {
-    for (int i = 0; i < 2; ++i) mbar_init(a_full + i, 4);
-    for (int i = 0; i < kFAccSlots; ++i) {
-      mbar_init(tmem_full + i, 1);
-      mbar_init(tmem_empty + i, 4);
-    }
+    for (int i = 0; i < 2; ++i) mbar_init(a_full + i, 1);
     for (int i = 0; i < n_slots; ++i) {
       mbar_init(b_full + i, 1);
-      mbar_init(b_empty + i, kCluster);   // the MMA warps of all CTAs that received the tile
+      mbar_init(b_empty + i, 8 * kCluster);   // the consumer warps of all CTAs that received the tile
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc<kFTmemCols>(tmem_base_smem);
-  tcgen05_fence_before();
   __syncthreads();
   if (kCluster == 2) cluster_sync_all();   // the peer's barriers exist before anything is multicast to them
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
-  long long dbg_clk = 0, dbg_ns = 0;
-  if (p.debug_mode != 0 && blockIdx.x == 0 && threadIdx.x == 64) {   // timing experiments: SM clock under this load
-    dbg_clk = clock64();
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(dbg_ns));
-  }
 
   if (warp == 0) {
     // ===================================== TMA producer ======================================
-    {   // warp-uniform control flow, one elected lane issues (see the MMA warp)
+    {   // warp-uniform control flow, one elected lane issues
       int ts = 0;
-      uint32_t ts_phase = 0, filled = 0;
+      uint32_t ts_phase = 0;
       for (int64_t w = w_first; w < n_work; w += w_step) {
         const int sp = static_cast<int>(w / n_groups);
         const int t0 = sp * p.tiles_per_split;
         const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
         for (int t = t0; t < t1; ++t) {
-          if (p.debug_mode == 6 && filled >= static_cast<uint32_t>(n_slots)) continue;   // timing: no B stream
-          mbar_wait(b_empty + ts, ts_phase ^ 1);
+          if (kCluster == 2)
+            mbar_wait_cluster(b_empty + ts, ts_phase ^ 1);
+          else
+            mbar_wait(b_empty + ts, ts_phase ^ 1);
           if (elect_one()) {
             mbar_arrive_expect_tx(b_full + ts, kSlotBytes);
 #pragma unroll
@@ -509,76 +516,6 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_items, const FilterP
             }
           }
           __syncwarp();
-          ++filled;
-          if (++ts == n_slots) {
-            ts = 0;
-            ts_phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================================== MMA issuer ========================================
-    // The whole warp runs the (warp-uniform) control flow and polls the barriers; one elected lane issues.  Issuing
-    // from inside `if (lane == 0)` makes ptxas wrap every tcgen05.mma in an ELECT / R2UR.BROADCAST loop (~17
-    // instructions per MMA) because it cannot prove the operands uniform.
-    //
-    // The user operand is read from TENSOR MEMORY (tcgen05.mma [d], [a], b-desc): with both operands in shared memory
-    // an M = 128, N = 128, K = 16 step takes 77 cycles instead of the 64 of the math (scripts/mma_probe).
-    //
-    // This loop has to stay LEAN: one thread issues every MMA of the SM, and 8 MMA steps are only 512 cycles of tensor
-    // work.  With a runtime stage count the ring arithmetic (fill % n_stages, fill / n_stages: ~25 dependent
-    // instructions each through I2F / MUFU.RCP / F2I) plus the R2UR moves put ~450 cycles of scalar latency in front of
-    // every 4 steps and the pipe ran at 112 cycles per step (TRK_FILTER_DEBUG=6).  Now: ring positions advance
-    // incrementally, one full/empty barrier per item tile, all 8 steps of an accumulator issued from one elected
-    // block with compile-time offsets.
-    {
-      constexpr uint32_t idesc = umma_idesc_f16_f32(kFBlockM, kFBlockN);
-      int ts = 0;
-      uint32_t ts_phase = 0, witer = 0, slot = 0, slot_phase = 0, consumed = 0;
-      const uint32_t b_base = smem_u32(smem + L.b_off);
-      for (int64_t w = w_first; w < n_work; w += w_step) {
-        const int sp = static_cast<int>(w / n_groups);
-        const int t0 = sp * p.tiles_per_split;
-        const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
-        if (t1 <= t0) continue;
-        mbar_wait(a_full + 0, witer & 1);   // both groups have written their user block into tensor memory
-        mbar_wait(a_full + 1, witer & 1);
-        tcgen05_fence_after();
-        ++witer;
-        for (int t = t0; t < t1; ++t) {
-          const bool streamed = !(p.debug_mode == 6 && consumed >= static_cast<uint32_t>(n_slots));
-          if (streamed) mbar_wait(b_full + ts, ts_phase);
-          const uint64_t db = umma_desc_k_major_sw128(b_base + ts * kSlotBytes);
-#pragma unroll
-          for (int b = 0; b < 2; ++b) {     // one B tile, two user blocks, one accumulator each
-            mbar_wait(tmem_empty + slot, slot_phase ^ 1);
-            tcgen05_fence_after();
-            const uint32_t d_tmem = tmem_base + kFTmemAccCol + slot * kFBlockN;
-            const uint32_t a_tmem = tmem_base + b * 64;
-            if (elect_one()) {
-#pragma unroll
-              for (int kb = 0; kb < kNKB; ++kb)
-#pragma unroll
-                for (int ks = 0; ks < kFKBlock / kFUmmaK; ++ks)
-                  umma_f16_ts(d_tmem, a_tmem + kb * (kFKBlock / 2) + ks * (kFUmmaK / 2),
-                              db + static_cast<uint64_t>(kb * (kFBTileBytes >> 4) + 2 * ks), idesc,
-                              static_cast<uint32_t>(kb > 0 || ks > 0));
-              umma_commit(tmem_full + slot);
-              if (b == 1 && streamed) {
-                if (kCluster == 2)
-                  umma_commit_multicast(b_empty + ts, kClusterMask);
-                else
-                  umma_commit(b_empty + ts);
-              }
-            }
-            __syncwarp();
-            if (++slot == kFAccSlots) {
-              slot = 0;
-              slot_phase ^= 1;
-            }
-          }
-          ++consumed;
           if (++ts == n_slots) {
             ts = 0;
             ts_phase ^= 1;
@@ -587,26 +524,31 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_items, const FilterP
       }
     }
   } else if (warp >= 4) {
-    // ===================================== epilogue ==========================================
-    const int group = (warp - 4) / 4;
-    const int quarter = warp % 4;
-    const int row = quarter * 32 + lane;
+    // ================================ consumers: wgmma + admission ================================
+    const int group = warp / 4 - 1;
+    const int wt = threadIdx.x % kFConsumerThreads;
+    const int row = wt;                              // row inside the user block
     const float kNegInf = -__int_as_float(0x7f800000);
     const uint32_t buf_row_addr =   // group g owns user block g of the pair
         smem_u32(smem + L.buf_off) + static_cast<uint32_t>((group * kFBlockM + row) * kBufEntries * 8);
+    float* acc_stage = reinterpret_cast<float*>(smem + L.acc_off + group * kFAccStageBytes);
+    const uint32_t a_base = smem_u32(smem + L.a_off) + group * kNKB * kFATileBytes;
+    const uint32_t b_base = smem_u32(smem + L.b_off);
     const float max_item_norm = __ldg(p.item_stats + 0);
     const float item_scale = fmaxf(__ldg(p.item_stats + 1), 1e-38f);
     const float max_item_bias = __ldg(p.item_stats + 2);
     const AdmitCtx ctx = {p.item_bias, p.item_perm, p.item_id_offset, static_cast<int32_t>(p.n_items)};
-    const uint32_t tmem_lane = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    uint32_t slot = group, slot_use = 0;   // accumulator number q = 2 (tile count) + group: slot q % 3, use q / 3
+    int ts = 0;
+    uint32_t ts_phase = 0, witer = 0;
+    float acc0[32], acc1[32];
 
     for (int64_t w = w_first; w < n_work; w += w_step) {
       const int up = static_cast<int>(w % n_groups) * kCluster + static_cast<int>(crank);
       const int sp = static_cast<int>(w / n_groups);
       const int t0 = sp * p.tiles_per_split;
       const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
-      const int64_t u = (static_cast<int64_t>(up) * 2 + group) * kFBlockM + row;
+      const int64_t ublock_row0 = (static_cast<int64_t>(up) * 2 + group) * kFBlockM;
+      const int64_t u = ublock_row0 + row;
       const bool u_ok = u < p.n_users;
       const float su = u_ok ? __ldg(p.user_scale + u) : 1.0f;
       const float ubias = (u_ok && p.user_bias != nullptr) ? __ldg(p.user_bias + u) : 0.0f;
@@ -615,61 +557,47 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_items, const FilterP
       const float inv_c = 1.0f / c;
       // error bound of one approximate score: operand rounding + the fp32 rounding of the two bias adds
       const float m3 = kThetaMargins * (kMarginFactor * unorm * max_item_norm + kBiasUlps * (fabsf(ubias) + max_item_bias));
-      float tau = p.debug_mode == 4 ? -kNegInf : kNegInf, theta = kNegInf;   // 4: timing experiment, nothing admitted
+      float tau = kNegInf, theta = kNegInf;
       int cnt = 0, n_res = 0, n_ovf = 0;
       float drop_max = kNegInf;
-      uint32_t ra[32], rb[32];
+      const uint32_t* ra = reinterpret_cast<const uint32_t*>(acc_stage + wt * kFStageStride);   // this row, staged
 
       if (t1 > t0) {
-        // This row of the user operand (hi half, fp16) goes to tensor memory: lane = row, two values per column,
-        // k-block kb in columns [64 group + 32 kb, +32).  Every MMA that read the previous unit's block completed
-        // before this warp saw the tmem_full of that unit's last accumulator, so the columns are free.
-        const uint4* src = reinterpret_cast<const uint4*>(p.user_split + u * 2 * p.d_pad);
-        for (int kb = 0; kb < n_kb; ++kb) {
+        // this group's user block (hi half, fp16; rows past n_users arrive as zeros) goes to shared memory.  Every
+        // wgmma of the previous unit has completed in all four warps once they pass this barrier.
+        named_barrier_sync(1 + group, kFConsumerThreads);
+        if (wt == 0) {
+          mbar_arrive_expect_tx(a_full + group, kNKB * kFATileBytes);
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const uint4 v = u_ok ? __ldg(src + kb * 8 + i) : make_uint4(0u, 0u, 0u, 0u);
-            ra[4 * i + 0] = v.x;
-            ra[4 * i + 1] = v.y;
-            ra[4 * i + 2] = v.z;
-            ra[4 * i + 3] = v.w;
-          }
-          tmem_st_32x32b_x32(tmem_lane + group * 64 + kb * (kFKBlock / 2), ra);
+          for (int kb = 0; kb < kNKB; ++kb)
+            tma_load_2d(smem + L.a_off + (group * kNKB + kb) * kFATileBytes, &map_users, a_full + group, kb * kFKBlock,
+                        static_cast<int32_t>(ublock_row0), kEvictFirst);
         }
-        tmem_st_wait();
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(a_full + group);
+        mbar_wait(a_full + group, witer & 1);
+        ++witer;
       }
 
       float bmax_next = t1 > t0 ? __ldg(p.block_bias_max + t0) : 0.0f;
       for (int t = t0; t < t1; ++t) {
         const float bmax_scaled = bmax_next * inv_c;
         if (t + 1 < t1) bmax_next = __ldg(p.block_bias_max + t + 1);   // in flight while this tile is filtered
-        mbar_wait(tmem_full + slot, slot_use & 1);
-        tcgen05_fence_after();
-        const uint32_t taddr = tmem_lane + kFTmemAccCol + slot * kFBlockN;
+        mbar_wait(b_full + ts, ts_phase);
+        const uint32_t b_slot = b_base + ts * kSlotBytes;
         const int32_t pos0 = t * kFBlockN;
-        if (t == t0 && p.block_bias_min != nullptr && p.debug_mode == 0) {
+        if (t == t0 && p.block_bias_min != nullptr) {
           const float bmin = __ldg(p.block_bias_min + t0);   // the same for the whole CTA: warp-uniform branch
           if (bmin > kNegInf) {
             float g[16];
-            tmem_ld_32x32b_x32(taddr, ra);
-            tmem_ld_wait();
-            tmem_ld_32x32b_x32(taddr + 32, rb);
 #pragma unroll
-            for (int q = 0; q < 4; ++q) g[q] = acc_max_8(ra + 8 * q);
-            tmem_ld_wait();
-            tmem_ld_32x32b_x32(taddr + 64, ra);
+            for (int h = 0; h < 2; ++h) {
+              filter_mma_half<kNKB>(acc0, acc1, a_base, b_slot, h);
+              stage_chunk<0>(acc0, acc1, acc_stage, wt, group);
 #pragma unroll
-            for (int q = 0; q < 4; ++q) g[4 + q] = acc_max_8(rb + 8 * q);
-            tmem_ld_wait();
-            tmem_ld_32x32b_x32(taddr + 96, rb);
+              for (int q = 0; q < 4; ++q) g[8 * h + q] = acc_max_8(ra + 8 * q);
+              stage_chunk<1>(acc0, acc1, acc_stage, wt, group);
 #pragma unroll
-            for (int q = 0; q < 4; ++q) g[8 + q] = acc_max_8(ra + 8 * q);
-            tmem_ld_wait();
-#pragma unroll
-            for (int q = 0; q < 4; ++q) g[12 + q] = acc_max_8(rb + 8 * q);
+              for (int q = 0; q < 4; ++q) g[8 * h + 4 + q] = acc_max_8(ra + 8 * q);
+            }
             sort16_desc(g);
             float a_k = g[0];
 #pragma unroll
@@ -682,55 +610,39 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_items, const FilterP
             }
           }
         }
-        if (p.debug_mode == 2 || p.debug_mode == 6) goto drained;
-        if (p.debug_mode == 1) {
-          float acc_dbg = 0.0f;
-          for (int ch = 0; ch < kFBlockN / 32; ch += 2) {
-            tmem_ld_32x32b_x32(taddr + ch * 32, ra);
-            tmem_ld_32x32b_x32(taddr + (ch + 1) * 32, rb);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              acc_dbg = fmaxf(acc_dbg, fmaxf(__uint_as_float(ra[j]), __uint_as_float(rb[j])));
-          }
-          if (acc_dbg == 1.2345e30f) cnt = 1;
-          goto drained;
-        }
-        tmem_ld_32x32b_x32(taddr, ra);
-        tmem_ld_wait();
 #pragma unroll 1
-        for (int ch = 0; ch < kFBlockN / 32; ch += 2) {   // (compile-time bounds: a run-time bound here cost 2.5 %)
-          tmem_ld_32x32b_x32(taddr + (ch + 1) * 32, rb);   // in flight while chunk ch is filtered
-          filter_32(ra, pos0 + ch * 32, bmax_scaled, ctx, c, inv_c, ubias, tau, theta, drop_max, n_ovf, m3, buf_row_addr,
+        for (int h = 0; h < 2; ++h) {
+          filter_mma_half<kNKB>(acc0, acc1, a_base, b_slot, h);
+          if (h == 1) {   // the tile's last MMAs of this warp are complete: release the B slot in every CTA that got it
+            __syncwarp();
+            if (lane == 0) {
+              if (kCluster == 2) {
+#pragma unroll
+                for (uint32_t r = 0; r < kCluster; ++r) mbar_arrive_cluster(b_empty + ts, r);
+              } else {
+                mbar_arrive(b_empty + ts);
+              }
+            }
+          }
+          stage_chunk<0>(acc0, acc1, acc_stage, wt, group);
+          filter_32(ra, pos0 + h * 64, bmax_scaled, ctx, c, inv_c, ubias, tau, theta, drop_max, n_ovf, m3, buf_row_addr,
                     cnt, n_res, lane, p.k);
-          tmem_ld_wait();
-          if (ch + 2 < kFBlockN / 32) tmem_ld_32x32b_x32(taddr + (ch + 2) * 32, ra);
-          filter_32(rb, pos0 + (ch + 1) * 32, bmax_scaled, ctx, c, inv_c, ubias, tau, theta, drop_max, n_ovf, m3,
+          stage_chunk<1>(acc0, acc1, acc_stage, wt, group);
+          filter_32(ra, pos0 + h * 64 + 32, bmax_scaled, ctx, c, inv_c, ubias, tau, theta, drop_max, n_ovf, m3,
                     buf_row_addr, cnt, n_res, lane, p.k);
-          tmem_ld_wait();
         }
-      drained:
-        // accumulator and bias slot drained
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tmem_empty + slot);
-        // A compaction waits one L2 round trip for the biases / item ids of its new entries (almost all of shared memory
-        // is carved out: there is no L1 to speak of) -- ~0.8 us during which, in the middle of a tile, the warp's 32 rows
-        // stand still AND their accumulator slot stays occupied: the admission path cost ~10 ms of a 31 ms sweep of a
-        // 125K-item shard, the same at 1.45 and at 1.9 GHz (profiles/probe_r2_v9_filter_shard8_cool.txt).  So rows whose
-        // buffer is filling up are compacted HERE, after the slot has gone back to the MMA warp: the round trip overlaps
-        // the MMAs of this group's next accumulator (-1.5 ms of 32 at the shard with the trigger at 26 of 32 entries,
-        // profiles/probe_r2_v10_filter_shard8_tile_end_trigger.txt).  The mid-tile path remains for a row that overflows
-        // inside a tile.  Compiled in only for kTileEnd (short sweeps; see the template parameter).  (Measured and not kept: releasing the slot before the last chunk is filtered, and giving the
-        // MMA / TMA warps the highest warp ids -- both neutral: the epilogue warps' own time per tile is the limit.)
-        if (kTileEnd && p.debug_mode == 0) {
+        if (++ts == n_slots) {
+          ts = 0;
+          ts_phase ^= 1;
+        }
+        // A compaction waits one L2 round trip for the biases / item ids of its new entries -- during which, in the
+        // middle of a tile, the warp's 32 rows stand still.  So rows whose buffer is filling up are compacted HERE, at
+        // the end of the tile, where the round trip overlaps the other warpgroup's MMAs.  The mid-tile path remains for
+        // a row that overflows inside a tile.  (Measured on an H100 80GB HBM3 at 400 W, against a build without this
+        // pass: 1M-item sweep 1570 -> 1560 ms, 125K-item shard 186.0 -> 183.6 ms.)
+        {
           const unsigned early = __ballot_sync(0xffffffffu, cnt > p.tile_end_trigger);
           compact_rows(early, buf_row_addr, lane, p.k, cnt, n_res, theta, tau, drop_max, n_ovf, m3, ubias, c, inv_c, ctx);
-        }
-        slot += 2;                          // q += 2
-        if (slot >= kFAccSlots) {
-          slot -= kFAccSlots;
-          ++slot_use;
         }
       }
 
@@ -757,19 +669,8 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_items, const FilterP
     }
   }
 
-  tcgen05_fence_before();
   __syncthreads();
-  if (kCluster == 2) cluster_sync_all();   // no CTA leaves while its peer may still multicast into it
-  if (p.debug_mode != 0 && blockIdx.x == 0 && threadIdx.x == 64) {
-    long long ns;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
-    g_filter_debug_clock[0] = clock64() - dbg_clk;
-    g_filter_debug_clock[1] = ns - dbg_ns;
-  }
-  if (warp == 2) {
-    tcgen05_fence_after();
-    tmem_dealloc<kFTmemCols>(tmem_base);
-  }
+  if (kCluster == 2) cluster_sync_all();   // no CTA leaves while its peer may still multicast into it or arrive on it
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -954,36 +855,27 @@ int score_filter_f16(const void* user_split, const float* user_scale, const floa
   p.tiles_per_split = static_cast<int32_t>(ceil_div(p.n_tiles, n_splits));
   p.n_user_pairs = static_cast<int32_t>(ceil_div(n_users, 2 * kFBlockM));
   p.item_id_offset = item_id_offset;
-  // Tile-end compaction for sweeps of up to kTileEndMaxTiles item tiles per split (measured: helps at 125K items,
-  // costs at 1M; the crossover interpolates to ~380K).  TRK_FILTER_TILE_END_TRIGGER (probe knob): a value below
-  // kBufEntries forces it on with that trigger, kBufEntries or more forces it off.
-  bool tile_end = p.tiles_per_split <= kTileEndMaxTiles;
+  // Tile-end compaction trigger.  TRK_FILTER_TILE_END_TRIGGER (probe knob) sets it; kBufEntries or more turns the
+  // tile-end pass off (no buffer holds more than kBufEntries entries).
   p.tile_end_trigger = 26;
   {
     const char* env = getenv("TRK_FILTER_TILE_END_TRIGGER");
-    if (env != nullptr) {
-      tile_end = atoi(env) < kBufEntries;
-      if (tile_end) p.tile_end_trigger = atoi(env);
-    }
+    if (env != nullptr) p.tile_end_trigger = atoi(env) < kBufEntries ? atoi(env) : kBufEntries;
     if (p.tile_end_trigger < kKeepMax + 2) p.tile_end_trigger = kKeepMax + 2;   // (a compaction leaves up to kKeepMax)
   }
   p.cand_score = cand_score;
   p.cand_item = cand_item;
   p.row_theta = row_theta;
-  {
-    const char* dbg = getenv("TRK_FILTER_DEBUG");
-    p.debug_mode = dbg != nullptr ? atoi(dbg) : 0;
-  }
-  CUtensorMap map_items;
+  CUtensorMap map_users, map_items;
   int rc;
   p.n_stages = 0;
   for (int s = kFMaxStages; s >= 2; --s)
-    if (s % p.n_kblocks == 0 && filter_layout(s).total + 1024 <= kFSmemLimit) {
+    if (s % p.n_kblocks == 0 && filter_layout(p.n_kblocks, s).total + 1024 <= kFSmemLimit) {
       p.n_stages = s;
       break;
     }
   TRK_CHECK_ARG(p.n_stages >= 2 * p.n_kblocks, "score_filter: shared memory budget exceeded");
-  const uint32_t smem_bytes = filter_layout(p.n_stages).total + 1024;
+  const uint32_t smem_bytes = filter_layout(p.n_kblocks, p.n_stages).total + 1024;
 
   // Launch form: clusters of two CTAs sharing every item tile through TMA multicast (default when the device can keep
   // (almost) all SMs busy with 2-CTA clusters), else independent CTAs.  TRK_FILTER_CLUSTER=1|2 forces one.
@@ -992,10 +884,8 @@ int score_filter_f16(const void* user_split, const float* user_scale, const floa
     const char* env = getenv("TRK_FILTER_CLUSTER");
     if (env != nullptr && (atoi(env) == 1 || atoi(env) == 2)) cluster = atoi(env);
   }
-  auto kernel2 = tile_end ? (p.n_kblocks == 2 ? score_filter_kernel<2, 2, true> : score_filter_kernel<1, 2, true>)
-                          : (p.n_kblocks == 2 ? score_filter_kernel<2, 2, false> : score_filter_kernel<1, 2, false>);
-  auto kernel1 = tile_end ? (p.n_kblocks == 2 ? score_filter_kernel<2, 1, true> : score_filter_kernel<1, 1, true>)
-                          : (p.n_kblocks == 2 ? score_filter_kernel<2, 1, false> : score_filter_kernel<1, 1, false>);
+  auto kernel2 = p.n_kblocks == 2 ? score_filter_kernel<2, 2> : score_filter_kernel<1, 2>;
+  auto kernel1 = p.n_kblocks == 2 ? score_filter_kernel<2, 1> : score_filter_kernel<1, 1>;
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
   int max_clusters = 0;
@@ -1012,11 +902,11 @@ int score_filter_f16(const void* user_split, const float* user_scale, const floa
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     // the answer depends on (device, kernel, shared memory) only: asked once per device and kernel variant
-    static int cached_clusters[64][4];
-    static bool cached_valid[64][4];
+    static int cached_clusters[64][2];
+    static bool cached_valid[64][2];
     int device = 0;
     TRK_CHECK_CUDA(cudaGetDevice(&device));
-    const int variant = (p.n_kblocks == 2 ? 1 : 0) + (tile_end ? 2 : 0);
+    const int variant = p.n_kblocks == 2 ? 1 : 0;
     if (device >= 0 && device < 64 && cached_valid[device][variant]) {
       max_clusters = cached_clusters[device][variant];
     } else {
@@ -1035,25 +925,20 @@ int score_filter_f16(const void* user_split, const float* user_scale, const floa
   }
   rc = make_hi_map(&map_items, item_hi, n_items, d_pad, d_pad, kFBlockN / cluster);
   if (rc != TRK_OK) return rc;
+  rc = make_hi_map(&map_users, user_split, n_users, 2 * d_pad, d_pad, kFBlockM);   // the hi half of the split rows
+  if (rc != TRK_OK) return rc;
   if (cluster == 2) {
     const int64_t n_work = ceil_div(static_cast<int64_t>(p.n_user_pairs), 2) * n_splits;
     const int n_clusters = static_cast<int>(n_work < max_clusters ? n_work : max_clusters);
     cfg.gridDim = dim3(static_cast<unsigned>(2 * n_clusters));
-    TRK_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel2, map_items, p));
+    TRK_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel2, map_users, map_items, p));
   } else {
     TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel1, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     const int64_t n_work = static_cast<int64_t>(p.n_user_pairs) * n_splits;
     const int grid = static_cast<int>(n_work < sm_count() ? n_work : sm_count());
-    kernel1<<<grid, kFThreads, smem_bytes, stream>>>(map_items, p);
+    kernel1<<<grid, kFThreads, smem_bytes, stream>>>(map_users, map_items, p);
   }
   TRK_CHECK_LAUNCH();
-  if (p.debug_mode != 0) {   // timing experiments only: report the SM clock CTA 0 saw (synchronises)
-    long long clk[2] = {0, 0};
-    TRK_CHECK_CUDA(cudaStreamSynchronize(stream));
-    TRK_CHECK_CUDA(cudaMemcpyFromSymbol(clk, g_filter_debug_clock, sizeof(clk)));
-    fprintf(stderr, "[trk] score_filter debug=%d: %lld cycles in %.3f ms -> %.0f MHz\n", p.debug_mode, clk[0],
-            clk[1] * 1e-6, clk[1] > 0 ? clk[0] * 1e3 / static_cast<double>(clk[1]) : 0.0);
-  }
   return TRK_OK;
 }
 

@@ -7,7 +7,7 @@
 //
 // This is the any-shape, bit-deterministic path (k ascending, one fp32 FMA chain per output) that backs the
 // reference API at small sizes (tests, n_components not a multiple of 16, n_tastes > 1, attention).  The
-// throughput path is the tcgen05 kernel in score_topk_tc.cu.
+// throughput path is the wgmma kernel in score_topk_tc.cu.
 #include "common.cuh"
 
 namespace trk {

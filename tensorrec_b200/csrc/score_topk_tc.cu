@@ -1,4 +1,4 @@
-// K2 + K3 fused on tcgen05 tensor cores: user x item scores and the per-user top-k (or the dense score matrix),
+// K2 + K3 fused on Hopper tensor cores (wgmma): user x item scores and the per-user top-k (or the dense score matrix),
 // without the [n_users, n_items] matrix ever reaching HBM in the top-k form.
 //
 // Reference chain replaced: tf.matmul(user_repr, item_repr, transpose_b=True) (tensorrec/prediction_graphs.py:49-50,
@@ -6,42 +6,42 @@
 // (tensorrec/recommendation_graphs.py:41) and rank_predictions (:73-82) restricted to rank <= k.
 //
 // Arithmetic: operands are the split-fp16 rows written by K1 (hi | lo, per-row power-of-two scale).  Per 64-wide
-// k-block three tcgen05.mma groups accumulate hi.hi + lo.hi + hi.lo into ONE fp32 accumulator in tensor memory,
-// i.e. an fp32-grade dot product (the dropped lo.lo term is < 2^-22 relative) that is exact for integer-valued
+// k-block three groups of wgmma accumulate hi.hi + lo.hi + hi.lo into ONE fp32 register accumulator, i.e. an
+// fp32-grade dot product (the dropped lo.lo term is < 2^-22 relative) that is exact for integer-valued
 // representations -- which is what makes rank parity with the reference testable bit for bit.
 //
-// CTA = 384 threads, one CTA per SM, persistent over work items (user block of 128 rows, item split):
-//   warp 0      TMA producer: the A block (all k-blocks, resident for the whole sweep) then a ring of B k-block
-//               tiles [128 items x 64 fp16, 128B-swizzled] over the item range;
-//   warp 1      MMA issuer (one elected thread): M=128, N=128, K=16 instructions, four 128-column accumulators in
-//               TMEM; tcgen05.commit releases smem stages and publishes finished accumulators;
-//   warp 2      TMEM allocator;
-//   warps 4-7   epilogue group 0, warps 8-11 epilogue group 1: tiles alternate between the groups, each group owns two
-//               accumulators and two {scale, bias} slots fed by TMA; one thread per user row: tcgen05.ld 32 columns at a time, score = acc * scale_u *
-//               scale_i + bias_u + bias_i, compare against the row's current k-th best, rare insert into the row's
-//               sorted list in shared memory.  Items are visited in ascending id order and the compare is strict,
-//               so equal scores keep the lower item id first -- tf.nn.top_k's order.
+// CTA = 384 threads (three warpgroups), one CTA per SM, persistent over work items (user block of 128 rows, item split):
+//   warp 0        TMA producer: the A block (all k-blocks, resident for the whole sweep) then a ring of B k-block
+//                 tiles [128 items x 64 fp16, 128B-swizzled] over the item range;
+//   warpgroups 1, 2  consumers: warpgroup g owns user rows [64 g, 64 g + 64) of the block and computes, per item tile,
+//                 their 64 x 128 scores with m64n128k16 wgmma into registers.  The accumulator goes through a small
+//                 shared-memory staging tile (32 columns per half at a time) so that the epilogue runs one thread per
+//                 (user row, column half): score = acc * scale_u * scale_i + bias_u + bias_i, compare against that
+//                 list's current k-th best, rare insert into the sorted list in shared memory.  The two half-lists of
+//                 a row are merged at the end of the item range.  Items are visited in ascending id order and the
+//                 compare is strict, so equal scores keep the lower item id first -- tf.nn.top_k's order.
 #include "common.cuh"
 
 namespace trk {
 
 constexpr int kBlockM = 128;
-constexpr int kBlockN = 128;          // item tile; 4 accumulators of 128 columns fill the 512 TMEM columns
+constexpr int kBlockN = 128;          // item tile
 constexpr int kKBlock = 64;           // fp16 per 128-byte swizzle row
-constexpr int kUmmaK = 16;
+constexpr int kMmaK = 16;
 constexpr int kTcThreads = 384;
-constexpr int kEpiThreads = 128;      // per epilogue group
+constexpr int kConsumerThreads = 128; // per consumer warpgroup
+constexpr int kWgRows = 64;           // user rows per consumer warpgroup
+constexpr int kStageStride = 33;      // fp32 per staged row (32 columns + 1: conflict-free row reads)
 constexpr uint32_t kATileBytes = kBlockM * kKBlock * 2;   // 16 KB
 constexpr uint32_t kBTileBytes = kBlockN * kKBlock * 2;   // 16 KB
-constexpr uint32_t kMetaBytes = kBlockN * 8;              // {item scale, item bias} per column: 1 KB per tile
+constexpr uint32_t kAccStageBytes = 2u * kWgRows * kStageStride * 4u;   // per warpgroup: 2 halves x 64 rows x 32 cols
 constexpr int kMaxStages = 10;
-constexpr uint32_t kTmemCols = 512;
 constexpr int kMaxK = 32;
 
 struct TcParams {
   const float* user_scale;
   const float* user_bias;   // may be null
-  const float2* item_meta;  // [tiles*256] {scale, bias}; padding {0, -inf}
+  const float2* item_meta;  // [tiles*128] {scale, bias}; padding {0, -inf}
   int64_t n_users;
   int64_t n_items;
   int32_t n_kblocks;        // d_pad / 64  (hi half); the operand has 2*n_kblocks k-blocks
@@ -49,7 +49,7 @@ struct TcParams {
   int32_t k;                // top-k mode
   int32_t n_splits;
   int32_t tiles_per_split;
-  int32_t n_tiles;          // ceil(n_items / 256)
+  int32_t n_tiles;          // ceil(n_items / 128)
   int32_t n_user_blocks;
   int32_t item_id_offset;
   float* cand_score;        // top-k mode outputs
@@ -63,7 +63,7 @@ struct TcParams {
 
 // shared-memory carve-up (offsets from a 1024-byte aligned base)
 struct SmemLayout {
-  uint32_t a_off, b_off, list_score_off, list_item_off, meta_off, bar_off, total;
+  uint32_t a_off, b_off, list_score_off, list_item_off, acc_off, bar_off, total;
 };
 constexpr uint32_t kStoreTileBytes = 32 * 32 * 4;   // one warp's 32 rows x 32 columns of fp32 scores
 __host__ __device__ inline SmemLayout make_layout(int n_kblocks, int n_stages, int k, bool dense_staging = false) {
@@ -72,17 +72,14 @@ __host__ __device__ inline SmemLayout make_layout(int n_kblocks, int n_stages, i
   L.b_off = L.a_off + 2u * n_kblocks * kATileBytes;
   L.list_score_off = L.b_off + static_cast<uint32_t>(n_stages) * kBTileBytes;
   L.list_item_off = L.list_score_off + (dense_staging ? 16u * kStoreTileBytes : 2u * k * kBlockM * 4u);
-  L.meta_off = L.list_item_off + (dense_staging ? 0u : 2u * k * kBlockM * 4u);
-  L.bar_off = L.meta_off + 4u * kMetaBytes;      // 2 groups x 2 slots, filled by the TMA warp
+  L.acc_off = L.list_item_off + (dense_staging ? 0u : 2u * k * kBlockM * 4u);
+  L.bar_off = L.acc_off + 2u * kAccStageBytes;
   L.total = L.bar_off + 512u;
   return L;
 }
 
-// barrier block (uint64 each): [0] a_full, [1] a_empty, [2..5] tmem_full, [6..9] tmem_empty, [10..13] meta_full,
-// [14..17] meta_empty, [18 .. 18+S) b_full, [18+S .. 18+2S) b_empty; then the TMEM base address (uint32) at byte 400.
-// Tile `it` is drained by epilogue group g = it & 1; use = it >> 1 counts that group's tiles and
-// slot = g * 2 + (use & 1) names its accumulator and meta slot: two accumulators per group, so the MMA warp fills
-// one while the group drains the other.
+// barrier block (uint64 each): [0] a_full, [1] a_empty, [2 .. 2+S) b_full, [2+S .. 2+2S) b_empty.
+// Both consumer warpgroups read every stage: the empty barriers count the 8 consumer warps.
 
 __device__ __noinline__ float list_insert(float s, int32_t id, float* ls, int32_t* li, int k) {
   // ls/li point at this row's column of the [k][128] arrays.  Entries are sorted by (score desc, id asc) and the
@@ -99,20 +96,16 @@ __device__ __noinline__ float list_insert(float s, int32_t id, float* ls, int32_
   return ls[(k - 1) * kBlockM];
 }
 
-// 16-byte shared-memory load through the shared window (keeps the hot loop on LDS instead of generic LD)
-__device__ __forceinline__ float4 lds128(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-  return v;
-}
+// 16-byte read-only global load ({scale, bias} of two item columns; the 1 KB of a tile stays in L1)
+__device__ __forceinline__ float4 ldg128(const float2* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 
 // Scores one 32-column chunk held in r[] (raw accumulators in, final scores out) and returns the chunk maximum.
-// Branch-free: the 16 LDS.128 and 96 FP ops of a chunk pipeline freely; the rare insert path is taken per chunk.
-__device__ __forceinline__ float score_chunk(uint32_t (&r)[32], uint32_t meta_addr, float su, float ubias) {
+// Branch-free: the 16 loads and 96 FP ops of a chunk pipeline freely; the rare insert path is taken per chunk.
+__device__ __forceinline__ float score_chunk(uint32_t (&r)[32], const float2* meta, float su, float ubias) {
   float cmax = -__int_as_float(0x7f800000);
 #pragma unroll
   for (int j = 0; j < 32; j += 2) {
-    const float4 m = lds128(meta_addr + j * 8);   // {scale_j, bias_j, scale_j+1, bias_j+1}
+    const float4 m = ldg128(meta + j);   // {scale_j, bias_j, scale_j+1, bias_j+1}
     const float s0 = fmaf(__uint_as_float(r[j]), m.x * su, ubias) + m.y;       // (acc*scales + ub) + ib
     const float s1 = fmaf(__uint_as_float(r[j + 1]), m.z * su, ubias) + m.w;
     r[j] = __float_as_uint(s0);
@@ -124,10 +117,10 @@ __device__ __forceinline__ float score_chunk(uint32_t (&r)[32], uint32_t meta_ad
 
 // One 32-column chunk of one user row: final scores, then (top-k mode) the rare inserts, or (dense mode) the store.
 template <bool kDense>
-__device__ __forceinline__ void process_chunk(uint32_t (&r)[32], int c, int t, int32_t id0, uint32_t meta_base,
+__device__ __forceinline__ void process_chunk(uint32_t (&r)[32], int c, int t, int32_t id0, const float2* meta,
                                               float su, float ubias, float& thr, float* ls, int32_t* li,
                                               const TcParams& p, int64_t u, bool u_ok) {
-  const float cmax = score_chunk(r, meta_base + c * 32 * 8, su, ubias);
+  const float cmax = score_chunk(r, meta + c * 32, su, ubias);
   if constexpr (!kDense) {
     if (cmax > thr) {   // some column of this chunk enters the row's list (probability ~ 32 k / items seen)
 #pragma unroll
@@ -189,22 +182,17 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
   uint64_t* a_full = bars + 0;
   uint64_t* a_empty = bars + 1;
-  uint64_t* tmem_full = bars + 2;
-  uint64_t* tmem_empty = bars + 6;
-  uint64_t* meta_full = bars + 10;
-  uint64_t* meta_empty = bars + 14;
-  uint64_t* b_full = bars + 18;
-  uint64_t* b_empty = bars + 18 + p.n_stages;
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(smem + L.bar_off + 400);
+  uint64_t* b_full = bars + 2;
+  uint64_t* b_empty = bars + 2 + p.n_stages;
 
   const int warp = threadIdx.x / 32;
   const int lane = threadIdx.x % 32;
   constexpr int n_kb2 = 2 * kNKB;
   // work item w = (user block w / n_splits, item split w % n_splits): the splits of ONE user block go to consecutive
   // CTAs, so a handful of live user blocks (the device-side fallback: ~100 rows of a million) still spreads over the
-  // whole machine -- with the block index minor, one live block of 8 x 148 items landed on 37 of the 148 CTAs
+  // whole machine -- with the block index minor, one live block of 8 x 132 items landed on a quarter of the CTAs
   const int64_t n_work = static_cast<int64_t>(p.n_user_blocks) * p.n_splits;
-  // user blocks at or beyond this one hold no rows (every role skips them: the same test in all three loops)
+  // user blocks at or beyond this one hold no rows (every role skips them: the same test in both loops)
   const int live_blocks = p.n_users_live != nullptr
                               ? static_cast<int>(min(static_cast<int64_t>(p.n_user_blocks),
                                                      ceil_div(static_cast<int64_t>(__ldg(p.n_users_live)), kBlockM)))
@@ -216,32 +204,21 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
   }
   if (warp == 1 && lane == 0) {
     mbar_init(a_full, 1);
-    mbar_init(a_empty, 1);
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(tmem_full + i, 1);
-      mbar_init(tmem_empty + i, kEpiThreads / 32);
-      mbar_init(meta_full + i, 1);
-      mbar_init(meta_empty + i, kEpiThreads / 32);
-    }
+    mbar_init(a_empty, 2 * kConsumerThreads / 32);
     for (int i = 0; i < p.n_stages; ++i) {
       mbar_init(b_full + i, 1);
-      mbar_init(b_empty + i, 1);
+      mbar_init(b_empty + i, 2 * kConsumerThreads / 32);
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc<kTmemCols>(tmem_base_smem);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
 
   if (warp == 0) {
     // ===================================== TMA producer ======================================
-    {   // warp-uniform control flow, one elected lane issues (see the MMA warp)
+    {   // warp-uniform control flow, one elected lane issues
       int stage = 0;       // B ring position
       uint32_t stage_phase = 0;
       uint32_t witer = 0;  // non-empty work items so far
-      uint32_t it = 0;     // tiles issued so far
       for (int64_t w = blockIdx.x; w < n_work; w += gridDim.x) {
         const int ub = static_cast<int>(w / p.n_splits);
         const int sp = static_cast<int>(w % p.n_splits);
@@ -257,16 +234,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
         }
         __syncwarp();
         ++witer;
-        for (int t = t0; t < t1; ++t, ++it) {
-          // {item scale, item bias} of this tile for the epilogue group that will drain it
-          const uint32_t use = it >> 1, slot = (it & 1) * 2 + (use & 1);
-          mbar_wait(meta_empty + slot, ((use >> 1) & 1) ^ 1);
-          if (elect_one()) {
-            mbar_arrive_expect_tx(meta_full + slot, kMetaBytes);
-            bulk_load_1d(smem + L.meta_off + slot * kMetaBytes, p.item_meta + static_cast<int64_t>(t) * kBlockN,
-                         kMetaBytes, meta_full + slot);
-          }
-          __syncwarp();
+        for (int t = t0; t < t1; ++t) {
 #pragma unroll
           for (int kb = 0; kb < n_kb2; ++kb) {
             mbar_wait(b_empty + stage, stage_phase ^ 1);
@@ -284,86 +252,30 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================================== MMA issuer ========================================
-    // The whole warp runs the (warp-uniform) control flow and polls the barriers; one elected lane issues.  Issuing
-    // from inside `if (lane == 0)` makes ptxas wrap every tcgen05.mma in an ELECT / R2UR.BROADCAST loop (~17
-    // instructions per MMA) because it cannot prove the operands uniform.
-    {
-      constexpr uint32_t idesc = umma_idesc_f16_f32(kBlockM, kBlockN);
-      int stage = 0;
-      uint32_t stage_phase = 0, witer = 0, it = 0;  // it = accumulator tiles produced so far
-      const uint32_t a_base = smem_u32(smem + L.a_off);
-      const uint32_t b_base = smem_u32(smem + L.b_off);
-      for (int64_t w = blockIdx.x; w < n_work; w += gridDim.x) {
-        const int sp = static_cast<int>(w % p.n_splits);
-        const int t0 = sp * p.tiles_per_split;
-        const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
-        if (t1 <= t0 || static_cast<int>(w / p.n_splits) >= live_blocks) continue;
-        mbar_wait(a_full, witer & 1);
-        ++witer;
-        for (int t = t0; t < t1; ++t, ++it) {
-          const uint32_t use = it >> 1, buf = (it & 1) * 2 + (use & 1);
-          mbar_wait(tmem_empty + buf, ((use >> 1) & 1) ^ 1);  // the epilogue has drained this accumulator
-          tcgen05_fence_after();
-          const uint32_t d_tmem = tmem_base + buf * kBlockN;
-          // One thread issues every MMA of the SM and a k-block is only 4-8 MMA steps: the loop is unrolled over the
-          // (compile-time) k-blocks and the ring position advances incrementally -- `fill % n_stages` with a runtime
-          // stage count cost ~25 dependent instructions (I2F / MUFU.RCP / F2I) in front of every k-block and kept the
-          // tensor pipe at half rate (the same finding as in score_filter_tc.cu).
-#pragma unroll
-          for (int kb2 = 0; kb2 < n_kb2; ++kb2) {
-            mbar_wait(b_full + stage, stage_phase);
-            tcgen05_fence_after();
-            const uint64_t db = umma_desc_k_major_sw128(b_base + stage * kBTileBytes);
-            constexpr int kNKBc = kNKB;
-            const bool b_is_hi = kb2 < kNKBc;
-            const int kb = b_is_hi ? kb2 : kb2 - kNKBc;
-            // B hi block: A_hi[kb] x B and A_lo[kb] x B ;  B lo block: A_hi[kb] x B
-            if (elect_one()) {
-#pragma unroll
-              for (int a = 0; a < (b_is_hi ? 2 : 1); ++a) {
-                const uint64_t da = umma_desc_k_major_sw128(a_base + (a == 0 ? kb : kNKBc + kb) * kATileBytes);
-#pragma unroll
-                for (int ks = 0; ks < kKBlock / kUmmaK; ++ks) {
-                  // advancing 16 fp16 (32 bytes) inside the 128-byte swizzle atom = +2 in the address field
-                  umma_f16_ss(d_tmem, da + 2u * ks, db + 2u * ks, idesc,
-                              static_cast<uint32_t>(kb2 > 0 || a > 0 || ks > 0));
-                }
-              }
-              umma_commit(b_empty + stage);  // stage reusable once these MMAs have read it
-            }
-            __syncwarp();
-            if (++stage == p.n_stages) {
-              stage = 0;
-              stage_phase ^= 1;
-            }
-          }
-          if (elect_one()) umma_commit(tmem_full + buf);  // accumulator complete
-          __syncwarp();
-        }
-        if (elect_one()) umma_commit(a_empty);
-        __syncwarp();
-      }
-    }
   } else if (warp >= 4) {
-    // ===================================== epilogue ==========================================
-    const int group = (warp - 4) / 4;               // 0 or 1
-    const int quarter = warp % 4;                   // TMEM lane quarter this warp may access
-    const int row = quarter * 32 + lane;            // row inside the user block == TMEM lane
-    float* ls = reinterpret_cast<float*>(smem + L.list_score_off) + group * (kDense ? 0 : p.k) * kBlockM + row;
-    int32_t* li = reinterpret_cast<int32_t*>(smem + L.list_item_off) + group * (kDense ? 0 : p.k) * kBlockM + row;
+    // ================================ consumers: wgmma + epilogue ================================
+    const int g = warp / 4 - 1;                       // consumer warpgroup: user rows [64 g, 64 g + 64) of the block
+    const int wt = threadIdx.x % kConsumerThreads;    // thread of the warpgroup
+    const int half = wt / kWgRows;                    // epilogue: column half of the tile this thread scans
+    const int row = g * kWgRows + wt % kWgRows;       // epilogue: row inside the user block
+    float* ls = reinterpret_cast<float*>(smem + L.list_score_off) + half * (kDense ? 0 : p.k) * kBlockM + row;
+    int32_t* li = reinterpret_cast<int32_t*>(smem + L.list_item_off) + half * (kDense ? 0 : p.k) * kBlockM + row;
+    float* acc_stage = reinterpret_cast<float*>(smem + L.acc_off + g * kAccStageBytes);
     const float kNegInf = -__int_as_float(0x7f800000);
-    uint32_t it = 0;
     uint32_t n_stored = 0;   // dense TMA path: chunks stored by this warp (selects the staging buffer)
     const uint32_t stage_base = smem_u32(smem + L.list_score_off) + static_cast<uint32_t>(warp - 4) * 2u * kStoreTileBytes;
+    const uint32_t a_base = smem_u32(smem + L.a_off) + g * (kWgRows * 128);   // this warpgroup's 64 rows
+    const uint32_t b_base = smem_u32(smem + L.b_off);
+    int stage = 0;
+    uint32_t stage_phase = 0, witer = 0;
+    float acc[64];
 
     for (int64_t w = blockIdx.x; w < n_work; w += gridDim.x) {
       const int ub = static_cast<int>(w / p.n_splits);
       const int sp = static_cast<int>(w % p.n_splits);
       const int t0 = sp * p.tiles_per_split;
       const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
-      if (ub >= live_blocks) continue;
+      if (ub >= live_blocks) continue;   // (an empty split still emits its sentinel candidates)
       const int64_t u = static_cast<int64_t>(ub) * kBlockM + row;
       const bool u_ok = u < p.n_users;
       const float su = u_ok ? __ldg(p.user_scale + u) : 0.0f;
@@ -375,55 +287,72 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
           li[j * kBlockM] = 0x7fffffff;
         }
       }
-
-      for (int t = t0; t < t1; ++t, ++it) {
-        if (static_cast<int>(it & 1) != group) continue;
-        const uint32_t use = it >> 1, slot = group * 2 + (use & 1);
-        mbar_wait(meta_full + slot, (use >> 1) & 1);     // this tile's {item scale, item bias}, put there by TMA
-        mbar_wait(tmem_full + slot, (use >> 1) & 1);
-        tcgen05_fence_after();
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + slot * kBlockN;
-        const int32_t id0 = p.item_id_offset + t * kBlockN;
-        const uint32_t meta_base = smem_u32(smem + L.meta_off) + slot * kMetaBytes;
-        uint32_t ra[32], rb[32];
-        tmem_ld_32x32b_x32(taddr, ra);
-        tmem_ld_wait();
-#pragma unroll 1
-        for (int c = 0; c < kBlockN / 32; c += 2) {
-          tmem_ld_32x32b_x32(taddr + (c + 1) * 32, rb);   // in flight while chunk c is scored
-          if (kDense && p.tma_store) {
-            score_chunk(ra, meta_base + c * 32 * 8, su, ubias);
-            store_chunk_tma(ra, stage_base + (n_stored & 1) * kStoreTileBytes, lane, &map_out, t * kBlockN + c * 32,
-                            ub * kBlockM + quarter * 32);
-            ++n_stored;
-          } else {
-            process_chunk<kDense>(ra, c, t, id0, meta_base, su, ubias, thr, ls, li, p, u, u_ok);
-          }
-          tmem_ld_wait();
-          if (c + 2 < kBlockN / 32) tmem_ld_32x32b_x32(taddr + (c + 2) * 32, ra);
-          if (kDense && p.tma_store) {
-            score_chunk(rb, meta_base + (c + 1) * 32 * 8, su, ubias);
-            store_chunk_tma(rb, stage_base + (n_stored & 1) * kStoreTileBytes, lane, &map_out,
-                            t * kBlockN + (c + 1) * 32, ub * kBlockM + quarter * 32);
-            ++n_stored;
-          } else {
-            process_chunk<kDense>(rb, c + 1, t, id0, meta_base, su, ubias, thr, ls, li, p, u, u_ok);
-          }
-          tmem_ld_wait();
-        }
-        // accumulator drained: hand the TMEM buffer back to the MMA warp
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(tmem_empty + slot);
-          mbar_arrive(meta_empty + slot);
-        }
+      if (t1 > t0) {
+        mbar_wait(a_full, witer & 1);
+        ++witer;
       }
 
+      for (int t = t0; t < t1; ++t) {
+        // ---- 64 rows x 128 items: per B k-block hi: A_hi[kb] B + A_lo[kb] B, per B k-block lo: A_hi[kb] B ----
+#pragma unroll
+        for (int kb2 = 0; kb2 < n_kb2; ++kb2) {
+          mbar_wait(b_full + stage, stage_phase);
+          const uint64_t db = wgmma_desc_k_major_sw128(b_base + stage * kBTileBytes);
+          const bool b_is_hi = kb2 < kNKB;
+          const int kb = b_is_hi ? kb2 : kb2 - kNKB;
+          wgmma_fence();
+#pragma unroll
+          for (int a = 0; a < (b_is_hi ? 2 : 1); ++a) {
+            const uint64_t da = wgmma_desc_k_major_sw128(a_base + (a == 0 ? kb : kNKB + kb) * kATileBytes);
+#pragma unroll
+            for (int ks = 0; ks < kKBlock / kMmaK; ++ks)   // 16 fp16 (32 bytes) inside the swizzle atom = +2
+              wgmma_m64n128k16_f16(acc, da + 2u * ks, db + 2u * ks, static_cast<uint32_t>(kb2 > 0 || a > 0 || ks > 0));
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(b_empty + stage);   // this warp's part of the MMAs no longer reads the stage
+          if (++stage == p.n_stages) {
+            stage = 0;
+            stage_phase ^= 1;
+          }
+        }
+        // ---- epilogue: two rounds, each stages columns [32 c, 32 c + 32) of both 64-column halves ----
+        const int32_t id0 = p.item_id_offset + t * kBlockN;
+        const float2* meta = p.item_meta + static_cast<int64_t>(t) * kBlockN;
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          named_barrier_sync(1 + g, kConsumerThreads);   // the previous round's rows have been read
+#pragma unroll
+          for (int i = 0; i < 64; ++i) {
+            const int nb = i / 4;                          // 8-column block of the accumulator
+            if ((nb % 8) / 4 != c) continue;
+            const int col = wgmma_acc_col(wt, i);          // 0..127
+            acc_stage[((col / 64) * kWgRows + wgmma_acc_row(wt, i)) * kStageStride + col % 32] = acc[i];
+          }
+          named_barrier_sync(1 + g, kConsumerThreads);
+          uint32_t r[32];
+          const float* src = acc_stage + (half * kWgRows + wt % kWgRows) * kStageStride;
+#pragma unroll
+          for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(src[j]);
+          const int chunk = half * 2 + c;
+          if (kDense && p.tma_store) {
+            score_chunk(r, meta + chunk * 32, su, ubias);
+            store_chunk_tma(r, stage_base + (n_stored & 1) * kStoreTileBytes, lane, &map_out, t * kBlockN + chunk * 32,
+                            ub * kBlockM + g * kWgRows + (warp % 2) * 32);
+            ++n_stored;
+          } else {
+            process_chunk<kDense>(r, chunk, t, id0, meta, su, ubias, thr, ls, li, p, u, u_ok);
+          }
+        }
+      }
+      __syncwarp();
+      if (t1 > t0 && lane == 0) mbar_arrive(a_empty);   // this warp's MMAs of the work item are complete
+
       if constexpr (!kDense) {
-        // both groups have finished the item range: merge the two lists of each row and emit the candidates
-        named_barrier_sync(1, 2 * kEpiThreads);
-        if (group == 0 && u_ok) {
+        // both halves have finished the item range: merge the two lists of each row and emit the candidates
+        named_barrier_sync(1 + g, kConsumerThreads);
+        if (half == 0 && u_ok) {
           const float* l0s = ls;
           const int32_t* l0i = li;
           const float* l1s = ls + p.k * kBlockM;
@@ -441,19 +370,14 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
             b += take_a ? 0 : 1;
           }
         }
-        named_barrier_sync(1, 2 * kEpiThreads);   // lists may be re-initialised for the next work item
+        named_barrier_sync(1 + g, kConsumerThreads);   // lists may be re-initialised for the next work item
       }
     }
   }
 
   // ---- teardown ----
   if (kDense && p.tma_store && warp >= 4 && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-  tcgen05_fence_before();
   __syncthreads();
-  if (warp == 2) {
-    tcgen05_fence_after();
-    tmem_dealloc<kTmemCols>(tmem_base);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -499,7 +423,7 @@ int make_operand_map(CUtensorMap* map, const void* base, int64_t rows, int d_pad
   return TRK_OK;
 }
 
-constexpr uint32_t kSmemLimit = 232448;  // 227 KB opt-in limit per CTA on sm_100
+constexpr uint32_t kSmemLimit = 232448;  // 227 KB opt-in limit per CTA on sm_90
 
 int pick_stages(int n_kblocks, int k, bool dense_staging) {
   for (int s = kMaxStages; s >= 2; --s)

@@ -17,7 +17,7 @@ TILE_USERS = 128
 
 def require_cuda():
     if not torch.cuda.is_available():
-        raise RuntimeError('tensorrec_b200 runs its predict / predict_rank path on a CUDA device (B200, sm_100a) only; '
+        raise RuntimeError('tensorrec_b200 runs its predict / predict_rank path on a CUDA device (H100, sm_90a) only; '
                            'no CUDA device is visible and there is no CPU fallback')
     return _lib.load()
 

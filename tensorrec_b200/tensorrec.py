@@ -1,10 +1,10 @@
 """The TensorRec model class: same constructor, fit / fit_partial / predict / predict_rank / predict_* / save / load
 signatures and error behaviour as tensorrec/tensorrec.py, with the predict / predict_rank hot path evaluated by
-hand-written sm_100a kernels through the C ABI (include/tensorrec_b200.h):
+hand-written sm_90a kernels through the C ABI (include/tensorrec_b200.h):
 
     sparse features --K1 trk_csr_gather_reduce_f32--> representations (fp32 and/or split-fp16 operand)
                     --trk_csr_project_biases_f32--> user / item biases
-    predict():       K2 trk_score_dense_f16x3 (tcgen05) or trk_score_f32 (exact fp32, any shape)  -> [U, I] float32
+    predict():       K2 trk_score_dense_f16x3 (wgmma)   or trk_score_f32 (exact fp32, any shape)  -> [U, I] float32
     predict_rank():  ... + K3 trk_rank_full                                                      -> [U, I] int32
     predict_rank(k): K2+K3 fused trk_score_topk_f16x3 + trk_topk_merge (+ one NCCL all-gather when the item axis is
                      sharded over GPUs)                                                           -> top-k ids, scores
@@ -518,7 +518,7 @@ class TensorRec(object):
         return kernels.project_biases(sparse_input.device_csr(device), self._var(name, device).reshape(-1))
 
     def _tensor_path_ok(self, allow_tastes=False):
-        """Can the tcgen05 kernels evaluate this model?  allow_tastes: the fused top-k also covers n_tastes > 1 without
+        """Can the tensor-core kernels evaluate this model?  allow_tastes: the fused top-k also covers n_tastes > 1 without
         attention (one sweep per taste, then a de-duplicating merge: the prediction is the maximum over the tastes)."""
         if SCORE_PATH == 'exact':
             return False
@@ -526,7 +526,7 @@ class TensorRec(object):
               and (self.n_tastes == 1 or allow_tastes) and self.attention_graph_factory is None
               and kernels.d_pad_for(self.n_components) <= 128)
         if SCORE_PATH == 'tensor' and not ok:
-            raise RuntimeError('TENSORREC_B200_SCORE_PATH=tensor but this model cannot use the tcgen05 kernel')
+            raise RuntimeError('TENSORREC_B200_SCORE_PATH=tensor but this model cannot use the tensor-core kernel')
         return ok
 
     def _side_operands(self, side, sparse_in, device, for_filter=False, taste=0):
@@ -621,7 +621,7 @@ class TensorRec(object):
         return self._score_plan(item_in, device)(user_in)
 
     # a dense [n_users, n_items] result beyond this many bytes is produced in user blocks (SURVEY 8d: BASELINE config #2,
-    # 1M x 100K = 400 GB, exceeds the 180 GB of HBM): two device buffers + two page-locked host buffers of this size
+    # 1M x 100K = 400 GB, exceeds the 80 GB of an H100): two device buffers + two page-locked host buffers of this size
     PREDICT_BLOCK_BYTES = 4 << 30
 
     def _user_blocks(self, user_in, n_items, user_batch_size):

@@ -1,4 +1,4 @@
-"""GPU parity tests of every C-ABI kernel against the oracle (run on the B200 box: pytest -m gpu).
+"""GPU parity tests of every C-ABI kernel against the oracle (needs an H100: pytest -m gpu).
 
 Bars (BASELINE.json north_star): integer / index results bit-exact; fp32 scores within 1e-5 relative to |u|.|i|."""
 import json
@@ -502,7 +502,7 @@ def test_filter_candidates_respect_the_error_bound(K, sort_by_bias):
                                              (513, 40000, 64, 10, False), (1100, 3000, 128, 10, False)])
 @pytest.mark.parametrize('cluster', ['1', '2'])
 def test_filter_user_block_and_kblock_shapes(K, monkeypatch, cluster, U, I, d, k, integer):
-    """Ragged user blocks (U not a multiple of 256: rows past the end are zero rows in tensor memory), one and two
+    """Ragged user blocks (U not a multiple of 256: rows past the end arrive as zero rows), one and two
     k-blocks (d_pad 64 / 128), several work units per CTA; both launch forms: independent CTAs and clusters of two
     CTAs sharing the item tiles by TMA multicast (an odd number of 256-user groups leaves one CTA of the last cluster
     without users)."""
@@ -604,8 +604,8 @@ def test_filter_cluster_pairs_with_splits_and_a_ragged_last_tile(K, monkeypatch)
 
 @pytest.mark.parametrize('cluster', ['1', '2'])
 def test_filter_variants_with_and_without_the_tile_end_pass_agree(K, monkeypatch, cluster):
-    """The launch picks one of two compiled forms by sweep length (tile-end compaction for up to 3072 tiles per split);
-    the probe knob forces either on any shape: same certified result, bit for bit, and equal to the oracle's."""
+    """Tile-end compaction at the default trigger, at another trigger, and turned off by the probe knob: same certified
+    result, bit for bit, and equal to the oracle's."""
     monkeypatch.setenv('TRK_FILTER_CLUSTER', cluster)
     for (U, I, d, k, splits) in [(700, 40000, 128, 10, 1), (300, 9000, 64, 12, 2)]:
         uf, itf, wu, wi, bu, bi = make_case(U, I, d, False, seed=I, regime='indicator')
