@@ -120,7 +120,8 @@ int trk_rank_full(const float* scores, int32_t* ranks, int64_t n_users, int64_t 
                   size_t workspace_bytes, void* stream);
 /* order[ranks[i] - 1] = i for ONE row of ranks: the items of that row listed by reference rank (tf.nn.top_k order).
  * trk_rank_full on the 1 x n_items row of item biases followed by this call is the stable descending sort that fixes the
- * filter kernel's processing order (no library sort on the predict path). */
+ * filter kernel's processing order (no library sort of the items or of any score on the predict path; the only sort is
+ * the O(nnz) ordering of exclusion lists, see trk_exclusion_positions). */
 int trk_order_from_ranks(const int32_t* ranks, int64_t n, int32_t* order, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------
@@ -154,6 +155,41 @@ int trk_score_topk_f16x3(const void* user_split, const float* user_scale, const 
                          const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
                          int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset,
                          float* cand_score, int32_t* cand_item, const int32_t* n_users_live, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------
+ * Exclusion: the top-k among the items a user has NOT interacted with (serving, and the held-out evaluation protocol
+ * of tensorrec/eval.py:23,49,68-69 with the training interactions removed).  The result is the chain above on a model
+ * whose excluded pairs score -inf, with excluded items never reported: for every user the k best non-excluded items in
+ * tf.nn.top_k order (score descending, lower item id first); a user with fewer than k eligible items gets the sentinel
+ * (-inf, INT32_MAX) in the remaining slots.  An empty list leaves a row's result bit-identical to the calls without
+ * exclusion.
+ *
+ * Lists are CSR over the launch's user rows: int32 excl_indptr [rows + 1], int32 values per row strictly ascending.
+ *   trk_score_topk_f16x3_excl  the arguments of trk_score_topk_f16x3 plus excl_ids = LOCAL item ids (global id -
+ *                              item_id_offset, in [0, n_items)) and excl_row_map (may be NULL): user row u of the
+ *                              launch reads list row excl_row_map[u] -- the idx array of trk_select_flagged_rows, so
+ *                              the device-side fallback over gathered rows needs no gathered lists.  Rows at or beyond
+ *                              *n_users_live exclude nothing (their results are discarded).
+ *   trk_exclusion_positions    the filter kernel walks items in PROCESSING order (item_perm: position -> local id), so
+ *                              it takes each row's list as processing positions: inv_perm (int32 [n_items], workspace)
+ *                              = the inverse of item_perm, then out_keys[e] (int64 [nnz]) = (row << 32) | inv_perm[id]
+ *                              for every entry e of row `row` (item_perm NULL = identity, inv_perm unused).  Sorting
+ *                              out_keys ascending orders every row (rows are contiguous: excl_indptr is unchanged); the
+ *                              low 32 bits of the sorted keys are excl_pos.  That O(nnz) sort prepares the lists -- it
+ *                              is not part of the scoring.
+ *   trk_score_filter_f16_excl  the arguments of trk_score_filter_f16 plus excl_pos (processing positions, ascending).
+ *                              Excluded items leave the candidate universe (also in the first tile the starting
+ *                              threshold is taken from); the certificate of trk_rescore_topk_split is unchanged, and
+ *                              rows it flags are re-run through trk_score_topk_f16x3_excl with the same lists.
+ * ---------------------------------------------------------------------------------------------------- */
+int trk_score_topk_f16x3_excl(const void* user_split, const float* user_scale, const float* user_bias,
+                              const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
+                              int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset,
+                              float* cand_score, int32_t* cand_item, const int32_t* n_users_live,
+                              const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
+                              void* stream);
+int trk_exclusion_positions(const int32_t* item_perm, int64_t n_items, int32_t* inv_perm, const int32_t* excl_indptr,
+                            const int32_t* excl_ids, int64_t n_rows, int64_t* out_keys, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------
  * K2+K3 fused, FILTER form (the throughput path of predict_rank(k)): one tensor-core pass over the fp16 "hi"
@@ -200,6 +236,12 @@ int trk_score_filter_f16(const void* user_split, const float* user_scale, const 
                          const int32_t* item_perm, int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k,
                          int32_t n_splits, int32_t item_id_offset, float* cand_score, int32_t* cand_item,
                          float* row_theta, void* stream);
+int trk_score_filter_f16_excl(const void* user_split, const float* user_scale, const float* user_bias,
+                              const float* user_norm, const void* item_hi_global, const float* item_stats,
+                              const float* item_bias_padded, const float* block_bias_max, const float* block_bias_min,
+                              const int32_t* item_perm, int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k,
+                              int32_t n_splits, int32_t item_id_offset, float* cand_score, int32_t* cand_item,
+                              float* row_theta, const int32_t* excl_indptr, const int32_t* excl_pos, void* stream);
 /* item_split / item_scale / item_bias hold the rows of THIS shard: global id g lives at row g - item_id_offset.
  * n_lists = n_splits, list_width = 16.  Row u of the result is written at out_score + u * out_row_stride and
  * out_item + u * out_row_stride (both may point into one [n_users, 2k] exchange buffer: stride 2k, out_item =

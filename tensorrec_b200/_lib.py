@@ -40,6 +40,9 @@ SIGNATURES = {
     'trk_pack_item_meta': (ctypes.c_int, [_c_p, _c_p, _c_i64, _c_p, _c_i64, _c_p]),
     'trk_score_topk_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_p, _c_i64, _c_i64, _c_i32, _c_i32, _c_i32,
                                             _c_i32, _c_p, _c_p, _c_p, _c_p]),
+    'trk_score_topk_f16x3_excl': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_p, _c_i64, _c_i64, _c_i32, _c_i32, _c_i32,
+                                                 _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p]),
+    'trk_exclusion_positions': (ctypes.c_int, [_c_p, _c_i64, _c_p, _c_p, _c_p, _c_i64, _c_p, _c_p]),
     'trk_score_dense_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_p, _c_i64, _c_i64, _c_i32, _c_p, _c_i64,
                                              _c_p]),
     'trk_topk_merge': (ctypes.c_int, [_c_p, _c_p, _c_i64, _c_i32, _c_i32, _c_i32, _c_i64, _c_i64, _c_p, _c_p, _c_i64,
@@ -51,6 +54,9 @@ SIGNATURES = {
     'trk_pack_item_bias': (ctypes.c_int, [_c_p, _c_p, _c_i64, _c_p, _c_i64, _c_p, _c_p, _c_p, _c_p]),
     'trk_score_filter_f16': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_i64, _c_i64,
                                             _c_i32, _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p]),
+    'trk_score_filter_f16_excl': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_i64,
+                                                 _c_i64, _c_i32, _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p,
+                                                 _c_p]),
     'trk_rescore_topk_split': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_i64, _c_i64,
                                               _c_i32, _c_i32, _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_i64, _c_p, _c_p]),
     'trk_select_flagged_rows': (ctypes.c_int, [_c_p, _c_i64, _c_p, _c_i32, _c_p, _c_p]),

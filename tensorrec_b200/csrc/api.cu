@@ -41,7 +41,8 @@ int rank_full(const float*, int32_t*, int64_t, int64_t, void*, size_t, cudaStrea
 int order_from_ranks(const int32_t*, int64_t, int32_t*, cudaStream_t);
 int score_topk_max_k(int32_t);
 int score_topk_f16x3(const void*, const float*, const float*, const void*, const float*, int64_t, int64_t, int32_t,
-                     int32_t, int32_t, int32_t, float*, int32_t*, const int32_t*, cudaStream_t);
+                     int32_t, int32_t, int32_t, float*, int32_t*, const int32_t*, const int32_t*, const int32_t*,
+                     const int32_t*, cudaStream_t);
 int score_dense_f16x3(const void*, const float*, const float*, const void*, const float*, int64_t, int64_t, int32_t,
                       float*, int64_t, cudaStream_t);
 int topk_merge(const float*, const int32_t*, int64_t, int32_t, int32_t, int32_t, int64_t, int64_t, float*, int32_t*,
@@ -53,7 +54,9 @@ int rescale_hi_global(const void*, const float*, const float*, const int32_t*, i
 int pack_item_bias(const float*, const int32_t*, int64_t, float*, int64_t, float*, float*, float*, cudaStream_t);
 int score_filter_f16(const void*, const float*, const float*, const float*, const void*, const float*, const float*,
                      const float*, const float*, const int32_t*, int64_t, int64_t, int32_t, int32_t, int32_t, int32_t,
-                     float*, int32_t*, float*, cudaStream_t);
+                     float*, int32_t*, float*, const int32_t*, const int32_t*, cudaStream_t);
+int exclusion_positions(const int32_t*, int64_t, int32_t*, const int32_t*, const int32_t*, int64_t, int64_t*,
+                        cudaStream_t);
 int rescore_topk(const void*, const float*, const void*, const float*, const float*, const float*, const int32_t*,
                  const float*, const float*, const float*, int64_t, int64_t, int32_t, int32_t, int32_t, int32_t, int32_t,
                  float*, int32_t*, int64_t, int32_t*, cudaStream_t);
@@ -144,7 +147,19 @@ int trk_score_topk_f16x3(const void* user_split, const float* user_scale, const 
                          int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset, float* cand_score,
                          int32_t* cand_item, const int32_t* n_users_live, void* stream) {
   return trk::score_topk_f16x3(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k,
-                               n_splits, item_id_offset, cand_score, cand_item, n_users_live, trk::as_stream(stream));
+                               n_splits, item_id_offset, cand_score, cand_item, n_users_live, nullptr, nullptr, nullptr,
+                               trk::as_stream(stream));
+}
+
+int trk_score_topk_f16x3_excl(const void* user_split, const float* user_scale, const float* user_bias,
+                              const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
+                              int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset, float* cand_score,
+                              int32_t* cand_item, const int32_t* n_users_live, const int32_t* excl_indptr,
+                              const int32_t* excl_ids, const int32_t* excl_row_map, void* stream) {
+  TRK_CHECK_ARG(excl_indptr != nullptr && excl_ids != nullptr, "trk_score_topk_f16x3_excl: null exclusion list");
+  return trk::score_topk_f16x3(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k,
+                               n_splits, item_id_offset, cand_score, cand_item, n_users_live, excl_indptr, excl_ids,
+                               excl_row_map, trk::as_stream(stream));
 }
 
 int trk_score_dense_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
@@ -189,7 +204,27 @@ int trk_score_filter_f16(const void* user_split, const float* user_scale, const 
                          float* row_theta, void* stream) {
   return trk::score_filter_f16(user_split, user_scale, user_bias, user_norm, item_hi_global, item_stats,
                                item_bias_padded, block_bias_max, block_bias_min, item_perm, n_users, n_items, d_pad, k,
-                               n_splits, item_id_offset, cand_score, cand_item, row_theta, trk::as_stream(stream));
+                               n_splits, item_id_offset, cand_score, cand_item, row_theta, nullptr, nullptr,
+                               trk::as_stream(stream));
+}
+
+int trk_exclusion_positions(const int32_t* item_perm, int64_t n_items, int32_t* inv_perm, const int32_t* excl_indptr,
+                            const int32_t* excl_ids, int64_t n_rows, int64_t* out_keys, void* stream) {
+  return trk::exclusion_positions(item_perm, n_items, inv_perm, excl_indptr, excl_ids, n_rows, out_keys,
+                                  trk::as_stream(stream));
+}
+
+int trk_score_filter_f16_excl(const void* user_split, const float* user_scale, const float* user_bias,
+                              const float* user_norm, const void* item_hi_global, const float* item_stats,
+                              const float* item_bias_padded, const float* block_bias_max, const float* block_bias_min,
+                              const int32_t* item_perm, int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k,
+                              int32_t n_splits, int32_t item_id_offset, float* cand_score, int32_t* cand_item,
+                              float* row_theta, const int32_t* excl_indptr, const int32_t* excl_pos, void* stream) {
+  TRK_CHECK_ARG(excl_indptr != nullptr && excl_pos != nullptr, "trk_score_filter_f16_excl: null exclusion list");
+  return trk::score_filter_f16(user_split, user_scale, user_bias, user_norm, item_hi_global, item_stats,
+                               item_bias_padded, block_bias_max, block_bias_min, item_perm, n_users, n_items, d_pad, k,
+                               n_splits, item_id_offset, cand_score, cand_item, row_theta, excl_indptr, excl_pos,
+                               trk::as_stream(stream));
 }
 
 int trk_rescore_topk_split(const void* user_split, const float* user_scale, const void* item_split,

@@ -232,6 +232,25 @@ __device__ __forceinline__ void named_barrier_sync(uint32_t id, uint32_t threads
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
+// Exclusion lists (top-k of the items a user has not seen): CSR rows of ascending int32 values (item ids or processing
+// positions).  Index of the first value >= x in v[lo, hi), hi if there is none.
+__device__ __forceinline__ int excl_lower_bound(const int32_t* v, int lo, int hi, int32_t x) {
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(v + mid) < x)
+      lo = mid + 1;
+    else
+      hi = mid;
+  }
+  return lo;
+}
+// The first value >= x of CSR row `row`, INT32_MAX if there is none.
+__device__ __forceinline__ int32_t excl_next_at(const int32_t* indptr, const int32_t* v, int64_t row, int32_t x) {
+  const int hi = __ldg(indptr + row + 1);
+  const int i = excl_lower_bound(v, __ldg(indptr + row), hi, x);
+  return i < hi ? __ldg(v + i) : 0x7fffffff;
+}
+
 #endif  // __CUDACC__
 
 }  // namespace trk

@@ -81,6 +81,10 @@ struct FilterParams {
   float* cand_score;           // [n_users, n_splits, kKeepMax] approximate scores (sentinel -inf)
   int32_t* cand_item;          // [n_users, n_splits, kKeepMax] global ids (sentinel INT32_MAX)
   float* row_theta;            // [n_users, n_splits] final admission threshold (certified by rescore_topk_kernel)
+  // exclusion lists (kExclude instantiations only): row u's excluded items as PROCESSING positions, ascending, at
+  // excl_pos[excl_indptr[u] .. excl_indptr[u + 1])
+  const int32_t* excl_indptr;
+  const int32_t* excl_pos;
 };
 
 struct FilterLayout {
@@ -427,6 +431,25 @@ __device__ __forceinline__ void stage_chunk(const float (&acc0)[32], const float
   named_barrier_sync(1 + group, kFConsumerThreads);
 }
 
+// Exclusion (kExclude): every consumer thread keeps ONE register, `next` = the first excluded processing position of its
+// row at or after the chunk being filtered (INT32_MAX: none left).  When it falls inside the staged chunk [base,
+// base + 32) -- rare, divergent -- this writes -inf over the thread's own staged raw accumulators of every listed
+// position of the chunk (only this thread reads that staged row: no synchronisation) and moves `next` past the chunk.
+// A -inf accumulator never passes the admission bound (-inf + x > tau is false even for tau = -inf), and it is the
+// neutral element of the warm start's group maxima, so an excluded item neither becomes a candidate nor sets a threshold.
+__device__ __noinline__ void excl_mask_chunk(const int32_t* indptr, const int32_t* pos, int64_t u, int32_t base,
+                                             float* staged_row, int32_t& next) {
+  const int hi = __ldg(indptr + u + 1);
+  int i = excl_lower_bound(pos, __ldg(indptr + u), hi, base);
+  int32_t e = i < hi ? __ldg(pos + i) : 0x7fffffff;
+  while (e < base + 32) {
+    staged_row[e - base] = -__int_as_float(0x7f800000);
+    ++i;
+    e = i < hi ? __ldg(pos + i) : 0x7fffffff;
+  }
+  next = e;
+}
+
 // 128 user rows x 64 items (column half `h` of the tile in B slot `b_slot`), fp16 hi x hi, fp32 accumulate
 template <int kNKB>
 __device__ __forceinline__ void filter_mma_half(float (&acc0)[32], float (&acc1)[32], uint32_t a_base, uint32_t b_slot,
@@ -449,8 +472,9 @@ __device__ __forceinline__ void filter_mma_half(float (&acc0)[32], float (&acc1)
 
 // kNKB: k-blocks of 64 per row (d_pad / 64).  kCluster: 1, or 2 = clusters of two CTAs that work on two different
 // 256-user groups over the SAME item tiles: each CTA fetches half of every tile and TMA-multicasts it into both CTAs'
-// shared memory, so the L2 -> SM stream of the item operand is halved.
-template <int kNKB, int kCluster>
+// shared memory, so the L2 -> SM stream of the item operand is halved.  kExclude: mask the items of each row's exclusion
+// list (p.excl_indptr / p.excl_pos) out of the candidate universe, see excl_mask_chunk.
+template <int kNKB, int kCluster, bool kExclude = false>
 __global__ void __launch_bounds__(kFThreads, 1)
 score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_constant__ CUtensorMap map_items,
                     const FilterParams p) {
@@ -561,6 +585,11 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
       int cnt = 0, n_res = 0, n_ovf = 0;
       float drop_max = kNegInf;
       const uint32_t* ra = reinterpret_cast<const uint32_t*>(acc_stage + wt * kFStageStride);   // this row, staged
+      float* const ra_w = acc_stage + wt * kFStageStride;
+      int32_t excl_next = 0x7fffffff;   // kExclude: next excluded processing position >= the current chunk
+      if constexpr (kExclude) {
+        if (u_ok && t1 > t0) excl_next = excl_next_at(p.excl_indptr, p.excl_pos, u, t0 * kFBlockN);
+      }
 
       if (t1 > t0) {
         // this group's user block (hi half, fp16; rows past n_users arrive as zeros) goes to shared memory.  Every
@@ -588,13 +617,23 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
           const float bmin = __ldg(p.block_bias_min + t0);   // the same for the whole CTA: warp-uniform branch
           if (bmin > kNegInf) {
             float g[16];
+            // the tile is staged again by the filter below: the pre-pass masks with a copy of the cursor
+            int32_t pre_next = excl_next;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               filter_mma_half<kNKB>(acc0, acc1, a_base, b_slot, h);
               stage_chunk<0>(acc0, acc1, acc_stage, wt, group);
+              if constexpr (kExclude) {
+                if (pre_next < pos0 + h * 64 + 32)
+                  excl_mask_chunk(p.excl_indptr, p.excl_pos, u, pos0 + h * 64, ra_w, pre_next);
+              }
 #pragma unroll
               for (int q = 0; q < 4; ++q) g[8 * h + q] = acc_max_8(ra + 8 * q);
               stage_chunk<1>(acc0, acc1, acc_stage, wt, group);
+              if constexpr (kExclude) {
+                if (pre_next < pos0 + h * 64 + 64)
+                  excl_mask_chunk(p.excl_indptr, p.excl_pos, u, pos0 + h * 64 + 32, ra_w, pre_next);
+              }
 #pragma unroll
               for (int q = 0; q < 4; ++q) g[8 * h + 4 + q] = acc_max_8(ra + 8 * q);
             }
@@ -625,9 +664,17 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
             }
           }
           stage_chunk<0>(acc0, acc1, acc_stage, wt, group);
+          if constexpr (kExclude) {
+            if (excl_next < pos0 + h * 64 + 32)
+              excl_mask_chunk(p.excl_indptr, p.excl_pos, u, pos0 + h * 64, ra_w, excl_next);
+          }
           filter_32(ra, pos0 + h * 64, bmax_scaled, ctx, c, inv_c, ubias, tau, theta, drop_max, n_ovf, m3, buf_row_addr,
                     cnt, n_res, lane, p.k);
           stage_chunk<1>(acc0, acc1, acc_stage, wt, group);
+          if constexpr (kExclude) {
+            if (excl_next < pos0 + h * 64 + 64)
+              excl_mask_chunk(p.excl_indptr, p.excl_pos, u, pos0 + h * 64 + 32, ra_w, excl_next);
+          }
           filter_32(ra, pos0 + h * 64 + 32, bmax_scaled, ctx, c, inv_c, ubias, tau, theta, drop_max, n_ovf, m3,
                     buf_row_addr, cnt, n_res, lane, p.k);
         }
@@ -736,6 +783,28 @@ __global__ void rescale_hi_global_kernel(const __half* __restrict__ split, const
   }
 }
 
+// Exclusion lists in processing order.  inv[perm[p]] = p, then one warp per list row writes, for every excluded local
+// id of the row, the key (row << 32) | position.  Sorting the keys ascending orders every row's positions (the rows are
+// already contiguous, so the row pointer is unchanged): the low 32 bits of the sorted keys are the filter's excl_pos.
+__global__ void invert_perm_kernel(const int32_t* __restrict__ perm, int64_t n, int32_t* __restrict__ inv) {
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x)
+    inv[perm[i]] = static_cast<int32_t>(i);
+}
+__global__ void exclusion_keys_kernel(const int32_t* __restrict__ indptr, const int32_t* __restrict__ ids,
+                                      const int32_t* __restrict__ inv, int64_t rows, int64_t* __restrict__ keys) {
+  const int lane = threadIdx.x % 32;
+  const int64_t warp = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) / 32;
+  const int64_t n_warps = static_cast<int64_t>(gridDim.x) * blockDim.x / 32;
+  for (int64_t r = warp; r < rows; r += n_warps) {
+    const int e1 = indptr[r + 1];
+    for (int e = indptr[r] + lane; e < e1; e += 32) {
+      const int32_t pos = inv != nullptr ? inv[ids[e]] : ids[e];
+      keys[e] = static_cast<int64_t>(static_cast<uint64_t>(r) << 32 | static_cast<uint32_t>(pos));
+    }
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
@@ -812,14 +881,35 @@ int rescale_hi_global(const void* split, const float* scale, const float* stats,
   return TRK_OK;
 }
 
+int exclusion_positions(const int32_t* item_perm, int64_t n_items, int32_t* inv_perm, const int32_t* excl_indptr,
+                        const int32_t* excl_ids, int64_t n_rows, int64_t* out_keys, cudaStream_t stream) {
+  TRK_CHECK_ARG(excl_indptr && excl_ids && out_keys && n_rows >= 0 && n_items >= 0, "exclusion_positions: bad arguments");
+  TRK_CHECK_ARG(item_perm == nullptr || inv_perm != nullptr, "exclusion_positions: item_perm needs inv_perm");
+  if (item_perm != nullptr && n_items > 0) {
+    const int64_t blocks = ceil_div(n_items, 256);
+    const int64_t cap = static_cast<int64_t>(sm_count()) * 16;
+    invert_perm_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), 256, 0, stream>>>(item_perm, n_items,
+                                                                                                inv_perm);
+    TRK_CHECK_LAUNCH();
+  }
+  if (n_rows == 0) return TRK_OK;
+  const int64_t blocks = ceil_div(n_rows, 256 / 32);
+  const int64_t cap = static_cast<int64_t>(sm_count()) * 16;
+  exclusion_keys_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), 256, 0, stream>>>(
+      excl_indptr, excl_ids, item_perm != nullptr ? inv_perm : nullptr, n_rows, out_keys);
+  TRK_CHECK_LAUNCH();
+  return TRK_OK;
+}
+
 int score_filter_f16(const void* user_split, const float* user_scale, const float* user_bias,
                      const float* user_norm, const void* item_hi, const float* item_stats, const float* item_bias,
                      const float* block_bias_max, const float* block_bias_min, const int32_t* item_perm,
                      int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k, int32_t n_splits,
                      int32_t item_id_offset, float* cand_score, int32_t* cand_item, float* row_theta,
-                     cudaStream_t stream) {
+                     const int32_t* excl_indptr, const int32_t* excl_pos, cudaStream_t stream) {
   TRK_CHECK_ARG(user_split && user_scale && user_norm && item_hi && item_stats && item_bias && block_bias_max,
                 "score_filter: null input");
+  TRK_CHECK_ARG((excl_indptr == nullptr) == (excl_pos == nullptr), "score_filter: excl_indptr and excl_pos go together");
   TRK_CHECK_ARG(cand_score && cand_item && row_theta, "score_filter: null output");
   TRK_CHECK_ARG(n_users >= 1 && n_items >= 1 && n_splits >= 1, "score_filter: empty shape");
   TRK_CHECK_ARG(n_users < (1ll << 31) && n_items < (1ll << 31) - 512, "score_filter: shape exceeds int32 indexing");
@@ -866,6 +956,9 @@ int score_filter_f16(const void* user_split, const float* user_scale, const floa
   p.cand_score = cand_score;
   p.cand_item = cand_item;
   p.row_theta = row_theta;
+  p.excl_indptr = excl_indptr;
+  p.excl_pos = excl_pos;
+  const bool excl = excl_indptr != nullptr;
   CUtensorMap map_users, map_items;
   int rc;
   p.n_stages = 0;
@@ -884,8 +977,10 @@ int score_filter_f16(const void* user_split, const float* user_scale, const floa
     const char* env = getenv("TRK_FILTER_CLUSTER");
     if (env != nullptr && (atoi(env) == 1 || atoi(env) == 2)) cluster = atoi(env);
   }
-  auto kernel2 = p.n_kblocks == 2 ? score_filter_kernel<2, 2> : score_filter_kernel<1, 2>;
-  auto kernel1 = p.n_kblocks == 2 ? score_filter_kernel<2, 1> : score_filter_kernel<1, 1>;
+  auto kernel2 = excl ? (p.n_kblocks == 2 ? score_filter_kernel<2, 2, true> : score_filter_kernel<1, 2, true>)
+                     : (p.n_kblocks == 2 ? score_filter_kernel<2, 2> : score_filter_kernel<1, 2>);
+  auto kernel1 = excl ? (p.n_kblocks == 2 ? score_filter_kernel<2, 1, true> : score_filter_kernel<1, 1, true>)
+                     : (p.n_kblocks == 2 ? score_filter_kernel<2, 1> : score_filter_kernel<1, 1>);
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
   int max_clusters = 0;
@@ -902,11 +997,12 @@ int score_filter_f16(const void* user_split, const float* user_scale, const floa
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     // the answer depends on (device, kernel, shared memory) only: asked once per device and kernel variant
-    static int cached_clusters[64][2];
-    static bool cached_valid[64][2];
+    // (n_kblocks x exclusion)
+    static int cached_clusters[64][4];
+    static bool cached_valid[64][4];
     int device = 0;
     TRK_CHECK_CUDA(cudaGetDevice(&device));
-    const int variant = p.n_kblocks == 2 ? 1 : 0;
+    const int variant = (p.n_kblocks == 2 ? 1 : 0) + (excl ? 2 : 0);
     if (device >= 0 && device < 64 && cached_valid[device][variant]) {
       max_clusters = cached_clusters[device][variant];
     } else {

@@ -61,6 +61,15 @@ struct TcParams {
                                 // by the filter's certificate, counted on the device) -- later user blocks are skipped
 };
 
+// Exclusion lists (kExclude instantiations, top-k mode only): the excluded LOCAL item ids of list row r, ascending, at
+// ids[indptr[r] .. indptr[r + 1]); user row u reads list row row_map[u] (null = u).  A kernel parameter of its own:
+// TcParams keeps its size, so the instantiations without exclusion compile exactly as before.
+struct TcExcl {
+  const int32_t* indptr;
+  const int32_t* ids;
+  const int32_t* row_map;
+};
+
 // shared-memory carve-up (offsets from a 1024-byte aligned base)
 struct SmemLayout {
   uint32_t a_off, b_off, list_score_off, list_item_off, acc_off, bar_off, total;
@@ -115,6 +124,31 @@ __device__ __forceinline__ float score_chunk(uint32_t (&r)[32], const float2* me
   return cmax;
 }
 
+// Exclusion (kExclude): the final scores of the chunk's columns [base, base + 32) named in list row `xr` become -inf
+// (never inserted: the compare is strict and the lists start at -inf).  A select per register, not r[dynamic index],
+// which would put r[] into local memory; the FINAL score is masked, not the accumulator (a zero scale would turn -inf into
+// NaN).  Returns the new chunk maximum and moves `next` to the row's first listed id >= base + 32.
+__device__ __forceinline__ float excl_mask_scores(uint32_t (&r)[32], const TcExcl& x, int32_t xr, int32_t base,
+                                                  int32_t& next) {
+  const int hi = __ldg(x.indptr + xr + 1);
+  int i = excl_lower_bound(x.ids, __ldg(x.indptr + xr), hi, base);
+  int32_t e = i < hi ? __ldg(x.ids + i) : 0x7fffffff;
+  uint32_t mask = 0;
+  while (e < base + 32) {
+    mask |= 1u << (e - base);
+    ++i;
+    e = i < hi ? __ldg(x.ids + i) : 0x7fffffff;
+  }
+  next = e;
+  float cmax = -__int_as_float(0x7f800000);
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    r[j] = ((mask >> j) & 1u) ? 0xff800000u : r[j];
+    cmax = fmaxf(cmax, __uint_as_float(r[j]));
+  }
+  return cmax;
+}
+
 // One 32-column chunk of one user row: final scores, then (top-k mode) the rare inserts, or (dense mode) the store.
 template <bool kDense>
 __device__ __forceinline__ void process_chunk(uint32_t (&r)[32], int c, int t, int32_t id0, const float2* meta,
@@ -146,6 +180,32 @@ __device__ __forceinline__ void process_chunk(uint32_t (&r)[32], int c, int t, i
   }
 }
 
+// Per-row exclusion state of the exact kernel (empty without exclusion).
+template <bool kOn>
+struct ExclCursor {
+  int32_t row = -1;            // list row of this user row (-1: none)
+  int32_t next = 0x7fffffff;   // first listed id >= the current chunk (INT32_MAX: none left)
+};
+template <>
+struct ExclCursor<false> {};
+
+// Top-k mode with exclusion: process_chunk<false> with the row's listed columns masked after scoring.
+__device__ __forceinline__ void process_chunk_excl(uint32_t (&r)[32], int c, int t, int32_t id0, const float2* meta,
+                                                   float su, float ubias, float& thr, float* ls, int32_t* li,
+                                                   const TcParams& p, const TcExcl& x, int32_t xr,
+                                                   int32_t& excl_next) {
+  float cmax = score_chunk(r, meta + c * 32, su, ubias);
+  const int32_t base = t * kBlockN + c * 32;   // local id of the chunk's first column
+  if (excl_next < base + 32) cmax = excl_mask_scores(r, x, xr, base, excl_next);
+  if (cmax > thr) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      const float s = __uint_as_float(r[j]);
+      if (s > thr) thr = list_insert(s, id0 + c * 32 + j, ls, li, p.k);
+    }
+  }
+}
+
 // Dense mode, TMA path: the warp's 32 rows x 32 columns go to a 128B-swizzled staging tile in shared memory and
 // leave as ONE cp.async.bulk.tensor store (full 128-byte lines per row, rows / columns beyond the matrix clipped by the
 // tensor map).  Direct stores from the row-per-thread layout write 16 bytes per lane to 32 different rows.
@@ -171,10 +231,12 @@ __device__ __forceinline__ void store_chunk_tma(const uint32_t (&r)[32], uint32_
   }
 }
 
-template <bool kDense, int kNKB>   // kNKB = d_pad / 64 k-blocks per operand half
+// kNKB = d_pad / 64 k-blocks per operand half.  kExclude (top-k mode): columns named in the row's exclusion list are
+// left out of the top-k (excl_mask_scores).
+template <bool kDense, int kNKB, bool kExclude = false>
 __global__ void __launch_bounds__(kTcThreads, 1)
 score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_constant__ CUtensorMap map_items,
-                const __grid_constant__ CUtensorMap map_out, const TcParams p) {
+                const __grid_constant__ CUtensorMap map_out, const TcParams p, const TcExcl x) {
   extern __shared__ uint8_t smem_raw[];
   // 128B-swizzled tiles need a 1024-byte aligned base
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -281,6 +343,15 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
       const float su = u_ok ? __ldg(p.user_scale + u) : 0.0f;
       const float ubias = (u_ok && p.user_bias != nullptr) ? __ldg(p.user_bias + u) : 0.0f;
       float thr = kNegInf;
+      // kExclude: this row's list row and the first listed id >= the current chunk.  Rows of a gathered launch beyond
+      // *n_users_live have no map entry and are discarded by the caller: they exclude nothing.
+      ExclCursor<kExclude> xc;
+      if constexpr (kExclude) {
+        if (u_ok && t1 > t0 && (p.n_users_live == nullptr || u < __ldg(p.n_users_live))) {
+          xc.row = x.row_map != nullptr ? __ldg(x.row_map + u) : static_cast<int32_t>(u);
+          xc.next = excl_next_at(x.indptr, x.ids, xc.row, t0 * kBlockN);
+        }
+      }
       if constexpr (!kDense) {
         for (int j = 0; j < p.k; ++j) {
           ls[j * kBlockM] = kNegInf;
@@ -342,7 +413,10 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
                             ub * kBlockM + g * kWgRows + (warp % 2) * 32);
             ++n_stored;
           } else {
-            process_chunk<kDense>(r, chunk, t, id0, meta, su, ubias, thr, ls, li, p, u, u_ok);
+            if constexpr (kExclude)
+              process_chunk_excl(r, chunk, t, id0, meta, su, ubias, thr, ls, li, p, x, xc.row, xc.next);
+            else
+              process_chunk<kDense>(r, chunk, t, id0, meta, su, ubias, thr, ls, li, p, u, u_ok);
           }
         }
       }
@@ -443,6 +517,7 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
                      const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
                      int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset, float* cand_score,
                      int32_t* cand_item, float* dense_out, int64_t dense_stride, const int32_t* n_users_live,
+                     const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
                      cudaStream_t stream) {
   TRK_CHECK_ARG(user_split && user_scale && item_split && item_meta, "score_tc: null operand");
   TRK_CHECK_ARG(n_users >= 1 && n_items >= 1, "score_tc: empty shape");
@@ -464,6 +539,8 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
     TRK_CHECK_ARG(dense_out && dense_stride >= n_items, "score_dense: bad output");
   }
   TRK_CHECK_ARG(n_splits >= 1, "score_tc: n_splits < 1");
+  TRK_CHECK_ARG((excl_indptr == nullptr) == (excl_ids == nullptr) && (excl_indptr != nullptr || excl_row_map == nullptr),
+                "score_topk: excl_indptr and excl_ids go together (excl_row_map needs both)");
 
   TcParams p;
   p.user_scale = user_scale;
@@ -483,6 +560,7 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
   p.dense_out = dense_out;
   p.dense_stride = dense_stride;
   p.n_users_live = n_users_live;
+  const TcExcl x = {excl_indptr, excl_ids, excl_row_map};
   p.tma_store = (kDense && dense_stride % 4 == 0 && reinterpret_cast<uintptr_t>(dense_out) % 16 == 0) ? 1 : 0;
   p.n_stages = pick_stages(p.n_kblocks, p.k, p.tma_store != 0);
   TRK_CHECK_ARG(p.n_stages >= 2, "score_tc: shared memory budget exceeded (d_pad=%d k=%d)", d_pad, k);
@@ -509,11 +587,15 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
     }
   }
   const uint32_t smem_bytes = make_layout(p.n_kblocks, p.n_stages, p.k, p.tma_store != 0).total + 1024;
-  auto kernel = p.n_kblocks == 2 ? score_tc_kernel<kDense, 2> : score_tc_kernel<kDense, 1>;
+  decltype(&score_tc_kernel<kDense, 1>) kernel = nullptr;
+  if constexpr (!kDense) {
+    if (excl_indptr != nullptr) kernel = p.n_kblocks == 2 ? score_tc_kernel<false, 2, true> : score_tc_kernel<false, 1, true>;
+  }
+  if (kernel == nullptr) kernel = p.n_kblocks == 2 ? score_tc_kernel<kDense, 2> : score_tc_kernel<kDense, 1>;
   TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
   const int64_t n_work = static_cast<int64_t>(p.n_user_blocks) * n_splits;
   const int grid = static_cast<int>(n_work < sm_count() ? n_work : sm_count());
-  kernel<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, map_out, p);
+  kernel<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, map_out, p, x);
   TRK_CHECK_LAUNCH();
   return TRK_OK;
 }
@@ -521,9 +603,11 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
 int score_topk_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
                      const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
                      int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset, float* cand_score,
-                     int32_t* cand_item, const int32_t* n_users_live, cudaStream_t stream) {
+                     int32_t* cand_item, const int32_t* n_users_live, const int32_t* excl_indptr,
+                     const int32_t* excl_ids, const int32_t* excl_row_map, cudaStream_t stream) {
   return launch_tc<false>(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k,
-                          n_splits, item_id_offset, cand_score, cand_item, nullptr, 0, n_users_live, stream);
+                          n_splits, item_id_offset, cand_score, cand_item, nullptr, 0, n_users_live, excl_indptr,
+                          excl_ids, excl_row_map, stream);
 }
 
 int score_dense_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
@@ -536,7 +620,8 @@ int score_dense_f16x3(const void* user_split, const float* user_scale, const flo
   if (splits > n_tiles) splits = n_tiles;
   if (splits < 1) splits = 1;
   return launch_tc<true>(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, 0,
-                         static_cast<int32_t>(splits), 0, nullptr, nullptr, out, out_row_stride, nullptr, stream);
+                         static_cast<int32_t>(splits), 0, nullptr, nullptr, out, out_row_stride, nullptr, nullptr,
+                         nullptr, nullptr, stream);
 }
 
 }  // namespace trk

@@ -76,13 +76,15 @@ def union_of_indices(indices, n, group, device):
 
 
 def predict_top_k_sharded(model, user_features, item_features, k, group=None, to_host=True, gather='all',
-                          user_batch_size=None):
+                          user_batch_size=None, exclude=None):
     """Item-sharded predict_rank(k).  `item_features` is the FULL item matrix (scipy sparse); each rank slices its
-    contiguous shard, runs the fused kernel on it and takes part in the exchange."""
+    contiguous shard, runs the fused kernel on it and takes part in the exchange.  `exclude` (global item ids, see
+    TensorRec.predict_top_k) is the same matrix on every rank; each rank uses the columns of its shard."""
     world = dist.get_world_size(group)
     rank = dist.get_rank(group)
     lo, hi = shard_bounds(item_features.shape[0], world, rank)
     local_items = item_features.tocsr()[lo:hi] if hasattr(item_features, 'tocsr') else item_features[lo:hi]
     return model.predict_top_k(user_features, local_items, k, item_id_offset=lo,
                                gather_group=group if group is not None else dist.group.WORLD, to_host=to_host,
-                               gather=gather, user_batch_size=user_batch_size)
+                               gather=gather, user_batch_size=user_batch_size, **({} if exclude is None else
+                                                                               {'exclude': exclude}))

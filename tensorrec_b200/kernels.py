@@ -274,19 +274,27 @@ def default_splits(n_users, n_items):
 
 
 def score_topk(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k, n_splits=None,
-               item_id_offset=0, n_users_live=None):
+               item_id_offset=0, n_users_live=None, excl=None, excl_row_map=None):
     """K2+K3 fused.  Returns (cand_score [U, n_splits, k] f32, cand_item [U, n_splits, k] i32).
-    n_users_live: device int32 tensor; only its first element's worth of user rows is processed."""
+    n_users_live: device int32 tensor; only its first element's worth of user rows is processed.
+    excl: DeviceExclusion -- its items are left out of every row's top-k (user row u reads list row excl_row_map[u])."""
     lib = require_cuda()
     if n_splits is None:
         n_splits = default_splits(n_users, n_items)
     dev = user_split.device
     cand_score = torch.empty((n_users, n_splits, k), dtype=torch.float32, device=dev)
     cand_item = torch.empty((n_users, n_splits, k), dtype=torch.int32, device=dev)
-    rc = lib.trk_score_topk_f16x3(_p(user_split), _p(user_scale), _p(user_bias), _p(item_split), _p(item_meta),
-                                  n_users, n_items, int(d_pad), int(k), int(n_splits), int(item_id_offset),
-                                  _p(cand_score), _p(cand_item), _p(n_users_live), _stream())
-    _lib.check(rc, 'trk_score_topk_f16x3')
+    if excl is None:
+        rc = lib.trk_score_topk_f16x3(_p(user_split), _p(user_scale), _p(user_bias), _p(item_split), _p(item_meta),
+                                      n_users, n_items, int(d_pad), int(k), int(n_splits), int(item_id_offset),
+                                      _p(cand_score), _p(cand_item), _p(n_users_live), _stream())
+        _lib.check(rc, 'trk_score_topk_f16x3')
+    else:
+        rc = lib.trk_score_topk_f16x3_excl(_p(user_split), _p(user_scale), _p(user_bias), _p(item_split), _p(item_meta),
+                                           n_users, n_items, int(d_pad), int(k), int(n_splits), int(item_id_offset),
+                                           _p(cand_score), _p(cand_item), _p(n_users_live), _p(excl.indptr),
+                                           _p(excl.ids), _p(excl_row_map), _stream())
+        _lib.check(rc, 'trk_score_topk_f16x3_excl')
     return cand_score, cand_item
 
 
@@ -420,8 +428,10 @@ def bias_processing_order(item_bias):
 
 
 def score_filter(user_split, user_scale, user_bias, user_norm, item_hi, item_stats, item_bias_pad, block_bias_max,
-                 item_perm, n_users, n_items, d_pad, k, n_splits=None, item_id_offset=0, block_bias_min=None):
-    """Filter pass.  Returns (cand_score, cand_item [U, n_splits, 16], theta [U, n_splits])."""
+                 item_perm, n_users, n_items, d_pad, k, n_splits=None, item_id_offset=0, block_bias_min=None,
+                 excl=None):
+    """Filter pass.  Returns (cand_score, cand_item [U, n_splits, 16], theta [U, n_splits]).
+    excl: DeviceExclusion with its processing positions formed (exclusion_positions)."""
     lib = require_cuda()
     if n_splits is None:
         n_splits = default_splits(n_users, n_items)
@@ -430,11 +440,19 @@ def score_filter(user_split, user_scale, user_bias, user_norm, item_hi, item_sta
     cand_s = torch.empty((n_users, n_splits, width), dtype=torch.float32, device=dev)
     cand_i = torch.empty((n_users, n_splits, width), dtype=torch.int32, device=dev)
     theta = torch.empty((n_users, n_splits), dtype=torch.float32, device=dev)
-    rc = lib.trk_score_filter_f16(_p(user_split), _p(user_scale), _p(user_bias), _p(user_norm), _p(item_hi),
-                                  _p(item_stats), _p(item_bias_pad), _p(block_bias_max), _p(block_bias_min),
-                                  _p(item_perm), n_users, n_items, int(d_pad), int(k), int(n_splits),
-                                  int(item_id_offset), _p(cand_s), _p(cand_i), _p(theta), _stream())
-    _lib.check(rc, 'trk_score_filter_f16')
+    if excl is None:
+        rc = lib.trk_score_filter_f16(_p(user_split), _p(user_scale), _p(user_bias), _p(user_norm), _p(item_hi),
+                                      _p(item_stats), _p(item_bias_pad), _p(block_bias_max), _p(block_bias_min),
+                                      _p(item_perm), n_users, n_items, int(d_pad), int(k), int(n_splits),
+                                      int(item_id_offset), _p(cand_s), _p(cand_i), _p(theta), _stream())
+        _lib.check(rc, 'trk_score_filter_f16')
+    else:
+        rc = lib.trk_score_filter_f16_excl(_p(user_split), _p(user_scale), _p(user_bias), _p(user_norm), _p(item_hi),
+                                           _p(item_stats), _p(item_bias_pad), _p(block_bias_max), _p(block_bias_min),
+                                           _p(item_perm), n_users, n_items, int(d_pad), int(k), int(n_splits),
+                                           int(item_id_offset), _p(cand_s), _p(cand_i), _p(theta), _p(excl.indptr),
+                                           _p(excl.pos), _stream())
+        _lib.check(rc, 'trk_score_filter_f16_excl')
     return cand_s, cand_i, theta
 
 
@@ -543,11 +561,13 @@ class SideOperands(object):
                             self.d_pad, norm=cut(self.norm), stats=self.stats)
 
 
-def topk_exact(users, items, k, n_splits=None, item_id_offset=0, out=None, n_users_live=None):
+def topk_exact(users, items, k, n_splits=None, item_id_offset=0, out=None, n_users_live=None, excl=None,
+               excl_row_map=None):
     """Exact 3-pass fused kernel + merge -> PackedTopK [U, k]."""
     meta = pack_item_meta(items.scale, items.bias, items.n_rows)
     cs, ci = score_topk(users.split, users.scale, users.bias, items.split, meta, users.n_rows, items.n_rows,
-                        users.d_pad, k, n_splits=n_splits, item_id_offset=item_id_offset, n_users_live=n_users_live)
+                        users.d_pad, k, n_splits=n_splits, item_id_offset=item_id_offset, n_users_live=n_users_live,
+                        excl=excl, excl_row_map=excl_row_map)
     return topk_merge(cs, ci, k, out=out, n_users_live=n_users_live)
 
 
@@ -568,12 +588,12 @@ class FilterItems(object):
                                                                        perm=self.perm, want_min=True)
 
 
-def filter_and_rescore(users, items, fitems, user_norm, k, n_splits=None, item_id_offset=0, out=None):
+def filter_and_rescore(users, items, fitems, user_norm, k, n_splits=None, item_id_offset=0, out=None, excl=None):
     """(PackedTopK [U, k], flags [U]) -- flags mark users the certificate did not cover."""
     _, ci, theta = score_filter(users.split, users.scale, users.bias, user_norm, fitems.hi, fitems.stats,
                                 fitems.bias_pad, fitems.block_max, fitems.perm, users.n_rows, items.n_rows,
                                 users.d_pad, k, n_splits=n_splits, item_id_offset=item_id_offset,
-                                block_bias_min=fitems.block_min)
+                                block_bias_min=fitems.block_min, excl=excl)
     return rescore_topk(users, items, ci, theta, user_norm, fitems.stats, k, item_id_offset=item_id_offset, out=out)
 
 
@@ -592,14 +612,14 @@ def _ptr_at(t, index):
     return ctypes.c_void_p(t.data_ptr() + index * t.element_size())
 
 
-def rerun_uncertified(users, items, bad, top, k, item_id_offset=0):
+def rerun_uncertified(users, items, bad, top, k, item_id_offset=0, excl=None):
     """Users flagged by the certificate go through the exact kernel WITHOUT a host round trip: the flagged rows are
     compacted on the device, their operands gathered into a fixed-capacity buffer, the exact kernel runs over that buffer
     with the device-side count and the rows are scattered back into `top`.  Two tiers are launched, exactly one does
     work (decided on the device): up to FALLBACK_SMALL_ROWS rows (the normal case: ~0.01 % of the users) with as many
     item splits as it takes to fill the machine from one or two user blocks, or up to `capacity` rows with few splits.
     Returns (counters, capacity); counters[0] = flagged rows, > capacity means overflow (the caller checks it at its
-    next synchronisation)."""
+    next synchronisation).  excl: the exclusion lists of the users; the gathered rows read them through idx."""
     lib = require_cuda()
     dev = users.split.device
     cap = fallback_capacity(users.n_rows)
@@ -621,20 +641,89 @@ def rerun_uncertified(users, items, bad, top, k, item_id_offset=0):
         tiers.append((sub, cap, 3, None))
     for tier_rows, n_rows, slot, n_splits in tiers:
         live = counters[slot:slot + 1]
-        exact = topk_exact(tier_rows, items, k, n_splits=n_splits, item_id_offset=item_id_offset, n_users_live=live)
+        exact = topk_exact(tier_rows, items, k, n_splits=n_splits, item_id_offset=item_id_offset, n_users_live=live,
+                           excl=excl, excl_row_map=None if excl is None else idx)
         rc = lib.trk_scatter_topk_rows(_p(idx), _ptr_at(counters, slot), n_rows, exact.score_ptr(), exact.item_ptr(),
                                        2 * exact.k, int(k), top.score_ptr(), top.item_ptr(), 2 * top.k, _stream())
         _lib.check(rc, 'trk_scatter_topk_rows')
     return counters, cap
 
 
-def topk_filter(users, items, k, n_splits=None, item_id_offset=0, fitems=None):
+def topk_filter(users, items, k, n_splits=None, item_id_offset=0, fitems=None, excl=None):
     """Filter form: one tensor pass + re-scoring from the split operands; users whose error bound cannot be certified
     (buffer overflow under massive ties, bound violated) are re-run through the exact kernel on the device.
+    excl: DeviceExclusion of the users (its positions are formed here for fitems' processing order if missing).
     Returns (PackedTopK, counters device int32[2], capacity)."""
     user_norm = users.norm if users.norm is not None else operand_stats(users.split, users.scale, users.d_pad)
     if fitems is None:
         fitems = FilterItems(items)
-    top, bad = filter_and_rescore(users, items, fitems, user_norm, k, n_splits=n_splits, item_id_offset=item_id_offset)
-    counters, cap = rerun_uncertified(users, items, bad, top, k, item_id_offset=item_id_offset)
+    if excl is not None and excl.pos is None:
+        exclusion_positions(excl, fitems.perm, items.n_rows)
+    top, bad = filter_and_rescore(users, items, fitems, user_norm, k, n_splits=n_splits, item_id_offset=item_id_offset,
+                                  excl=excl)
+    counters, cap = rerun_uncertified(users, items, bad, top, k, item_id_offset=item_id_offset, excl=excl)
     return top, counters, cap
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# exclusion lists: the top-k among the items a user has not interacted with
+# ---------------------------------------------------------------------------------------------------------------
+def exclusion_host_csr(exclude, item_id_offset, n_items, u0=0, u1=None):
+    """Host preparation of an exclusion matrix (pure numpy / scipy, no device).
+
+    exclude: scipy sparse [n_users, >= item_id_offset + n_items], column = GLOBAL item id.  Returns the lists of user
+    rows [u0, u1) over the items [item_id_offset, item_id_offset + n_items) as (indptr int32 [rows + 1], ids int32):
+    duplicates summed, entries that are zero afterwards dropped (explicit zeros exclude nothing; negative values do
+    exclude), ids LOCAL (global - item_id_offset) and ascending within each row."""
+    csr = sp.csr_matrix(exclude)
+    u1 = csr.shape[0] if u1 is None else int(u1)
+    block = csr[int(u0):u1]
+    csr = block.copy() if np.shares_memory(block.data, csr.data) else block   # the caller's matrix is never modified
+    csr.sum_duplicates()             # sums duplicates and sorts the indices of every row
+    csr.eliminate_zeros()
+    keep = (csr.indices >= item_id_offset) & (csr.indices < item_id_offset + n_items)
+    rows = np.repeat(np.arange(csr.shape[0]), np.diff(csr.indptr))[keep]
+    ids = (csr.indices[keep].astype(np.int64) - item_id_offset).astype(np.int32)
+    indptr = np.zeros(csr.shape[0] + 1, dtype=np.int64)
+    np.cumsum(np.bincount(rows, minlength=csr.shape[0]), out=indptr[1:])
+    if indptr[-1] >= 2 ** 31 - 1:
+        raise ValueError('exclude holds more entries than int32 indexing covers')
+    return indptr.astype(np.int32), np.ascontiguousarray(ids)
+
+
+class DeviceExclusion(object):
+    """Exclusion lists of a block of user rows on the device: int32 indptr [rows + 1], int32 ids (local item ids,
+    ascending per row) for the exact kernel and -- once exclusion_positions ran -- int32 pos (processing positions,
+    ascending per row) for the filter kernel."""
+
+    def __init__(self, indptr, ids):
+        self.indptr, self.ids, self.pos = indptr, ids, None
+
+    @property
+    def n_rows(self):
+        return int(self.indptr.numel()) - 1
+
+    @classmethod
+    def upload(cls, indptr, ids, device):
+        require_cuda()
+        up = lambda a: torch.from_numpy(a).to(device, non_blocking=True)   # noqa: E731
+        # (an empty id array still gets a valid device pointer)
+        return cls(up(indptr), up(ids) if ids.size else torch.zeros((1,), dtype=torch.int32, device=device))
+
+
+def exclusion_positions(excl, perm, n_items):
+    """excl.pos = every row's excluded items as filter processing positions (perm: position -> local id, None =
+    identity), ascending: one kernel writes (row << 32 | position) keys, one sort of the keys orders every row (the
+    rows are contiguous, so indptr is unchanged)."""
+    if perm is None:
+        excl.pos = excl.ids         # identity order: the ascending ids are the positions
+        return excl
+    lib = require_cuda()
+    dev = excl.indptr.device
+    keys = torch.empty((int(excl.ids.numel()),), dtype=torch.int64, device=dev)   # (an empty list: one unused key)
+    inv = torch.empty((max(int(n_items), 1),), dtype=torch.int32, device=dev)
+    rc = lib.trk_exclusion_positions(_p(perm), int(n_items), _p(inv), _p(excl.indptr), _p(excl.ids), excl.n_rows,
+                                     _p(keys), _stream())
+    _lib.check(rc, 'trk_exclusion_positions')
+    excl.pos = (torch.sort(keys).values & 0xffffffff).to(torch.int32)
+    return excl

@@ -75,6 +75,23 @@ class _Hook(object):
         return '<graph hook {}>'.format(self.name)
 
 
+def _checked_exclude(exclude, n_users, n_items, k, item_id_offset, sharded):
+    """Validates predict_top_k's `exclude` (no device work) and returns it as a CSR matrix."""
+    if k is None:
+        raise ValueError('exclude needs k: exclusion applies to the top-k only, not to full ranks')
+    if not sp.issparse(exclude):
+        raise ValueError('exclude must be a scipy sparse matrix with one row per user')
+    if exclude.shape[0] != n_users:
+        raise ValueError('exclude has %d rows but there are %d users' % (exclude.shape[0], n_users))
+    if sharded:
+        if exclude.shape[1] < int(item_id_offset) + n_items:
+            raise ValueError('exclude has %d columns; this shard needs >= item_id_offset + n_items = %d'
+                             % (exclude.shape[1], int(item_id_offset) + n_items))
+    elif exclude.shape[1] != n_items:
+        raise ValueError('exclude has %d columns but there are %d items' % (exclude.shape[1], n_items))
+    return exclude if isinstance(exclude, sp.csr_matrix) else sp.csr_matrix(exclude)
+
+
 class TensorRec(object):
 
     def __init__(self,
@@ -717,14 +734,19 @@ class TensorRec(object):
             out[u0:u1] = block
         return out
 
-    def predict_rank(self, user_features, item_features, k=None):
+    def predict_rank(self, user_features, item_features, k=None, exclude=None):
         """Ranks for every user x item pair: int32 ndarray [n_users, n_items], 1 = best, ties by lower item index
         (tensorrec/tensorrec.py:705-733).  With k (an addition for shapes whose rank matrix cannot be materialised)
-        only the entries with rank <= k are produced, as a TopK(items, scores) -- see predict_top_k."""
+        only the entries with rank <= k are produced, as a TopK(items, scores) -- see predict_top_k, also for
+        `exclude` (top-k only: full ranks with exclusion raise ValueError)."""
         if self.tf_prediction is None:
             raise ModelNotFitException(method='predict_rank')
         if k is not None:
-            return self.predict_top_k(user_features, item_features, k)
+            if exclude is None:
+                return self.predict_top_k(user_features, item_features, k)
+            return self.predict_top_k(user_features, item_features, k, exclude=exclude)
+        if exclude is not None:
+            raise ValueError('exclude needs k: exclusion applies to the top-k only, not to full ranks')
         device = self._cuda_device()
         user_in = self._single_input(user_features, 'user_features')
         item_in = self._single_input(item_features, 'item_features')
@@ -734,7 +756,7 @@ class TensorRec(object):
         return kernels.to_host(kernels.rank_full(scores))
 
     def predict_top_k(self, user_features, item_features, k, item_id_offset=0, gather_group=None, to_host=True,
-                      gather='all', user_batch_size=None):
+                      gather='all', user_batch_size=None, exclude=None):
         """The k best items per user in reference rank order, without materialising the score matrix.
 
         Single GPU: K2+K3 fused kernel (filter form: one tensor pass + re-scoring of the survivors; users the
@@ -744,9 +766,23 @@ class TensorRec(object):
         top-k -- rank r receives the candidates of ITS slice of the users from every shard and merges them -- and,
         with gather='all', one all-gather of the merged slices so that every rank returns all users.  gather='slice'
         returns this rank's users only (rows `last_topk_info['user_rows']`).
-        user_batch_size: users are processed in blocks of this many rows (bounds device memory at 10M+ users)."""
+        user_batch_size: users are processed in blocks of this many rows (bounds device memory at 10M+ users).
+
+        exclude: None, or a scipy sparse matrix (any format) with n_users rows whose column index is the GLOBAL item id
+        (the numbering of TopK.items).  The pair (u, i) is excluded when exclude[u, i] != 0 after duplicates are summed
+        (explicit zeros exclude nothing, negative values do: "disliked" counts as seen).  Result: for every user the k
+        best NON-excluded items in reference rank order (score descending, lower item id on ties) -- the result of a
+        model whose excluded pairs score -inf, with excluded items never appearing; a user with fewer than k eligible
+        items gets (id 2**31 - 1, score -inf) in the remaining slots.  With n_tastes > 1 an item is excluded for every
+        taste.  exclude.shape[1] must equal n_items, or -- in sharded calls (item_id_offset != 0 or gather_group) -- be
+        >= item_id_offset + n_items; entries outside this shard are ignored, so every rank can pass the same matrix.
+        An exclude without non-zero entries gives results bit-identical to exclude=None."""
         if self.tf_prediction is None:
             raise ModelNotFitException(method='predict_rank')
+        if exclude is not None:      # validated before any device work
+            exclude = _checked_exclude(exclude, self._single_input(user_features, 'user_features').shape[0],
+                                       self._single_input(item_features, 'item_features').shape[0], k,
+                                       item_id_offset, item_id_offset != 0 or gather_group is not None)
         device = self._cuda_device()
         user_in = self._single_input(user_features, 'user_features')
         item_in = self._single_input(item_features, 'item_features')
@@ -761,6 +797,12 @@ class TensorRec(object):
         if n_users == 0:
             return TopK(np.zeros((0, k), np.int32), np.zeros((0, k), np.float32))
         from . import distributed
+
+        def block_exclusion(u0, u1):
+            """-> host lists (indptr, ids) of user rows [u0, u1) over this shard's items, or None"""
+            if exclude is None:
+                return None
+            return kernels.exclusion_host_csr(exclude, item_id_offset, n_items, u0, u1)
 
         fused = (self._tensor_path_ok(allow_tastes=True) and n_items > 0 and
                  k <= kernels.topk_max_k(kernels.d_pad_for(self.n_components)))
@@ -781,22 +823,29 @@ class TensorRec(object):
             blocks = [(u0, min(n_users, u0 + step), SparseInput(csr[u0:min(n_users, u0 + step)]))
                       for u0 in range(0, n_users, step)]
 
-        def run_taste(block_in, taste, force_exact):
+        def run_taste(block_in, taste, force_exact, excl):
             users = self._side_operands('user', block_in, device, for_filter=use_filter and not force_exact, taste=taste)
             if use_filter and not force_exact:
-                return kernels.topk_filter(users, items, k, item_id_offset=item_id_offset, fitems=fitems)
-            return kernels.topk_exact(users, items, k, item_id_offset=item_id_offset), None, 0
+                if excl is None:
+                    return kernels.topk_filter(users, items, k, item_id_offset=item_id_offset, fitems=fitems)
+                return kernels.topk_filter(users, items, k, item_id_offset=item_id_offset, fitems=fitems, excl=excl)
+            if excl is None:
+                return kernels.topk_exact(users, items, k, item_id_offset=item_id_offset), None, 0
+            return kernels.topk_exact(users, items, k, item_id_offset=item_id_offset, excl=excl), None, 0
 
-        def run_block(block_in, force_exact=False):
+        def run_block(block_in, u0, u1, force_exact=False):
             """-> (PackedTopK of the block, [(device counters | None, capacity)] of its sweeps)"""
+            host_excl = block_exclusion(u0, u1)
             if not fused:
-                return self._topk_from_dense(block_in, item_in, k, item_id_offset, device), [(None, 0)]
+                return self._topk_from_dense(block_in, item_in, k, item_id_offset, device, host_excl), [(None, 0)]
+            # every taste sweep of the block uses the same lists (an item is excluded for every taste)
+            excl = None if host_excl is None else kernels.DeviceExclusion.upload(*host_excl, device=device)
             if self.n_tastes == 1:
-                top, cnt, cap = run_taste(block_in, 0, force_exact)
+                top, cnt, cap = run_taste(block_in, 0, force_exact, excl)
                 return top, [(cnt, cap)]
             # mixture of tastes (no attention): prediction = max over tastes (recommendation_graphs.py:107), so the top-k
             # lies in the union of the per-taste top-k lists: one fused sweep per taste, then a de-duplicating merge
-            per_taste = [run_taste(block_in, t, force_exact) for t in range(self.n_tastes)]
+            per_taste = [run_taste(block_in, t, force_exact, excl) for t in range(self.n_tastes)]
             stacked = torch.stack([top.buf for top, _, _ in per_taste]).contiguous()          # [T, U_block, 2k]
             merged = kernels.topk_merge_received(stacked, block_in.shape[0], self.n_tastes, k, dedup=True)
             return merged, [(cnt, cap) for _, cnt, cap in per_taste]
@@ -811,7 +860,7 @@ class TensorRec(object):
 
         results, counters, rows = [], [], []
         for (u0, u1, block_in) in blocks:
-            top, sweeps = run_block(block_in)
+            top, sweeps = run_block(block_in, u0, u1)
             top, user_rows = exchange(top, u0, u1)
             results.append(top)
             counters.append(sweeps)
@@ -835,7 +884,7 @@ class TensorRec(object):
                 overflow = distributed.union_of_indices(overflow, len(blocks), gather_group, device)
             for b in overflow:
                 u0, u1, block_in = blocks[b]
-                top, _ = run_block(block_in, force_exact=True)
+                top, _ = run_block(block_in, u0, u1, force_exact=True)
                 results[b], rows[b] = exchange(top, u0, u1)
             info['overflow_blocks'] = len(overflow)
         info['user_rows'] = rows[0] if len(rows) == 1 else np.concatenate(rows)
@@ -845,16 +894,28 @@ class TensorRec(object):
             return TopK(top_i, top_s)
         return TopK(*kernels.to_host(top_i, top_s))
 
-    def _topk_from_dense(self, user_in, item_in, k, item_id_offset, device):
-        """Any model the fused kernel does not cover: dense scores -> exact full ranks -> the rank <= k entries."""
+    def _topk_from_dense(self, user_in, item_in, k, item_id_offset, device, host_excl=None):
+        """Any model the fused kernel does not cover: dense scores -> exact full ranks -> the rank <= k entries.
+        host_excl: exclusion lists (indptr, local ids) of the rows -- those scores become -inf before the ranking and
+        those entries are never emitted (their slots keep the sentinel)."""
         n_users, n_items = user_in.shape[0], item_in.shape[0]
         top = kernels.PackedTopK(n_users, k, device)
         top.scores.fill_(float('-inf'))
         top.items.fill_(2 ** 31 - 1)
         if n_items > 0:
             scores = self._predict_device(user_in, item_in, device)
+            excluded = None
+            if host_excl is not None:
+                indptr, ids = host_excl
+                ex_rows = torch.from_numpy(np.repeat(np.arange(n_users, dtype=np.int64), np.diff(indptr))).to(device)
+                ex_cols = torch.from_numpy(ids.astype(np.int64)).to(device)
+                scores[ex_rows, ex_cols] = float('-inf')
+                excluded = torch.zeros((n_users, n_items), dtype=torch.bool, device=device)
+                excluded[ex_rows, ex_cols] = True
             ranks = kernels.rank_full(scores).long()
             sel = ranks <= k
+            if excluded is not None:
+                sel &= ~excluded
             rows, cols = sel.nonzero(as_tuple=True)
             pos = ranks[rows, cols] - 1
             top.scores[rows, pos] = scores[rows, cols]
