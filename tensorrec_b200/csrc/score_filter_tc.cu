@@ -8,18 +8,20 @@
 //
 // CTA = 256 user rows (two 128-row blocks) x a sweep over 128-item tiles: every B tile fetched from L2 feeds two
 // warpgroups.  Warp 0 streams the item tiles with TMA; consumer warpgroup g (warps 4+4g..7+4g) loads user block g
-// (hi half, TMA) into shared memory once per work unit, computes each tile's 128 x 128 accumulator in two 64-column
-// halves with m64n64k16 wgmma into registers, and passes it through a 32-column shared-memory staging tile so that the
-// admission code runs one thread per user row.  While one warpgroup filters, the other's wgmma keeps the tensor cores
-// busy.
+// (hi half, TMA) into shared memory once per work unit and computes each tile's 128 x 128 accumulator in two 64-column
+// halves with m64n64k16 wgmma into registers.  Each consumer warp owns the 32 user rows whose accumulator fragments it
+// holds (lane l: row 16 w + l % 16 + 64 (l / 16) of the block), so the admission test of a 32-column chunk is a
+// register reduction plus shuffles inside the warp; only a chunk in which some row passes goes through the warp's own
+// shared-memory staging tile, where the admission code runs one lane per user row.  While one warpgroup filters, the
+// other's wgmma keeps the tensor cores busy.
 //
 // Why: the exact split-product kernel issues 3 tensor passes and its per-row sorted-list inserts serialise a warp.
 // Here
 //   * tensor work is 1 pass (2*U*I*d flops = the algorithmic count);
 //   * items are processed in descending-bias order (host side), so within a 128-item block the biases are almost equal
 //     and the admission test v_j = acc_j + bias_j / c > tau (c = user scale x GLOBAL item scale, both powers of two)
-//     is bounded by max_j acc_j + blockmax / c: the hot loop is an FMNMX3 tree over the raw accumulators, one add and
-//     one warp vote per 32 columns;
+//     is bounded by max_j acc_j + blockmax / c: the hot loop is an FMNMX tree over the raw accumulators in the wgmma
+//     fragments, four shuffles, one add and one warp vote per 32 columns;
 //   * a passing column is APPENDED raw (accumulator, position) to the row's 32-entry buffer in shared memory; when
 //     some row's buffer passes half full the whole warp compacts it cooperatively: one entry per lane, raw entries
 //     resolved to (approximate score, item id), a 15-step bitonic sort through shuffles, keep everything >= (k-th best
@@ -43,10 +45,10 @@ constexpr int kFKBlock = 64;
 constexpr int kFMmaK = 16;
 constexpr int kFThreads = 384;
 constexpr int kFConsumerThreads = 128; // per consumer warpgroup (= user rows of its block)
-constexpr int kFStageStride = 33;      // fp32 per staged row (32 columns + 1: conflict-free row reads)
 constexpr uint32_t kFBTileBytes = kFBlockN * kFKBlock * 2;   // 16 KB
 constexpr uint32_t kFATileBytes = kFBlockM * kFKBlock * 2;   // 16 KB
-constexpr uint32_t kFAccStageBytes = kFBlockM * kFStageStride * 4u;   // per warpgroup
+constexpr uint32_t kFWarpStageBytes = 32 * 32 * 4u;                     // 32 rows x 32 fp32 per consumer warp
+constexpr uint32_t kFAccStageBytes = 4 * kFWarpStageBytes;              // per warpgroup
 constexpr int kFMaxStages = 10;
 constexpr int kBufEntries = 32;      // candidate buffer per (row, epilogue group)
 constexpr int kKeepMax = 16;         // entries kept by a compaction (>= k + slack); also the per-group output width
@@ -268,10 +270,10 @@ __device__ __forceinline__ void compact_rows(unsigned rows, uint32_t buf_row_add
 
 // 16 columns of one user row per lane.  The admission test is v_j = acc_j + bias_j / c > tau.  Items are processed in
 // bias-sorted order, so the biases of one 128-item block differ by ~1e-4 of their range and v_j <= max_j acc_j +
-// bmax_block / c is a tight upper bound: the fast path is a pure FMNMX3 reduction of the raw accumulators plus ONE add
-// (no per-score bias load, no per-score FFMA) and one vote; only when some lane's bound passes are the exact v_j
-// formed.  The hitting lanes then append their survivors (approximate score + original item id) and rows whose buffer
-// passed half full are compacted by the whole warp.
+// bmax_block / c is a tight upper bound: the fast path (chunk_row_max in the kernel) is an FMNMX reduction of the raw
+// accumulators plus ONE add (no per-score bias load, no per-score FFMA) and one vote; only when some lane's bound
+// passes is the chunk staged and are the exact v_j formed.  The hitting lanes then append their survivors (approximate
+// score + original item id) and rows whose buffer passed half full are compacted by the whole warp.
 // maximum of 16 columns; g[q] = maximum of columns [4q, 4q + 4) (the slow path looks only into the groups that pass)
 __device__ __forceinline__ float acc_max_16(const uint32_t* acc, float (&g)[4]) {
 #pragma unroll
@@ -351,8 +353,9 @@ __device__ __forceinline__ void append_16(const uint32_t* acc, uint32_t mask, fl
   }
 }
 
-// 32 columns behind ONE vote (the two 16-column maxima are independent chains).  Slow path, taken when some lane's bound
-// passes (~8 % of the chunks of a 1M-item sweep, ~40 % at a 125K-item shard: 32 rows share the instruction stream): the
+// 32 columns of a staged row behind ONE vote (the two 16-column maxima are independent chains).  Runs only on a chunk
+// that the register fast path flagged, i.e. when some row of the warp passes its bound (32 rows share the instruction
+// stream; the vote here is the same predicate, so it passes too unless only an exclusion flagged the chunk): the
 // hitting lanes form the pass masks, ONE ballot tells whether every row's buffer can take its new entries -- the common
 // case: the hitting lanes append, nobody else does anything -- and only otherwise the chunk goes through the two-step
 // path (compact the rows that need it, append 16 columns at a time so that the 32-entry buffer cannot overflow between
@@ -415,39 +418,124 @@ __device__ __forceinline__ void sort16_desc(float (&g)[16]) {
   }
 }
 
-// Writes columns [32 c, 32 c + 32) of the warpgroup's 128 x 64 accumulator half (acc[m] = rows [64 m, 64 m + 64)) to
-// the staging tile: afterwards thread `wt` finds its row's 32 raw accumulators at stage + wt * kFStageStride (valid
-// until the next call), row-per-thread from the wgmma register layout.  The admission code reads them from there.
-template <int c>
-__device__ __forceinline__ void stage_chunk(const float (&acc0)[32], const float (&acc1)[32], float* stage, int wt,
-                                            int group) {
-  named_barrier_sync(1 + group, kFConsumerThreads);   // the previous chunk's rows have been read
-#pragma unroll
-  for (int i = 16 * c; i < 16 * c + 16; ++i) {
-    const int row = wgmma_acc_row(wt, i), col = wgmma_acc_col(wt, i) - 32 * c;
-    stage[row * kFStageStride + col] = acc0[i];
-    stage[(64 + row) * kFStageStride + col] = acc1[i];
-  }
-  named_barrier_sync(1 + group, kFConsumerThreads);
+// ---- a consumer warp's 32 rows: fragments, fast path, staging ------------------------------------------------------
+// wgmma_acc_row: lane l of warp w holds columns of block rows 16 w + l / 4 (+ 8) in acc0 and 64 + the same in acc1.
+// Lane L of the warp OWNS (keeps the admission state of) the row of class q = L / 8, quad g = L % 8, where class 0/1 =
+// acc0 row +0 / +8 and class 2/3 = acc1 row +0 / +8: block row 16 w + L % 16 + 64 (L / 16).  Its staged row is row L of
+// the warp's 32 x 32 staging tile.
+__device__ __forceinline__ int filter_owned_row(int warp_in_group, int lane) {
+  return 16 * warp_in_group + (lane & 15) + 64 * (lane >> 4);
 }
 
-// Exclusion (kExclude): every consumer thread keeps ONE register, `next` = the first excluded processing position of its
+// Maximum of the raw accumulators of columns [32 c, 32 c + 32) of the half, for the row this lane owns.  Each lane
+// reduces the 8 columns it holds of each of its 4 rows; a reduce-scatter through the quad (2 + 1 shuffles) leaves lane
+// l with the full maximum of class l % 4 of quad l / 4, and one more shuffle brings it to the owner.  fmaxf is exact,
+// so this is the maximum the staged row would give.
+template <int c>
+__device__ __forceinline__ float chunk_row_max(const float (&acc0)[32], const float (&acc1)[32], int lane) {
+  float m[4];
+#pragma unroll
+  for (int s = 0; s < 2; ++s) {   // registers 16 c + 4 j + 2 s + {0, 1}, j < 4: row +8 s, 8 columns
+    const int i = 16 * c + 2 * s;
+    m[s] = fmaxf(fmaxf(fmaxf(acc0[i], acc0[i + 1]), fmaxf(acc0[i + 4], acc0[i + 5])),
+                 fmaxf(fmaxf(acc0[i + 8], acc0[i + 9]), fmaxf(acc0[i + 12], acc0[i + 13])));
+    m[2 + s] = fmaxf(fmaxf(fmaxf(acc1[i], acc1[i + 1]), fmaxf(acc1[i + 4], acc1[i + 5])),
+                     fmaxf(fmaxf(acc1[i + 8], acc1[i + 9]), fmaxf(acc1[i + 12], acc1[i + 13])));
+  }
+  const bool b0 = (lane & 1) != 0, b1 = (lane & 2) != 0;
+  // step 1 (lane ^ 1): keep the classes with bit 0 = b0, send the other two
+  const float k0 = fmaxf(b0 ? m[1] : m[0], __shfl_xor_sync(0xffffffffu, b0 ? m[0] : m[1], 1));   // class b0
+  const float k1 = fmaxf(b0 ? m[3] : m[2], __shfl_xor_sync(0xffffffffu, b0 ? m[2] : m[3], 1));   // class 2 + b0
+  // step 2 (lane ^ 2): keep class b0 + 2 b1 = lane % 4
+  const float r = fmaxf(b1 ? k1 : k0, __shfl_xor_sync(0xffffffffu, b1 ? k0 : k1, 2));
+  return __shfl_sync(0xffffffffu, r, 4 * (lane & 7) + (lane >> 3));   // owner 8 q + g <- lane 4 g + q
+}
+
+// The staging tile of a warp: row r at r * 128 bytes, column x at word x ^ stage_swizzle(r % 8), an XOR of bits 2..4
+// that keeps 2- and 4-word groups together.  Stores (st.shared.v2: one quad-row of 8 columns per lane pair) and the
+// owner's row loads (ld.shared.v4) are both free of bank conflicts: a half-warp of stores covers quads g = 0..3 or
+// 4..7, whose swizzles 8 (g % 4) (+ 4) send its 16 column pairs to 16 different bank pairs; a quarter-warp of loads
+// reads 8 rows whose swizzles 4 * {0..7} differ, so its 16-byte groups land in 8 different bank quads.
+__device__ __forceinline__ uint32_t stage_swizzle(int g) { return 4u * static_cast<uint32_t>(((g & 3) << 1) | (g >> 2)); }
+__device__ __forceinline__ void f_sts32(uint32_t addr, float v) {
+  asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
+}
+
+// Writes columns [32 c, 32 c + 32) of the warp's four fragment rows of the 128 x 64 half to its staging tile (base
+// `stage`): afterwards lane L finds its row's 32 raw accumulators with load_staged_row.  Called warp-uniformly.
+template <int c>
+__device__ __forceinline__ void stage_warp_chunk(const float (&acc0)[32], const float (&acc1)[32], uint32_t stage,
+                                                 int lane) {
+  __syncwarp();   // every lane has read its row of the previous staged chunk
+  const int g = lane >> 2;
+  const uint32_t col0 = 2u * static_cast<uint32_t>(lane & 3) ^ stage_swizzle(g);
+  const uint32_t row_g = stage + 128u * g;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const uint32_t a = row_g + 4u * (col0 ^ (8u * j));
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      const int i = 16 * c + 4 * j + 2 * s;   // rows of class s (acc0) and 2 + s (acc1): tile rows 8 s + g, 16 + 8 s + g
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a + 1024u * s), "f"(acc0[i]), "f"(acc0[i + 1]) : "memory");
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a + 1024u * (2 + s)), "f"(acc1[i]), "f"(acc1[i + 1])
+                   : "memory");
+    }
+  }
+  __syncwarp();
+}
+// the 32 staged raw accumulators of the lane's own row, in column order
+__device__ __forceinline__ void load_staged_row(uint32_t stage, int lane, uint32_t (&v)[32]) {
+  const uint32_t row = stage + 128u * lane, sw = stage_swizzle(lane & 7);
+#pragma unroll
+  for (uint32_t q = 0; q < 8; ++q)
+    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(v[4 * q]), "=r"(v[4 * q + 1]), "=r"(v[4 * q + 2]), "=r"(v[4 * q + 3])
+                 : "r"(row + 4u * ((4u * q) ^ sw))
+                 : "memory");
+}
+
+// Exclusion (kExclude): every consumer lane keeps ONE register, `next` = the first excluded processing position of its
 // row at or after the chunk being filtered (INT32_MAX: none left).  When it falls inside the staged chunk [base,
-// base + 32) -- rare, divergent -- this writes -inf over the thread's own staged raw accumulators of every listed
-// position of the chunk (only this thread reads that staged row: no synchronisation) and moves `next` past the chunk.
-// A -inf accumulator never passes the admission bound (-inf + x > tau is false even for tau = -inf), and it is the
+// base + 32) -- rare, divergent -- this writes -inf over the lane's own staged raw accumulators of every listed
+// position of the chunk (only this lane reads that staged row: no synchronisation) and returns the new `next`, the
+// first listed position past the chunk.  A -inf accumulator never passes the admission bound (-inf + x > tau is false even for tau = -inf), and it is the
 // neutral element of the warm start's group maxima, so an excluded item neither becomes a candidate nor sets a threshold.
-__device__ __noinline__ void excl_mask_chunk(const int32_t* indptr, const int32_t* pos, int64_t u, int32_t base,
-                                             float* staged_row, int32_t& next) {
+__device__ __noinline__ int32_t excl_mask_chunk(const int32_t* indptr, const int32_t* pos, int64_t u, int32_t base,
+                                                uint32_t stage, int lane) {
+  const uint32_t row = stage + 128u * lane, sw = stage_swizzle(lane & 7);
   const int hi = __ldg(indptr + u + 1);
   int i = excl_lower_bound(pos, __ldg(indptr + u), hi, base);
   int32_t e = i < hi ? __ldg(pos + i) : 0x7fffffff;
   while (e < base + 32) {
-    staged_row[e - base] = -__int_as_float(0x7f800000);
+    f_sts32(row + 4u * (static_cast<uint32_t>(e - base) ^ sw), -__int_as_float(0x7f800000));
     ++i;
     e = i < hi ? __ldg(pos + i) : 0x7fffffff;
   }
-  next = e;
+  return e;
+}
+
+// Columns [32 kC, 32 kC + 32) of the half in acc0 / acc1, processing positions [base, base + 32).  Fast path: the owner
+// of each row tests its register maximum against tau (and, kExclude, whether its next excluded position lies in the
+// chunk); one vote.  Most chunks stop here with no shared-memory traffic.  Otherwise the warp stages the chunk, masks
+// excluded positions, and every lane runs filter_32 on its row from registers.  Called warp-uniformly.
+template <int kC, bool kExclude>
+__device__ __forceinline__ void filter_chunk(const float (&acc0)[32], const float (&acc1)[32], int32_t base,
+                                             float bmax_scaled, uint32_t stage, int lane, int64_t u,
+                                             const FilterParams& p, int32_t& excl_next, const AdmitCtx& ctx, float c,
+                                             float inv_c, float ubias, float& tau, float& theta, float& drop_max,
+                                             int& n_ovf, float m3, uint32_t buf_row_addr, int& cnt, int& n_res) {
+  const float amax = chunk_row_max<kC>(acc0, acc1, lane);
+  bool flag = amax + bmax_scaled > tau;   // == the h0 || h1 of filter_32: x -> x + bmax is monotonic
+  if constexpr (kExclude) flag = flag || excl_next < base + 32;
+  if (!__any_sync(0xffffffffu, flag)) return;
+  stage_warp_chunk<kC>(acc0, acc1, stage, lane);
+  if constexpr (kExclude) {
+    if (excl_next < base + 32) excl_next = excl_mask_chunk(p.excl_indptr, p.excl_pos, u, base, stage, lane);
+  }
+  uint32_t v[32];
+  load_staged_row(stage, lane, v);
+  filter_32(v, base, bmax_scaled, ctx, c, inv_c, ubias, tau, theta, drop_max, n_ovf, m3, buf_row_addr, cnt, n_res, lane,
+            p.k);
 }
 
 // 128 user rows x 64 items (column half `h` of the tile in B slot `b_slot`), fp16 hi x hi, fp32 accumulate
@@ -512,9 +600,12 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
   __syncthreads();
   if (kCluster == 2) cluster_sync_all();   // the peer's barriers exist before anything is multicast to them
 
-  if (warp == 0) {
+  // register budget: the producer warpgroup (one issuing warp) needs few, the consumers hold 64 accumulators, a staged
+  // row and the admission state per thread (40 x 128 + 232 x 256 = 64,512 of the 65,536 registers)
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
     // ===================================== TMA producer ======================================
-    {   // warp-uniform control flow, one elected lane issues
+    if (warp == 0) {   // warp-uniform control flow, one elected lane issues
       int ts = 0;
       uint32_t ts_phase = 0;
       for (int64_t w = w_first; w < n_work; w += w_step) {
@@ -547,15 +638,15 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
         }
       }
     }
-  } else if (warp >= 4) {
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
     // ================================ consumers: wgmma + admission ================================
     const int group = warp / 4 - 1;
-    const int wt = threadIdx.x % kFConsumerThreads;
-    const int row = wt;                              // row inside the user block
+    const int row = filter_owned_row(warp % 4, lane);   // row inside the user block
     const float kNegInf = -__int_as_float(0x7f800000);
     const uint32_t buf_row_addr =   // group g owns user block g of the pair
         smem_u32(smem + L.buf_off) + static_cast<uint32_t>((group * kFBlockM + row) * kBufEntries * 8);
-    float* acc_stage = reinterpret_cast<float*>(smem + L.acc_off + group * kFAccStageBytes);
+    const uint32_t stage = smem_u32(smem + L.acc_off) + static_cast<uint32_t>(warp - 4) * kFWarpStageBytes;
     const uint32_t a_base = smem_u32(smem + L.a_off) + group * kNKB * kFATileBytes;
     const uint32_t b_base = smem_u32(smem + L.b_off);
     const float max_item_norm = __ldg(p.item_stats + 0);
@@ -584,8 +675,6 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
       float tau = kNegInf, theta = kNegInf;
       int cnt = 0, n_res = 0, n_ovf = 0;
       float drop_max = kNegInf;
-      const uint32_t* ra = reinterpret_cast<const uint32_t*>(acc_stage + wt * kFStageStride);   // this row, staged
-      float* const ra_w = acc_stage + wt * kFStageStride;
       int32_t excl_next = 0x7fffffff;   // kExclude: next excluded processing position >= the current chunk
       if constexpr (kExclude) {
         if (u_ok && t1 > t0) excl_next = excl_next_at(p.excl_indptr, p.excl_pos, u, t0 * kFBlockN);
@@ -595,7 +684,7 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
         // this group's user block (hi half, fp16; rows past n_users arrive as zeros) goes to shared memory.  Every
         // wgmma of the previous unit has completed in all four warps once they pass this barrier.
         named_barrier_sync(1 + group, kFConsumerThreads);
-        if (wt == 0) {
+        if (warp % 4 == 0 && lane == 0) {
           mbar_arrive_expect_tx(a_full + group, kNKB * kFATileBytes);
 #pragma unroll
           for (int kb = 0; kb < kNKB; ++kb)
@@ -617,25 +706,28 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
           const float bmin = __ldg(p.block_bias_min + t0);   // the same for the whole CTA: warp-uniform branch
           if (bmin > kNegInf) {
             float g[16];
-            // the tile is staged again by the filter below: the pre-pass masks with a copy of the cursor
+            // the tile is filtered again below: the pre-pass masks with a copy of the cursor
             int32_t pre_next = excl_next;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
               filter_mma_half<kNKB>(acc0, acc1, a_base, b_slot, h);
-              stage_chunk<0>(acc0, acc1, acc_stage, wt, group);
+              uint32_t v[32];
+              stage_warp_chunk<0>(acc0, acc1, stage, lane);
               if constexpr (kExclude) {
                 if (pre_next < pos0 + h * 64 + 32)
-                  excl_mask_chunk(p.excl_indptr, p.excl_pos, u, pos0 + h * 64, ra_w, pre_next);
+                  pre_next = excl_mask_chunk(p.excl_indptr, p.excl_pos, u, pos0 + h * 64, stage, lane);
               }
+              load_staged_row(stage, lane, v);
 #pragma unroll
-              for (int q = 0; q < 4; ++q) g[8 * h + q] = acc_max_8(ra + 8 * q);
-              stage_chunk<1>(acc0, acc1, acc_stage, wt, group);
+              for (int q = 0; q < 4; ++q) g[8 * h + q] = acc_max_8(v + 8 * q);
+              stage_warp_chunk<1>(acc0, acc1, stage, lane);
               if constexpr (kExclude) {
                 if (pre_next < pos0 + h * 64 + 64)
-                  excl_mask_chunk(p.excl_indptr, p.excl_pos, u, pos0 + h * 64 + 32, ra_w, pre_next);
+                  pre_next = excl_mask_chunk(p.excl_indptr, p.excl_pos, u, pos0 + h * 64 + 32, stage, lane);
               }
+              load_staged_row(stage, lane, v);
 #pragma unroll
-              for (int q = 0; q < 4; ++q) g[8 * h + 4 + q] = acc_max_8(ra + 8 * q);
+              for (int q = 0; q < 4; ++q) g[8 * h + 4 + q] = acc_max_8(v + 8 * q);
             }
             sort16_desc(g);
             float a_k = g[0];
@@ -663,20 +755,10 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
               }
             }
           }
-          stage_chunk<0>(acc0, acc1, acc_stage, wt, group);
-          if constexpr (kExclude) {
-            if (excl_next < pos0 + h * 64 + 32)
-              excl_mask_chunk(p.excl_indptr, p.excl_pos, u, pos0 + h * 64, ra_w, excl_next);
-          }
-          filter_32(ra, pos0 + h * 64, bmax_scaled, ctx, c, inv_c, ubias, tau, theta, drop_max, n_ovf, m3, buf_row_addr,
-                    cnt, n_res, lane, p.k);
-          stage_chunk<1>(acc0, acc1, acc_stage, wt, group);
-          if constexpr (kExclude) {
-            if (excl_next < pos0 + h * 64 + 64)
-              excl_mask_chunk(p.excl_indptr, p.excl_pos, u, pos0 + h * 64 + 32, ra_w, excl_next);
-          }
-          filter_32(ra, pos0 + h * 64 + 32, bmax_scaled, ctx, c, inv_c, ubias, tau, theta, drop_max, n_ovf, m3,
-                    buf_row_addr, cnt, n_res, lane, p.k);
+          filter_chunk<0, kExclude>(acc0, acc1, pos0 + h * 64, bmax_scaled, stage, lane, u, p, excl_next, ctx, c, inv_c,
+                                    ubias, tau, theta, drop_max, n_ovf, m3, buf_row_addr, cnt, n_res);
+          filter_chunk<1, kExclude>(acc0, acc1, pos0 + h * 64 + 32, bmax_scaled, stage, lane, u, p, excl_next, ctx, c,
+                                    inv_c, ubias, tau, theta, drop_max, n_ovf, m3, buf_row_addr, cnt, n_res);
         }
         if (++ts == n_slots) {
           ts = 0;
