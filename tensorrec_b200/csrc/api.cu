@@ -27,6 +27,44 @@ int sm_count() {
   return cached[dev];
 }
 
+int capped_grid(int64_t blocks, int per_sm) {
+  const int64_t cap = static_cast<int64_t>(sm_count()) * per_sm;
+  return static_cast<int>(blocks < 1 ? 1 : (blocks < cap ? blocks : cap));
+}
+
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+int encode_tiled_2d(CUtensorMap* map, CUtensorMapDataType type, const void* base, uint64_t cols, uint64_t rows,
+                    uint64_t row_bytes, uint32_t box_cols, uint32_t box_rows, CUtensorMapL2promotion l2_promotion) {
+  static EncodeTiledFn encode = nullptr;   // the library links no driver: the entry point is looked up at run time
+  if (encode == nullptr) {
+    void* ptr = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
+        qres == cudaDriverEntryPointSuccess)
+      encode = reinterpret_cast<EncodeTiledFn>(ptr);
+  }
+  if (encode == nullptr) {
+    set_error("cuTensorMapEncodeTiled is not available from the CUDA driver");
+    return TRK_ERR_CUDA;
+  }
+  const cuuint64_t dims[2] = {cols, rows};
+  const cuuint64_t strides[1] = {row_bytes};
+  const cuuint32_t box[2] = {box_cols, box_rows};
+  const cuuint32_t elem_strides[2] = {1, 1};
+  const CUresult r = encode(map, type, 2, const_cast<void*>(base), dims, strides, box, elem_strides,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, l2_promotion,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled failed with CUresult %d (rows=%llu cols=%llu)", static_cast<int>(r),
+              static_cast<unsigned long long>(rows), static_cast<unsigned long long>(cols));
+    return TRK_ERR_CUDA;
+  }
+  return TRK_OK;
+}
+
 // implemented in the kernel translation units
 int csr_gather_reduce(const int32_t*, const int32_t*, const float*, const float*, int64_t, int32_t, int32_t, int32_t,
                       float*, void*, int32_t, float*, float*, float*, cudaStream_t);

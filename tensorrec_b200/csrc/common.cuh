@@ -43,8 +43,30 @@ void set_error(const char* fmt, ...);
 // Number of SMs of the current device (cached per device id).
 int sm_count();
 
+// Grid of a grid-stride launch: `blocks` CTAs, at most per_sm x sm_count(), at least 1.
+int capped_grid(int64_t blocks, int per_sm);
+
+// Encodes a 2-D row-major tensor map with the 128-byte swizzle: `rows` rows of `cols` elements of `type`, row_bytes
+// apart, loaded / stored in boxes of box_cols x box_rows.
+int encode_tiled_2d(CUtensorMap* map, CUtensorMapDataType type, const void* base, uint64_t cols, uint64_t rows,
+                    uint64_t row_bytes, uint32_t box_cols, uint32_t box_rows, CUtensorMapL2promotion l2_promotion);
+
 constexpr int kWarp = 32;
 constexpr int kSMsH100 = 132;
+
+// Tile geometry of the two tensor-core kernels (score_topk_tc.cu, score_filter_tc.cu): a producer warpgroup streams
+// 128-row operand tiles of 64 fp16 (one 128-byte swizzle row) per k-block, two consumer warpgroups issue wgmma.
+constexpr int kBlockM = 128;          // user tile
+constexpr int kBlockN = 128;          // item tile
+constexpr int kKBlock = 64;           // fp16 per 128-byte swizzle row
+constexpr int kMmaK = 16;
+constexpr int kTcThreads = 384;
+constexpr int kConsumerThreads = 128; // per consumer warpgroup
+constexpr uint32_t kATileBytes = kBlockM * kKBlock * 2;   // 16 KB
+constexpr uint32_t kBTileBytes = kBlockN * kKBlock * 2;   // 16 KB
+constexpr int kMaxStages = 10;
+constexpr uint32_t kSmemLimit = 232448;   // 227 KB opt-in limit per CTA on sm_90
+constexpr uint32_t kSmemAlignSlack = 1024;   // dynamic shared memory requested beyond the layout: see smem_base_1024
 
 __host__ __device__ constexpr int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 __host__ __device__ constexpr int64_t round_up(int64_t a, int64_t b) { return ceil_div(a, b) * b; }
@@ -56,6 +78,12 @@ __host__ __device__ constexpr int64_t round_up(int64_t a, int64_t b) { return ce
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
+}
+
+// The dynamic shared memory rounded up to 1024 bytes: 128B-swizzled tiles need a 1024-byte aligned base.
+__device__ __forceinline__ uint8_t* smem_base_1024() {
+  extern __shared__ uint8_t smem_raw[];
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 }
 
 __device__ __forceinline__ bool elect_one() {

@@ -412,11 +412,6 @@ bool pick_shape(int d, int d_pad, bool want_split, bool aligned16, RowShape* s) 
   return true;
 }
 
-int gather_grid(int64_t n_tiles) {
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 8;  // 8 x 256 threads resident per SM
-  return static_cast<int>(n_tiles < cap ? (n_tiles > 0 ? n_tiles : 1) : cap);
-}
-
 #define TRK_DISPATCH_ROWSHAPE(S, CALL)                          \
   do {                                                          \
     if ((S).vec) {                                              \
@@ -459,7 +454,7 @@ int csr_gather_reduce(const int32_t* indptr, const int32_t* col, const float* va
     set_error("csr_gather_reduce: n_components=%d (d_pad=%d) exceeds the fused row width", d, d_pad);
     return TRK_ERR_UNSUPPORTED;
   }
-  const int grid = gather_grid(ceil_div(rows, kTileRows));
+  const int grid = capped_grid(ceil_div(rows, kTileRows), 8);   // 8 x 256 threads resident per SM
 #define CALL(G, CH, VEC)                                                                                     \
   csr_gather_reduce_kernel<G, CH, VEC><<<grid, kGatherThreads, 0, stream>>>(                                 \
       indptr, col, val, weights, rows, d, n_normalize, out_f32, static_cast<__half*>(out_split), d_pad, out_scale, \
@@ -487,7 +482,7 @@ int split_rows(const float* repr, int64_t rows, int32_t d, int32_t n_normalize, 
     return TRK_ERR_UNSUPPORTED;
   }
   const int groups = kGatherThreads / s.g;
-  const int grid = gather_grid(ceil_div(rows, groups));
+  const int grid = capped_grid(ceil_div(rows, groups), 8);
 #define CALL(G, CH, VEC)                                                 \
   split_rows_kernel<G, CH, VEC><<<grid, kGatherThreads, 0, stream>>>(    \
       repr, rows, d, n_normalize, normalized_inplace, static_cast<__half*>(out_split), d_pad, out_scale)
@@ -502,7 +497,7 @@ int csr_project_biases(const int32_t* indptr, const int32_t* col, const float* v
   TRK_CHECK_ARG(indptr && biases && out, "csr_project_biases: null pointer");
   TRK_CHECK_ARG(rows >= 0, "csr_project_biases: rows < 0");
   if (rows == 0) return TRK_OK;
-  const int grid = gather_grid(ceil_div(rows, kBiasTileRows));
+  const int grid = capped_grid(ceil_div(rows, kBiasTileRows), 8);
   csr_project_biases_kernel<<<grid, kBiasTileRows, 0, stream>>>(indptr, col, val, biases, rows, out);
   TRK_CHECK_LAUNCH();
   return TRK_OK;

@@ -268,9 +268,7 @@ __global__ void order_from_ranks_kernel(const int32_t* __restrict__ ranks, int64
 int order_from_ranks(const int32_t* ranks, int64_t n, int32_t* order, cudaStream_t stream) {
   TRK_CHECK_ARG(ranks && order && n >= 0 && n < (1ll << 31), "order_from_ranks: bad arguments");
   if (n == 0) return TRK_OK;
-  const int64_t blocks = ceil_div(n, 256);
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 8;
-  order_from_ranks_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), 256, 0, stream>>>(ranks, n, order);
+  order_from_ranks_kernel<<<capped_grid(ceil_div(n, 256), 8), 256, 0, stream>>>(ranks, n, order);
   TRK_CHECK_LAUNCH();
   return TRK_OK;
 }

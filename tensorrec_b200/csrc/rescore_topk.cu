@@ -303,9 +303,7 @@ int rescore_topk(const void* user_split, const float* user_scale, const void* it
                 "rescore_topk: operands must be 16-byte aligned");
   if (n_users == 0) return TRK_OK;
   const int threads = 256;
-  const int64_t blocks = ceil_div(n_users, threads / 32);
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 8;
-  rescore_topk_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), threads, 0, stream>>>(
+  rescore_topk_kernel<<<capped_grid(ceil_div(n_users, threads / 32), 8), threads, 0, stream>>>(
       static_cast<const __half*>(user_split), user_scale, static_cast<const __half*>(item_split), item_scale, user_bias,
       item_bias, cand_item, row_theta, user_norm, item_stats, n_users, n_items_local, d_pad, n_lists, list_width, k,
       item_id_offset, out_score, out_item, out_row_stride, out_flag);
@@ -319,9 +317,7 @@ int select_flagged_rows(const int32_t* flags, int64_t n, int32_t* idx, int32_t c
   TRK_CHECK_CUDA(cudaMemsetAsync(counters, 0, 4 * sizeof(int32_t), stream));
   if (n == 0) return TRK_OK;
   const int threads = 256;
-  const int64_t blocks = ceil_div(n, threads);
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 8;
-  select_flagged_rows_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), threads, 0, stream>>>(
+  select_flagged_rows_kernel<<<capped_grid(ceil_div(n, threads), 8), threads, 0, stream>>>(
       flags, n, idx, capacity, counters);
   TRK_CHECK_LAUNCH();
   return TRK_OK;
@@ -336,8 +332,7 @@ int gather_operand_rows(const int32_t* idx, int32_t* counters, int32_t capacity,
   TRK_CHECK_ARG(bias == nullptr || sub_bias != nullptr, "gather_operand_rows: bias without sub_bias");
   const int threads = 256;
   const int64_t blocks = ceil_div(static_cast<int64_t>(capacity), threads / 32);
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 8;
-  gather_operand_rows_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), threads, 0, stream>>>(
+  gather_operand_rows_kernel<<<capped_grid(blocks, 8), threads, 0, stream>>>(
       idx, counters, capacity, small_capacity, static_cast<const uint4*>(split), scale, bias, 2 * d_pad * 2 / 16,
       static_cast<uint4*>(sub_split), sub_scale, sub_bias);
   TRK_CHECK_LAUNCH();
@@ -352,8 +347,7 @@ int scatter_topk_rows(const int32_t* idx, const int32_t* counters, int32_t capac
                 "scatter_topk_rows: bad arguments");
   const int threads = 256;
   const int64_t blocks = ceil_div(static_cast<int64_t>(capacity) * k, threads);
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 8;
-  scatter_topk_rows_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), threads, 0, stream>>>(
+  scatter_topk_rows_kernel<<<capped_grid(blocks, 8), threads, 0, stream>>>(
       idx, counters, capacity, sub_score, sub_item, sub_row_stride, k, out_score, out_item, out_row_stride);
   TRK_CHECK_LAUNCH();
   return TRK_OK;

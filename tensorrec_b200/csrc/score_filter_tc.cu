@@ -39,17 +39,8 @@
 
 namespace trk {
 
-constexpr int kFBlockM = 128;
-constexpr int kFBlockN = 128;          // item tile
-constexpr int kFKBlock = 64;
-constexpr int kFMmaK = 16;
-constexpr int kFThreads = 384;
-constexpr int kFConsumerThreads = 128; // per consumer warpgroup (= user rows of its block)
-constexpr uint32_t kFBTileBytes = kFBlockN * kFKBlock * 2;   // 16 KB
-constexpr uint32_t kFATileBytes = kFBlockM * kFKBlock * 2;   // 16 KB
-constexpr uint32_t kFWarpStageBytes = 32 * 32 * 4u;                     // 32 rows x 32 fp32 per consumer warp
-constexpr uint32_t kFAccStageBytes = 4 * kFWarpStageBytes;              // per warpgroup
-constexpr int kFMaxStages = 10;
+constexpr uint32_t kWarpStageBytes = 32 * 32 * 4u;   // 32 rows x 32 fp32 per consumer warp
+constexpr uint32_t kAccStageBytes = 4 * kWarpStageBytes;   // per warpgroup
 constexpr int kBufEntries = 32;      // candidate buffer per (row, epilogue group)
 constexpr int kKeepMax = 16;         // entries kept by a compaction (>= k + slack); also the per-group output width
 constexpr int kFilterMaxK = 12;
@@ -95,10 +86,10 @@ struct FilterLayout {
 __host__ __device__ inline FilterLayout filter_layout(int n_kblocks, int n_stages) {
   FilterLayout L;
   L.a_off = 0;                                                    // user blocks 0 and 1, n_kblocks tiles each
-  L.b_off = L.a_off + 2u * static_cast<uint32_t>(n_kblocks) * kFATileBytes;
-  L.buf_off = L.b_off + static_cast<uint32_t>(n_stages) * kFBTileBytes;
-  L.acc_off = L.buf_off + 2u * kFBlockM * kBufEntries * 8u;       // 64 KB of candidate buffers
-  L.bar_off = L.acc_off + 2u * kFAccStageBytes;
+  L.b_off = L.a_off + 2u * static_cast<uint32_t>(n_kblocks) * kATileBytes;
+  L.buf_off = L.b_off + static_cast<uint32_t>(n_stages) * kBTileBytes;
+  L.acc_off = L.buf_off + 2u * kBlockM * kBufEntries * 8u;        // 64 KB of candidate buffers
+  L.bar_off = L.acc_off + 2u * kAccStageBytes;
   L.total = L.bar_off + 512u;
   return L;
 }
@@ -128,7 +119,29 @@ struct AdmitCtx {
   const int32_t* perm;   // processing position -> local item index, or null = identity
   int32_t id_offset;
   int32_t n_items;
+  int32_t k;
 };
+
+// Admission state of the user row a consumer lane owns (filter_owned_row).  Only ever passed to __forceinline__
+// functions, so that it stays in registers.
+struct RowState {
+  uint32_t buf;     // shared-memory address of the row's candidate buffer (kBufEntries entries of 8 bytes)
+  int cnt;          // entries in the buffer
+  int n_res;        // entries [0, n_res) are resolved (approximate score, item id), [n_res, cnt) raw
+  int n_ovf;        // compactions that overflowed, see compact_finish
+  float tau;        // admission threshold on v = acc + bias / c
+  float theta;      // admission threshold on the approximate score
+  float drop_max;   // best score a compaction dropped
+  // row constants: the margin 2.25 m, the user bias, c = user scale x global item scale (a power of two) and 1 / c
+  float m3, ubias, c, inv_c;
+};
+
+// theta -> tau: the admission test runs on v = acc + bias / c; a few ulps of slack (extra survivors are harmless, a
+// missed one is not)
+__device__ __forceinline__ void set_tau(RowState& r) {
+  const float t = (r.theta - r.ubias) * r.inv_c;
+  r.tau = t - 8.0f * 1.1920929e-7f * fabsf(t) - 1e-30f;
+}
 
 // Warp-cooperative compaction of the candidate buffer of lane `src`'s row: one entry per lane, bitonic sort by
 // (score desc, id asc), keep everything >= k-th best - 2.25m (at most kKeepMax), tighten that row's thresholds.
@@ -156,12 +169,11 @@ __device__ __forceinline__ int32_t ldg_nc_s32(const int32_t* p) {
   asm volatile("ld.global.nc.s32 %0, [%1];" : "=r"(v) : "l"(p));
   return v;
 }
-__device__ __forceinline__ RowFetch compact_fetch(uint32_t buf_row_addr, int lane, int src, int cnt, int n_res,
-                                                  const AdmitCtx& ctx) {
+__device__ __forceinline__ RowFetch compact_fetch(const RowState& r, int lane, int src, const AdmitCtx& ctx) {
   RowFetch f;
-  f.n = __shfl_sync(0xffffffffu, cnt, src);
-  f.n_res = __shfl_sync(0xffffffffu, n_res, src);
-  f.addr = __shfl_sync(0xffffffffu, buf_row_addr, src);
+  f.n = __shfl_sync(0xffffffffu, r.cnt, src);
+  f.n_res = __shfl_sync(0xffffffffu, r.n_res, src);
+  f.addr = __shfl_sync(0xffffffffu, r.buf, src);
   f.s = -__int_as_float(0x7f800000);
   f.id = 0x7fffffff;
   f.bias = 0.0f;
@@ -181,15 +193,14 @@ __device__ __forceinline__ RowFetch compact_fetch(uint32_t buf_row_addr, int lan
 // massive near-ties (all-equal scores in the limit: EVERY column passes, every chunk takes the slow path and the sweep of
 // 1M x 1M took 43 s instead of 0.2): after kGiveUpOverflows of them the row stops admitting (tau = +inf) and is marked
 // uncertifiable (drop_max = +inf), i.e. it goes through the exact kernel -- where a tie-heavy row belongs anyway.
-__device__ __forceinline__ void compact_finish(const RowFetch& f, int lane, int src, int k, int& cnt, int& n_res,
-                                               float& theta, float& tau, float& drop_max, int& n_ovf, float m3,
-                                               float ubias, float c, float inv_c, const AdmitCtx& ctx) {
+__device__ __forceinline__ void compact_finish(const RowFetch& f, int lane, int src, RowState& r, const AdmitCtx& ctx) {
   const float kNegInf = -__int_as_float(0x7f800000);
+  const int k = ctx.k;
   const int n = f.n;
   const uint32_t addr = f.addr;
-  const float m3s = __shfl_sync(0xffffffffu, m3, src);
-  const float cs = __shfl_sync(0xffffffffu, c, src);
-  const float ubs = __shfl_sync(0xffffffffu, ubias, src);
+  const float m3s = __shfl_sync(0xffffffffu, r.m3, src);
+  const float cs = __shfl_sync(0xffffffffu, r.c, src);
+  const float ubs = __shfl_sync(0xffffffffu, r.ubias, src);
   float s = f.s;
   int32_t id = f.id;
   if (lane < n && lane >= f.n_res) {
@@ -228,40 +239,35 @@ __device__ __forceinline__ void compact_finish(const RowFetch& f, int lane, int 
   const float first_dropped = __shfl_sync(0xffffffffu, s, kKeepMax & 31);
   if (lane < n_keep) f_sts64(addr + lane * 8, s, id);
   if (lane == src) {
-    cnt = n_keep;
-    n_res = n_keep;
+    r.cnt = n_keep;
+    r.n_res = n_keep;
     if (ovf) {
-      drop_max = fmaxf(drop_max, first_dropped);
-      n_ovf += 1;
+      r.drop_max = fmaxf(r.drop_max, first_dropped);
+      r.n_ovf += 1;
     }
     if (have_k) {
-      theta = floor_s;
-      // admission test runs on v = acc + bias/c; move theta there and leave a few ulps of slack (extra survivors are
-      // harmless, a missed one is not)
-      const float t = (theta - ubias) * inv_c;
-      tau = t - 8.0f * 1.1920929e-7f * fabsf(t) - 1e-30f;
+      r.theta = floor_s;
+      set_tau(r);
     }
-    if (n_ovf >= kGiveUpOverflows) {
-      tau = __int_as_float(0x7f800000);
-      drop_max = __int_as_float(0x7f800000);
+    if (r.n_ovf >= kGiveUpOverflows) {
+      r.tau = __int_as_float(0x7f800000);
+      r.drop_max = __int_as_float(0x7f800000);
     }
   }
   __syncwarp();
 }
 // compacts every row of `rows` (bit = lane), the lookups of the next row in flight while the current one is sorted
-__device__ __forceinline__ void compact_rows(unsigned rows, uint32_t buf_row_addr, int lane, int k, int& cnt, int& n_res,
-                                             float& theta, float& tau, float& drop_max, int& n_ovf, float m3,
-                                             float ubias, float c, float inv_c, const AdmitCtx& ctx) {
+__device__ __forceinline__ void compact_rows(unsigned rows, int lane, RowState& r, const AdmitCtx& ctx) {
   if (rows == 0u) return;
   int src = __ffs(rows) - 1;
   rows &= rows - 1;
-  RowFetch cur = compact_fetch(buf_row_addr, lane, src, cnt, n_res, ctx);
+  RowFetch cur = compact_fetch(r, lane, src, ctx);
   while (true) {
     const int nxt = rows != 0u ? __ffs(rows) - 1 : -1;
     rows &= rows - 1;     // (0 stays 0)
     RowFetch ahead = cur;
-    if (nxt >= 0) ahead = compact_fetch(buf_row_addr, lane, nxt, cnt, n_res, ctx);
-    compact_finish(cur, lane, src, k, cnt, n_res, theta, tau, drop_max, n_ovf, m3, ubias, c, inv_c, ctx);
+    if (nxt >= 0) ahead = compact_fetch(r, lane, nxt, ctx);
+    compact_finish(cur, lane, src, r, ctx);
     if (nxt < 0) break;
     cur = ahead;
     src = nxt;
@@ -292,24 +298,22 @@ __device__ __forceinline__ float acc_max_16(const uint32_t* acc) {
 // rounding is monotonic; no memory is read here.  A row is compacted (by the whole warp) only when its buffer could not
 // take the new entries: ~4 compactions per user at 1M items instead of 9 with a "more than half full" trigger.
 // Called warp-uniformly.
-__device__ __forceinline__ void admit_16(const uint32_t* acc, bool hit, int32_t pos_base, float bmax_scaled,
-                                         const AdmitCtx& ctx, float c, float inv_c, float ubias, float& tau,
-                                         float& theta, float& drop_max, int& n_ovf, float m3, uint32_t buf_row_addr,
-                                         int& cnt, int& n_res, int lane, int k) {
+__device__ __forceinline__ void admit_16(const uint32_t* acc, bool hit, int32_t pos_base, float bmax_scaled, int lane,
+                                         RowState& r, const AdmitCtx& ctx) {
   uint32_t pass = 0;
   if (hit) {
 #pragma unroll
-    for (int j = 0; j < 16; ++j) pass |= (__uint_as_float(acc[j]) + bmax_scaled > tau) ? (1u << j) : 0u;
+    for (int j = 0; j < 16; ++j) pass |= (__uint_as_float(acc[j]) + bmax_scaled > r.tau) ? (1u << j) : 0u;
   }
   __syncwarp();   // earlier appends of every lane are visible to the lanes that may now compact its row
-  const unsigned need = __ballot_sync(0xffffffffu, cnt + __popc(pass) > kBufEntries);
-  compact_rows(need, buf_row_addr, lane, k, cnt, n_res, theta, tau, drop_max, n_ovf, m3, ubias, c, inv_c, ctx);
-  if (pass != 0 && n_ovf < kGiveUpOverflows) {   // (a row that has just given up appends nothing more)   // cnt + popc(pass) <= kBufEntries holds here (a compaction leaves at most kKeepMax = 16)
+  const unsigned need = __ballot_sync(0xffffffffu, r.cnt + __popc(pass) > kBufEntries);
+  compact_rows(need, lane, r, ctx);
+  if (pass != 0 && r.n_ovf < kGiveUpOverflows) {   // (a row that has just given up appends nothing more)   // cnt + popc(pass) <= kBufEntries holds here (a compaction leaves at most kKeepMax = 16)
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       if ((pass >> j) & 1u) {
-        f_sts64(buf_row_addr + cnt * 8, __uint_as_float(acc[j]), pos_base + j);
-        cnt += 1;
+        f_sts64(r.buf + r.cnt * 8, __uint_as_float(acc[j]), pos_base + j);
+        r.cnt += 1;
       }
     }
   }
@@ -339,17 +343,17 @@ __device__ __forceinline__ uint32_t pass_mask_16(const uint32_t* acc, const floa
 // does): one store, no search through the registers.  Several: every slot is addressed by a prefix popcount, the
 // stores are independent.
 __device__ __forceinline__ void append_16(const uint32_t* acc, uint32_t mask, float amax, int32_t pos_base,
-                                          uint32_t buf_row_addr, int& cnt) {
+                                          RowState& r) {
   if ((mask & (mask - 1u)) == 0u) {
-    f_sts64(buf_row_addr + cnt * 8, amax, pos_base + __ffs(mask) - 1);
-    cnt += 1;
+    f_sts64(r.buf + r.cnt * 8, amax, pos_base + __ffs(mask) - 1);
+    r.cnt += 1;
   } else {
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       if ((mask >> j) & 1u)
-        f_sts64(buf_row_addr + (cnt + __popc(mask & ((1u << j) - 1u))) * 8, __uint_as_float(acc[j]), pos_base + j);
+        f_sts64(r.buf + (r.cnt + __popc(mask & ((1u << j) - 1u))) * 8, __uint_as_float(acc[j]), pos_base + j);
     }
-    cnt += __popc(mask);
+    r.cnt += __popc(mask);
   }
 }
 
@@ -360,25 +364,21 @@ __device__ __forceinline__ void append_16(const uint32_t* acc, uint32_t mask, fl
 // case: the hitting lanes append, nobody else does anything -- and only otherwise the chunk goes through the two-step
 // path (compact the rows that need it, append 16 columns at a time so that the 32-entry buffer cannot overflow between
 // compactions).
-__device__ __forceinline__ void filter_32(const uint32_t* acc, int32_t pos_base, float bmax_scaled, const AdmitCtx& ctx,
-                                          float c, float inv_c, float ubias, float& tau, float& theta,
-                                          float& drop_max, int& n_ovf, float m3, uint32_t buf_row_addr, int& cnt,
-                                          int& n_res, int lane, int k) {
+__device__ __forceinline__ void filter_32(const uint32_t* acc, int32_t pos_base, float bmax_scaled, int lane,
+                                          RowState& r, const AdmitCtx& ctx) {
   float g0[4], g1[4];
   const float a0 = acc_max_16(acc, g0), a1 = acc_max_16(acc + 16, g1);
-  const bool h0 = a0 + bmax_scaled > tau, h1 = a1 + bmax_scaled > tau;
+  const bool h0 = a0 + bmax_scaled > r.tau, h1 = a1 + bmax_scaled > r.tau;
   if (__any_sync(0xffffffffu, h0 || h1)) {
     uint32_t lo = 0, hi = 0;
-    if (h0) lo = pass_mask_16(acc, g0, bmax_scaled, tau);
-    if (h1) hi = pass_mask_16(acc + 16, g1, bmax_scaled, tau);
-    if (__ballot_sync(0xffffffffu, cnt + __popc(lo) + __popc(hi) > kBufEntries) == 0u) {
-      if (lo != 0u) append_16(acc, lo, a0, pos_base, buf_row_addr, cnt);
-      if (hi != 0u) append_16(acc + 16, hi, a1, pos_base + 16, buf_row_addr, cnt);
+    if (h0) lo = pass_mask_16(acc, g0, bmax_scaled, r.tau);
+    if (h1) hi = pass_mask_16(acc + 16, g1, bmax_scaled, r.tau);
+    if (__ballot_sync(0xffffffffu, r.cnt + __popc(lo) + __popc(hi) > kBufEntries) == 0u) {
+      if (lo != 0u) append_16(acc, lo, a0, pos_base, r);
+      if (hi != 0u) append_16(acc + 16, hi, a1, pos_base + 16, r);
     } else {
-      admit_16(acc, h0, pos_base, bmax_scaled, ctx, c, inv_c, ubias, tau, theta, drop_max, n_ovf, m3, buf_row_addr, cnt,
-               n_res, lane, k);
-      admit_16(acc + 16, h1, pos_base + 16, bmax_scaled, ctx, c, inv_c, ubias, tau, theta, drop_max, n_ovf, m3,
-               buf_row_addr, cnt, n_res, lane, k);
+      admit_16(acc, h0, pos_base, bmax_scaled, lane, r, ctx);
+      admit_16(acc + 16, h1, pos_base + 16, bmax_scaled, lane, r, ctx);
     }
   }
 }
@@ -521,11 +521,10 @@ __device__ __noinline__ int32_t excl_mask_chunk(const int32_t* indptr, const int
 template <int kC, bool kExclude>
 __device__ __forceinline__ void filter_chunk(const float (&acc0)[32], const float (&acc1)[32], int32_t base,
                                              float bmax_scaled, uint32_t stage, int lane, int64_t u,
-                                             const FilterParams& p, int32_t& excl_next, const AdmitCtx& ctx, float c,
-                                             float inv_c, float ubias, float& tau, float& theta, float& drop_max,
-                                             int& n_ovf, float m3, uint32_t buf_row_addr, int& cnt, int& n_res) {
+                                             const FilterParams& p, int32_t& excl_next, RowState& r,
+                                             const AdmitCtx& ctx) {
   const float amax = chunk_row_max<kC>(acc0, acc1, lane);
-  bool flag = amax + bmax_scaled > tau;   // == the h0 || h1 of filter_32: x -> x + bmax is monotonic
+  bool flag = amax + bmax_scaled > r.tau;   // == the h0 || h1 of filter_32: x -> x + bmax is monotonic
   if constexpr (kExclude) flag = flag || excl_next < base + 32;
   if (!__any_sync(0xffffffffu, flag)) return;
   stage_warp_chunk<kC>(acc0, acc1, stage, lane);
@@ -534,8 +533,7 @@ __device__ __forceinline__ void filter_chunk(const float (&acc0)[32], const floa
   }
   uint32_t v[32];
   load_staged_row(stage, lane, v);
-  filter_32(v, base, bmax_scaled, ctx, c, inv_c, ubias, tau, theta, drop_max, n_ovf, m3, buf_row_addr, cnt, n_res, lane,
-            p.k);
+  filter_32(v, base, bmax_scaled, lane, r, ctx);
 }
 
 // 128 user rows x 64 items (column half `h` of the tile in B slot `b_slot`), fp16 hi x hi, fp32 accumulate
@@ -546,12 +544,12 @@ __device__ __forceinline__ void filter_mma_half(float (&acc0)[32], float (&acc1)
 #pragma unroll
   for (int kb = 0; kb < kNKB; ++kb) {
 #pragma unroll
-    for (int ks = 0; ks < kFKBlock / kFMmaK; ++ks) {
-      const uint64_t db = wgmma_desc_k_major_sw128(b_slot + kb * kFBTileBytes + h * (kFBTileBytes / 2)) + 2u * ks;
-      const uint64_t da = wgmma_desc_k_major_sw128(a_base + kb * kFATileBytes) + 2u * ks;
+    for (int ks = 0; ks < kKBlock / kMmaK; ++ks) {
+      const uint64_t db = wgmma_desc_k_major_sw128(b_slot + kb * kBTileBytes + h * (kBTileBytes / 2)) + 2u * ks;
+      const uint64_t da = wgmma_desc_k_major_sw128(a_base + kb * kATileBytes) + 2u * ks;
       const uint32_t accumulate = static_cast<uint32_t>(kb > 0 || ks > 0);
       wgmma_m64n64k16_f16(acc0, da, db, accumulate);
-      wgmma_m64n64k16_f16(acc1, da + ((kFATileBytes / 2) >> 4), db, accumulate);   // rows 64..127: +8 KB
+      wgmma_m64n64k16_f16(acc1, da + ((kATileBytes / 2) >> 4), db, accumulate);   // rows 64..127: +8 KB
     }
   }
   wgmma_commit();
@@ -563,18 +561,17 @@ __device__ __forceinline__ void filter_mma_half(float (&acc0)[32], float (&acc1)
 // shared memory, so the L2 -> SM stream of the item operand is halved.  kExclude: mask the items of each row's exclusion
 // list (p.excl_indptr / p.excl_pos) out of the candidate universe, see excl_mask_chunk.
 template <int kNKB, int kCluster, bool kExclude = false>
-__global__ void __launch_bounds__(kFThreads, 1)
+__global__ void __launch_bounds__(kTcThreads, 1)
 score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_constant__ CUtensorMap map_items,
                     const FilterParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_base_1024();
   const FilterLayout L = filter_layout(kNKB, p.n_stages);
   const int n_slots = p.n_stages / kNKB;   // B tile slots
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
   uint64_t* a_full = bars + 0;        // [user block]
   uint64_t* b_full = bars + 2;
   uint64_t* b_empty = bars + 2 + n_slots;
-  constexpr uint32_t kSlotBytes = kNKB * kFBTileBytes;
+  constexpr uint32_t kSlotBytes = kNKB * kBTileBytes;
 
   const int warp = threadIdx.x / 32;
   const int lane = threadIdx.x % 32;
@@ -622,12 +619,12 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
 #pragma unroll
             for (int kb = 0; kb < kNKB; ++kb) {
               if (kCluster == 2)   // this CTA's half of the tile rows (box = 64 rows), delivered to both CTAs
-                tma_load_2d_multicast(smem + L.b_off + ts * kSlotBytes + kb * kFBTileBytes + crank * (kFBTileBytes / 2),
-                                      &map_items, b_full + ts, kb * kFKBlock,
-                                      t * kFBlockN + static_cast<int>(crank) * (kFBlockN / 2), kClusterMask, kEvictLast);
+                tma_load_2d_multicast(smem + L.b_off + ts * kSlotBytes + kb * kBTileBytes + crank * (kBTileBytes / 2),
+                                      &map_items, b_full + ts, kb * kKBlock,
+                                      t * kBlockN + static_cast<int>(crank) * (kBlockN / 2), kClusterMask, kEvictLast);
               else
-                tma_load_2d(smem + L.b_off + ts * kSlotBytes + kb * kFBTileBytes, &map_items, b_full + ts,
-                            kb * kFKBlock, t * kFBlockN, kEvictLast);
+                tma_load_2d(smem + L.b_off + ts * kSlotBytes + kb * kBTileBytes, &map_items, b_full + ts,
+                            kb * kKBlock, t * kBlockN, kEvictLast);
             }
           }
           __syncwarp();
@@ -645,14 +642,14 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
     const int row = filter_owned_row(warp % 4, lane);   // row inside the user block
     const float kNegInf = -__int_as_float(0x7f800000);
     const uint32_t buf_row_addr =   // group g owns user block g of the pair
-        smem_u32(smem + L.buf_off) + static_cast<uint32_t>((group * kFBlockM + row) * kBufEntries * 8);
-    const uint32_t stage = smem_u32(smem + L.acc_off) + static_cast<uint32_t>(warp - 4) * kFWarpStageBytes;
-    const uint32_t a_base = smem_u32(smem + L.a_off) + group * kNKB * kFATileBytes;
+        smem_u32(smem + L.buf_off) + static_cast<uint32_t>((group * kBlockM + row) * kBufEntries * 8);
+    const uint32_t stage = smem_u32(smem + L.acc_off) + static_cast<uint32_t>(warp - 4) * kWarpStageBytes;
+    const uint32_t a_base = smem_u32(smem + L.a_off) + group * kNKB * kATileBytes;
     const uint32_t b_base = smem_u32(smem + L.b_off);
     const float max_item_norm = __ldg(p.item_stats + 0);
     const float item_scale = fmaxf(__ldg(p.item_stats + 1), 1e-38f);
     const float max_item_bias = __ldg(p.item_stats + 2);
-    const AdmitCtx ctx = {p.item_bias, p.item_perm, p.item_id_offset, static_cast<int32_t>(p.n_items)};
+    const AdmitCtx ctx = {p.item_bias, p.item_perm, p.item_id_offset, static_cast<int32_t>(p.n_items), p.k};
     int ts = 0;
     uint32_t ts_phase = 0, witer = 0;
     float acc0[32], acc1[32];
@@ -662,33 +659,35 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
       const int sp = static_cast<int>(w / n_groups);
       const int t0 = sp * p.tiles_per_split;
       const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
-      const int64_t ublock_row0 = (static_cast<int64_t>(up) * 2 + group) * kFBlockM;
+      const int64_t ublock_row0 = (static_cast<int64_t>(up) * 2 + group) * kBlockM;
       const int64_t u = ublock_row0 + row;
       const bool u_ok = u < p.n_users;
       const float su = u_ok ? __ldg(p.user_scale + u) : 1.0f;
       const float ubias = (u_ok && p.user_bias != nullptr) ? __ldg(p.user_bias + u) : 0.0f;
       const float unorm = u_ok ? __ldg(p.user_norm + u) : 0.0f;
-      const float c = su * item_scale;          // powers of two: exact
-      const float inv_c = 1.0f / c;
+      RowState rs;
+      rs.buf = buf_row_addr;
+      rs.cnt = rs.n_res = rs.n_ovf = 0;
+      rs.tau = rs.theta = rs.drop_max = kNegInf;
+      rs.ubias = ubias;
+      rs.c = su * item_scale;          // powers of two: exact
+      rs.inv_c = 1.0f / rs.c;
       // error bound of one approximate score: operand rounding + the fp32 rounding of the two bias adds
-      const float m3 = kThetaMargins * (kMarginFactor * unorm * max_item_norm + kBiasUlps * (fabsf(ubias) + max_item_bias));
-      float tau = kNegInf, theta = kNegInf;
-      int cnt = 0, n_res = 0, n_ovf = 0;
-      float drop_max = kNegInf;
+      rs.m3 = kThetaMargins * (kMarginFactor * unorm * max_item_norm + kBiasUlps * (fabsf(ubias) + max_item_bias));
       int32_t excl_next = 0x7fffffff;   // kExclude: next excluded processing position >= the current chunk
       if constexpr (kExclude) {
-        if (u_ok && t1 > t0) excl_next = excl_next_at(p.excl_indptr, p.excl_pos, u, t0 * kFBlockN);
+        if (u_ok && t1 > t0) excl_next = excl_next_at(p.excl_indptr, p.excl_pos, u, t0 * kBlockN);
       }
 
       if (t1 > t0) {
         // this group's user block (hi half, fp16; rows past n_users arrive as zeros) goes to shared memory.  Every
         // wgmma of the previous unit has completed in all four warps once they pass this barrier.
-        named_barrier_sync(1 + group, kFConsumerThreads);
+        named_barrier_sync(1 + group, kConsumerThreads);
         if (warp % 4 == 0 && lane == 0) {
-          mbar_arrive_expect_tx(a_full + group, kNKB * kFATileBytes);
+          mbar_arrive_expect_tx(a_full + group, kNKB * kATileBytes);
 #pragma unroll
           for (int kb = 0; kb < kNKB; ++kb)
-            tma_load_2d(smem + L.a_off + (group * kNKB + kb) * kFATileBytes, &map_users, a_full + group, kb * kFKBlock,
+            tma_load_2d(smem + L.a_off + (group * kNKB + kb) * kATileBytes, &map_users, a_full + group, kb * kKBlock,
                         static_cast<int32_t>(ublock_row0), kEvictFirst);
         }
         mbar_wait(a_full + group, witer & 1);
@@ -697,11 +696,11 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
 
       float bmax_next = t1 > t0 ? __ldg(p.block_bias_max + t0) : 0.0f;
       for (int t = t0; t < t1; ++t) {
-        const float bmax_scaled = bmax_next * inv_c;
+        const float bmax_scaled = bmax_next * rs.inv_c;
         if (t + 1 < t1) bmax_next = __ldg(p.block_bias_max + t + 1);   // in flight while this tile is filtered
         mbar_wait(b_full + ts, ts_phase);
         const uint32_t b_slot = b_base + ts * kSlotBytes;
-        const int32_t pos0 = t * kFBlockN;
+        const int32_t pos0 = t * kBlockN;
         if (t == t0 && p.block_bias_min != nullptr) {
           const float bmin = __ldg(p.block_bias_min + t0);   // the same for the whole CTA: warp-uniform branch
           if (bmin > kNegInf) {
@@ -733,11 +732,10 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
             float a_k = g[0];
 #pragma unroll
             for (int i = 1; i < 16; ++i) a_k = (i < p.k) ? g[i] : a_k;   // g[k - 1]: the k-th largest group maximum
-            const float th0 = (fmaf(a_k, c, ubias) + bmin) - m3;
+            const float th0 = (fmaf(a_k, rs.c, ubias) + bmin) - rs.m3;
             if (th0 == th0) {   // not NaN (infinite biases / margins): otherwise the sweep starts from -inf as before
-              theta = th0;
-              const float tt = (theta - ubias) * inv_c;
-              tau = tt - 8.0f * 1.1920929e-7f * fabsf(tt) - 1e-30f;
+              rs.theta = th0;
+              set_tau(rs);
             }
           }
         }
@@ -755,10 +753,8 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
               }
             }
           }
-          filter_chunk<0, kExclude>(acc0, acc1, pos0 + h * 64, bmax_scaled, stage, lane, u, p, excl_next, ctx, c, inv_c,
-                                    ubias, tau, theta, drop_max, n_ovf, m3, buf_row_addr, cnt, n_res);
-          filter_chunk<1, kExclude>(acc0, acc1, pos0 + h * 64 + 32, bmax_scaled, stage, lane, u, p, excl_next, ctx, c,
-                                    inv_c, ubias, tau, theta, drop_max, n_ovf, m3, buf_row_addr, cnt, n_res);
+          filter_chunk<0, kExclude>(acc0, acc1, pos0 + h * 64, bmax_scaled, stage, lane, u, p, excl_next, rs, ctx);
+          filter_chunk<1, kExclude>(acc0, acc1, pos0 + h * 64 + 32, bmax_scaled, stage, lane, u, p, excl_next, rs, ctx);
         }
         if (++ts == n_slots) {
           ts = 0;
@@ -770,14 +766,13 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
         // a row that overflows inside a tile.  (Measured on an H100 80GB HBM3 at 400 W, against a build without this
         // pass: 1M-item sweep 1570 -> 1560 ms, 125K-item shard 186.0 -> 183.6 ms.)
         {
-          const unsigned early = __ballot_sync(0xffffffffu, cnt > p.tile_end_trigger);
-          compact_rows(early, buf_row_addr, lane, p.k, cnt, n_res, theta, tau, drop_max, n_ovf, m3, ubias, c, inv_c, ctx);
+          const unsigned early = __ballot_sync(0xffffffffu, rs.cnt > p.tile_end_trigger);
+          compact_rows(early, lane, rs, ctx);
         }
       }
 
       // end of the item range: final compaction of every row of this warp, then emit the survivors
-      compact_rows(0xffffffffu, buf_row_addr, lane, p.k, cnt, n_res, theta, tau, drop_max, n_ovf, m3, ubias, c, inv_c,
-                   ctx);
+      compact_rows(0xffffffffu, lane, rs, ctx);
       if (u_ok) {
         const int64_t base = u * p.n_splits + sp;
         float* os = p.cand_score + base * kKeepMax;
@@ -785,14 +780,14 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
         for (int e = 0; e < kKeepMax; ++e) {
           float s = kNegInf;
           int32_t id = 0x7fffffff;
-          if (e < cnt) f_lds64(buf_row_addr + e * 8, &s, &id);
+          if (e < rs.cnt) f_lds64(rs.buf + e * 8, &s, &id);
           os[e] = s;
           oi[e] = id;
         }
         // every excluded item has an approximate score <= this; a NaN (inf - inf with infinite biases) must not read
         // as "nothing was excluded": +inf makes the certificate fail and the row goes through the exact kernel
-        const bool th_nan = theta != theta || drop_max != drop_max;
-        p.row_theta[base] = th_nan ? __int_as_float(0x7f800000) : fmaxf(theta, drop_max);
+        const bool th_nan = rs.theta != rs.theta || rs.drop_max != rs.drop_max;
+        p.row_theta[base] = th_nan ? __int_as_float(0x7f800000) : fmaxf(rs.theta, rs.drop_max);
       }
       __syncwarp();
     }
@@ -890,49 +885,6 @@ __global__ void exclusion_keys_kernel(const int32_t* __restrict__ indptr, const 
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
-namespace {
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn filter_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  }
-  return fn;
-}
-
-// fp16 [rows, row_elems] row-major (only the first d_pad columns are addressed), boxes 64 x box_rows, 128B swizzle
-int make_hi_map(CUtensorMap* map, const void* base, int64_t rows, int row_elems, int d_pad, int box_rows) {
-  EncodeTiledFn encode = filter_encode_fn();
-  if (encode == nullptr) {
-    set_error("cuTensorMapEncodeTiled is not available from the CUDA driver");
-    return TRK_ERR_CUDA;
-  }
-  const cuuint64_t dims[2] = {static_cast<cuuint64_t>(d_pad), static_cast<cuuint64_t>(rows)};
-  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(row_elems) * 2};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(kFKBlock), static_cast<cuuint32_t>(box_rows)};
-  const cuuint32_t elem_strides[2] = {1, 1};
-  const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box,
-                            elem_strides, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed with CUresult %d", static_cast<int>(r));
-    return TRK_ERR_CUDA;
-  }
-  return TRK_OK;
-}
-
-constexpr uint32_t kFSmemLimit = 232448;
-
-}  // namespace
-
 int score_filter_max_k() { return kFilterMaxK; }
 int score_filter_list_width() { return kKeepMax; }
 
@@ -941,9 +893,7 @@ int operand_stats(const void* split, const float* scale, int64_t rows, int32_t d
   TRK_CHECK_ARG(split && scale && rows >= 0 && d_pad >= 64 && d_pad % 64 == 0, "operand_stats: bad arguments");
   if (rows == 0) return TRK_OK;
   const int threads = 256;
-  const int64_t blocks = ceil_div(rows, threads / 32);
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 8;
-  operand_stats_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), threads, 0, stream>>>(
+  operand_stats_kernel<<<capped_grid(ceil_div(rows, threads / 32), 8), threads, 0, stream>>>(
       static_cast<const __half*>(split), scale, rows, d_pad, out_norm, stats);
   TRK_CHECK_LAUNCH();
   return TRK_OK;
@@ -955,9 +905,7 @@ int rescale_hi_global(const void* split, const float* scale, const float* stats,
                 "rescale_hi_global: bad arguments");
   if (rows == 0) return TRK_OK;
   const int threads = 256;
-  const int64_t blocks = ceil_div(rows * (d_pad / 8), threads);
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 16;
-  rescale_hi_global_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), threads, 0, stream>>>(
+  rescale_hi_global_kernel<<<capped_grid(ceil_div(rows * (d_pad / 8), threads), 16), threads, 0, stream>>>(
       static_cast<const __half*>(split), scale, stats, perm, rows, d_pad, static_cast<__half*>(out_hi));
   TRK_CHECK_LAUNCH();
   return TRK_OK;
@@ -968,16 +916,11 @@ int exclusion_positions(const int32_t* item_perm, int64_t n_items, int32_t* inv_
   TRK_CHECK_ARG(excl_indptr && excl_ids && out_keys && n_rows >= 0 && n_items >= 0, "exclusion_positions: bad arguments");
   TRK_CHECK_ARG(item_perm == nullptr || inv_perm != nullptr, "exclusion_positions: item_perm needs inv_perm");
   if (item_perm != nullptr && n_items > 0) {
-    const int64_t blocks = ceil_div(n_items, 256);
-    const int64_t cap = static_cast<int64_t>(sm_count()) * 16;
-    invert_perm_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), 256, 0, stream>>>(item_perm, n_items,
-                                                                                                inv_perm);
+    invert_perm_kernel<<<capped_grid(ceil_div(n_items, 256), 16), 256, 0, stream>>>(item_perm, n_items, inv_perm);
     TRK_CHECK_LAUNCH();
   }
   if (n_rows == 0) return TRK_OK;
-  const int64_t blocks = ceil_div(n_rows, 256 / 32);
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 16;
-  exclusion_keys_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), 256, 0, stream>>>(
+  exclusion_keys_kernel<<<capped_grid(ceil_div(n_rows, 256 / 32), 16), 256, 0, stream>>>(
       excl_indptr, excl_ids, item_perm != nullptr ? inv_perm : nullptr, n_rows, out_keys);
   TRK_CHECK_LAUNCH();
   return TRK_OK;
@@ -1015,17 +958,17 @@ int score_filter_f16(const void* user_split, const float* user_scale, const floa
   p.user_norm = user_norm;
   p.item_bias = item_bias;
   p.block_bias_max = block_bias_max;
-  p.block_bias_min = getenv("TRK_FILTER_NO_WARMSTART") != nullptr ? nullptr : block_bias_min;
+  p.block_bias_min = block_bias_min;
   p.item_perm = item_perm;
   p.item_stats = item_stats;
   p.n_users = n_users;
   p.n_items = n_items;
-  p.n_kblocks = d_pad / kFKBlock;
+  p.n_kblocks = d_pad / kKBlock;
   p.k = k;
-  p.n_tiles = static_cast<int32_t>(ceil_div(n_items, kFBlockN));
+  p.n_tiles = static_cast<int32_t>(ceil_div(n_items, kBlockN));
   p.n_splits = n_splits;
   p.tiles_per_split = static_cast<int32_t>(ceil_div(p.n_tiles, n_splits));
-  p.n_user_pairs = static_cast<int32_t>(ceil_div(n_users, 2 * kFBlockM));
+  p.n_user_pairs = static_cast<int32_t>(ceil_div(n_users, 2 * kBlockM));
   p.item_id_offset = item_id_offset;
   // Tile-end compaction trigger.  TRK_FILTER_TILE_END_TRIGGER (probe knob) sets it; kBufEntries or more turns the
   // tile-end pass off (no buffer holds more than kBufEntries entries).
@@ -1044,13 +987,13 @@ int score_filter_f16(const void* user_split, const float* user_scale, const floa
   CUtensorMap map_users, map_items;
   int rc;
   p.n_stages = 0;
-  for (int s = kFMaxStages; s >= 2; --s)
-    if (s % p.n_kblocks == 0 && filter_layout(p.n_kblocks, s).total + 1024 <= kFSmemLimit) {
+  for (int s = kMaxStages; s >= 2; --s)
+    if (s % p.n_kblocks == 0 && filter_layout(p.n_kblocks, s).total + kSmemAlignSlack <= kSmemLimit) {
       p.n_stages = s;
       break;
     }
   TRK_CHECK_ARG(p.n_stages >= 2 * p.n_kblocks, "score_filter: shared memory budget exceeded");
-  const uint32_t smem_bytes = filter_layout(p.n_kblocks, p.n_stages).total + 1024;
+  const uint32_t smem_bytes = filter_layout(p.n_kblocks, p.n_stages).total + kSmemAlignSlack;
 
   // Launch form: clusters of two CTAs sharing every item tile through TMA multicast (default when the device can keep
   // (almost) all SMs busy with 2-CTA clusters), else independent CTAs.  TRK_FILTER_CLUSTER=1|2 forces one.
@@ -1069,7 +1012,7 @@ int score_filter_f16(const void* user_split, const float* user_scale, const floa
   if (cluster == 2) {
     TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel2, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     cfg.gridDim = dim3(2);
-    cfg.blockDim = dim3(kFThreads);
+    cfg.blockDim = dim3(kTcThreads);
     cfg.dynamicSmemBytes = smem_bytes;
     cfg.stream = stream;
     attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -1101,9 +1044,13 @@ int score_filter_f16(const void* user_split, const float* user_scale, const floa
     if (max_clusters * 2 < sm_count() - 8 && env == nullptr) cluster = 1;   // too many SMs would sit idle
     if (max_clusters < 1) cluster = 1;
   }
-  rc = make_hi_map(&map_items, item_hi, n_items, d_pad, d_pad, kFBlockN / cluster);
+  // fp16 operands, boxes of one k-block: the items [n_items, d_pad] (each CTA of a cluster fetches half of a tile) and
+  // the hi half of the split user rows [n_users, 2 d_pad]
+  rc = encode_tiled_2d(&map_items, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, item_hi, d_pad, n_items, 2 * d_pad, kKBlock,
+                       kBlockN / cluster, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   if (rc != TRK_OK) return rc;
-  rc = make_hi_map(&map_users, user_split, n_users, 2 * d_pad, d_pad, kFBlockM);   // the hi half of the split rows
+  rc = encode_tiled_2d(&map_users, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, user_split, d_pad, n_users, 4 * d_pad, kKBlock,
+                       kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   if (rc != TRK_OK) return rc;
   if (cluster == 2) {
     const int64_t n_work = ceil_div(static_cast<int64_t>(p.n_user_pairs), 2) * n_splits;
@@ -1112,9 +1059,8 @@ int score_filter_f16(const void* user_split, const float* user_scale, const floa
     TRK_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel2, map_users, map_items, p));
   } else {
     TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel1, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    const int64_t n_work = static_cast<int64_t>(p.n_user_pairs) * n_splits;
-    const int grid = static_cast<int>(n_work < sm_count() ? n_work : sm_count());
-    kernel1<<<grid, kFThreads, smem_bytes, stream>>>(map_users, map_items, p);
+    const int grid = capped_grid(static_cast<int64_t>(p.n_user_pairs) * n_splits, 1);
+    kernel1<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, p);
   }
   TRK_CHECK_LAUNCH();
   return TRK_OK;

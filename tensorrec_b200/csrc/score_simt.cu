@@ -182,9 +182,7 @@ int l2_normalize_rows(float* x, int64_t rows, int32_t d, cudaStream_t stream) {
   TRK_CHECK_ARG(x && rows >= 0 && d >= 1, "l2_normalize_rows: bad arguments");
   if (rows == 0) return TRK_OK;
   const int threads = 256;
-  const int64_t blocks = ceil_div(rows, threads / 32);
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 8;
-  l2_normalize_rows_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), threads, 0, stream>>>(x, rows, d);
+  l2_normalize_rows_kernel<<<capped_grid(ceil_div(rows, threads / 32), 8), threads, 0, stream>>>(x, rows, d);
   TRK_CHECK_LAUNCH();
   return TRK_OK;
 }

@@ -24,18 +24,9 @@
 
 namespace trk {
 
-constexpr int kBlockM = 128;
-constexpr int kBlockN = 128;          // item tile
-constexpr int kKBlock = 64;           // fp16 per 128-byte swizzle row
-constexpr int kMmaK = 16;
-constexpr int kTcThreads = 384;
-constexpr int kConsumerThreads = 128; // per consumer warpgroup
 constexpr int kWgRows = 64;           // user rows per consumer warpgroup
 constexpr int kStageStride = 33;      // fp32 per staged row (32 columns + 1: conflict-free row reads)
-constexpr uint32_t kATileBytes = kBlockM * kKBlock * 2;   // 16 KB
-constexpr uint32_t kBTileBytes = kBlockN * kKBlock * 2;   // 16 KB
 constexpr uint32_t kAccStageBytes = 2u * kWgRows * kStageStride * 4u;   // per warpgroup: 2 halves x 64 rows x 32 cols
-constexpr int kMaxStages = 10;
 constexpr int kMaxK = 32;
 
 struct TcParams {
@@ -149,13 +140,29 @@ __device__ __forceinline__ float excl_mask_scores(uint32_t (&r)[32], const TcExc
   return cmax;
 }
 
-// One 32-column chunk of one user row: final scores, then (top-k mode) the rare inserts, or (dense mode) the store.
-template <bool kDense>
+// Per-row exclusion state of the exact kernel (empty without exclusion).
+template <bool kOn>
+struct ExclCursor {
+  int32_t row = -1;            // list row of this user row (-1: none)
+  int32_t next = 0x7fffffff;   // first listed id >= the current chunk (INT32_MAX: none left)
+};
+template <>
+struct ExclCursor<false> {};
+
+// One 32-column chunk of one user row: final scores, then (top-k mode) the row's listed columns masked (kExclude) and
+// the rare inserts, or (dense mode) the store.  `x` is taken by value: a reference bound to the kernel parameter
+// changes the generated code of the instantiations without exclusion.
+template <bool kDense, bool kExclude>
 __device__ __forceinline__ void process_chunk(uint32_t (&r)[32], int c, int t, int32_t id0, const float2* meta,
                                               float su, float ubias, float& thr, float* ls, int32_t* li,
-                                              const TcParams& p, int64_t u, bool u_ok) {
-  const float cmax = score_chunk(r, meta + c * 32, su, ubias);
+                                              const TcParams& p, int64_t u, bool u_ok, const TcExcl x,
+                                              ExclCursor<kExclude>& xc) {
+  float cmax = score_chunk(r, meta + c * 32, su, ubias);
   if constexpr (!kDense) {
+    if constexpr (kExclude) {
+      const int32_t base = t * kBlockN + c * 32;   // local id of the chunk's first column
+      if (xc.next < base + 32) cmax = excl_mask_scores(r, x, xc.row, base, xc.next);
+    }
     if (cmax > thr) {   // some column of this chunk enters the row's list (probability ~ 32 k / items seen)
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
@@ -176,32 +183,6 @@ __device__ __forceinline__ void process_chunk(uint32_t (&r)[32], int c, int t, i
         for (int j = 0; j < 32; ++j)
           if (i0 + j < p.n_items) dst[j] = __uint_as_float(r[j]);
       }
-    }
-  }
-}
-
-// Per-row exclusion state of the exact kernel (empty without exclusion).
-template <bool kOn>
-struct ExclCursor {
-  int32_t row = -1;            // list row of this user row (-1: none)
-  int32_t next = 0x7fffffff;   // first listed id >= the current chunk (INT32_MAX: none left)
-};
-template <>
-struct ExclCursor<false> {};
-
-// Top-k mode with exclusion: process_chunk<false> with the row's listed columns masked after scoring.
-__device__ __forceinline__ void process_chunk_excl(uint32_t (&r)[32], int c, int t, int32_t id0, const float2* meta,
-                                                   float su, float ubias, float& thr, float* ls, int32_t* li,
-                                                   const TcParams& p, const TcExcl& x, int32_t xr,
-                                                   int32_t& excl_next) {
-  float cmax = score_chunk(r, meta + c * 32, su, ubias);
-  const int32_t base = t * kBlockN + c * 32;   // local id of the chunk's first column
-  if (excl_next < base + 32) cmax = excl_mask_scores(r, x, xr, base, excl_next);
-  if (cmax > thr) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      const float s = __uint_as_float(r[j]);
-      if (s > thr) thr = list_insert(s, id0 + c * 32 + j, ls, li, p.k);
     }
   }
 }
@@ -237,9 +218,7 @@ template <bool kDense, int kNKB, bool kExclude = false>
 __global__ void __launch_bounds__(kTcThreads, 1)
 score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_constant__ CUtensorMap map_items,
                 const __grid_constant__ CUtensorMap map_out, const TcParams p, const TcExcl x) {
-  extern __shared__ uint8_t smem_raw[];
-  // 128B-swizzled tiles need a 1024-byte aligned base
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_base_1024();
   const SmemLayout L = make_layout(p.n_kblocks, p.n_stages, kDense ? 0 : p.k, kDense && p.tma_store != 0);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
   uint64_t* a_full = bars + 0;
@@ -413,10 +392,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
                             ub * kBlockM + g * kWgRows + (warp % 2) * 32);
             ++n_stored;
           } else {
-            if constexpr (kExclude)
-              process_chunk_excl(r, chunk, t, id0, meta, su, ubias, thr, ls, li, p, x, xc.row, xc.next);
-            else
-              process_chunk<kDense>(r, chunk, t, id0, meta, su, ubias, thr, ls, li, p, u, u_ok);
+            process_chunk<kDense, kExclude>(r, chunk, t, id0, meta, su, ubias, thr, ls, li, p, u, u_ok, x, xc);
           }
         }
       }
@@ -459,49 +435,9 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
 // ---------------------------------------------------------------------------------------------------------
 namespace {
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  }
-  return fn;
-}
-
-// [rows, 2*d_pad] fp16 row-major, boxes of 64 columns x box_rows rows, 128-byte swizzle
-int make_operand_map(CUtensorMap* map, const void* base, int64_t rows, int d_pad, int box_rows) {
-  EncodeTiledFn encode = get_encode_fn();
-  if (encode == nullptr) {
-    set_error("cuTensorMapEncodeTiled is not available from the CUDA driver");
-    return TRK_ERR_CUDA;
-  }
-  const cuuint64_t dims[2] = {static_cast<cuuint64_t>(2 * d_pad), static_cast<cuuint64_t>(rows)};
-  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(2 * d_pad) * 2};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(kKBlock), static_cast<cuuint32_t>(box_rows)};
-  const cuuint32_t elem_strides[2] = {1, 1};
-  const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box,
-                            elem_strides, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed with CUresult %d (rows=%lld d_pad=%d)", static_cast<int>(r),
-              static_cast<long long>(rows), d_pad);
-    return TRK_ERR_CUDA;
-  }
-  return TRK_OK;
-}
-
-constexpr uint32_t kSmemLimit = 232448;  // 227 KB opt-in limit per CTA on sm_90
-
 int pick_stages(int n_kblocks, int k, bool dense_staging) {
   for (int s = kMaxStages; s >= 2; --s)
-    if (make_layout(n_kblocks, s, k, dense_staging).total + 1024 <= kSmemLimit) return s;
+    if (make_layout(n_kblocks, s, k, dense_staging).total + kSmemAlignSlack <= kSmemLimit) return s;
   return 0;
 }
 
@@ -565,36 +501,29 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
   p.n_stages = pick_stages(p.n_kblocks, p.k, p.tma_store != 0);
   TRK_CHECK_ARG(p.n_stages >= 2, "score_tc: shared memory budget exceeded (d_pad=%d k=%d)", d_pad, k);
 
+  // operands: [rows, 2 d_pad] fp16 (hi | lo), boxes of one k-block x one tile
   CUtensorMap map_users, map_items;
-  int rc = make_operand_map(&map_users, user_split, n_users, d_pad, kBlockM);
+  int rc = encode_tiled_2d(&map_users, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, user_split, 2 * d_pad, n_users, 4 * d_pad,
+                           kKBlock, kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   if (rc != TRK_OK) return rc;
-  rc = make_operand_map(&map_items, item_split, n_items, d_pad, kBlockN);
+  rc = encode_tiled_2d(&map_items, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, item_split, 2 * d_pad, n_items, 4 * d_pad, kKBlock,
+                       kBlockN, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   if (rc != TRK_OK) return rc;
 
   CUtensorMap map_out = map_items;   // placeholder when the TMA store path is off
   if (p.tma_store) {
-    EncodeTiledFn encode = get_encode_fn();
-    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(n_items), static_cast<cuuint64_t>(n_users)};
-    const cuuint64_t strides[1] = {static_cast<cuuint64_t>(dense_stride) * 4};
-    const cuuint32_t box[2] = {32, 32};
-    const cuuint32_t elem_strides[2] = {1, 1};
-    const CUresult r = encode(&map_out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, dense_out, dims, strides, box,
-                              elem_strides, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                              CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      set_error("cuTensorMapEncodeTiled (output) failed with CUresult %d", static_cast<int>(r));
-      return TRK_ERR_CUDA;
-    }
+    rc = encode_tiled_2d(&map_out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, dense_out, n_items, n_users, 4 * dense_stride, 32,
+                         32, CU_TENSOR_MAP_L2_PROMOTION_NONE);
+    if (rc != TRK_OK) return rc;
   }
-  const uint32_t smem_bytes = make_layout(p.n_kblocks, p.n_stages, p.k, p.tma_store != 0).total + 1024;
+  const uint32_t smem_bytes = make_layout(p.n_kblocks, p.n_stages, p.k, p.tma_store != 0).total + kSmemAlignSlack;
   decltype(&score_tc_kernel<kDense, 1>) kernel = nullptr;
   if constexpr (!kDense) {
     if (excl_indptr != nullptr) kernel = p.n_kblocks == 2 ? score_tc_kernel<false, 2, true> : score_tc_kernel<false, 1, true>;
   }
   if (kernel == nullptr) kernel = p.n_kblocks == 2 ? score_tc_kernel<kDense, 2> : score_tc_kernel<kDense, 1>;
   TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-  const int64_t n_work = static_cast<int64_t>(p.n_user_blocks) * n_splits;
-  const int grid = static_cast<int>(n_work < sm_count() ? n_work : sm_count());
+  const int grid = capped_grid(static_cast<int64_t>(p.n_user_blocks) * n_splits, 1);
   kernel<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, map_out, p, x);
   TRK_CHECK_LAUNCH();
   return TRK_OK;

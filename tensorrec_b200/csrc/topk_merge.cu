@@ -99,9 +99,7 @@ int topk_merge(const float* cand_score, const int32_t* cand_item, int64_t n_user
                 32 * kMergeMaxListsPerLane);
   if (n_users == 0) return TRK_OK;
   const int threads = 256;
-  const int64_t blocks = ceil_div(n_users, threads / 32);
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 8;
-  topk_merge_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), threads, 0, stream>>>(
+  topk_merge_kernel<<<capped_grid(ceil_div(n_users, threads / 32), 8), threads, 0, stream>>>(
       cand_score, cand_item, n_users, n_lists, k_in, k_out, user_stride, list_stride, out_score, out_item,
       out_row_stride, n_users_live, dedup);
   TRK_CHECK_LAUNCH();

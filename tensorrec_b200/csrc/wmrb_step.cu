@@ -373,9 +373,7 @@ int sample_items(int64_t n_users, int64_t n_items, int32_t n_sampled, int32_t re
     return TRK_ERR_UNSUPPORTED;
   }
   if (n_users == 0) return TRK_OK;
-  const int64_t blocks = ceil_div(n_users, kSampleWarps);
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 8;
-  const unsigned grid = static_cast<unsigned>(blocks < cap ? blocks : cap);
+  const int grid = capped_grid(ceil_div(n_users, kSampleWarps), 8);
   if (replace) {
     sample_items_kernel<true><<<grid, kSampleWarps * 32, 0, stream>>>(n_users, static_cast<uint32_t>(n_items), n_sampled,
                                                                       seed, step, out);
@@ -395,9 +393,7 @@ template <typename T>
 static int launch_wmrb(const WmrbParams& p, cudaStream_t stream) {
   const int ch = static_cast<int>(ceil_div(p.d, 128));
   const size_t smem = static_cast<size_t>(kWmrbWarps) * 2 * p.n_sampled * sizeof(float);
-  const int64_t blocks = ceil_div(p.n_users, kWmrbWarps);
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 16;
-  const unsigned grid = static_cast<unsigned>(blocks < cap ? blocks : cap);
+  const int grid = capped_grid(ceil_div(p.n_users, kWmrbWarps), 16);
 #define TRK_WMRB_LAUNCH(CH)                                                                                   \
   do {                                                                                                        \
     if (smem > 48 * 1024)                                                                                     \
@@ -461,9 +457,7 @@ int wmrb_step(const void* user_repr, const void* item_repr, int32_t repr_is_bf16
 int f32_to_bf16(const float* x, int64_t n, void* out, cudaStream_t stream) {
   TRK_CHECK_ARG(x && out && n >= 0, "f32_to_bf16: bad arguments");
   if (n == 0) return TRK_OK;
-  const int64_t blocks = ceil_div(n, 256);
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 16;
-  f32_to_bf16_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), 256, 0, stream>>>(
+  f32_to_bf16_kernel<<<capped_grid(ceil_div(n, 256), 16), 256, 0, stream>>>(
       x, n, static_cast<__nv_bfloat16*>(out));
   TRK_CHECK_LAUNCH();
   return TRK_OK;
@@ -473,10 +467,8 @@ int adam_step(float* w, const float* grad, float* m, float* v, int64_t n, float 
               float epsilon, float l2, cudaStream_t stream) {
   TRK_CHECK_ARG(w && grad && m && v && n >= 0, "adam_step: bad arguments");
   if (n == 0) return TRK_OK;
-  const int64_t blocks = ceil_div(n, 256);
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 16;
-  adam_step_kernel<<<static_cast<unsigned>(blocks < cap ? blocks : cap), 256, 0, stream>>>(w, grad, m, v, n, lr_t, beta1,
-                                                                                         beta2, epsilon, l2);
+  adam_step_kernel<<<capped_grid(ceil_div(n, 256), 16), 256, 0, stream>>>(w, grad, m, v, n, lr_t, beta1, beta2, epsilon,
+                                                                         l2);
   TRK_CHECK_LAUNCH();
   return TRK_OK;
 }

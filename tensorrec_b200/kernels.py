@@ -285,16 +285,13 @@ def score_topk(user_split, user_scale, user_bias, item_split, item_meta, n_users
     cand_score = torch.empty((n_users, n_splits, k), dtype=torch.float32, device=dev)
     cand_item = torch.empty((n_users, n_splits, k), dtype=torch.int32, device=dev)
     if excl is None:
-        rc = lib.trk_score_topk_f16x3(_p(user_split), _p(user_scale), _p(user_bias), _p(item_split), _p(item_meta),
-                                      n_users, n_items, int(d_pad), int(k), int(n_splits), int(item_id_offset),
-                                      _p(cand_score), _p(cand_item), _p(n_users_live), _stream())
-        _lib.check(rc, 'trk_score_topk_f16x3')
+        name, extra = 'trk_score_topk_f16x3', ()
     else:
-        rc = lib.trk_score_topk_f16x3_excl(_p(user_split), _p(user_scale), _p(user_bias), _p(item_split), _p(item_meta),
-                                           n_users, n_items, int(d_pad), int(k), int(n_splits), int(item_id_offset),
-                                           _p(cand_score), _p(cand_item), _p(n_users_live), _p(excl.indptr),
-                                           _p(excl.ids), _p(excl_row_map), _stream())
-        _lib.check(rc, 'trk_score_topk_f16x3_excl')
+        name, extra = 'trk_score_topk_f16x3_excl', (_p(excl.indptr), _p(excl.ids), _p(excl_row_map))
+    rc = getattr(lib, name)(_p(user_split), _p(user_scale), _p(user_bias), _p(item_split), _p(item_meta), n_users,
+                            n_items, int(d_pad), int(k), int(n_splits), int(item_id_offset), _p(cand_score),
+                            _p(cand_item), _p(n_users_live), *extra, _stream())
+    _lib.check(rc, name)
     return cand_score, cand_item
 
 
@@ -441,18 +438,14 @@ def score_filter(user_split, user_scale, user_bias, user_norm, item_hi, item_sta
     cand_i = torch.empty((n_users, n_splits, width), dtype=torch.int32, device=dev)
     theta = torch.empty((n_users, n_splits), dtype=torch.float32, device=dev)
     if excl is None:
-        rc = lib.trk_score_filter_f16(_p(user_split), _p(user_scale), _p(user_bias), _p(user_norm), _p(item_hi),
-                                      _p(item_stats), _p(item_bias_pad), _p(block_bias_max), _p(block_bias_min),
-                                      _p(item_perm), n_users, n_items, int(d_pad), int(k), int(n_splits),
-                                      int(item_id_offset), _p(cand_s), _p(cand_i), _p(theta), _stream())
-        _lib.check(rc, 'trk_score_filter_f16')
+        name, extra = 'trk_score_filter_f16', ()
     else:
-        rc = lib.trk_score_filter_f16_excl(_p(user_split), _p(user_scale), _p(user_bias), _p(user_norm), _p(item_hi),
-                                           _p(item_stats), _p(item_bias_pad), _p(block_bias_max), _p(block_bias_min),
-                                           _p(item_perm), n_users, n_items, int(d_pad), int(k), int(n_splits),
-                                           int(item_id_offset), _p(cand_s), _p(cand_i), _p(theta), _p(excl.indptr),
-                                           _p(excl.pos), _stream())
-        _lib.check(rc, 'trk_score_filter_f16_excl')
+        name, extra = 'trk_score_filter_f16_excl', (_p(excl.indptr), _p(excl.pos))
+    rc = getattr(lib, name)(_p(user_split), _p(user_scale), _p(user_bias), _p(user_norm), _p(item_hi), _p(item_stats),
+                            _p(item_bias_pad), _p(block_bias_max), _p(block_bias_min), _p(item_perm), n_users, n_items,
+                            int(d_pad), int(k), int(n_splits), int(item_id_offset), _p(cand_s), _p(cand_i), _p(theta),
+                            *extra, _stream())
+    _lib.check(rc, name)
     return cand_s, cand_i, theta
 
 

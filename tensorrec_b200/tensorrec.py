@@ -815,22 +815,12 @@ class TensorRec(object):
             if use_filter:
                 fitems = kernels.FilterItems(items)
 
-        if user_batch_size is None or user_batch_size >= n_users:
-            blocks = [(0, n_users, user_in)]
-        else:
-            step = max(1, int(user_batch_size))
-            csr = user_in.matrix if isinstance(user_in.matrix, sp.csr_matrix) else sp.csr_matrix(user_in.matrix)
-            blocks = [(u0, min(n_users, u0 + step), SparseInput(csr[u0:min(n_users, u0 + step)]))
-                      for u0 in range(0, n_users, step)]
+        blocks = self._user_blocks(user_in, n_items, n_users if user_batch_size is None else user_batch_size)
 
         def run_taste(block_in, taste, force_exact, excl):
             users = self._side_operands('user', block_in, device, for_filter=use_filter and not force_exact, taste=taste)
             if use_filter and not force_exact:
-                if excl is None:
-                    return kernels.topk_filter(users, items, k, item_id_offset=item_id_offset, fitems=fitems)
                 return kernels.topk_filter(users, items, k, item_id_offset=item_id_offset, fitems=fitems, excl=excl)
-            if excl is None:
-                return kernels.topk_exact(users, items, k, item_id_offset=item_id_offset), None, 0
             return kernels.topk_exact(users, items, k, item_id_offset=item_id_offset, excl=excl), None, 0
 
         def run_block(block_in, u0, u1, force_exact=False):
