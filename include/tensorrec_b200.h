@@ -273,6 +273,22 @@ int trk_scatter_topk_rows(const int32_t* idx, const int32_t* counters, int32_t c
                           const int32_t* sub_item, int64_t sub_row_stride, int32_t k, float* out_score,
                           int32_t* out_item, int64_t out_row_stride, void* stream);
 
+/* Similar items with Euclidean similarity (EuclideanSimilarityPredictionGraph, tensorrec/prediction_graphs.py:84-100;
+ * similar-items scores carry no biases, recommendation_graphs.py:124-137) on the fused top-k kernels above.  With
+ * user bias -1/2 |q|^2 and item bias -1/2 |i|^2 their score q.i + ub + ib is -1/2 d^2(q, i), which ranks the items as
+ * the reference's -sqrt(max(d^2, 1e-16)) does; the error bound of the filter covers the biases as for any model.
+ *   trk_operand_half_sqnorm    out[r] = -1/2 sum_j (scale[r] (hi + lo)_j)^2 of a split operand [rows, 2 d_pad]
+ *                              (fp32, fixed reduction order: deterministic).
+ *   trk_topk_euclidean_finish  in place on k <= 32 (score, id) entries per row (row r at scores / items +
+ *                              r * row_stride, e.g. a [n_rows, 2k] exchange-layout buffer with items = scores + k):
+ *                              s = -sqrt(max(-2 s, 1e-16)) (sentinels stay -inf), then each row is re-sorted by
+ *                              (score desc, id asc): distances the sqrt or the clamp makes equal are ordered by id, as
+ *                              tf.nn.top_k orders them. */
+int trk_operand_half_sqnorm(const void* split, const float* scale, int64_t rows, int32_t d_pad, float* out,
+                            void* stream);
+int trk_topk_euclidean_finish(float* scores, int32_t* items, int64_t row_stride, int64_t n_rows, int32_t k,
+                              void* stream);
+
 /* Tensor-core dense prediction with the same operands, writing the full fp32 matrix out[n_users, n_items]
  * (predict(); tensorrec/tensorrec.py:636-664).  HBM-write bound. */
 int trk_score_dense_f16x3(const void* user_split, const float* user_scale, const float* user_bias,

@@ -103,6 +103,8 @@ int gather_operand_rows(const int32_t*, int32_t*, int32_t, int32_t, const void*,
                         void*, float*, float*, cudaStream_t);
 int scatter_topk_rows(const int32_t*, const int32_t*, int32_t, const float*, const int32_t*, int64_t, int32_t, float*,
                       int32_t*, int64_t, cudaStream_t);
+int operand_half_sqnorm(const void*, const float*, int64_t, int32_t, float*, cudaStream_t);
+int topk_euclidean_finish(float*, int32_t*, int64_t, int64_t, int32_t, cudaStream_t);
 
 int sample_items(int64_t, int64_t, int32_t, int32_t, uint64_t, uint32_t, int32_t*, cudaStream_t);
 int wmrb_step(const void*, const void*, int32_t, const float*, const float*, const int32_t*, const int32_t*, const float*,
@@ -293,6 +295,16 @@ int trk_scatter_topk_rows(const int32_t* idx, const int32_t* counters, int32_t c
                           int32_t* out_item, int64_t out_row_stride, void* stream) {
   return trk::scatter_topk_rows(idx, counters, capacity, sub_score, sub_item, sub_row_stride, k, out_score, out_item,
                                 out_row_stride, trk::as_stream(stream));
+}
+
+int trk_operand_half_sqnorm(const void* split, const float* scale, int64_t rows, int32_t d_pad, float* out,
+                            void* stream) {
+  return trk::operand_half_sqnorm(split, scale, rows, d_pad, out, trk::as_stream(stream));
+}
+
+int trk_topk_euclidean_finish(float* scores, int32_t* items, int64_t row_stride, int64_t n_rows, int32_t k,
+                              void* stream) {
+  return trk::topk_euclidean_finish(scores, items, row_stride, n_rows, k, trk::as_stream(stream));
 }
 
 int trk_sample_items(int64_t n_users, int64_t n_items, int32_t n_sampled, int32_t replace, uint64_t seed,

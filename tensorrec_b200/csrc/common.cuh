@@ -279,6 +279,31 @@ __device__ __forceinline__ int32_t excl_next_at(const int32_t* indptr, const int
   return i < hi ? __ldg(v + i) : 0x7fffffff;
 }
 
+// tf.nn.top_k order of two (score, id) entries: score descending, lower id first on ties
+__device__ __forceinline__ bool r_before(float xs, int32_t xi, float ys, int32_t yi) {
+  return xs > ys || (xs == ys && xi < yi);
+}
+
+// bitonic sort of one (score, id) entry per lane into (score desc, id asc) order; sentinels (-inf, INT32_MAX) go last
+__device__ __forceinline__ void warp_sort_desc(float& s, int32_t& id, int lane) {
+#pragma unroll
+  for (int size = 2; size <= 32; size <<= 1) {
+#pragma unroll
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      const float os = __shfl_xor_sync(0xffffffffu, s, stride);
+      const int32_t oi = __shfl_xor_sync(0xffffffffu, id, stride);
+      const bool lower = (lane & stride) == 0;
+      const bool descending = (lane & size) == 0;
+      const bool other_first = r_before(os, oi, s, id);
+      const bool take_other = (lower == descending) ? other_first : !other_first;
+      if (take_other) {
+        s = os;
+        id = oi;
+      }
+    }
+  }
+}
+
 #endif  // __CUDACC__
 
 }  // namespace trk

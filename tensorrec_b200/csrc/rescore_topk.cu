@@ -21,10 +21,6 @@ namespace trk {
 constexpr float kRMarginFactor = 1.5f * 0.0009765625f;
 constexpr float kRBiasUlps = 4.0f * 1.1920929e-7f;
 
-__device__ __forceinline__ bool r_before(float xs, int32_t xi, float ys, int32_t yi) {
-  return xs > ys || (xs == ys && xi < yi);
-}
-
 // four consecutive elements of a split row (hi | lo halves, d_pad apart) as fp32 values hi + lo; zeros past d_pad
 __device__ __forceinline__ void load_split4(const __half* __restrict__ row, int d_pad, int lane, bool ok, float (&x)[4]) {
   const int e = lane * 4;
@@ -59,26 +55,6 @@ __device__ __forceinline__ float transpose_sum_16(float (&v)[16], int lane) {
     }
   }
   return v[0] + __shfl_xor_sync(0xffffffffu, v[0], 1);
-}
-
-// bitonic sort of one (score, id) entry per lane into (score desc, id asc) order; sentinels (-inf, INT32_MAX) go last
-__device__ __forceinline__ void warp_sort_desc(float& s, int32_t& id, int lane) {
-#pragma unroll
-  for (int size = 2; size <= 32; size <<= 1) {
-#pragma unroll
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      const float os = __shfl_xor_sync(0xffffffffu, s, stride);
-      const int32_t oi = __shfl_xor_sync(0xffffffffu, id, stride);
-      const bool lower = (lane & stride) == 0;
-      const bool descending = (lane & size) == 0;
-      const bool other_first = r_before(os, oi, s, id);
-      const bool take_other = (lower == descending) ? other_first : !other_first;
-      if (take_other) {
-        s = os;
-        id = oi;
-      }
-    }
-  }
 }
 
 // One warp per user, 16 candidates (one filter list) at a time: the 16 item rows are requested together, the 16 dot

@@ -383,6 +383,25 @@ def operand_stats(split, scale, d_pad, want_norm=True, stats=None):
     return norm
 
 
+def operand_half_sqnorm(split, scale, d_pad):
+    """-1/2 |row|^2 of every row of a split operand (fp32 [rows]): the biases that turn the fused top-k kernels' score
+    q.i + ub + ib into -1/2 d^2(q, i) for Euclidean similar items."""
+    lib = require_cuda()
+    out = torch.empty((split.shape[0],), dtype=torch.float32, device=split.device)
+    rc = lib.trk_operand_half_sqnorm(_p(split), _p(scale), split.shape[0], int(d_pad), _p(out), _stream())
+    _lib.check(rc, 'trk_operand_half_sqnorm')
+    return out
+
+
+def topk_euclidean_finish(top):
+    """In place on a PackedTopK whose scores are -1/2 d^2: scores become -sqrt(max(d^2, 1e-16)) (the reference's
+    Euclidean similarity) and every row is re-sorted by (score desc, id asc)."""
+    lib = require_cuda()
+    rc = lib.trk_topk_euclidean_finish(top.score_ptr(), top.item_ptr(), 2 * top.k, top.n_users, top.k, _stream())
+    _lib.check(rc, 'trk_topk_euclidean_finish')
+    return top
+
+
 def rescale_hi_global(split, scale, stats, d_pad, perm=None):
     lib = require_cuda()
     rows = split.shape[0]

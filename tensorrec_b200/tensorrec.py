@@ -92,6 +92,24 @@ def _checked_exclude(exclude, n_users, n_items, k, item_id_offset, sharded):
     return exclude if isinstance(exclude, sp.csr_matrix) else sp.csr_matrix(exclude)
 
 
+def _similar_exclusion_mask(exclude, exclude_self, ids, n_queries, n_items):
+    """The excluded (query, item) pairs of predict_similar_items_top_k as a CSR matrix of ones (None = nothing excluded
+    at all): the non-zero pairs of `exclude` (duplicates summed first) united with every query's own id when
+    exclude_self.  A union of masks, not a sum of values: a -1 entry on the query's own id stays excluded."""
+    mask = None
+    if exclude is not None:
+        mask = exclude.copy()
+        mask.sum_duplicates()
+        mask.eliminate_zeros()
+        mask = sp.csr_matrix((np.ones(mask.nnz, np.float32), mask.indices, mask.indptr), shape=mask.shape)
+    if exclude_self:
+        own = np.arange(n_queries, dtype=np.int64) if ids is None else ids
+        self_mask = sp.csr_matrix((np.ones(n_queries, np.float32), own, np.arange(n_queries + 1)),
+                                  shape=(n_queries, n_items))
+        mask = self_mask if mask is None else mask.maximum(self_mask)
+    return mask
+
+
 class TensorRec(object):
 
     def __init__(self,
@@ -827,7 +845,9 @@ class TensorRec(object):
             """-> (PackedTopK of the block, [(device counters | None, capacity)] of its sweeps)"""
             host_excl = block_exclusion(u0, u1)
             if not fused:
-                return self._topk_from_dense(block_in, item_in, k, item_id_offset, device, host_excl), [(None, 0)]
+                return self._topk_from_dense(block_in.shape[0], n_items, k, item_id_offset, device,
+                                             lambda: self._predict_device(block_in, item_in, device),
+                                             host_excl), [(None, 0)]
             # every taste sweep of the block uses the same lists (an item is excluded for every taste)
             excl = None if host_excl is None else kernels.DeviceExclusion.upload(*host_excl, device=device)
             if self.n_tastes == 1:
@@ -848,16 +868,25 @@ class TensorRec(object):
                 return distributed.all_gather_rows(merged, u1 - u0, gather_group), np.arange(u0, u1)
             return merged, np.arange(u0 + lo, u0 + hi)
 
+        results, rows = self._run_topk_blocks(blocks, run_block, exchange, info, gather_group, device)
+        info['user_rows'] = rows[0] if len(rows) == 1 else np.concatenate(rows)
+        return self._topk_result(results, to_host)
+
+    @staticmethod
+    def _run_topk_blocks(blocks, run_block, exchange, info, gather_group=None, device=None):
+        """The block loop of the fused top-k: run_block(block_in, r0, r1, force_exact=False) -> (PackedTopK, [(device
+        counters | None, capacity)] of its sweeps) for every (r0, r1, block_in) of `blocks`, exchange(top, r0, r1) ->
+        (top, result rows).  Then one synchronisation for the whole call: how many rows the certificate rejected per
+        sweep (device counters, summed into info['fallback_rows']); a block with more rejected rows than the device-side
+        fallback holds is re-run through the exact kernel.  Returns (the PackedTopK of every block, its result rows)."""
         results, counters, rows = [], [], []
-        for (u0, u1, block_in) in blocks:
-            top, sweeps = run_block(block_in, u0, u1)
-            top, user_rows = exchange(top, u0, u1)
+        for (r0, r1, block_in) in blocks:
+            top, sweeps = run_block(block_in, r0, r1)
+            top, block_rows = exchange(top, r0, r1)
             results.append(top)
             counters.append(sweeps)
-            rows.append(user_rows)
+            rows.append(block_rows)
 
-        # one synchronisation for the whole call: how many rows the certificate rejected per sweep (device counters);
-        # a block with more rejected rows than the device-side fallback holds is re-run through the exact kernel
         live = [c for sweeps in counters for c, _ in sweeps if c is not None]
         if live:
             counts = iter(torch.stack([c[0] for c in live]).cpu().numpy().tolist())
@@ -871,29 +900,34 @@ class TensorRec(object):
                     if n_bad > cap and b not in overflow:
                         overflow.append(b)
             if gather_group is not None:     # every rank must take the same decision: the exchange is collective
+                from . import distributed
                 overflow = distributed.union_of_indices(overflow, len(blocks), gather_group, device)
             for b in overflow:
-                u0, u1, block_in = blocks[b]
-                top, _ = run_block(block_in, u0, u1, force_exact=True)
-                results[b], rows[b] = exchange(top, u0, u1)
+                r0, r1, block_in = blocks[b]
+                top, _ = run_block(block_in, r0, r1, force_exact=True)
+                results[b], rows[b] = exchange(top, r0, r1)
             info['overflow_blocks'] = len(overflow)
-        info['user_rows'] = rows[0] if len(rows) == 1 else np.concatenate(rows)
+        return results, rows
+
+    @staticmethod
+    def _topk_result(results, to_host):
+        """The PackedTopK of consecutive row blocks -> one TopK (device tensors, or numpy arrays with to_host)."""
         top_s = results[0].scores if len(results) == 1 else torch.cat([r.scores for r in results])
         top_i = results[0].items if len(results) == 1 else torch.cat([r.items for r in results])
         if not to_host:
             return TopK(top_i, top_s)
         return TopK(*kernels.to_host(top_i, top_s))
 
-    def _topk_from_dense(self, user_in, item_in, k, item_id_offset, device, host_excl=None):
+    def _topk_from_dense(self, n_users, n_items, k, item_id_offset, device, score, host_excl=None):
         """Any model the fused kernel does not cover: dense scores -> exact full ranks -> the rank <= k entries.
-        host_excl: exclusion lists (indptr, local ids) of the rows -- those scores become -inf before the ranking and
-        those entries are never emitted (their slots keep the sentinel)."""
-        n_users, n_items = user_in.shape[0], item_in.shape[0]
+        score() -> the float32 [n_users, n_items] scores of the rows on the device.  host_excl: exclusion lists (indptr,
+        local ids) of the rows -- those scores become -inf before the ranking and those entries are never emitted (their
+        slots keep the sentinel)."""
         top = kernels.PackedTopK(n_users, k, device)
         top.scores.fill_(float('-inf'))
         top.items.fill_(2 ** 31 - 1)
         if n_items > 0:
-            scores = self._predict_device(user_in, item_in, device)
+            scores = score()
             excluded = None
             if host_excl is not None:
                 indptr, ids = host_excl
@@ -914,7 +948,8 @@ class TensorRec(object):
 
     def predict_similar_items(self, item_features, item_ids, n_similar):
         """tensorrec/tensorrec.py:666-703: for each id, the n_similar (item_id, score) pairs of highest prediction
-        between that item's representation and every item's."""
+        between that item's representation and every item's.
+        For whole catalogues (no [len(item_ids), n_items] matrix), use predict_similar_items_top_k."""
         if self.tf_prediction is None:
             raise ModelNotFitException(method='predict_similar_items')
         device = self._cuda_device()
@@ -939,6 +974,128 @@ class TensorRec(object):
             best = np.argpartition(item_sims, -n_similar)[-n_similar:]
             results.append(sorted(zip(best, item_sims[best]), key=lambda x: -x[1]))
         return results
+
+    def predict_similar_items_top_k(self, item_features, n_similar, item_ids=None, exclude=None, exclude_self=False,
+                                    to_host=True, item_batch_size=None):
+        """The n_similar most similar items of every query item, without materialising the [n_queries, n_items]
+        similarity matrix: TopK(items int32 [n_queries, n_similar], scores float32 [n_queries, n_similar]).
+
+        Similarity is predict_similar_items' score: the prediction graph (dot, cosine or Euclidean for the built-in
+        graphs) between the query's item representation and every item's, without biases (biased, n_tastes and the
+        attention graph do not enter it).  Row q holds the n_similar best items of query q in reference rank order
+        (score descending, lower item id first on ties); slots that cannot be filled hold (id 2**31 - 1, score -inf).
+
+        item_ids: 1-D integer array-like of query item ids in [0, n_items) (duplicates allowed); None = every item, in
+        order (the whole "related items" table).  exclude: None or a scipy sparse matrix [n_queries, n_items] with the
+        rules of predict_top_k's `exclude` (duplicates summed; a pair is excluded when its sum is non-zero).
+        exclude_self: also exclude every query's own id (the reference returns the item itself, hence the default False).
+        item_batch_size: queries are processed in blocks of this many rows (bit-identical results).
+
+        Built-in prediction and representation graphs with n_components <= 128 and n_similar <= 32 run on the fused
+        tensor-core top-k kernels (filter + re-scoring for n_similar <= 12, else the exact 3-pass kernel); Euclidean
+        similarity ranks -1/2 d^2 = q.i - 1/2 |q|^2 - 1/2 |i|^2 there and is mapped to -sqrt(d^2) at the end.  Everything
+        else scores dense query blocks and ranks them.  last_topk_info['path'] names the route.  Single GPU: queries
+        and items live on one device (there is no item-sharded form)."""
+        if self.tf_prediction is None:
+            raise ModelNotFitException(method='predict_similar_items_top_k')
+        item_in = self._single_input(item_features, 'item_features')
+        self._check_features(item_in, self.n_item_features, 'item')
+        n_items = item_in.shape[0]
+        n = int(n_similar)
+        if n < 1:
+            raise ValueError('n_similar must be >= 1')
+        ids = None
+        if item_ids is not None:
+            ids = np.asarray(item_ids)
+            if ids.ndim != 1:
+                raise ValueError('item_ids must be a 1-D array of item ids')
+            if ids.size == 0:
+                ids = ids.astype(np.int64)
+            if not np.issubdtype(ids.dtype, np.integer):
+                raise ValueError('item_ids must hold integers')
+            if ids.size and (ids.min() < 0 or ids.max() >= n_items):
+                raise ValueError('item_ids must lie in [0, %d)' % n_items)
+            ids = ids.astype(np.int64)
+        n_queries = n_items if ids is None else ids.shape[0]
+        if exclude is not None:
+            exclude = _checked_exclude(exclude, n_queries, n_items, n, 0, False)
+        mask = _similar_exclusion_mask(exclude, exclude_self, ids, n_queries, n_items)
+
+        pred_graph = self.prediction_graph_factory
+        kind = pred_graph.b200_kind if type(pred_graph) in _BUILTIN_PRED else None
+        euclidean = kind == 'euclidean'
+        device = self._cuda_device()
+        d_pad = kernels.d_pad_for(self.n_components)
+        model_ok = (SCORE_PATH != 'exact' and kind is not None and type(self.item_repr_graph_factory) in _BUILTIN_REPR
+                    and d_pad <= 128)
+        if SCORE_PATH == 'tensor' and not model_ok:
+            raise RuntimeError('TENSORREC_B200_SCORE_PATH=tensor but this model cannot use the tensor-core kernel')
+        fused = model_ok and n_items > 0 and n <= kernels.topk_max_k(d_pad)
+        use_filter = fused and TOPK_PATH != 'exact' and n <= kernels.filter_max_k()
+        info = self.last_topk_info = {'path': 'filter' if use_filter else ('exact3' if fused else 'dense+rank'),
+                                      'fallback_rows': 0}
+        if n_queries == 0:
+            return TopK(np.zeros((0, n), np.int32), np.zeros((0, n), np.float32))
+        ids_dev = None if ids is None else torch.from_numpy(ids).to(device)
+
+        def take(t, q0, q1):
+            """Rows of the queries [q0, q1) of a per-item tensor (a view when the queries are all items in order)."""
+            if t is None:
+                return None
+            return t[q0:q1] if ids_dev is None else t.index_select(0, ids_dev[q0:q1])
+
+        extra = 1 if kind == 'cosine' else 0
+        if fused:
+            # the item operand once: split fp16 + scale (+ row norms and statistics for the filter), no projected biases;
+            # Euclidean: bias -1/2 |i|^2.  The queries are rows of this same operand.
+            stats = torch.empty((3,), dtype=torch.float32, device=device) if use_filter else None
+            out = self._represent(self.item_repr_graph_factory, item_in, self.n_item_features, 'item', device, extra,
+                                  want_f32=False, split_d_pad=d_pad, want_norm=use_filter, stats=stats)
+            split, scale, norm = out[1], out[2], (out[3] if use_filter else None)
+            bias = kernels.operand_half_sqnorm(split, scale, d_pad) if euclidean else None
+            items = kernels.SideOperands(None, split, scale, bias, n_items, self.n_components, d_pad, stats=stats)
+            fitems = kernels.FilterItems(items) if use_filter else None
+
+            def query_rows(q0, q1):
+                return kernels.SideOperands(None, take(split, q0, q1), take(scale, q0, q1), take(bias, q0, q1), q1 - q0,
+                                            self.n_components, d_pad, norm=take(norm, q0, q1))
+        else:
+            item_repr = self._represent(self.item_repr_graph_factory, item_in, self.n_item_features, 'item', device,
+                                        extra)[0]
+
+            def dense_scores(q0, q1):
+                gathered = take(item_repr, q0, q1).contiguous()
+                if kind is not None:
+                    return kernels.score_exact(gathered, item_repr, mode=1 if euclidean else 0)
+                with torch.no_grad():
+                    sims = pred_graph.connect_dense_prediction_graph(tf_user_representation=gathered,
+                                                                     tf_item_representation=item_repr)
+                return sims.to(torch.float32).contiguous()
+
+        def run_block(_, q0, q1, force_exact=False):
+            host_excl = None if mask is None else kernels.exclusion_host_csr(mask, 0, n_items, q0, q1)
+            if not fused:
+                return self._topk_from_dense(q1 - q0, n_items, n, 0, device, lambda: dense_scores(q0, q1),
+                                             host_excl), [(None, 0)]
+            excl = None if host_excl is None else kernels.DeviceExclusion.upload(*host_excl, device=device)
+            queries = query_rows(q0, q1)
+            if use_filter and not force_exact:
+                top, cnt, cap = kernels.topk_filter(queries, items, n, fitems=fitems, excl=excl)
+                return top, [(cnt, cap)]
+            return kernels.topk_exact(queries, items, n, excl=excl), [(None, 0)]
+
+        if item_batch_size is not None:
+            step = max(1, int(item_batch_size))
+        elif fused:
+            step = n_queries
+        else:
+            step = max(1, self.PREDICT_BLOCK_BYTES // max(4 * n_items, 1))
+        blocks = [(q0, min(n_queries, q0 + step), None) for q0 in range(0, n_queries, step)]
+        results, _ = self._run_topk_blocks(blocks, run_block, lambda top, q0, q1: (top, None), info)
+        if fused and euclidean:
+            for top in results:
+                kernels.topk_euclidean_finish(top)
+        return self._topk_result(results, to_host)
 
     def predict_user_representation(self, user_features):
         """[n_users, n_components] (or [n_tastes, n_users, n_components] when n_tastes > 1) (tensorrec.py:735-762)."""
