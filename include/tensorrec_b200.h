@@ -289,6 +289,48 @@ int trk_operand_half_sqnorm(const void* split, const float* scale, int64_t rows,
 int trk_topk_euclidean_finish(float* scores, int32_t* items, int64_t row_stride, int64_t n_rows, int32_t k,
                               void* stream);
 
+/* Wide form of the filter top-k: 32 < k <= trk_score_wide_max_k() (1024), same inputs as trk_score_filter_f16 (the
+ * hi item operand in processing order, packed biases, block maxima, perm, statistics) except block_bias_min: the wide
+ * form has no warm start.  Every (user, split) keeps its candidates in a list in global memory of
+ * trk_score_wide_list_capacity(k) entries; a warp compacts a full list by a radix select of the k-th best approximate
+ * score, keeps everything within the error bound of it (at most half the capacity) and raises its threshold.
+ *   trk_score_wide_f16        list_score / list_item [n_users, n_splits, capacity] (scratch while the kernel runs; on
+ *                             return entries [0, list_count) hold (approximate score, global item id)), list_count
+ *                             [n_users, n_splits], row_theta [n_users, n_splits] = max(theta, best dropped score).
+ *   trk_score_wide_f16_excl   the same plus the exclusion lists as processing positions (see
+ *                             trk_score_filter_f16_excl).
+ *   trk_select_wide_topk      per row: the candidate ids cand_item[row * cand_row_stride + l * list_width + e] for
+ *                             the n_lists lists l and e < list_count[row * n_lists + l] (list_count NULL: every entry;
+ *                             ids outside [item_id_offset, item_id_offset + n_items_local) and INT32_MAX are not
+ *                             candidates) are re-scored with the arithmetic of trk_rescore_topk_split, sorted by
+ *                             (score desc, id asc) and the first k written to out_score / out_item (row stride
+ *                             out_row_stride; sentinels (-inf, INT32_MAX)).  out_flag (may be NULL: no certificate)
+ *                             receives 1 for rows the certificate of trk_rescore_topk_split rejects (row_theta
+ *                             [n_rows, n_lists], user_norm, item_stats are then required).  euclidean != 0: the
+ *                             scores (-1/2 d^2) are mapped to -sqrt(max(d^2, 1e-16)) after the certificate and the
+ *                             row is sorted again.  n_lists * list_width <= 16384. */
+int trk_score_wide_max_k(void);
+int trk_score_wide_list_capacity(int32_t k);
+int trk_score_wide_f16(const void* user_split, const float* user_scale, const float* user_bias,
+                       const float* user_norm, const void* item_hi_global, const float* item_stats,
+                       const float* item_bias_padded, const float* block_bias_max, const int32_t* item_perm,
+                       int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k, int32_t n_splits,
+                       int32_t item_id_offset, float* list_score, int32_t* list_item, int32_t* list_count,
+                       float* row_theta, void* stream);
+int trk_score_wide_f16_excl(const void* user_split, const float* user_scale, const float* user_bias,
+                            const float* user_norm, const void* item_hi_global, const float* item_stats,
+                            const float* item_bias_padded, const float* block_bias_max, const int32_t* item_perm,
+                            int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k, int32_t n_splits,
+                            int32_t item_id_offset, float* list_score, int32_t* list_item, int32_t* list_count,
+                            float* row_theta, const int32_t* excl_indptr, const int32_t* excl_pos, void* stream);
+int trk_select_wide_topk(const void* user_split, const float* user_scale, const void* item_split,
+                         const float* item_scale, const float* user_bias, const float* item_bias,
+                         const int32_t* cand_item, int64_t cand_row_stride, int32_t n_lists, int32_t list_width,
+                         const int32_t* list_count, const float* row_theta, const float* user_norm,
+                         const float* item_stats, int64_t n_rows, int64_t n_items_local, int32_t d_pad, int32_t k,
+                         int32_t item_id_offset, int32_t euclidean, float* out_score, int32_t* out_item,
+                         int64_t out_row_stride, int32_t* out_flag, void* stream);
+
 /* Tensor-core dense prediction with the same operands, writing the full fp32 matrix out[n_users, n_items]
  * (predict(); tensorrec/tensorrec.py:636-664).  HBM-write bound. */
 int trk_score_dense_f16x3(const void* user_split, const float* user_scale, const float* user_bias,

@@ -65,6 +65,15 @@ SIGNATURES = {
     'trk_scatter_topk_rows': (ctypes.c_int, [_c_p, _c_p, _c_i32, _c_p, _c_p, _c_i64, _c_i32, _c_p, _c_p, _c_i64, _c_p]),
     'trk_operand_half_sqnorm': (ctypes.c_int, [_c_p, _c_p, _c_i64, _c_i32, _c_p, _c_p]),
     'trk_topk_euclidean_finish': (ctypes.c_int, [_c_p, _c_p, _c_i64, _c_i64, _c_i32, _c_p]),
+    'trk_score_wide_max_k': (ctypes.c_int, []),
+    'trk_score_wide_list_capacity': (ctypes.c_int, [_c_i32]),
+    'trk_score_wide_f16': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_i64, _c_i64, _c_i32,
+                                          _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p]),
+    'trk_score_wide_f16_excl': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_i64, _c_i64,
+                                               _c_i32, _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p]),
+    'trk_select_wide_topk': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_i64, _c_i32, _c_i32, _c_p, _c_p,
+                                            _c_p, _c_p, _c_i64, _c_i64, _c_i32, _c_i32, _c_i32, _c_i32, _c_p, _c_p,
+                                            _c_i64, _c_p, _c_p]),
     'trk_sample_items': (ctypes.c_int, [_c_i64, _c_i64, _c_i32, _c_i32, ctypes.c_uint64, ctypes.c_uint32, _c_p, _c_p]),
     'trk_sample_stream_u64': (ctypes.c_uint64, [ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32]),
     'trk_wmrb_step': (ctypes.c_int, [_c_p, _c_p, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_i64, _c_i64, _c_i32,

@@ -105,6 +105,14 @@ int scatter_topk_rows(const int32_t*, const int32_t*, int32_t, const float*, con
                       int32_t*, int64_t, cudaStream_t);
 int operand_half_sqnorm(const void*, const float*, int64_t, int32_t, float*, cudaStream_t);
 int topk_euclidean_finish(float*, int32_t*, int64_t, int64_t, int32_t, cudaStream_t);
+int score_wide_max_k();
+int score_wide_list_capacity(int32_t);
+int score_wide_f16(const void*, const float*, const float*, const float*, const void*, const float*, const float*,
+                   const float*, const int32_t*, int64_t, int64_t, int32_t, int32_t, int32_t, int32_t, float*, int32_t*,
+                   int32_t*, float*, const int32_t*, const int32_t*, cudaStream_t);
+int select_wide_topk(const void*, const float*, const void*, const float*, const float*, const float*, const int32_t*,
+                     int64_t, int32_t, int32_t, const int32_t*, const float*, const float*, const float*, int64_t,
+                     int64_t, int32_t, int32_t, int32_t, int32_t, float*, int32_t*, int64_t, int32_t*, cudaStream_t);
 
 int sample_items(int64_t, int64_t, int32_t, int32_t, uint64_t, uint32_t, int32_t*, cudaStream_t);
 int wmrb_step(const void*, const void*, int32_t, const float*, const float*, const int32_t*, const int32_t*, const float*,
@@ -305,6 +313,48 @@ int trk_operand_half_sqnorm(const void* split, const float* scale, int64_t rows,
 int trk_topk_euclidean_finish(float* scores, int32_t* items, int64_t row_stride, int64_t n_rows, int32_t k,
                               void* stream) {
   return trk::topk_euclidean_finish(scores, items, row_stride, n_rows, k, trk::as_stream(stream));
+}
+
+int trk_score_wide_max_k(void) { return trk::score_wide_max_k(); }
+
+int trk_score_wide_list_capacity(int32_t k) { return trk::score_wide_list_capacity(k); }
+
+int trk_score_wide_f16(const void* user_split, const float* user_scale, const float* user_bias,
+                       const float* user_norm, const void* item_hi_global, const float* item_stats,
+                       const float* item_bias_padded, const float* block_bias_max, const int32_t* item_perm,
+                       int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k, int32_t n_splits,
+                       int32_t item_id_offset, float* list_score, int32_t* list_item, int32_t* list_count,
+                       float* row_theta, void* stream) {
+  return trk::score_wide_f16(user_split, user_scale, user_bias, user_norm, item_hi_global, item_stats,
+                             item_bias_padded, block_bias_max, item_perm, n_users, n_items, d_pad, k, n_splits,
+                             item_id_offset, list_score, list_item, list_count, row_theta, nullptr, nullptr,
+                             trk::as_stream(stream));
+}
+
+int trk_score_wide_f16_excl(const void* user_split, const float* user_scale, const float* user_bias,
+                            const float* user_norm, const void* item_hi_global, const float* item_stats,
+                            const float* item_bias_padded, const float* block_bias_max, const int32_t* item_perm,
+                            int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k, int32_t n_splits,
+                            int32_t item_id_offset, float* list_score, int32_t* list_item, int32_t* list_count,
+                            float* row_theta, const int32_t* excl_indptr, const int32_t* excl_pos, void* stream) {
+  TRK_CHECK_ARG(excl_indptr != nullptr && excl_pos != nullptr, "trk_score_wide_f16_excl: null exclusion list");
+  return trk::score_wide_f16(user_split, user_scale, user_bias, user_norm, item_hi_global, item_stats,
+                             item_bias_padded, block_bias_max, item_perm, n_users, n_items, d_pad, k, n_splits,
+                             item_id_offset, list_score, list_item, list_count, row_theta, excl_indptr, excl_pos,
+                             trk::as_stream(stream));
+}
+
+int trk_select_wide_topk(const void* user_split, const float* user_scale, const void* item_split,
+                         const float* item_scale, const float* user_bias, const float* item_bias,
+                         const int32_t* cand_item, int64_t cand_row_stride, int32_t n_lists, int32_t list_width,
+                         const int32_t* list_count, const float* row_theta, const float* user_norm,
+                         const float* item_stats, int64_t n_rows, int64_t n_items_local, int32_t d_pad, int32_t k,
+                         int32_t item_id_offset, int32_t euclidean, float* out_score, int32_t* out_item,
+                         int64_t out_row_stride, int32_t* out_flag, void* stream) {
+  return trk::select_wide_topk(user_split, user_scale, item_split, item_scale, user_bias, item_bias, cand_item,
+                               cand_row_stride, n_lists, list_width, list_count, row_theta, user_norm, item_stats,
+                               n_rows, n_items_local, d_pad, k, item_id_offset, euclidean, out_score, out_item,
+                               out_row_stride, out_flag, trk::as_stream(stream));
 }
 
 int trk_sample_items(int64_t n_users, int64_t n_items, int32_t n_sampled, int32_t replace, uint64_t seed,

@@ -304,6 +304,25 @@ __device__ __forceinline__ void warp_sort_desc(float& s, int32_t& id, int lane) 
   }
 }
 
+// four consecutive elements of a split row (hi | lo halves, d_pad apart) as fp32 values hi + lo; zeros past d_pad
+__device__ __forceinline__ void load_split4(const __half* __restrict__ row, int d_pad, int lane, bool ok, float (&x)[4]) {
+  const int e = lane * 4;
+  if (ok && e < d_pad) {
+    const uint2 h = __ldg(reinterpret_cast<const uint2*>(row + e));
+    const uint2 l = __ldg(reinterpret_cast<const uint2*>(row + d_pad + e));
+    const float2 h0 = __half22float2(*reinterpret_cast<const __half2*>(&h.x));
+    const float2 h1 = __half22float2(*reinterpret_cast<const __half2*>(&h.y));
+    const float2 l0 = __half22float2(*reinterpret_cast<const __half2*>(&l.x));
+    const float2 l1 = __half22float2(*reinterpret_cast<const __half2*>(&l.y));
+    x[0] = h0.x + l0.x;
+    x[1] = h0.y + l0.y;
+    x[2] = h1.x + l1.x;
+    x[3] = h1.y + l1.y;
+  } else {
+    x[0] = x[1] = x[2] = x[3] = 0.0f;
+  }
+}
+
 #endif  // __CUDACC__
 
 }  // namespace trk

@@ -88,3 +88,12 @@ def predict_top_k_sharded(model, user_features, item_features, k, group=None, to
                                gather_group=group if group is not None else dist.group.WORLD, to_host=to_host,
                                gather=gather, user_batch_size=user_batch_size, **({} if exclude is None else
                                                                                {'exclude': exclude}))
+
+
+def common_block_rows(rows, group, device):
+    """The smallest of the block sizes (user rows per block) the ranks chose.  Each rank sizes its blocks from its own
+    item shard, and shards differ in size; but every block ends in the collective exchange, so every rank must cut the
+    users into the same blocks."""
+    t = torch.tensor([int(rows)], dtype=torch.int64, device=device)
+    dist.all_reduce(t, op=dist.ReduceOp.MIN, group=group)
+    return int(t.item())

@@ -332,6 +332,14 @@ class PackedTopK(object):
         return ctypes.c_void_p(self.buf.data_ptr() + 4 * self.k)
 
 
+def empty_topk(n_rows, k, device):
+    """PackedTopK [n_rows, k] of sentinels only (id 2**31 - 1, score -inf): the result over an empty catalogue."""
+    top = PackedTopK(n_rows, k, device)
+    top.scores.fill_(float('-inf'))
+    top.items.fill_(2 ** 31 - 1)
+    return top
+
+
 def topk_merge(cand_score, cand_item, k_out, out=None, n_users_live=None):
     """[U, L, k_in] candidate lists -> PackedTopK [U, k_out] (top scores, top item ids)."""
     lib = require_cuda()
@@ -675,6 +683,178 @@ def topk_filter(users, items, k, n_splits=None, item_id_offset=0, fitems=None, e
                                   excl=excl)
     counters, cap = rerun_uncertified(users, items, bad, top, k, item_id_offset=item_id_offset, excl=excl)
     return top, counters, cap
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# wide form of the filter (32 < k <= 1024): candidate lists in global memory, re-scoring + selection + certificate in
+# one CTA per row, rows the certificate rejects scored dense and ranked
+# ---------------------------------------------------------------------------------------------------------------
+WIDE_MAX_SLOTS = 16384      # candidates of one row trk_select_wide_topk sorts at once (n_splits x list capacity)
+DENSE_RANK_BYTES_PER_PAIR = 35   # device bytes per (row, item) pair that dense scores + rank_full + selection hold
+
+
+def wide_max_k():
+    return int(require_cuda().trk_score_wide_max_k())
+
+
+def wide_list_capacity(k):
+    """Entries of one wide candidate list (per user and item split) for this k."""
+    return int(require_cuda().trk_score_wide_list_capacity(int(k)))
+
+
+def wide_splits(n_users, n_items, k):
+    """default_splits, bounded so that a row's lists fit one selection (n_splits x capacity <= WIDE_MAX_SLOTS)."""
+    return int(max(1, min(default_splits(n_users, n_items), WIDE_MAX_SLOTS // wide_list_capacity(k))))
+
+
+def score_wide(users, user_norm, fitems, n_items, k, n_splits, item_id_offset=0, excl=None):
+    """Wide filter pass.  Returns (list_item [U, n_splits, capacity], list_count [U, n_splits], theta [U, n_splits])."""
+    lib = require_cuda()
+    dev = users.split.device
+    cap = wide_list_capacity(k)
+    list_s = torch.empty((users.n_rows, n_splits, cap), dtype=torch.float32, device=dev)
+    list_i = torch.empty((users.n_rows, n_splits, cap), dtype=torch.int32, device=dev)
+    count = torch.empty((users.n_rows, n_splits), dtype=torch.int32, device=dev)
+    theta = torch.empty((users.n_rows, n_splits), dtype=torch.float32, device=dev)
+    if excl is None:
+        name, extra = 'trk_score_wide_f16', ()
+    else:
+        name, extra = 'trk_score_wide_f16_excl', (_p(excl.indptr), _p(excl.pos))
+    rc = getattr(lib, name)(_p(users.split), _p(users.scale), _p(users.bias), _p(user_norm), _p(fitems.hi),
+                            _p(fitems.stats), _p(fitems.bias_pad), _p(fitems.block_max), _p(fitems.perm), users.n_rows,
+                            n_items, int(users.d_pad), int(k), int(n_splits), int(item_id_offset), _p(list_s),
+                            _p(list_i), _p(count), _p(theta), *extra, _stream())
+    _lib.check(rc, name)
+    return list_i, count, theta
+
+
+def select_wide(users, items, cand_item, n_lists, width, k, count=None, theta=None, user_norm=None, item_stats=None,
+                item_id_offset=0, euclidean=False, out=None):
+    """Candidate ids per row (cand_item[row, l * width + e], e < count[row, l]) -> PackedTopK [U, k] re-scored from the
+    split operands in (score desc, id asc) order, and -- when theta is given -- flags int32 [U] of the rows the
+    certificate rejects (else None).  euclidean: scores -1/2 d^2 become -sqrt(max(d^2, 1e-16))."""
+    lib = require_cuda()
+    dev = users.split.device
+    if out is None:
+        out = PackedTopK(users.n_rows, k, dev)
+    flags = None if theta is None else torch.empty((users.n_rows,), dtype=torch.int32, device=dev)
+    rc = lib.trk_select_wide_topk(_p(users.split), _p(users.scale), _p(items.split), _p(items.scale), _p(users.bias),
+                                  _p(items.bias), _p(cand_item), cand_item.stride(0), int(n_lists), int(width),
+                                  _p(count), _p(theta), _p(user_norm), _p(item_stats), users.n_rows, items.n_rows,
+                                  int(users.d_pad), int(k), int(item_id_offset), 1 if euclidean else 0,
+                                  out.score_ptr(), out.item_ptr(), 2 * out.k, _p(flags), _stream())
+    _lib.check(rc, 'trk_select_wide_topk')
+    return out, flags
+
+
+def exclusion_pairs(excl, rows):
+    """(row position, local item id) long tensors of the excluded pairs of the list rows `rows` (long [n])."""
+    dev = excl.indptr.device
+    starts = excl.indptr[rows].long()
+    lens = excl.indptr[rows + 1].long() - starts
+    pair_row = torch.repeat_interleave(torch.arange(rows.numel(), device=dev), lens)
+    first = torch.repeat_interleave(torch.cumsum(lens, 0) - lens, lens)
+    offs = torch.arange(pair_row.numel(), device=dev) - first
+    return pair_row, excl.ids[starts[pair_row] + offs].long()
+
+
+def topk_from_scores(scores, k, item_id_offset=0, ex_rows=None, ex_cols=None):
+    """Dense scores [n, n_items] (modified in place) -> PackedTopK [n, k] of the entries of rank <= k (exact full ranks,
+    trk_rank_full).  ex_rows / ex_cols: excluded pairs -- they score -inf before the ranking and are never emitted
+    (their slots keep the sentinel (-inf, 2**31 - 1))."""
+    n_rows, n_items = scores.shape
+    top = empty_topk(n_rows, k, scores.device)
+    excluded = None
+    if ex_rows is not None:
+        scores[ex_rows, ex_cols] = float('-inf')
+        excluded = torch.zeros((n_rows, n_items), dtype=torch.bool, device=scores.device)
+        excluded[ex_rows, ex_cols] = True
+    ranks = rank_full(scores).long()
+    sel = ranks <= k
+    if excluded is not None:
+        sel &= ~excluded
+    rows, cols = sel.nonzero(as_tuple=True)
+    pos = ranks[rows, cols] - 1
+    top.scores[rows, pos] = scores[rows, cols]
+    top.items[rows, pos] = (cols + item_id_offset).to(torch.int32)
+    return top
+
+
+def dense_rank_rows(n_items, block_bytes):
+    """Rows of one dense-score + full-rank block that stay within block_bytes (DENSE_RANK_BYTES_PER_PAIR per pair)."""
+    return int(max(1, block_bytes // max(DENSE_RANK_BYTES_PER_PAIR * int(n_items), 1)))
+
+
+def rerun_flagged_dense(users, items, bad, top, k, item_id_offset=0, excl=None, euclidean=False,
+                        block_bytes=4 << 30):
+    """Rows of `top` whose certificate failed (bad != 0): compacted on the device, their operands gathered, scored dense
+    by the exact 3-pass kernel in blocks of at most block_bytes, ranked (trk_rank_full, exclusion as a mask), and their
+    rank <= k items re-scored and ordered by trk_select_wide_topk (the arithmetic of every other row) before they are
+    scattered back into `top`.  One host synchronisation per call, i.e. per user block: the count, which sizes the dense
+    work.  (The default wide blocks are large: one block at k = 100 for up to 1.68M users, six at k = 1000 for 1M.)
+    Returns the device counters (counters[0] = rows)."""
+    lib = require_cuda()
+    dev = users.split.device
+    n = users.n_rows
+    idx = torch.empty((max(n, 1),), dtype=torch.int32, device=dev)
+    counters = torch.zeros((4,), dtype=torch.int32, device=dev)
+    if n == 0:
+        return counters
+    rc = lib.trk_select_flagged_rows(_p(bad), n, _p(idx), n, _p(counters), _stream())
+    _lib.check(rc, 'trk_select_flagged_rows')
+    n_bad = int(counters[0].item())
+    if n_bad == 0:
+        return counters
+    sub_split = torch.empty((n_bad, 2 * users.d_pad), dtype=torch.float16, device=dev)
+    sub_scale = torch.empty((n_bad,), dtype=torch.float32, device=dev)
+    sub_bias = None if users.bias is None else torch.empty((n_bad,), dtype=torch.float32, device=dev)
+    rc = lib.trk_gather_operand_rows(_p(idx), _p(counters), n_bad, n_bad, _p(users.split), _p(users.scale),
+                                     _p(users.bias), int(users.d_pad), _p(sub_split), _p(sub_scale), _p(sub_bias),
+                                     _stream())
+    _lib.check(rc, 'trk_gather_operand_rows')
+    sub = SideOperands(None, sub_split, sub_scale, sub_bias, n_bad, users.d, users.d_pad)
+    meta = pack_item_meta(items.scale, items.bias, items.n_rows)
+    cand = torch.empty((n_bad, k), dtype=torch.int32, device=dev)
+    step = dense_rank_rows(items.n_rows, block_bytes)
+    rows = idx[:n_bad].long()
+    for r0 in range(0, n_bad, step):
+        r1 = min(n_bad, r0 + step)
+        part = sub.rows(r0, r1)
+        scores = score_dense_tc(part.split, part.scale, part.bias, items.split, meta, r1 - r0, items.n_rows,
+                                users.d_pad)
+        ex = (None, None) if excl is None else exclusion_pairs(excl, rows[r0:r1])
+        cand[r0:r1] = topk_from_scores(scores, k, item_id_offset, *ex).items
+        del scores
+    fixed, _ = select_wide(sub, items, cand, 1, k, k, item_id_offset=item_id_offset, euclidean=euclidean)
+    rc = lib.trk_scatter_topk_rows(_p(idx), _p(counters), n_bad, fixed.score_ptr(), fixed.item_ptr(), 2 * fixed.k,
+                                   int(k), top.score_ptr(), top.item_ptr(), 2 * top.k, _stream())
+    _lib.check(rc, 'trk_scatter_topk_rows')
+    return counters
+
+
+def topk_wide(users, items, k, n_splits=None, item_id_offset=0, fitems=None, excl=None, euclidean=False,
+              block_bytes=4 << 30):
+    """Wide filter form for 32 < k <= wide_max_k(): one tensor pass that keeps every row's candidates in global memory,
+    re-scoring + selection + certificate (trk_select_wide_topk), and the rows the certificate rejects scored dense and
+    ranked (rerun_flagged_dense).  Returns (PackedTopK, counters device int32[4], capacity); counters[0] = rows that
+    took the dense fallback (every flagged row fits: capacity = the number of rows)."""
+    user_norm = users.norm if users.norm is not None else operand_stats(users.split, users.scale, users.d_pad)
+    if fitems is None:
+        fitems = FilterItems(items)
+    if excl is not None and excl.pos is None:
+        exclusion_positions(excl, fitems.perm, items.n_rows)
+    if n_splits is None:
+        n_splits = wide_splits(users.n_rows, items.n_rows, k)
+    cand, count, theta = score_wide(users, user_norm, fitems, items.n_rows, k, n_splits,
+                                    item_id_offset=item_id_offset, excl=excl)
+    cap = cand.shape[2]
+    top, bad = select_wide(users, items, cand.view(users.n_rows, n_splits * cap), n_splits, cap, k, count=count,
+                           theta=theta, user_norm=user_norm, item_stats=fitems.stats, item_id_offset=item_id_offset,
+                           euclidean=euclidean)
+    del cand, count, theta
+    counters = rerun_flagged_dense(users, items, bad, top, k, item_id_offset=item_id_offset, excl=excl,
+                                   euclidean=euclidean, block_bytes=block_bytes)
+    return top, counters, users.n_rows
 
 
 # ---------------------------------------------------------------------------------------------------------------

@@ -54,6 +54,30 @@ SCORE_PATH = os.environ.get('TENSORREC_B200_SCORE_PATH', 'auto')
 # 3-pass split-product kernel
 TOPK_PATH = os.environ.get('TENSORREC_B200_TOPK_PATH', 'auto')
 
+# The wide form of the filter serves 32 < k <= WIDE_MAX_K on catalogues of at least WIDE_MIN_ITEMS items; below that,
+# scoring the catalogue densely and ranking it costs less than a sweep (see README, "Large k").
+WIDE_MAX_K = 1024
+WIDE_MIN_ITEMS = 4096
+
+
+def topk_route(k, n_items, model_ok, single_taste, filter_max_k, exact_max_k, sharded=False):
+    """The route of a top-k call -- 'filter', 'exact3', 'wide' or 'dense+rank' -- from k, the catalogue size and the
+    model alone.  model_ok: the tensor-core kernels evaluate the model (built-in dot / cosine prediction, or any
+    built-in similar-items graph, no attention, d_pad <= 128); single_taste: one taste (the wide route has no
+    de-duplicating merge); filter_max_k / exact_max_k: the k limits of the filter and of the exact 3-pass kernel.
+    sharded: an item-sharded call, where every rank must take the same route (the exchange is collective), so a
+    rank's shard size does not decide the wide route.  TOPK_PATH='exact' means "no filter": k > exact_max_k then
+    goes to dense+rank."""
+    if not model_ok:
+        return 'dense+rank'
+    if k <= exact_max_k:
+        if n_items == 0:
+            return 'dense+rank'
+        return 'filter' if TOPK_PATH != 'exact' and k <= filter_max_k else 'exact3'
+    if TOPK_PATH == 'exact' or not single_taste or k > WIDE_MAX_K:
+        return 'dense+rank'
+    return 'wide' if sharded or n_items >= WIDE_MIN_ITEMS else 'dense+rank'
+
 
 def _names_argument(method, name):
     """Does `method` declare `name` as an explicit parameter (not just **kwargs)?"""
@@ -785,6 +809,10 @@ class TensorRec(object):
         with gather='all', one all-gather of the merged slices so that every rank returns all users.  gather='slice'
         returns this rank's users only (rows `last_topk_info['user_rows']`).
         user_batch_size: users are processed in blocks of this many rows (bounds device memory at 10M+ users).
+        32 < k <= WIDE_MAX_K on catalogues of at least WIDE_MIN_ITEMS items runs on the wide form of the filter (each
+        user's candidates in a list in device memory, rows the certificate rejects scored dense and ranked); the default
+        user blocks then keep those lists within PREDICT_BLOCK_BYTES.  last_topk_info['path'] names the route
+        (topk_route).
 
         exclude: None, or a scipy sparse matrix (any format) with n_users rows whose column index is the GLOBAL item id
         (the numbering of TopK.items).  The pair (u, i) is excluded when exclude[u, i] != 0 after duplicates are summed
@@ -822,21 +850,34 @@ class TensorRec(object):
                 return None
             return kernels.exclusion_host_csr(exclude, item_id_offset, n_items, u0, u1)
 
-        fused = (self._tensor_path_ok(allow_tastes=True) and n_items > 0 and
-                 k <= kernels.topk_max_k(kernels.d_pad_for(self.n_components)))
-        use_filter = fused and TOPK_PATH != 'exact' and k <= kernels.filter_max_k()
-        info = self.last_topk_info = {'path': 'filter' if use_filter else ('exact3' if fused else 'dense+rank'),
-                                      'fallback_rows': 0}
+        model_ok = self._tensor_path_ok(allow_tastes=True)
+        d_pad = kernels.d_pad_for(self.n_components)
+        limits = (kernels.filter_max_k(), kernels.topk_max_k(d_pad)) if model_ok else (0, 0)
+        path = topk_route(k, n_items, model_ok, self.n_tastes == 1, *limits,
+                          sharded=item_id_offset != 0 or gather_group is not None)
+        fused = path != 'dense+rank'
+        use_filter = path == 'filter'
+        wide = path == 'wide'
+        info = self.last_topk_info = {'path': path, 'fallback_rows': 0}
         items = fitems = None
-        if fused:
-            items = self._side_operands('item', item_in, device, for_filter=use_filter)
-            if use_filter:
+        if fused and n_items > 0:
+            items = self._side_operands('item', item_in, device, for_filter=use_filter or wide)
+            if use_filter or wide:
                 fitems = kernels.FilterItems(items)
 
-        blocks = self._user_blocks(user_in, n_items, n_users if user_batch_size is None else user_batch_size)
+        if user_batch_size is None:
+            user_batch_size = self._topk_block_rows(path, n_users, n_items, k, gather_group, device)
+        blocks = self._user_blocks(user_in, n_items, user_batch_size)
 
         def run_taste(block_in, taste, force_exact, excl):
-            users = self._side_operands('user', block_in, device, for_filter=use_filter and not force_exact, taste=taste)
+            if wide and n_items == 0:     # an empty item shard: no candidates, but the same calls as the other ranks
+                return kernels.empty_topk(block_in.shape[0], k, device), torch.zeros((4,), dtype=torch.int32,
+                                                                                     device=device), 0
+            users = self._side_operands('user', block_in, device, for_filter=(use_filter or wide) and not force_exact,
+                                        taste=taste)
+            if wide:
+                return kernels.topk_wide(users, items, k, item_id_offset=item_id_offset, fitems=fitems, excl=excl,
+                                         block_bytes=self.PREDICT_BLOCK_BYTES)
             if use_filter and not force_exact:
                 return kernels.topk_filter(users, items, k, item_id_offset=item_id_offset, fitems=fitems, excl=excl)
             return kernels.topk_exact(users, items, k, item_id_offset=item_id_offset, excl=excl), None, 0
@@ -918,33 +959,38 @@ class TensorRec(object):
             return TopK(top_i, top_s)
         return TopK(*kernels.to_host(top_i, top_s))
 
+    def _topk_block_rows(self, path, n_rows, n_items, k, gather_group=None, device=None):
+        """Default rows per block of a top-k call: every row at once on the k <= 32 fused routes; on dense+rank as many
+        as keep the dense scores, ranks and selection masks within PREDICT_BLOCK_BYTES; on the wide route as many as
+        keep the candidate lists within PREDICT_BLOCK_BYTES at one item split per row.  (A block splits the items only
+        when it has fewer user blocks than the device has SMs; its rows x splits then stay below ~3 x 128 x the SM count,
+        about 1.2 GB of lists at k = 1024 on an H100.)  In a sharded call (gather_group) every rank takes the smallest
+        of the ranks' choices: each block ends in the collective exchange, so all ranks must cut the same blocks."""
+        if path == 'wide':
+            per_row = 8 * kernels.wide_list_capacity(k)
+            rows = max(2 * kernels.TILE_USERS, self.PREDICT_BLOCK_BYTES // per_row // 256 * 256)
+        elif path == 'dense+rank':
+            rows = kernels.dense_rank_rows(n_items, self.PREDICT_BLOCK_BYTES)
+        else:
+            rows = n_rows
+        if gather_group is not None:
+            from . import distributed
+            rows = distributed.common_block_rows(rows, gather_group, device)
+        return rows
+
     def _topk_from_dense(self, n_users, n_items, k, item_id_offset, device, score, host_excl=None):
         """Any model the fused kernel does not cover: dense scores -> exact full ranks -> the rank <= k entries.
         score() -> the float32 [n_users, n_items] scores of the rows on the device.  host_excl: exclusion lists (indptr,
         local ids) of the rows -- those scores become -inf before the ranking and those entries are never emitted (their
         slots keep the sentinel)."""
-        top = kernels.PackedTopK(n_users, k, device)
-        top.scores.fill_(float('-inf'))
-        top.items.fill_(2 ** 31 - 1)
-        if n_items > 0:
-            scores = score()
-            excluded = None
-            if host_excl is not None:
-                indptr, ids = host_excl
-                ex_rows = torch.from_numpy(np.repeat(np.arange(n_users, dtype=np.int64), np.diff(indptr))).to(device)
-                ex_cols = torch.from_numpy(ids.astype(np.int64)).to(device)
-                scores[ex_rows, ex_cols] = float('-inf')
-                excluded = torch.zeros((n_users, n_items), dtype=torch.bool, device=device)
-                excluded[ex_rows, ex_cols] = True
-            ranks = kernels.rank_full(scores).long()
-            sel = ranks <= k
-            if excluded is not None:
-                sel &= ~excluded
-            rows, cols = sel.nonzero(as_tuple=True)
-            pos = ranks[rows, cols] - 1
-            top.scores[rows, pos] = scores[rows, cols]
-            top.items[rows, pos] = (cols + item_id_offset).to(torch.int32)
-        return top
+        if n_items == 0:
+            return kernels.empty_topk(n_users, k, device)
+        ex_rows = ex_cols = None
+        if host_excl is not None:
+            indptr, ids = host_excl
+            ex_rows = torch.from_numpy(np.repeat(np.arange(n_users, dtype=np.int64), np.diff(indptr))).to(device)
+            ex_cols = torch.from_numpy(ids.astype(np.int64)).to(device)
+        return kernels.topk_from_scores(score(), k, item_id_offset, ex_rows, ex_cols)
 
     def predict_similar_items(self, item_features, item_ids, n_similar):
         """tensorrec/tensorrec.py:666-703: for each id, the n_similar (item_id, score) pairs of highest prediction
@@ -992,7 +1038,8 @@ class TensorRec(object):
         item_batch_size: queries are processed in blocks of this many rows (bit-identical results).
 
         Built-in prediction and representation graphs with n_components <= 128 and n_similar <= 32 run on the fused
-        tensor-core top-k kernels (filter + re-scoring for n_similar <= 12, else the exact 3-pass kernel); Euclidean
+        tensor-core top-k kernels (filter + re-scoring for n_similar <= 12, else the exact 3-pass kernel), and with
+        32 < n_similar <= WIDE_MAX_K on catalogues of at least WIDE_MIN_ITEMS items on the wide filter; Euclidean
         similarity ranks -1/2 d^2 = q.i - 1/2 |q|^2 - 1/2 |i|^2 there and is mapped to -sqrt(d^2) at the end.  Everything
         else scores dense query blocks and ranks them.  last_topk_info['path'] names the route.  Single GPU: queries
         and items live on one device (there is no item-sharded form)."""
@@ -1030,10 +1077,12 @@ class TensorRec(object):
                     and d_pad <= 128)
         if SCORE_PATH == 'tensor' and not model_ok:
             raise RuntimeError('TENSORREC_B200_SCORE_PATH=tensor but this model cannot use the tensor-core kernel')
-        fused = model_ok and n_items > 0 and n <= kernels.topk_max_k(d_pad)
-        use_filter = fused and TOPK_PATH != 'exact' and n <= kernels.filter_max_k()
-        info = self.last_topk_info = {'path': 'filter' if use_filter else ('exact3' if fused else 'dense+rank'),
-                                      'fallback_rows': 0}
+        limits = (kernels.filter_max_k(), kernels.topk_max_k(d_pad)) if model_ok else (0, 0)
+        path = topk_route(n, n_items, model_ok, True, *limits)
+        fused = path != 'dense+rank'
+        use_filter = path == 'filter'
+        wide = path == 'wide'
+        info = self.last_topk_info = {'path': path, 'fallback_rows': 0}
         if n_queries == 0:
             return TopK(np.zeros((0, n), np.int32), np.zeros((0, n), np.float32))
         ids_dev = None if ids is None else torch.from_numpy(ids).to(device)
@@ -1048,13 +1097,14 @@ class TensorRec(object):
         if fused:
             # the item operand once: split fp16 + scale (+ row norms and statistics for the filter), no projected biases;
             # Euclidean: bias -1/2 |i|^2.  The queries are rows of this same operand.
-            stats = torch.empty((3,), dtype=torch.float32, device=device) if use_filter else None
+            one_pass = use_filter or wide
+            stats = torch.empty((3,), dtype=torch.float32, device=device) if one_pass else None
             out = self._represent(self.item_repr_graph_factory, item_in, self.n_item_features, 'item', device, extra,
-                                  want_f32=False, split_d_pad=d_pad, want_norm=use_filter, stats=stats)
-            split, scale, norm = out[1], out[2], (out[3] if use_filter else None)
+                                  want_f32=False, split_d_pad=d_pad, want_norm=one_pass, stats=stats)
+            split, scale, norm = out[1], out[2], (out[3] if one_pass else None)
             bias = kernels.operand_half_sqnorm(split, scale, d_pad) if euclidean else None
             items = kernels.SideOperands(None, split, scale, bias, n_items, self.n_components, d_pad, stats=stats)
-            fitems = kernels.FilterItems(items) if use_filter else None
+            fitems = kernels.FilterItems(items) if one_pass else None
 
             def query_rows(q0, q1):
                 return kernels.SideOperands(None, take(split, q0, q1), take(scale, q0, q1), take(bias, q0, q1), q1 - q0,
@@ -1079,6 +1129,10 @@ class TensorRec(object):
                                              host_excl), [(None, 0)]
             excl = None if host_excl is None else kernels.DeviceExclusion.upload(*host_excl, device=device)
             queries = query_rows(q0, q1)
+            if wide:
+                top, cnt, cap = kernels.topk_wide(queries, items, n, fitems=fitems, excl=excl, euclidean=euclidean,
+                                                  block_bytes=self.PREDICT_BLOCK_BYTES)
+                return top, [(cnt, cap)]
             if use_filter and not force_exact:
                 top, cnt, cap = kernels.topk_filter(queries, items, n, fitems=fitems, excl=excl)
                 return top, [(cnt, cap)]
@@ -1086,13 +1140,11 @@ class TensorRec(object):
 
         if item_batch_size is not None:
             step = max(1, int(item_batch_size))
-        elif fused:
-            step = n_queries
         else:
-            step = max(1, self.PREDICT_BLOCK_BYTES // max(4 * n_items, 1))
+            step = self._topk_block_rows(path, n_queries, n_items, n)
         blocks = [(q0, min(n_queries, q0 + step), None) for q0 in range(0, n_queries, step)]
         results, _ = self._run_topk_blocks(blocks, run_block, lambda top, q0, q1: (top, None), info)
-        if fused and euclidean:
+        if fused and euclidean and not wide:     # (the wide route maps its survivors in the selection kernel)
             for top in results:
                 kernels.topk_euclidean_finish(top)
         return self._topk_result(results, to_host)
