@@ -337,6 +337,30 @@ int trk_score_dense_f16x3(const void* user_split, const float* user_scale, const
                           const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
                           int32_t d_pad, float* out, int64_t out_row_stride, void* stream);
 
+/* Euclidean user x item models (EuclideanSimilarityPredictionGraph, tensorrec/prediction_graphs.py:84-100, then
+ * bias_prediction_dense, recommendation_graphs.py:41) on the same tensor-core kernels: the epilogue turns each
+ * accumulator into the final score
+ *   p = acc * scale_u * scale_i,  d2 = (|u|^2 - 2 p) + |i|^2,  s = -sqrt(max(d2, 1e-16)) + user_bias[u] + item_bias[i]
+ * (left to right, correctly rounded sqrt; exact for integer-valued representations), then compares / stores it as the
+ * dot forms do.  The squared norms come from the split operands, as -1/2 |row|^2 written by trk_operand_half_sqnorm:
+ *   user_half_sqnorm [n_users];
+ *   item_half_sqnorm [n_items_padded256] (16-byte aligned), entries beyond n_items = 0 (any finite value).
+ *   trk_score_dense_euclid_f16x3  the arguments of trk_score_dense_f16x3 plus the two norm arrays.
+ *   trk_score_topk_euclid_f16x3   the arguments of trk_score_topk_f16x3_excl plus the two norm arrays; excl_indptr /
+ *                                 excl_ids / excl_row_map may all be NULL (no exclusion).
+ * Constraints: d_pad in {64, 128}; top-k: 1 <= k <= trk_score_topk_max_k(d_pad).  The top-k of a mixture of tastes is
+ * one call per taste and trk_topk_merge with dedup, as for the dot form: every step after the sqrt is monotone. */
+int trk_score_dense_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                 const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
+                                 int32_t d_pad, float* out, int64_t out_row_stride, const float* user_half_sqnorm,
+                                 const float* item_half_sqnorm, void* stream);
+int trk_score_topk_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
+                                int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset,
+                                float* cand_score, int32_t* cand_item, const int32_t* n_users_live,
+                                const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
+                                const float* user_half_sqnorm, const float* item_half_sqnorm, void* stream);
+
 /* Merges n_lists candidate lists per user (each sorted by (score desc, id asc), k_in entries) into the global
  * top k_out per user, same order.  Lists are the n_splits of one GPU and/or the shards received from the other GPUs
  * (item-axis sharding; the exchange itself is one NCCL all-to-all done by the host layer, SURVEY 8e).

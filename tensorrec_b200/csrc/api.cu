@@ -80,9 +80,9 @@ int order_from_ranks(const int32_t*, int64_t, int32_t*, cudaStream_t);
 int score_topk_max_k(int32_t);
 int score_topk_f16x3(const void*, const float*, const float*, const void*, const float*, int64_t, int64_t, int32_t,
                      int32_t, int32_t, int32_t, float*, int32_t*, const int32_t*, const int32_t*, const int32_t*,
-                     const int32_t*, cudaStream_t);
+                     const int32_t*, const float*, const float*, cudaStream_t);
 int score_dense_f16x3(const void*, const float*, const float*, const void*, const float*, int64_t, int64_t, int32_t,
-                      float*, int64_t, cudaStream_t);
+                      float*, int64_t, const float*, const float*, cudaStream_t);
 int topk_merge(const float*, const int32_t*, int64_t, int32_t, int32_t, int32_t, int64_t, int64_t, float*, int32_t*,
                int64_t, const int32_t*, int32_t, cudaStream_t);
 int score_filter_max_k();
@@ -196,7 +196,7 @@ int trk_score_topk_f16x3(const void* user_split, const float* user_scale, const 
                          int32_t* cand_item, const int32_t* n_users_live, void* stream) {
   return trk::score_topk_f16x3(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k,
                                n_splits, item_id_offset, cand_score, cand_item, n_users_live, nullptr, nullptr, nullptr,
-                               trk::as_stream(stream));
+                               nullptr, nullptr, trk::as_stream(stream));
 }
 
 int trk_score_topk_f16x3_excl(const void* user_split, const float* user_scale, const float* user_bias,
@@ -207,14 +207,37 @@ int trk_score_topk_f16x3_excl(const void* user_split, const float* user_scale, c
   TRK_CHECK_ARG(excl_indptr != nullptr && excl_ids != nullptr, "trk_score_topk_f16x3_excl: null exclusion list");
   return trk::score_topk_f16x3(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k,
                                n_splits, item_id_offset, cand_score, cand_item, n_users_live, excl_indptr, excl_ids,
-                               excl_row_map, trk::as_stream(stream));
+                               excl_row_map, nullptr, nullptr, trk::as_stream(stream));
+}
+
+int trk_score_topk_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
+                                int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset, float* cand_score,
+                                int32_t* cand_item, const int32_t* n_users_live, const int32_t* excl_indptr,
+                                const int32_t* excl_ids, const int32_t* excl_row_map, const float* user_half_sqnorm,
+                                const float* item_half_sqnorm, void* stream) {
+  TRK_CHECK_ARG(user_half_sqnorm != nullptr && item_half_sqnorm != nullptr,
+                "trk_score_topk_euclid_f16x3: null squared norms");
+  return trk::score_topk_f16x3(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k,
+                               n_splits, item_id_offset, cand_score, cand_item, n_users_live, excl_indptr, excl_ids,
+                               excl_row_map, user_half_sqnorm, item_half_sqnorm, trk::as_stream(stream));
 }
 
 int trk_score_dense_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
                           const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
                           int32_t d_pad, float* out, int64_t out_row_stride, void* stream) {
   return trk::score_dense_f16x3(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad,
-                                out, out_row_stride, trk::as_stream(stream));
+                                out, out_row_stride, nullptr, nullptr, trk::as_stream(stream));
+}
+
+int trk_score_dense_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                 const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
+                                 int32_t d_pad, float* out, int64_t out_row_stride, const float* user_half_sqnorm,
+                                 const float* item_half_sqnorm, void* stream) {
+  TRK_CHECK_ARG(user_half_sqnorm != nullptr && item_half_sqnorm != nullptr,
+                "trk_score_dense_euclid_f16x3: null squared norms");
+  return trk::score_dense_f16x3(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad,
+                                out, out_row_stride, user_half_sqnorm, item_half_sqnorm, trk::as_stream(stream));
 }
 
 int trk_topk_merge(const float* cand_score, const int32_t* cand_item, int64_t n_users, int32_t n_lists,

@@ -61,6 +61,16 @@ struct TcExcl {
   const int32_t* row_map;
 };
 
+// Euclidean similarity (kEuclid instantiations): -1/2 |row|^2 of every user row [n_users] and item column, as
+// operand_half_sqnorm_kernel (similar_items.cu) computes them from the split operands -- the norms see exactly the values
+// the dot product sees.  The epilogue reads item norms for whole 128-column tiles, so item_half_sqnorm holds
+// n_items_padded256 entries, 0 beyond n_items (finite: the meta's -inf bias still gives those columns -inf).  Also a
+// kernel parameter of its own, for the same reason as TcExcl.
+struct TcEuclid {
+  const float* user_half_sqnorm;
+  const float* item_half_sqnorm;
+};
+
 // shared-memory carve-up (offsets from a 1024-byte aligned base)
 struct SmemLayout {
   uint32_t a_off, b_off, list_score_off, list_item_off, acc_off, bar_off, total;
@@ -115,6 +125,44 @@ __device__ __forceinline__ float score_chunk(uint32_t (&r)[32], const float2* me
   return cmax;
 }
 
+// The Euclidean form of score_chunk: EuclideanSimilarityPredictionGraph dense (prediction_graphs.py:84-100) then
+// bias_prediction_dense (recommendation_graphs.py:41), every step in the reference's order:
+//   p = acc * (scale_u * scale_i)  (powers of two: exact),  d2 = (|u|^2 - 2 p) + |i|^2,
+//   s = (-sqrt(max(d2, 1e-16)) + ub) + ib
+// with |row|^2 = -2 * (-1/2 |row|^2) (exact) and a correctly rounded sqrtf.  A missing bias is 0 here, and s <= -1e-8
+// is never zero, so adding it changes nothing.  usq = |u|^2 of the row, ihsq = the chunk's -1/2 |i|^2 (16-byte aligned).
+__device__ __forceinline__ float score_chunk_euclid(uint32_t (&r)[32], const float2* meta, const float* ihsq, float su,
+                                                    float usq, float ubias) {
+  float cmax = -__int_as_float(0x7f800000);
+#pragma unroll
+  for (int j = 0; j < 32; j += 4) {
+    const float4 h = __ldg(reinterpret_cast<const float4*>(ihsq + j));
+    const float hq[4] = {h.x, h.y, h.z, h.w};
+#pragma unroll
+    for (int q = 0; q < 4; q += 2) {
+      const float4 m = ldg128(meta + j + q);   // {scale_j, bias_j, scale_j+1, bias_j+1}
+      const float p0 = __uint_as_float(r[j + q]) * (m.x * su);
+      const float p1 = __uint_as_float(r[j + q + 1]) * (m.z * su);
+      const float d0 = (usq - 2.0f * p0) + -2.0f * hq[q];
+      const float d1 = (usq - 2.0f * p1) + -2.0f * hq[q + 1];
+      const float s0 = (-sqrtf(fmaxf(d0, 1e-16f)) + ubias) + m.y;
+      const float s1 = (-sqrtf(fmaxf(d1, 1e-16f)) + ubias) + m.w;
+      r[j + q] = __float_as_uint(s0);
+      r[j + q + 1] = __float_as_uint(s1);
+      cmax = fmaxf(cmax, fmaxf(s0, s1));
+    }
+  }
+  return cmax;
+}
+
+// Final scores of one 32-column chunk, dot / cosine or Euclidean.
+template <bool kEuclid>
+__device__ __forceinline__ float score_chunk_as(uint32_t (&r)[32], const float2* meta, const float* ihsq, float su,
+                                                float usq, float ubias) {
+  if constexpr (kEuclid) return score_chunk_euclid(r, meta, ihsq, su, usq, ubias);
+  else return score_chunk(r, meta, su, ubias);
+}
+
 // Exclusion (kExclude): the final scores of the chunk's columns [base, base + 32) named in list row `xr` become -inf
 // (never inserted: the compare is strict and the lists start at -inf).  A select per register, not r[dynamic index],
 // which would put r[] into local memory; the FINAL score is masked, not the accumulator (a zero scale would turn -inf into
@@ -151,13 +199,14 @@ struct ExclCursor<false> {};
 
 // One 32-column chunk of one user row: final scores, then (top-k mode) the row's listed columns masked (kExclude) and
 // the rare inserts, or (dense mode) the store.  `x` is taken by value: a reference bound to the kernel parameter
-// changes the generated code of the instantiations without exclusion.
-template <bool kDense, bool kExclude>
+// changes the generated code of the instantiations without exclusion.  kEuclid: the Euclidean score (ihsq = the tile's
+// item norms, usq = the row's |u|^2).
+template <bool kDense, bool kExclude, bool kEuclid>
 __device__ __forceinline__ void process_chunk(uint32_t (&r)[32], int c, int t, int32_t id0, const float2* meta,
-                                              float su, float ubias, float& thr, float* ls, int32_t* li,
-                                              const TcParams& p, int64_t u, bool u_ok, const TcExcl x,
-                                              ExclCursor<kExclude>& xc) {
-  float cmax = score_chunk(r, meta + c * 32, su, ubias);
+                                              const float* ihsq, float su, float usq, float ubias, float& thr,
+                                              float* ls, int32_t* li, const TcParams& p, int64_t u, bool u_ok,
+                                              const TcExcl x, ExclCursor<kExclude>& xc) {
+  float cmax = score_chunk_as<kEuclid>(r, meta + c * 32, ihsq + c * 32, su, usq, ubias);
   if constexpr (!kDense) {
     if constexpr (kExclude) {
       const int32_t base = t * kBlockN + c * 32;   // local id of the chunk's first column
@@ -213,11 +262,11 @@ __device__ __forceinline__ void store_chunk_tma(const uint32_t (&r)[32], uint32_
 }
 
 // kNKB = d_pad / 64 k-blocks per operand half.  kExclude (top-k mode): columns named in the row's exclusion list are
-// left out of the top-k (excl_mask_scores).
-template <bool kDense, int kNKB, bool kExclude = false>
+// left out of the top-k (excl_mask_scores).  kEuclid: Euclidean similarity (score_chunk_euclid) in either mode.
+template <bool kDense, int kNKB, bool kExclude = false, bool kEuclid = false>
 __global__ void __launch_bounds__(kTcThreads, 1)
 score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_constant__ CUtensorMap map_items,
-                const __grid_constant__ CUtensorMap map_out, const TcParams p, const TcExcl x) {
+                const __grid_constant__ CUtensorMap map_out, const TcParams p, const TcExcl x, const TcEuclid e) {
   uint8_t* smem = smem_base_1024();
   const SmemLayout L = make_layout(p.n_kblocks, p.n_stages, kDense ? 0 : p.k, kDense && p.tma_store != 0);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
@@ -321,6 +370,8 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
       const bool u_ok = u < p.n_users;
       const float su = u_ok ? __ldg(p.user_scale + u) : 0.0f;
       const float ubias = (u_ok && p.user_bias != nullptr) ? __ldg(p.user_bias + u) : 0.0f;
+      float usq = 0.0f;   // kEuclid: |u|^2 (rows at or beyond n_users read nothing)
+      if constexpr (kEuclid) usq = u_ok ? -2.0f * __ldg(e.user_half_sqnorm + u) : 0.0f;
       float thr = kNegInf;
       // kExclude: this row's list row and the first listed id >= the current chunk.  Rows of a gathered launch beyond
       // *n_users_live have no map entry and are discarded by the caller: they exclude nothing.
@@ -370,6 +421,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
         // ---- epilogue: two rounds, each stages columns [32 c, 32 c + 32) of both 64-column halves ----
         const int32_t id0 = p.item_id_offset + t * kBlockN;
         const float2* meta = p.item_meta + static_cast<int64_t>(t) * kBlockN;
+        const float* ihsq = kEuclid ? e.item_half_sqnorm + static_cast<int64_t>(t) * kBlockN : nullptr;
 #pragma unroll
         for (int c = 0; c < 2; ++c) {
           named_barrier_sync(1 + g, kConsumerThreads);   // the previous round's rows have been read
@@ -387,12 +439,13 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
           for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(src[j]);
           const int chunk = half * 2 + c;
           if (kDense && p.tma_store) {
-            score_chunk(r, meta + chunk * 32, su, ubias);
+            score_chunk_as<kEuclid>(r, meta + chunk * 32, ihsq + chunk * 32, su, usq, ubias);
             store_chunk_tma(r, stage_base + (n_stored & 1) * kStoreTileBytes, lane, &map_out, t * kBlockN + chunk * 32,
                             ub * kBlockM + g * kWgRows + (warp % 2) * 32);
             ++n_stored;
           } else {
-            process_chunk<kDense, kExclude>(r, chunk, t, id0, meta, su, ubias, thr, ls, li, p, u, u_ok, x, xc);
+            process_chunk<kDense, kExclude, kEuclid>(r, chunk, t, id0, meta, ihsq, su, usq, ubias, thr, ls, li, p, u,
+                                                     u_ok, x, xc);
           }
         }
       }
@@ -454,8 +507,12 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
                      int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset, float* cand_score,
                      int32_t* cand_item, float* dense_out, int64_t dense_stride, const int32_t* n_users_live,
                      const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
-                     cudaStream_t stream) {
+                     const float* user_half_sqnorm, const float* item_half_sqnorm, cudaStream_t stream) {
   TRK_CHECK_ARG(user_split && user_scale && item_split && item_meta, "score_tc: null operand");
+  TRK_CHECK_ARG((user_half_sqnorm == nullptr) == (item_half_sqnorm == nullptr),
+                "score_tc: user_half_sqnorm and item_half_sqnorm go together");
+  TRK_CHECK_ARG(reinterpret_cast<uintptr_t>(item_half_sqnorm) % 16 == 0, "score_tc: item_half_sqnorm must be 16-byte aligned");
+  const bool euclid = user_half_sqnorm != nullptr;
   TRK_CHECK_ARG(n_users >= 1 && n_items >= 1, "score_tc: empty shape");
   TRK_CHECK_ARG(n_users < (1ll << 31) && n_items < (1ll << 31) - 512, "score_tc: shape exceeds int32 indexing");
   if (d_pad != 64 && d_pad != 128) {
@@ -497,6 +554,7 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
   p.dense_stride = dense_stride;
   p.n_users_live = n_users_live;
   const TcExcl x = {excl_indptr, excl_ids, excl_row_map};
+  const TcEuclid e = {user_half_sqnorm, item_half_sqnorm};
   p.tma_store = (kDense && dense_stride % 4 == 0 && reinterpret_cast<uintptr_t>(dense_out) % 16 == 0) ? 1 : 0;
   p.n_stages = pick_stages(p.n_kblocks, p.k, p.tma_store != 0);
   TRK_CHECK_ARG(p.n_stages >= 2, "score_tc: shared memory budget exceeded (d_pad=%d k=%d)", d_pad, k);
@@ -522,9 +580,18 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
     if (excl_indptr != nullptr) kernel = p.n_kblocks == 2 ? score_tc_kernel<false, 2, true> : score_tc_kernel<false, 1, true>;
   }
   if (kernel == nullptr) kernel = p.n_kblocks == 2 ? score_tc_kernel<kDense, 2> : score_tc_kernel<kDense, 1>;
+  if (euclid) {
+    if constexpr (kDense) {
+      kernel = p.n_kblocks == 2 ? score_tc_kernel<true, 2, false, true> : score_tc_kernel<true, 1, false, true>;
+    } else if (excl_indptr != nullptr) {
+      kernel = p.n_kblocks == 2 ? score_tc_kernel<false, 2, true, true> : score_tc_kernel<false, 1, true, true>;
+    } else {
+      kernel = p.n_kblocks == 2 ? score_tc_kernel<false, 2, false, true> : score_tc_kernel<false, 1, false, true>;
+    }
+  }
   TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
   const int grid = capped_grid(static_cast<int64_t>(p.n_user_blocks) * n_splits, 1);
-  kernel<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, map_out, p, x);
+  kernel<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, map_out, p, x, e);
   TRK_CHECK_LAUNCH();
   return TRK_OK;
 }
@@ -533,15 +600,17 @@ int score_topk_f16x3(const void* user_split, const float* user_scale, const floa
                      const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
                      int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset, float* cand_score,
                      int32_t* cand_item, const int32_t* n_users_live, const int32_t* excl_indptr,
-                     const int32_t* excl_ids, const int32_t* excl_row_map, cudaStream_t stream) {
+                     const int32_t* excl_ids, const int32_t* excl_row_map, const float* user_half_sqnorm,
+                     const float* item_half_sqnorm, cudaStream_t stream) {
   return launch_tc<false>(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k,
                           n_splits, item_id_offset, cand_score, cand_item, nullptr, 0, n_users_live, excl_indptr,
-                          excl_ids, excl_row_map, stream);
+                          excl_ids, excl_row_map, user_half_sqnorm, item_half_sqnorm, stream);
 }
 
 int score_dense_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
                       const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
-                      int32_t d_pad, float* out, int64_t out_row_stride, cudaStream_t stream) {
+                      int32_t d_pad, float* out, int64_t out_row_stride, const float* user_half_sqnorm,
+                      const float* item_half_sqnorm, cudaStream_t stream) {
   // split the item axis so that every SM gets work even when there are few user blocks
   const int64_t n_ub = ceil_div(n_users, kBlockM);
   const int64_t n_tiles = ceil_div(n_items, kBlockN);
@@ -550,7 +619,7 @@ int score_dense_f16x3(const void* user_split, const float* user_scale, const flo
   if (splits < 1) splits = 1;
   return launch_tc<true>(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, 0,
                          static_cast<int32_t>(splits), 0, nullptr, nullptr, out, out_row_stride, nullptr, nullptr,
-                         nullptr, nullptr, stream);
+                         nullptr, nullptr, user_half_sqnorm, item_half_sqnorm, stream);
 }
 
 }  // namespace trk

@@ -274,17 +274,22 @@ def default_splits(n_users, n_items):
 
 
 def score_topk(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k, n_splits=None,
-               item_id_offset=0, n_users_live=None, excl=None, excl_row_map=None):
+               item_id_offset=0, n_users_live=None, excl=None, excl_row_map=None, sqnorms=None):
     """K2+K3 fused.  Returns (cand_score [U, n_splits, k] f32, cand_item [U, n_splits, k] i32).
     n_users_live: device int32 tensor; only its first element's worth of user rows is processed.
-    excl: DeviceExclusion -- its items are left out of every row's top-k (user row u reads list row excl_row_map[u])."""
+    excl: DeviceExclusion -- its items are left out of every row's top-k (user row u reads list row excl_row_map[u]).
+    sqnorms: (user -1/2 |u|^2, item -1/2 |i|^2 padded by item_half_sqnorm) -> Euclidean similarity scores."""
     lib = require_cuda()
     if n_splits is None:
         n_splits = default_splits(n_users, n_items)
     dev = user_split.device
     cand_score = torch.empty((n_users, n_splits, k), dtype=torch.float32, device=dev)
     cand_item = torch.empty((n_users, n_splits, k), dtype=torch.int32, device=dev)
-    if excl is None:
+    if sqnorms is not None:
+        name = 'trk_score_topk_euclid_f16x3'
+        extra = (None, None, None) if excl is None else (_p(excl.indptr), _p(excl.ids), _p(excl_row_map))
+        extra += (_p(sqnorms[0]), _p(sqnorms[1]))
+    elif excl is None:
         name, extra = 'trk_score_topk_f16x3', ()
     else:
         name, extra = 'trk_score_topk_f16x3_excl', (_p(excl.indptr), _p(excl.ids), _p(excl_row_map))
@@ -295,13 +300,20 @@ def score_topk(user_split, user_scale, user_bias, item_split, item_meta, n_users
     return cand_score, cand_item
 
 
-def score_dense_tc(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, out=None):
+def score_dense_tc(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, out=None,
+                   sqnorms=None):
+    """sqnorms: as for score_topk (Euclidean similarity)."""
     lib = require_cuda()
     if out is None:
         out = torch.empty((n_users, n_items), dtype=torch.float32, device=user_split.device)
-    rc = lib.trk_score_dense_f16x3(_p(user_split), _p(user_scale), _p(user_bias), _p(item_split), _p(item_meta),
-                                   n_users, n_items, int(d_pad), _p(out), out.stride(0), _stream())
-    _lib.check(rc, 'trk_score_dense_f16x3')
+    args = (_p(user_split), _p(user_scale), _p(user_bias), _p(item_split), _p(item_meta), n_users, n_items, int(d_pad),
+            _p(out), out.stride(0))
+    if sqnorms is None:
+        name, extra = 'trk_score_dense_f16x3', ()
+    else:
+        name, extra = 'trk_score_dense_euclid_f16x3', (_p(sqnorms[0]), _p(sqnorms[1]))
+    rc = getattr(lib, name)(*args, *extra, _stream())
+    _lib.check(rc, name)
     return out
 
 
@@ -391,14 +403,23 @@ def operand_stats(split, scale, d_pad, want_norm=True, stats=None):
     return norm
 
 
-def operand_half_sqnorm(split, scale, d_pad):
-    """-1/2 |row|^2 of every row of a split operand (fp32 [rows]): the biases that turn the fused top-k kernels' score
-    q.i + ub + ib into -1/2 d^2(q, i) for Euclidean similar items."""
+def operand_half_sqnorm(split, scale, d_pad, out=None):
+    """-1/2 |row|^2 of every row of a split operand (fp32 [rows], or the first rows entries of `out`): the biases that
+    turn the fused top-k kernels' score q.i + ub + ib into -1/2 d^2(q, i) for Euclidean similar items, and the norms of
+    the Euclidean user x item kernels."""
     lib = require_cuda()
-    out = torch.empty((split.shape[0],), dtype=torch.float32, device=split.device)
+    if out is None:
+        out = torch.empty((split.shape[0],), dtype=torch.float32, device=split.device)
     rc = lib.trk_operand_half_sqnorm(_p(split), _p(scale), split.shape[0], int(d_pad), _p(out), _stream())
     _lib.check(rc, 'trk_operand_half_sqnorm')
     return out
+
+
+def item_half_sqnorm(items):
+    """-1/2 |i|^2 of an item SideOperands, zero-padded to padded_items(n) entries (the Euclidean kernels read whole
+    item tiles)."""
+    out = torch.zeros((padded_items(items.n_rows),), dtype=torch.float32, device=items.split.device)
+    return operand_half_sqnorm(items.split, items.scale, items.d_pad, out=out)
 
 
 def topk_euclidean_finish(top):
@@ -582,12 +603,16 @@ class SideOperands(object):
 
 
 def topk_exact(users, items, k, n_splits=None, item_id_offset=0, out=None, n_users_live=None, excl=None,
-               excl_row_map=None):
-    """Exact 3-pass fused kernel + merge -> PackedTopK [U, k]."""
+               excl_row_map=None, item_hsq=None):
+    """Exact 3-pass fused kernel + merge -> PackedTopK [U, k].  item_hsq (item_half_sqnorm(items)): Euclidean
+    similarity, with the user norms taken from users.split here."""
     meta = pack_item_meta(items.scale, items.bias, items.n_rows)
+    sqnorms = None
+    if item_hsq is not None:
+        sqnorms = (operand_half_sqnorm(users.split, users.scale, users.d_pad), item_hsq)
     cs, ci = score_topk(users.split, users.scale, users.bias, items.split, meta, users.n_rows, items.n_rows,
                         users.d_pad, k, n_splits=n_splits, item_id_offset=item_id_offset, n_users_live=n_users_live,
-                        excl=excl, excl_row_map=excl_row_map)
+                        excl=excl, excl_row_map=excl_row_map, sqnorms=sqnorms)
     return topk_merge(cs, ci, k, out=out, n_users_live=n_users_live)
 
 

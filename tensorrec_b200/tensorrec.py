@@ -4,7 +4,7 @@ hand-written sm_90a kernels through the C ABI (include/tensorrec_b200.h):
 
     sparse features --K1 trk_csr_gather_reduce_f32--> representations (fp32 and/or split-fp16 operand)
                     --trk_csr_project_biases_f32--> user / item biases
-    predict():       K2 trk_score_dense_f16x3 (wgmma)   or trk_score_f32 (exact fp32, any shape)  -> [U, I] float32
+    predict():       K2 trk_score_dense_(euclid_)f16x3 (wgmma) or trk_score_f32 (exact fp32, any shape) -> [U, I] f32
     predict_rank():  ... + K3 trk_rank_full                                                      -> [U, I] int32
     predict_rank(k): K2+K3 fused trk_score_topk_f16x3 + trk_topk_merge (+ one NCCL all-gather when the item axis is
                      sharded over GPUs)                                                           -> top-k ids, scores
@@ -58,18 +58,28 @@ TOPK_PATH = os.environ.get('TENSORREC_B200_TOPK_PATH', 'auto')
 # scoring the catalogue densely and ranking it costs less than a sweep (see README, "Large k").
 WIDE_MAX_K = 1024
 WIDE_MIN_ITEMS = 4096
+# Euclidean user x item models take the exact 3-pass kernel for k <= 32 on catalogues of at least EUCLIDEAN_MIN_ITEMS
+# items.  The fused route was faster at every measured catalogue size, from 1024 items up (see README, "Euclidean
+# models"); smaller catalogues stay on dense scoring and ranking.
+EUCLIDEAN_MIN_ITEMS = 1024
 
 
-def topk_route(k, n_items, model_ok, single_taste, filter_max_k, exact_max_k, sharded=False):
+def topk_route(k, n_items, model_ok, single_taste, filter_max_k, exact_max_k, sharded=False, euclidean=False):
     """The route of a top-k call -- 'filter', 'exact3', 'wide' or 'dense+rank' -- from k, the catalogue size and the
     model alone.  model_ok: the tensor-core kernels evaluate the model (built-in dot / cosine prediction, or any
     built-in similar-items graph, no attention, d_pad <= 128); single_taste: one taste (the wide route has no
     de-duplicating merge); filter_max_k / exact_max_k: the k limits of the filter and of the exact 3-pass kernel.
     sharded: an item-sharded call, where every rank must take the same route (the exchange is collective), so a
     rank's shard size does not decide the wide route.  TOPK_PATH='exact' means "no filter": k > exact_max_k then
-    goes to dense+rank."""
+    goes to dense+rank.  euclidean: a Euclidean user x item model (model_ok from _euclidean_tensor_ok), which has no
+    filter or wide form: 'exact3' for k <= exact_max_k on catalogues of at least EUCLIDEAN_MIN_ITEMS items (any shard
+    size in a sharded call), 'dense+rank' otherwise."""
     if not model_ok:
         return 'dense+rank'
+    if euclidean:
+        if k > exact_max_k or n_items == 0:
+            return 'dense+rank'
+        return 'exact3' if sharded or n_items >= EUCLIDEAN_MIN_ITEMS else 'dense+rank'
     if k <= exact_max_k:
         if n_items == 0:
             return 'dense+rank'
@@ -588,6 +598,13 @@ class TensorRec(object):
             raise RuntimeError('TENSORREC_B200_SCORE_PATH=tensor but this model cannot use the tensor-core kernel')
         return ok
 
+    def _euclidean_tensor_ok(self):
+        """Can the tensor-core kernels evaluate this Euclidean user x item model?  The built-in Euclidean graph, no
+        attention, d_pad <= 128; any number of tastes (the fused top-k merges one sweep per taste; dense scoring takes
+        one taste only -- _score_plan checks that)."""
+        return (SCORE_PATH != 'exact' and type(self.prediction_graph_factory) is EuclideanSimilarityPredictionGraph
+                and self.attention_graph_factory is None and kernels.d_pad_for(self.n_components) <= 128)
+
     def _side_operands(self, side, sparse_in, device, for_filter=False, taste=0):
         """One side ('user' or 'item') as kernels.SideOperands: split-fp16 operand + scale, projected biases and -- for
         the filter form of the fused top-k -- the row norms (users) / the global statistics (items), all from K1."""
@@ -615,17 +632,23 @@ class TensorRec(object):
 
     def _score_plan(self, item_in, device):
         """Item-side work of the dense prediction, done once per call: returns score(user_block_in, out=None) ->
-        float32 [rows, n_items] on the device.  Tensor cores (split-product kernel) when the model allows, the exact
-        CUDA-core kernel (tastes, attention, Euclidean, wide rows) or the plugin's own dense form otherwise."""
+        float32 [rows, n_items] on the device.  Tensor cores (split-product kernel, dot / cosine / Euclidean) when the
+        model allows, the exact CUDA-core kernel (tastes, attention, wide rows) or the plugin's own dense form
+        otherwise."""
         n_items = item_in.shape[0]
-        if self._tensor_path_ok():
+        euclidean = self.n_tastes == 1 and self._euclidean_tensor_ok()
+        if euclidean or self._tensor_path_ok():
             items = self._side_operands('item', item_in, device)
             meta = kernels.pack_item_meta(items.scale, items.bias, n_items)
+            item_hsq = kernels.item_half_sqnorm(items) if euclidean else None
 
             def score(block_in, out=None):
                 users = self._side_operands('user', block_in, device)
+                sqnorms = None
+                if euclidean:
+                    sqnorms = (kernels.operand_half_sqnorm(users.split, users.scale, users.d_pad), item_hsq)
                 return kernels.score_dense_tc(users.split, users.scale, users.bias, items.split, meta,
-                                              block_in.shape[0], n_items, users.d_pad, out=out)
+                                              block_in.shape[0], n_items, users.d_pad, out=out, sqnorms=sqnorms)
             return score
 
         pred_graph = self.prediction_graph_factory
@@ -811,8 +834,9 @@ class TensorRec(object):
         user_batch_size: users are processed in blocks of this many rows (bounds device memory at 10M+ users).
         32 < k <= WIDE_MAX_K on catalogues of at least WIDE_MIN_ITEMS items runs on the wide form of the filter (each
         user's candidates in a list in device memory, rows the certificate rejects scored dense and ranked); the default
-        user blocks then keep those lists within PREDICT_BLOCK_BYTES.  last_topk_info['path'] names the route
-        (topk_route).
+        user blocks then keep those lists within PREDICT_BLOCK_BYTES.  Euclidean models run k <= 32 on the exact kernel
+        (catalogues of at least EUCLIDEAN_MIN_ITEMS items) and larger k on dense+rank with tensor-core scoring.
+        last_topk_info['path'] names the route (topk_route).
 
         exclude: None, or a scipy sparse matrix (any format) with n_users rows whose column index is the GLOBAL item id
         (the numbering of TopK.items).  The pair (u, i) is excluded when exclude[u, i] != 0 after duplicates are summed
@@ -850,20 +874,23 @@ class TensorRec(object):
                 return None
             return kernels.exclusion_host_csr(exclude, item_id_offset, n_items, u0, u1)
 
-        model_ok = self._tensor_path_ok(allow_tastes=True)
+        euclidean = self._euclidean_tensor_ok()      # (checked first: SCORE_PATH='tensor' accepts these models)
+        model_ok = euclidean or self._tensor_path_ok(allow_tastes=True)
         d_pad = kernels.d_pad_for(self.n_components)
         limits = (kernels.filter_max_k(), kernels.topk_max_k(d_pad)) if model_ok else (0, 0)
         path = topk_route(k, n_items, model_ok, self.n_tastes == 1, *limits,
-                          sharded=item_id_offset != 0 or gather_group is not None)
+                          sharded=item_id_offset != 0 or gather_group is not None, euclidean=euclidean)
         fused = path != 'dense+rank'
         use_filter = path == 'filter'
         wide = path == 'wide'
         info = self.last_topk_info = {'path': path, 'fallback_rows': 0}
-        items = fitems = None
+        items = fitems = item_hsq = None
         if fused and n_items > 0:
             items = self._side_operands('item', item_in, device, for_filter=use_filter or wide)
             if use_filter or wide:
                 fitems = kernels.FilterItems(items)
+            if euclidean:
+                item_hsq = kernels.item_half_sqnorm(items)
 
         if user_batch_size is None:
             user_batch_size = self._topk_block_rows(path, n_users, n_items, k, gather_group, device)
@@ -880,7 +907,8 @@ class TensorRec(object):
                                          block_bytes=self.PREDICT_BLOCK_BYTES)
             if use_filter and not force_exact:
                 return kernels.topk_filter(users, items, k, item_id_offset=item_id_offset, fitems=fitems, excl=excl)
-            return kernels.topk_exact(users, items, k, item_id_offset=item_id_offset, excl=excl), None, 0
+            return kernels.topk_exact(users, items, k, item_id_offset=item_id_offset, excl=excl,
+                                      item_hsq=item_hsq), None, 0
 
         def run_block(block_in, u0, u1, force_exact=False):
             """-> (PackedTopK of the block, [(device counters | None, capacity)] of its sweeps)"""
