@@ -234,13 +234,16 @@ __device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUte
         "h"(cta_mask), "l"(cache_hint)
       : "memory");
 }
-// arrive on the barrier at the same shared-memory offset in CTA `rank` of the cluster (the own CTA included)
+// arrive on the barrier at the same shared-memory offset in CTA `rank` of the cluster (the own CTA included), with the
+// default semantics (release at CTA scope).  That is all that handing back a ring slot needs: the slot's readers are
+// wgmma that have completed before the arrival, and nothing the arriving thread wrote is read by the other side.  A
+// .release.cluster arrive would put a GPU-scope memory barrier (MEMBAR.ALL.GPU) in front of every arrival on sm_90.
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
   uint32_t remote;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
-// wait that also acquires what other CTAs of the cluster released with mbar_arrive_cluster
+// wait on a barrier that other CTAs of the cluster arrive on (mbar_arrive_cluster), with cluster-scope acquire
 __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
   uint32_t ok = 0;
   while (!ok) {

@@ -12,8 +12,8 @@
 // halves with m64n64k16 wgmma into registers.  Each consumer warp owns the 32 user rows whose accumulator fragments it
 // holds (lane l: row 16 w + l % 16 + 64 (l / 16) of the block), so the admission test of a 32-column chunk is a
 // register reduction plus shuffles inside the warp; only a chunk in which some row passes goes through the warp's own
-// shared-memory staging tile, where the admission code runs one lane per user row.  While one warpgroup filters, the
-// other's wgmma keeps the tensor cores busy.
+// shared-memory staging tile, where the admission code runs one lane per user row.  The two warpgroups issue their
+// wgmma independently and share the tensor pipe (DESIGN §2).
 //
 // Why: the exact split-product kernel issues 3 tensor passes and its per-row sorted-list inserts serialise a warp.
 // Here
@@ -357,16 +357,15 @@ __device__ __forceinline__ void sort16_desc(float (&g)[16]) {
 }
 
 
-// Columns [32 kC, 32 kC + 32) of the half in acc0 / acc1, processing positions [base, base + 32).  Fast path: the owner
-// of each row tests its register maximum against tau (and, kExclude, whether its next excluded position lies in the
-// chunk); one vote.  Most chunks stop here with no shared-memory traffic.  Otherwise the warp stages the chunk, masks
+// Columns [32 kC, 32 kC + 32) of the half in acc0 / acc1, processing positions [base, base + 32), amax =
+// chunk_row_max<kC>.  Fast path: the owner of each row tests its register maximum against tau (and, kExclude, whether
+// its next excluded position lies in the chunk); one vote.  Most chunks stop here with no shared-memory traffic.  Otherwise the warp stages the chunk, masks
 // excluded positions, and every lane runs filter_32 on its row from registers.  Called warp-uniformly.
 template <int kC, bool kExclude>
-__device__ __forceinline__ void filter_chunk(const float (&acc0)[32], const float (&acc1)[32], int32_t base,
+__device__ __forceinline__ void filter_chunk(const float (&acc0)[32], const float (&acc1)[32], float amax, int32_t base,
                                              float bmax_scaled, uint32_t stage, int lane, int64_t u,
                                              const FilterParams& p, int32_t& excl_next, RowState& r,
                                              const AdmitCtx& ctx) {
-  const float amax = chunk_row_max<kC>(acc0, acc1, lane);
   bool flag = amax + bmax_scaled > r.tau;   // == the h0 || h1 of filter_32: x -> x + bmax is monotonic
   if constexpr (kExclude) flag = flag || excl_next < base + 32;
   if (!__any_sync(0xffffffffu, flag)) return;
@@ -577,8 +576,13 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
               }
             }
           }
-          filter_chunk<0, kExclude>(acc0, acc1, pos0 + h * 64, bmax_scaled, stage, lane, u, p, excl_next, rs, ctx);
-          filter_chunk<1, kExclude>(acc0, acc1, pos0 + h * 64 + 32, bmax_scaled, stage, lane, u, p, excl_next, rs, ctx);
+          // both chunk maxima first: their shuffle chains overlap (the accumulators are read-only from here on, and the
+          // second chunk's vote still sees the tau the first chunk left)
+          const float amax0 = chunk_row_max<0>(acc0, acc1, lane), amax1 = chunk_row_max<1>(acc0, acc1, lane);
+          filter_chunk<0, kExclude>(acc0, acc1, amax0, pos0 + h * 64, bmax_scaled, stage, lane, u, p, excl_next, rs,
+                                    ctx);
+          filter_chunk<1, kExclude>(acc0, acc1, amax1, pos0 + h * 64 + 32, bmax_scaled, stage, lane, u, p, excl_next,
+                                    rs, ctx);
         }
         if (++ts == n_slots) {
           ts = 0;

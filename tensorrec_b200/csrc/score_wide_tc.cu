@@ -244,12 +244,11 @@ __device__ __forceinline__ void wide_32(const uint32_t* v, int32_t pos_base, flo
   }
 }
 
-// filter_chunk of the narrow form with wide_32 as its slow path
+// filter_chunk of the narrow form with wide_32 as its slow path (amax = chunk_row_max<kC>)
 template <int kC, bool kExclude>
-__device__ __forceinline__ void wide_chunk(const float (&acc0)[32], const float (&acc1)[32], int32_t base,
+__device__ __forceinline__ void wide_chunk(const float (&acc0)[32], const float (&acc1)[32], float amax, int32_t base,
                                            float bmax_scaled, uint32_t stage, int lane, int64_t u, const WideParams& p,
                                            int32_t& excl_next, WideRow& r, const AdmitCtx& ctx, uint32_t* hist) {
-  const float amax = chunk_row_max<kC>(acc0, acc1, lane);
   bool flag = amax + bmax_scaled > r.tau;
   if constexpr (kExclude) flag = flag || excl_next < base + 32;
   if (!__any_sync(0xffffffffu, flag)) return;
@@ -415,9 +414,11 @@ score_wide_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_co
               }
             }
           }
-          wide_chunk<0, kExclude>(acc0, acc1, pos0 + h * 64, bmax_scaled, stage, lane, u, p, excl_next, rs, ctx, hist);
-          wide_chunk<1, kExclude>(acc0, acc1, pos0 + h * 64 + 32, bmax_scaled, stage, lane, u, p, excl_next, rs, ctx,
+          const float amax0 = chunk_row_max<0>(acc0, acc1, lane), amax1 = chunk_row_max<1>(acc0, acc1, lane);
+          wide_chunk<0, kExclude>(acc0, acc1, amax0, pos0 + h * 64, bmax_scaled, stage, lane, u, p, excl_next, rs, ctx,
                                   hist);
+          wide_chunk<1, kExclude>(acc0, acc1, amax1, pos0 + h * 64 + 32, bmax_scaled, stage, lane, u, p, excl_next, rs,
+                                  ctx, hist);
         }
         if (++ts == n_slots) {
           ts = 0;
