@@ -8,11 +8,11 @@
 //
 // CTA = 256 user rows (two 128-row blocks) x a sweep over 128-item tiles: every B tile fetched from L2 feeds two
 // warpgroups.  Warp 0 streams the item tiles with TMA; consumer warpgroup g (warps 4+4g..7+4g) loads user block g
-// (hi half, TMA) into shared memory once per work unit and computes each tile's 128 x 128 accumulator in two 64-column
-// halves with m64n64k16 wgmma into registers.  Each consumer warp owns the 32 user rows whose accumulator fragments it
+// (hi half, TMA) into shared memory once per work unit and computes each tile's 128 x 128 accumulator in two 64-row
+// halves with m64n128k16 wgmma into registers.  Each consumer warp owns the 32 user rows whose accumulator fragments it
 // holds (lane l: row 16 w + l % 16 + 64 (l / 16) of the block), so the admission test of a 32-column chunk is a
-// register reduction plus shuffles inside the warp; only a chunk in which some row passes goes through the warp's own
-// shared-memory staging tile, where the admission code runs one lane per user row.  The two warpgroups issue their
+// register reduction in every lane and one warp vote; only a chunk in which some row passes goes through the warp's
+// own shared-memory staging tile, where the admission code runs one lane per user row.  The two warpgroups issue their
 // wgmma independently and share the tensor pipe (DESIGN §2).
 //
 // Why: the exact split-product kernel issues 3 tensor passes and its per-row sorted-list inserts serialise a warp.
@@ -21,7 +21,7 @@
 //   * items are processed in descending-bias order (host side), so within a 128-item block the biases are almost equal
 //     and the admission test v_j = acc_j + bias_j / c > tau (c = user scale x GLOBAL item scale, both powers of two)
 //     is bounded by max_j acc_j + blockmax / c: the hot loop is an FMNMX tree over the raw accumulators in the wgmma
-//     fragments, four shuffles, one add and one warp vote per 32 columns;
+//     fragments, two adds and one warp vote per 32 columns of 16 rows;
 //   * a passing column is APPENDED raw (accumulator, position) to the row's 32-entry buffer in shared memory; when
 //     some row's buffer passes half full the whole warp compacts it cooperatively: one entry per lane, raw entries
 //     resolved to (approximate score, item id), a 15-step bitonic sort through shuffles, keep everything >= (k-th best
@@ -245,7 +245,7 @@ __device__ __forceinline__ void compact_rows(unsigned rows, int lane, RowState& 
 
 // 16 columns of one user row per lane.  The admission test is v_j = acc_j + bias_j / c > tau.  Items are processed in
 // bias-sorted order, so the biases of one 128-item block differ by ~1e-4 of their range and v_j <= max_j acc_j +
-// bmax_block / c is a tight upper bound: the fast path (chunk_row_max in the kernel) is an FMNMX reduction of the raw
+// bmax_block / c is a tight upper bound: the fast path (chunk_frag_pass in the kernel) is an FMNMX reduction of the raw
 // accumulators plus ONE add (no per-score bias load, no per-score FFMA) and one vote; only when some lane's bound
 // passes is the chunk staged and are the exact v_j formed.  The hitting lanes then append their survivors (approximate
 // score + original item id) and rows whose buffer passed half full are compacted by the whole warp.
@@ -301,12 +301,13 @@ __device__ __forceinline__ void append_16(const uint32_t* acc, uint32_t mask, fl
 // hitting lanes form the pass masks, ONE ballot tells whether every row's buffer can take its new entries -- the common
 // case: the hitting lanes append, nobody else does anything -- and only otherwise the chunk goes through the two-step
 // path (compact the rows that need it, append 16 columns at a time so that the 32-entry buffer cannot overflow between
-// compactions).
-__device__ __forceinline__ void filter_32(const uint32_t* acc, int32_t pos_base, float bmax_scaled, int lane,
+// compactions).  Only the lanes with `own` set (the owners of the staged rows) test their row; the others take part in
+// the votes and compactions only.
+__device__ __forceinline__ void filter_32(const uint32_t* acc, bool own, int32_t pos_base, float bmax_scaled, int lane,
                                           RowState& r, const AdmitCtx& ctx) {
   float g0[4], g1[4];
   const float a0 = acc_max_16(acc, g0), a1 = acc_max_16(acc + 16, g1);
-  const bool h0 = a0 + bmax_scaled > r.tau, h1 = a1 + bmax_scaled > r.tau;
+  const bool h0 = own && a0 + bmax_scaled > r.tau, h1 = own && a1 + bmax_scaled > r.tau;
   if (__any_sync(0xffffffffu, h0 || h1)) {
     uint32_t lo = 0, hi = 0;
     if (h0) lo = pass_mask_16(acc, g0, bmax_scaled, r.tau);
@@ -357,25 +358,61 @@ __device__ __forceinline__ void sort16_desc(float (&g)[16]) {
 }
 
 
-// Columns [32 kC, 32 kC + 32) of the half in acc0 / acc1, processing positions [base, base + 32), amax =
-// chunk_row_max<kC>.  Fast path: the owner of each row tests its register maximum against tau (and, kExclude, whether
-// its next excluded position lies in the chunk); one vote.  Most chunks stop here with no shared-memory traffic.  Otherwise the warp stages the chunk, masks
-// excluded positions, and every lane runs filter_32 on its row from registers.  Called warp-uniformly.
+// Columns [32 kC, 32 kC + 32) of row half rh in acc, processing positions [base, base + 32); bf / tf = frag_rows of
+// the row half's bias bounds and tau.  Fast path: every lane tests the maxima of the 8 columns it holds of its two rows
+// (and, kExclude, the owners of the row half whether their next excluded position lies in the chunk); one vote, no
+// shuffles.  Most chunks stop here with no shared-memory traffic.  Otherwise the warp stages the chunk, masks excluded
+// positions, and the owner lanes of the row half run filter_32 on their rows from registers.  Called warp-uniformly.
 template <int kC, bool kExclude>
-__device__ __forceinline__ void filter_chunk(const float (&acc0)[32], const float (&acc1)[32], float amax, int32_t base,
-                                             float bmax_scaled, uint32_t stage, int lane, int64_t u,
+__device__ __forceinline__ void filter_chunk(const float (&acc)[64], int rh, int32_t base, float bmax_scaled,
+                                             const float (&bf)[2], float (&tf)[2], uint32_t stage, int lane, int64_t u,
                                              const FilterParams& p, int32_t& excl_next, RowState& r,
                                              const AdmitCtx& ctx) {
-  bool flag = amax + bmax_scaled > r.tau;   // == the h0 || h1 of filter_32: x -> x + bmax is monotonic
-  if constexpr (kExclude) flag = flag || excl_next < base + 32;
+  const bool own = (lane >> 4) == rh;
+  bool flag = chunk_frag_pass<kC>(acc, bf, tf);   // == the h0 || h1 of filter_32 over the quad
+  if constexpr (kExclude) flag = flag || (own && excl_next < base + 32);
   if (!__any_sync(0xffffffffu, flag)) return;
-  stage_warp_chunk<kC>(acc0, acc1, stage, lane);
+  stage_warp_chunk<kC>(acc, rh, stage, lane);
   if constexpr (kExclude) {
-    if (excl_next < base + 32) excl_next = excl_mask_chunk(p.excl_indptr, p.excl_pos, u, base, stage, lane);
+    if (own && excl_next < base + 32) excl_next = excl_mask_chunk(p.excl_indptr, p.excl_pos, u, base, stage, lane);
   }
   uint32_t v[32];
   load_staged_row(stage, lane, v);
-  filter_32(v, base, bmax_scaled, lane, r, ctx);
+  filter_32(v, own, base, bmax_scaled, lane, r, ctx);
+  frag_rows(r.tau, rh, lane, tf);
+}
+
+// The four chunks of row half rh, processing positions [pos0, pos0 + 128): every row's columns in ascending order, and
+// a chunk's test sees the tau the chunks before it left.  Called warp-uniformly.
+template <bool kExclude>
+__device__ __forceinline__ void filter_row_half(const float (&acc)[64], int rh, int32_t pos0, float bmax_scaled,
+                                                uint32_t stage, int lane, int64_t u, const FilterParams& p,
+                                                int32_t& excl_next, RowState& r, const AdmitCtx& ctx) {
+  float bf[2], tf[2];
+  frag_rows(bmax_scaled, rh, lane, bf);
+  frag_rows(r.tau, rh, lane, tf);
+  filter_chunk<0, kExclude>(acc, rh, pos0, bmax_scaled, bf, tf, stage, lane, u, p, excl_next, r, ctx);
+  filter_chunk<1, kExclude>(acc, rh, pos0 + 32, bmax_scaled, bf, tf, stage, lane, u, p, excl_next, r, ctx);
+  filter_chunk<2, kExclude>(acc, rh, pos0 + 64, bmax_scaled, bf, tf, stage, lane, u, p, excl_next, r, ctx);
+  filter_chunk<3, kExclude>(acc, rh, pos0 + 96, bmax_scaled, bf, tf, stage, lane, u, p, excl_next, r, ctx);
+}
+
+// Warm start: the 8-column group maxima g[4 kC + q] of columns [32 kC, 32 kC + 32) of the lane's row, for the owner
+// lanes of row half rh; excluded positions are masked with the pre-pass cursor `pre_next`.  Called warp-uniformly.
+template <int kC, bool kExclude>
+__device__ __forceinline__ void warm_chunk(const float (&acc)[64], int rh, int32_t pos0, uint32_t stage, int lane,
+                                           int64_t u, const FilterParams& p, int32_t& pre_next, float (&g)[16]) {
+  const bool own = (lane >> 4) == rh;
+  stage_warp_chunk<kC>(acc, rh, stage, lane);
+  if constexpr (kExclude) {
+    if (own && pre_next < pos0 + 32 * kC + 32)
+      pre_next = excl_mask_chunk(p.excl_indptr, p.excl_pos, u, pos0 + 32 * kC, stage, lane);
+  }
+  uint32_t v[32];
+  load_staged_row(stage, lane, v);
+#pragma unroll
+  for (int q = 0; q < 4; ++q)
+    if (own) g[4 * kC + q] = acc_max_8(v + 8 * q);
 }
 
 
@@ -475,7 +512,7 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
     const AdmitCtx ctx = {p.item_bias, p.item_perm, p.item_id_offset, static_cast<int32_t>(p.n_items), p.k};
     int ts = 0;
     uint32_t ts_phase = 0, witer = 0;
-    float acc0[32], acc1[32];
+    float acc[64];
 
     for (int64_t w = w_first; w < n_work; w += w_step) {
       const int up = static_cast<int>(w % n_groups) * kCluster + static_cast<int>(crank);
@@ -531,25 +568,12 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
             // the tile is filtered again below: the pre-pass masks with a copy of the cursor
             int32_t pre_next = excl_next;
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              filter_mma_half<kNKB>(acc0, acc1, a_base, b_slot, h);
-              uint32_t v[32];
-              stage_warp_chunk<0>(acc0, acc1, stage, lane);
-              if constexpr (kExclude) {
-                if (pre_next < pos0 + h * 64 + 32)
-                  pre_next = excl_mask_chunk(p.excl_indptr, p.excl_pos, u, pos0 + h * 64, stage, lane);
-              }
-              load_staged_row(stage, lane, v);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) g[8 * h + q] = acc_max_8(v + 8 * q);
-              stage_warp_chunk<1>(acc0, acc1, stage, lane);
-              if constexpr (kExclude) {
-                if (pre_next < pos0 + h * 64 + 64)
-                  pre_next = excl_mask_chunk(p.excl_indptr, p.excl_pos, u, pos0 + h * 64 + 32, stage, lane);
-              }
-              load_staged_row(stage, lane, v);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) g[8 * h + 4 + q] = acc_max_8(v + 8 * q);
+            for (int rh = 0; rh < 2; ++rh) {   // each lane's row is in one row half: its 16 groups come from that one
+              filter_mma_rows<kNKB>(acc, a_base, b_slot, rh);
+              warm_chunk<0, kExclude>(acc, rh, pos0, stage, lane, u, p, pre_next, g);
+              warm_chunk<1, kExclude>(acc, rh, pos0, stage, lane, u, p, pre_next, g);
+              warm_chunk<2, kExclude>(acc, rh, pos0, stage, lane, u, p, pre_next, g);
+              warm_chunk<3, kExclude>(acc, rh, pos0, stage, lane, u, p, pre_next, g);
             }
             sort16_desc(g);
             float a_k = g[0];
@@ -563,9 +587,9 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
           }
         }
 #pragma unroll 1
-        for (int h = 0; h < 2; ++h) {
-          filter_mma_half<kNKB>(acc0, acc1, a_base, b_slot, h);
-          if (h == 1) {   // the tile's last MMAs of this warp are complete: release the B slot in every CTA that got it
+        for (int rh = 0; rh < 2; ++rh) {
+          filter_mma_rows<kNKB>(acc, a_base, b_slot, rh);
+          if (rh == 1) {   // the tile's last MMAs of this warp are complete: release the B slot in every CTA that got it
             __syncwarp();
             if (lane == 0) {
               if (kCluster == 2) {
@@ -576,13 +600,15 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
               }
             }
           }
-          // both chunk maxima first: their shuffle chains overlap (the accumulators are read-only from here on, and the
-          // second chunk's vote still sees the tau the first chunk left)
-          const float amax0 = chunk_row_max<0>(acc0, acc1, lane), amax1 = chunk_row_max<1>(acc0, acc1, lane);
-          filter_chunk<0, kExclude>(acc0, acc1, amax0, pos0 + h * 64, bmax_scaled, stage, lane, u, p, excl_next, rs,
-                                    ctx);
-          filter_chunk<1, kExclude>(acc0, acc1, amax1, pos0 + h * 64 + 32, bmax_scaled, stage, lane, u, p, excl_next,
-                                    rs, ctx);
+          // kExclude: one vote per row half.  Only a row half in which some owner's next excluded position lies runs
+          // the exclusion test of every chunk; every other one (all of them with empty lists) runs the exclusion-free
+          // code, which decides exactly as the exclusion test would there.
+          bool excl_rh = false;
+          if constexpr (kExclude) excl_rh = __any_sync(0xffffffffu, (lane >> 4) == rh && excl_next < pos0 + kBlockN);
+          if (excl_rh)
+            filter_row_half<kExclude>(acc, rh, pos0, bmax_scaled, stage, lane, u, p, excl_next, rs, ctx);
+          else
+            filter_row_half<false>(acc, rh, pos0, bmax_scaled, stage, lane, u, p, excl_next, rs, ctx);
         }
         if (++ts == n_slots) {
           ts = 0;
