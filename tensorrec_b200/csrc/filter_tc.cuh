@@ -1,9 +1,16 @@
 // Pieces of the one-pass tensor-core filter (DESIGN §2-3) shared by its narrow form (score_filter_tc.cu, a
 // 32-entry candidate buffer per row in shared memory, k <= 12) and its wide form (score_wide_tc.cu, a candidate list
-// per row in global memory, k <= 1024): the error-bound constants, the warpgroup's tile MMA (m64n128k16 row halves for
-// the narrow form, m64n64k16 column halves for the wide form), the register fast path on the wgmma fragments and the
-// per-warp staging of a flagged chunk, with the exclusion cursor.
+// per row in global memory, k <= 1024):
+//   * the sweep skeleton: the parameters both forms read, the shared-memory layout and barriers, the TMA producer warp,
+//     the consumers' work-unit decode, row constants, user-block load and B-slot release, and the host launcher (stage
+//     count, launch form, tensor maps).  None of it depends on how a form stores its candidates;
+//   * the error-bound constants, the warpgroup's tile MMA (m64n128k16 row halves for the narrow form, m64n64k16 column
+//     halves for the wide form), the register fast path on the wgmma fragments and the per-warp staging of a flagged
+//     chunk, with the exclusion cursor.
+// Each form keeps its own kernel body: its tile epilogue, compaction and output.
 #pragma once
+
+#include <stdlib.h>
 
 #include "common.cuh"
 
@@ -33,6 +40,253 @@ __device__ __forceinline__ void set_tau(Row& r) {
   r.tau = t - 8.0f * 1.1920929e-7f * fabsf(t) - 1e-30f;
 }
 
+// ---- the sweep skeleton ---------------------------------------------------------------------------------------------
+// A work unit is 256 user rows (two 128-row blocks, one per consumer warpgroup) x an item split.  Warp 0 streams the
+// split's 128-item tiles with TMA into a ring of tile slots; consumer warpgroup g (warps 4+4g..7+4g) loads user block g
+// once per unit and runs the form's epilogue on every tile, so every B tile fetched from L2 feeds two warpgroups.
+// Template parameters of both kernels: kNKB = k-blocks of 64 per row (d_pad / 64); kCluster = 1, or 2 = clusters of two
+// CTAs on two different user pairs over the SAME item tiles, each CTA fetching half of every tile and TMA-multicasting it
+// into both (the L2 -> SM stream of the item operand is halved); kExclude = mask each row's exclusion list
+// (excl_indptr / excl_pos) out of the candidate universe, see excl_mask_chunk.
+
+// The inputs and shapes both forms read (FilterParams / WideParams hold one, plus their candidate storage).
+struct SweepParams {
+  const float* user_scale;
+  const float* user_bias;      // may be null
+  const float* user_norm;      // |u|_2 per user
+  const float* item_bias;      // [padded items] in PROCESSING order (see item_perm), padding = -inf
+  const float* block_bias_max; // max item bias of every block of 128 processing positions (-inf for all-padding)
+  const int32_t* item_perm;    // processing position -> local item index (items sorted by bias), or null = identity
+  const float* item_stats;     // device: [0] = max_j |i_j|_2, [1] = global item scale (2^-E), [2] = max_j |bias_j|
+  int64_t n_users;
+  int64_t n_items;
+  int32_t n_stages;            // B ring in k-block tiles
+  int32_t k;
+  int32_t n_splits;
+  int32_t tiles_per_split;
+  int32_t n_tiles;
+  int32_t n_user_pairs;        // ceil(n_users / 256)
+  int32_t item_id_offset;
+  float* row_theta;            // [n_users, n_splits] max(theta, drop_max), certified by the form's rescore kernel
+  // exclusion lists (kExclude instantiations only): row u's excluded items as PROCESSING positions, ascending, at
+  // excl_pos[excl_indptr[u] .. excl_indptr[u + 1])
+  const int32_t* excl_indptr;
+  const int32_t* excl_pos;
+};
+
+// Shared memory: user blocks 0 and 1 (n_kblocks tiles each), the B ring, `extra_bytes` of the form's own at extra_off,
+// the consumer warps' staging tiles and the barriers.
+struct SweepLayout {
+  uint32_t a_off, b_off, extra_off, acc_off, bar_off, total;
+};
+__host__ __device__ inline SweepLayout sweep_layout(int n_kblocks, int n_stages, uint32_t extra_bytes) {
+  SweepLayout L;
+  L.a_off = 0;
+  L.b_off = L.a_off + 2u * static_cast<uint32_t>(n_kblocks) * kATileBytes;
+  L.extra_off = L.b_off + static_cast<uint32_t>(n_stages) * kBTileBytes;
+  L.acc_off = L.extra_off + extra_bytes;
+  L.bar_off = L.acc_off + 2u * kAccStageBytes;
+  L.total = L.bar_off + 512u;
+  return L;
+}
+// The B ring is organised in TILE slots of n_kblocks k-blocks (16 KB each): one full / one empty barrier per item tile.
+// barriers (uint64): [0..1] a_full (per user block) [2 .. 2+T) b_full [2+T .. 2+2T) b_empty, T = n_stages / n_kblocks
+// tile slots.  b_empty counts the 8 consumer warps of every CTA that received the tile.
+// The item biases are NOT staged: the hot loop needs only the block maximum (one cached global load per tile,
+// prefetched a tile ahead) and the rare admission path reads the few biases it needs through L2.
+
+// What every thread of the CTA knows about the sweep after sweep_prologue.
+struct SweepCta {
+  uint8_t* smem;
+  SweepLayout L;
+  int n_slots;                  // B tile slots
+  uint64_t* a_full;             // [user block]
+  uint64_t* b_full;             // [slot]
+  uint64_t* b_empty;            // [slot]
+  uint32_t crank;               // rank in the cluster
+  int n_groups;                 // groups of kCluster user pairs
+  int64_t n_work, w_first, w_step;   // work units, this CTA's first one and its stride
+};
+
+// Tensor-map prefetch, barrier init and (kCluster = 2) the cluster sync after which the peer's barriers exist.
+template <int kNKB, int kCluster>
+__device__ __forceinline__ SweepCta sweep_prologue(const SweepParams& p, uint32_t extra_bytes,
+                                                   const CUtensorMap* map_users, const CUtensorMap* map_items) {
+  SweepCta cta;
+  cta.smem = smem_base_1024();
+  cta.L = sweep_layout(kNKB, p.n_stages, extra_bytes);
+  cta.n_slots = p.n_stages / kNKB;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(cta.smem + cta.L.bar_off);
+  cta.a_full = bars + 0;
+  cta.b_full = bars + 2;
+  cta.b_empty = bars + 2 + cta.n_slots;
+
+  const int warp = threadIdx.x / 32;
+  const int lane = threadIdx.x % 32;
+  // work unit = (group of kCluster user pairs, item split); CTA `crank` of the cluster takes pair kCluster * g + crank
+  cta.crank = kCluster == 2 ? cluster_ctarank() : 0u;
+  cta.n_groups = (p.n_user_pairs + kCluster - 1) / kCluster;
+  cta.n_work = static_cast<int64_t>(cta.n_groups) * p.n_splits;
+  cta.w_first = blockIdx.x / kCluster;
+  cta.w_step = gridDim.x / kCluster;
+
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(map_items);
+    tma_prefetch_desc(map_users);
+  }
+  if (warp == 1 && lane == 0) {
+    for (int i = 0; i < 2; ++i) mbar_init(cta.a_full + i, 1);
+    for (int i = 0; i < cta.n_slots; ++i) {
+      mbar_init(cta.b_full + i, 1);
+      mbar_init(cta.b_empty + i, 8 * kCluster);   // the consumer warps of all CTAs that received the tile
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  if (kCluster == 2) cluster_sync_all();   // the peer's barriers exist before anything is multicast to them
+  return cta;
+}
+
+// Register budget: the producer warpgroup (one issuing warp) needs few, the consumers hold the accumulators, a staged
+// row and the admission state per thread (40 x 128 + 232 x 256 = 64,512 of the 65,536 registers).  Returns whether
+// `warp` is in the producer warpgroup.
+__device__ __forceinline__ bool sweep_split_registers(int warp) {
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    return true;
+  }
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+  return false;
+}
+
+// Work unit w as a consumer thread of warpgroup `group` that owns block row `row` sees it (the producer passes 0, 0
+// and reads the tile range only).
+struct SweepUnit {
+  int sp, t0, t1;               // item split, its tiles [t0, t1)
+  int64_t ublock_row0;          // first row of the warpgroup's user block
+  int64_t u;                    // the thread's user row
+  bool u_ok;                    // u < n_users
+};
+template <int kCluster>
+__device__ __forceinline__ SweepUnit sweep_unit(const SweepParams& p, const SweepCta& cta, int64_t w, int group,
+                                                int row) {
+  SweepUnit wu;
+  const int up = static_cast<int>(w % cta.n_groups) * kCluster + static_cast<int>(cta.crank);
+  wu.sp = static_cast<int>(w / cta.n_groups);
+  wu.t0 = wu.sp * p.tiles_per_split;
+  wu.t1 = min(wu.t0 + p.tiles_per_split, p.n_tiles);
+  wu.ublock_row0 = (static_cast<int64_t>(up) * 2 + group) * kBlockM;
+  wu.u = wu.ublock_row0 + row;
+  wu.u_ok = wu.u < p.n_users;
+  return wu;
+}
+
+__device__ __forceinline__ void sweep_ring_advance(int& ts, uint32_t& ts_phase, int n_slots) {
+  if (++ts == n_slots) {
+    ts = 0;
+    ts_phase ^= 1;
+  }
+}
+
+// Warp 0: every tile of every work unit of this CTA into the ring, warp-uniform control flow, one elected lane issues.
+template <int kNKB, int kCluster>
+__device__ __forceinline__ void sweep_producer(const SweepParams& p, const SweepCta& cta,
+                                               const CUtensorMap* map_items) {
+  constexpr uint32_t kSlotBytes = kNKB * kBTileBytes;
+  constexpr uint16_t kClusterMask = (1u << kCluster) - 1u;
+  uint8_t* const ring = cta.smem + cta.L.b_off;
+  int ts = 0;
+  uint32_t ts_phase = 0;
+  for (int64_t w = cta.w_first; w < cta.n_work; w += cta.w_step) {
+    const SweepUnit wu = sweep_unit<kCluster>(p, cta, w, 0, 0);
+    for (int t = wu.t0; t < wu.t1; ++t) {
+      if (kCluster == 2)
+        mbar_wait_cluster(cta.b_empty + ts, ts_phase ^ 1);
+      else
+        mbar_wait(cta.b_empty + ts, ts_phase ^ 1);
+      if (elect_one()) {
+        mbar_arrive_expect_tx(cta.b_full + ts, kSlotBytes);
+#pragma unroll
+        for (int kb = 0; kb < kNKB; ++kb) {
+          if (kCluster == 2)   // this CTA's half of the tile rows (box = 64 rows), delivered to both CTAs
+            tma_load_2d_multicast(ring + ts * kSlotBytes + kb * kBTileBytes + cta.crank * (kBTileBytes / 2), map_items,
+                                  cta.b_full + ts, kb * kKBlock,
+                                  t * kBlockN + static_cast<int>(cta.crank) * (kBlockN / 2), kClusterMask, kEvictLast);
+          else
+            tma_load_2d(ring + ts * kSlotBytes + kb * kBTileBytes, map_items, cta.b_full + ts, kb * kKBlock,
+                        t * kBlockN, kEvictLast);
+        }
+      }
+      __syncwarp();
+      sweep_ring_advance(ts, ts_phase, cta.n_slots);
+    }
+  }
+}
+
+// The row constants of the unit's user row (fields m3, ubias, c, inv_c of the form's row state): the margin 2.25 m,
+// the user bias, c = user scale x global item scale (powers of two: exact) and 1 / c.  Returns the exclusion cursor
+// (kExclude): the first excluded processing position of the row in the unit's tiles, INT32_MAX if none.
+template <bool kExclude, class Row>
+__device__ __forceinline__ int32_t sweep_row_start(Row& r, const SweepParams& p, const SweepUnit& wu,
+                                                   float max_item_norm, float item_scale, float max_item_bias) {
+  const float su = wu.u_ok ? __ldg(p.user_scale + wu.u) : 1.0f;
+  const float ubias = (wu.u_ok && p.user_bias != nullptr) ? __ldg(p.user_bias + wu.u) : 0.0f;
+  const float unorm = wu.u_ok ? __ldg(p.user_norm + wu.u) : 0.0f;
+  r.ubias = ubias;
+  r.c = su * item_scale;
+  r.inv_c = 1.0f / r.c;
+  // error bound of one approximate score: operand rounding + the fp32 rounding of the two bias adds
+  r.m3 = kThetaMargins * (kMarginFactor * unorm * max_item_norm + kBiasUlps * (fabsf(ubias) + max_item_bias));
+  int32_t excl_next = 0x7fffffff;
+  if constexpr (kExclude) {
+    if (wu.u_ok && wu.t1 > wu.t0) excl_next = excl_next_at(p.excl_indptr, p.excl_pos, wu.u, wu.t0 * kBlockN);
+  }
+  return excl_next;
+}
+
+// The warpgroup's user block (hi half, fp16; rows past n_users arrive as zeros) goes to shared memory.  Every wgmma of
+// the previous unit has completed in all four warps once they pass the named barrier.  Called by the whole warpgroup.
+template <int kNKB>
+__device__ __forceinline__ void sweep_load_user_block(const SweepCta& cta, const CUtensorMap* map_users,
+                                                      const SweepUnit& wu, int group, int warp, int lane,
+                                                      uint32_t& witer) {
+  if (wu.t1 > wu.t0) {
+    named_barrier_sync(1 + group, kConsumerThreads);
+    if (warp % 4 == 0 && lane == 0) {
+      mbar_arrive_expect_tx(cta.a_full + group, kNKB * kATileBytes);
+#pragma unroll
+      for (int kb = 0; kb < kNKB; ++kb)
+        tma_load_2d(cta.smem + cta.L.a_off + (group * kNKB + kb) * kATileBytes, map_users, cta.a_full + group,
+                    kb * kKBlock, static_cast<int32_t>(wu.ublock_row0), kEvictFirst);
+    }
+    mbar_wait(cta.a_full + group, witer & 1);
+    ++witer;
+  }
+}
+
+// After the warp's last MMAs of a tile: release B slot ts in every CTA that received it.  Called warp-uniformly.
+template <int kCluster>
+__device__ __forceinline__ void sweep_release_slot(const SweepCta& cta, int ts, int lane) {
+  __syncwarp();
+  if (lane == 0) {
+    if (kCluster == 2) {
+#pragma unroll
+      for (uint32_t r = 0; r < kCluster; ++r) mbar_arrive_cluster(cta.b_empty + ts, r);
+    } else {
+      mbar_arrive(cta.b_empty + ts);
+    }
+  }
+}
+
+// Every excluded or dropped item has an approximate score <= max(theta, drop_max); a NaN (inf - inf with infinite
+// biases) must not read as "nothing was excluded": +inf makes the certificate fail and the row goes through the exact
+// kernel.
+template <class Row>
+__device__ __forceinline__ void sweep_store_theta(const SweepParams& p, int64_t list, const Row& r) {
+  const bool th_nan = r.theta != r.theta || r.drop_max != r.drop_max;
+  p.row_theta[list] = th_nan ? __int_as_float(0x7f800000) : fmaxf(r.theta, r.drop_max);
+}
+
 __device__ __forceinline__ float ldg_nc_f32(const float* p) {
   float v;
   asm volatile("ld.global.nc.f32 %0, [%1];" : "=f"(v) : "l"(p));
@@ -51,10 +305,6 @@ __device__ __forceinline__ float acc_max_16(const uint32_t* acc, float (&g)[4]) 
     g[q] = fmaxf(fmaxf(__uint_as_float(acc[4 * q]), __uint_as_float(acc[4 * q + 1])),
                  fmaxf(__uint_as_float(acc[4 * q + 2]), __uint_as_float(acc[4 * q + 3])));
   return fmaxf(fmaxf(g[0], g[1]), fmaxf(g[2], g[3]));
-}
-__device__ __forceinline__ float acc_max_16(const uint32_t* acc) {
-  float g[4];
-  return acc_max_16(acc, g);
 }
 
 // Bit mask of the columns of acc[0, 16) whose admission bound passes.  g[q] = maximum of columns [4q, 4q + 4) from the
@@ -276,6 +526,129 @@ __device__ __forceinline__ uint32_t wide_key(float s) {
 }
 __device__ __forceinline__ float wide_unkey(uint32_t key) {
   return __uint_as_float((key & 0x80000000u) ? (key & 0x7fffffffu) : ~key);
+}
+
+// ---- host: the launcher of both forms -------------------------------------------------------------------------------
+// Checks the arguments both C entry points take (messages prefixed with `name`), fills p.sweep, picks the stage count
+// and the launch form, encodes the two tensor maps and launches Kernel<d_pad / 64, cluster, exclusion>::fn.  The
+// caller has checked and filled its own part of p; `extra_bytes` is its shared memory (sweep_layout).
+//
+// Launch form: clusters of two CTAs sharing every item tile through TMA multicast (default when the device can keep
+// (almost) all SMs busy with 2-CTA clusters), else independent CTAs.  TRK_FILTER_CLUSTER=1|2 forces one.
+template <template <int, int, bool> class Kernel, class P>
+int launch_sweep(const char* name, P p, uint32_t extra_bytes, const void* user_split, const float* user_scale,
+                 const float* user_bias, const float* user_norm, const void* item_hi, const float* item_stats,
+                 const float* item_bias, const float* block_bias_max, const int32_t* item_perm, int64_t n_users,
+                 int64_t n_items, int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset,
+                 float* row_theta, const int32_t* excl_indptr, const int32_t* excl_pos, cudaStream_t stream) {
+  TRK_CHECK_ARG(user_split && user_scale && user_norm && item_hi && item_stats && item_bias && block_bias_max,
+                "%s: null input", name);
+  TRK_CHECK_ARG((excl_indptr == nullptr) == (excl_pos == nullptr), "%s: excl_indptr and excl_pos go together", name);
+  TRK_CHECK_ARG(n_users >= 1 && n_items >= 1 && n_splits >= 1, "%s: empty shape", name);
+  TRK_CHECK_ARG(n_users < (1ll << 31) && n_items < (1ll << 31) - 512, "%s: shape exceeds int32 indexing", name);
+  if (d_pad != 64 && d_pad != 128) {
+    set_error("%s: d_pad=%d not supported (64 or 128)", name, d_pad);
+    return TRK_ERR_UNSUPPORTED;
+  }
+  TRK_CHECK_ARG(reinterpret_cast<uintptr_t>(user_split) % 16 == 0 && reinterpret_cast<uintptr_t>(item_hi) % 16 == 0,
+                "%s: operands must be 16-byte aligned", name);
+
+  SweepParams& s = p.sweep;
+  s.user_scale = user_scale;
+  s.user_bias = user_bias;
+  s.user_norm = user_norm;
+  s.item_bias = item_bias;
+  s.block_bias_max = block_bias_max;
+  s.item_perm = item_perm;
+  s.item_stats = item_stats;
+  s.n_users = n_users;
+  s.n_items = n_items;
+  s.k = k;
+  s.n_tiles = static_cast<int32_t>(ceil_div(n_items, kBlockN));
+  s.n_splits = n_splits;
+  s.tiles_per_split = static_cast<int32_t>(ceil_div(s.n_tiles, n_splits));
+  s.n_user_pairs = static_cast<int32_t>(ceil_div(n_users, 2 * kBlockM));
+  s.item_id_offset = item_id_offset;
+  s.row_theta = row_theta;
+  s.excl_indptr = excl_indptr;
+  s.excl_pos = excl_pos;
+  const int n_kblocks = d_pad / kKBlock;
+  s.n_stages = 0;
+  for (int st = kMaxStages; st >= 2; --st)
+    if (st % n_kblocks == 0 && sweep_layout(n_kblocks, st, extra_bytes).total + kSmemAlignSlack <= kSmemLimit) {
+      s.n_stages = st;
+      break;
+    }
+  TRK_CHECK_ARG(s.n_stages >= 2 * n_kblocks, "%s: shared memory budget exceeded", name);
+  const uint32_t smem_bytes = sweep_layout(n_kblocks, s.n_stages, extra_bytes).total + kSmemAlignSlack;
+
+  const bool excl = excl_indptr != nullptr;
+  using KernelFn = void (*)(CUtensorMap, CUtensorMap, P);
+  const KernelFn kernel2 = excl ? (n_kblocks == 2 ? Kernel<2, 2, true>::fn : Kernel<1, 2, true>::fn)
+                                : (n_kblocks == 2 ? Kernel<2, 2, false>::fn : Kernel<1, 2, false>::fn);
+  const KernelFn kernel1 = excl ? (n_kblocks == 2 ? Kernel<2, 1, true>::fn : Kernel<1, 1, true>::fn)
+                                : (n_kblocks == 2 ? Kernel<2, 1, false>::fn : Kernel<1, 1, false>::fn);
+  int cluster = 2;
+  const char* env = getenv("TRK_FILTER_CLUSTER");
+  if (env != nullptr && (atoi(env) == 1 || atoi(env) == 2)) cluster = atoi(env);
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr[1];
+  int max_clusters = 0;
+  if (cluster == 2) {
+    TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel2, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    cfg.gridDim = dim3(2);
+    cfg.blockDim = dim3(kTcThreads);
+    cfg.dynamicSmemBytes = smem_bytes;
+    cfg.stream = stream;
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    // the answer depends on (device, kernel, shared memory) only: asked once per device and kernel (one table per
+    // form, indexed by n_kblocks x exclusion)
+    static int cached_clusters[64][4];
+    static bool cached_valid[64][4];
+    int device = 0;
+    TRK_CHECK_CUDA(cudaGetDevice(&device));
+    const int variant = (n_kblocks == 2 ? 1 : 0) + (excl ? 2 : 0);
+    if (device >= 0 && device < 64 && cached_valid[device][variant]) {
+      max_clusters = cached_clusters[device][variant];
+    } else {
+      if (cudaOccupancyMaxActiveClusters(&max_clusters, kernel2, &cfg) != cudaSuccess) {
+        (void)cudaGetLastError();
+        max_clusters = 0;
+      }
+      if (device >= 0 && device < 64) {
+        cached_clusters[device][variant] = max_clusters;
+        cached_valid[device][variant] = true;
+      }
+    }
+    if (max_clusters * 2 < sm_count() - 8 && env == nullptr) cluster = 1;   // too many SMs would sit idle
+    if (max_clusters < 1) cluster = 1;
+  }
+  // fp16 operands, boxes of one k-block: the items [n_items, d_pad] (each CTA of a cluster fetches half of a tile) and
+  // the hi half of the split user rows [n_users, 2 d_pad]
+  CUtensorMap map_users, map_items;
+  int rc = encode_tiled_2d(&map_items, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, item_hi, d_pad, n_items, 2 * d_pad, kKBlock,
+                           kBlockN / cluster, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  if (rc != TRK_OK) return rc;
+  rc = encode_tiled_2d(&map_users, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, user_split, d_pad, n_users, 4 * d_pad, kKBlock,
+                       kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  if (rc != TRK_OK) return rc;
+  if (cluster == 2) {
+    const int64_t n_work = ceil_div(static_cast<int64_t>(s.n_user_pairs), 2) * n_splits;
+    const int n_clusters = static_cast<int>(n_work < max_clusters ? n_work : max_clusters);
+    cfg.gridDim = dim3(static_cast<unsigned>(2 * n_clusters));
+    TRK_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel2, map_users, map_items, p));
+  } else {
+    TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel1, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    const int grid = capped_grid(static_cast<int64_t>(s.n_user_pairs) * n_splits, 1);
+    kernel1<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, p);
+  }
+  TRK_CHECK_LAUNCH();
+  return TRK_OK;
 }
 
 }  // namespace trk

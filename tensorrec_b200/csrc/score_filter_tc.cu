@@ -6,10 +6,9 @@
 // (tensorrec/prediction_graphs.py:49-50), bias_prediction_dense (tensorrec/recommendation_graphs.py:41),
 // rank_predictions (:73-82) restricted to rank <= k.
 //
-// CTA = 256 user rows (two 128-row blocks) x a sweep over 128-item tiles: every B tile fetched from L2 feeds two
-// warpgroups.  Warp 0 streams the item tiles with TMA; consumer warpgroup g (warps 4+4g..7+4g) loads user block g
-// (hi half, TMA) into shared memory once per work unit and computes each tile's 128 x 128 accumulator in two 64-row
-// halves with m64n128k16 wgmma into registers.  Each consumer warp owns the 32 user rows whose accumulator fragments it
+// The CTA runs the sweep skeleton of filter_tc.cuh (256 user rows x a sweep over 128-item tiles).  Consumer warpgroup
+// g computes each tile's 128 x 128 accumulator of user block g in two 64-row halves with m64n128k16 wgmma into
+// registers.  Each consumer warp owns the 32 user rows whose accumulator fragments it
 // holds (lane l: row 16 w + l % 16 + 64 (l / 16) of the block), so the admission test of a 32-column chunk is a
 // register reduction in every lane and one warp vote; only a chunk in which some row passes goes through the warp's
 // own shared-memory staging tile, where the admission code runs one lane per user row.  The two warpgroups issue their
@@ -43,55 +42,15 @@ constexpr int kBufEntries = 32;      // candidate buffer per (row, epilogue grou
 constexpr int kKeepMax = 16;         // entries kept by a compaction (>= k + slack); also the per-group output width
 constexpr int kFilterMaxK = 12;
 
+constexpr uint32_t kBufBytes = 2u * kBlockM * kBufEntries * 8u;   // 64 KB of candidate buffers, after the B ring
+
 struct FilterParams {
-  const __half* user_split;    // [n_users, 2 d_pad] hi | lo; the filter reads the hi half
-  const float* user_scale;
-  const float* user_bias;      // may be null
-  const float* user_norm;      // |u|_2 per user
-  const float* item_bias;      // [padded items] in PROCESSING order (see item_perm), padding = -inf
-  const float* block_bias_max; // max item bias of every block of 128 processing positions (-inf for all-padding)
+  SweepParams sweep;
   const float* block_bias_min; // min item bias of every block (-inf as soon as the block holds padding); may be null
-  const int32_t* item_perm;    // processing position -> local item index (items sorted by bias), or null = identity
-  const float* item_stats;     // device: [0] = max_j |i_j|_2, [1] = global item scale (2^-E), [2] = max_j |bias_j|
-  int64_t n_users;
-  int64_t n_items;
-  int32_t n_kblocks;           // d_pad / 64
-  int32_t d_pad;
-  int32_t n_stages;
-  int32_t k;
-  int32_t n_splits;
-  int32_t tiles_per_split;
-  int32_t n_tiles;
-  int32_t n_user_pairs;        // ceil(n_users / 256)
-  int32_t item_id_offset;
   int32_t tile_end_trigger;    // rows holding more entries than this are compacted at the END of a tile
   float* cand_score;           // [n_users, n_splits, kKeepMax] approximate scores (sentinel -inf)
   int32_t* cand_item;          // [n_users, n_splits, kKeepMax] global ids (sentinel INT32_MAX)
-  float* row_theta;            // [n_users, n_splits] final admission threshold (certified by rescore_topk_kernel)
-  // exclusion lists (kExclude instantiations only): row u's excluded items as PROCESSING positions, ascending, at
-  // excl_pos[excl_indptr[u] .. excl_indptr[u + 1])
-  const int32_t* excl_indptr;
-  const int32_t* excl_pos;
 };
-
-struct FilterLayout {
-  uint32_t a_off, b_off, buf_off, acc_off, bar_off, total;
-};
-__host__ __device__ inline FilterLayout filter_layout(int n_kblocks, int n_stages) {
-  FilterLayout L;
-  L.a_off = 0;                                                    // user blocks 0 and 1, n_kblocks tiles each
-  L.b_off = L.a_off + 2u * static_cast<uint32_t>(n_kblocks) * kATileBytes;
-  L.buf_off = L.b_off + static_cast<uint32_t>(n_stages) * kBTileBytes;
-  L.acc_off = L.buf_off + 2u * kBlockM * kBufEntries * 8u;        // 64 KB of candidate buffers
-  L.bar_off = L.acc_off + 2u * kAccStageBytes;
-  L.total = L.bar_off + 512u;
-  return L;
-}
-// The B ring is organised in TILE slots of n_kblocks k-blocks (16 KB each): one full / one empty barrier per item tile.
-// barriers (uint64): [0..1] a_full (per user block) [2 .. 2+T) b_full [2+T .. 2+2T) b_empty, T = n_stages / n_kblocks
-// tile slots.  b_empty counts the 8 consumer warps of every CTA that received the tile.
-// The item biases are NOT staged: the hot loop needs only the block maximum (one cached global load per tile,
-// prefetched a tile ahead) and the rare admission path reads the few biases it needs through L2.
 
 __device__ __forceinline__ void f_sts64(uint32_t addr, float s, int32_t id) {
   asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(__float_as_uint(s)), "r"(id) : "memory");
@@ -101,10 +60,6 @@ __device__ __forceinline__ void f_lds64(uint32_t addr, float* s, int32_t* id) {
   asm volatile("ld.shared.v2.b32 {%0, %1}, [%2];" : "=r"(a), "=r"(b) : "r"(addr) : "memory");
   *s = __uint_as_float(a);
   *id = static_cast<int32_t>(b);
-}
-// (score desc, id asc): does x come before y ?
-__device__ __forceinline__ bool cand_before(float xs, int32_t xi, float ys, int32_t yi) {
-  return xs > ys || (xs == ys && xi < yi);
 }
 
 // Admission state of the user row a consumer lane owns (filter_owned_row).  Only ever passed to __forceinline__
@@ -177,23 +132,7 @@ __device__ __forceinline__ void compact_finish(const RowFetch& f, int lane, int 
     id = pos < ctx.n_items ? ctx.id_offset + f.perm : 0x7fffffff;
     s = fmaf(s, cs, ubs) + f.bias;   // approximate score: (acc * c + user bias) + item bias
   }
-#pragma unroll
-  for (int size = 2; size <= 32; size <<= 1) {
-#pragma unroll
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      const float os = __shfl_xor_sync(0xffffffffu, s, stride);
-      const int32_t oi = __shfl_xor_sync(0xffffffffu, id, stride);
-      const bool lower = (lane & stride) == 0;           // this lane holds the earlier position of the pair
-      const bool descending = (lane & size) == 0;        // block direction: "before" elements first
-      const bool other_first = cand_before(os, oi, s, id);
-      // earlier position wants the element that comes first in a descending block (and vice versa)
-      const bool take_other = (lower == descending) ? other_first : !other_first;
-      if (take_other) {
-        s = os;
-        id = oi;
-      }
-    }
-  }
+  warp_sort_desc(s, id, lane);
   // lanes now hold the entries in (score desc, id asc) order, sentinels last
   const float kth = __shfl_sync(0xffffffffu, s, k - 1);
   const bool have_k = n >= k;
@@ -366,7 +305,7 @@ __device__ __forceinline__ void sort16_desc(float (&g)[16]) {
 template <int kC, bool kExclude>
 __device__ __forceinline__ void filter_chunk(const float (&acc)[64], int rh, int32_t base, float bmax_scaled,
                                              const float (&bf)[2], float (&tf)[2], uint32_t stage, int lane, int64_t u,
-                                             const FilterParams& p, int32_t& excl_next, RowState& r,
+                                             const SweepParams& p, int32_t& excl_next, RowState& r,
                                              const AdmitCtx& ctx) {
   const bool own = (lane >> 4) == rh;
   bool flag = chunk_frag_pass<kC>(acc, bf, tf);   // == the h0 || h1 of filter_32 over the quad
@@ -386,7 +325,7 @@ __device__ __forceinline__ void filter_chunk(const float (&acc)[64], int rh, int
 // a chunk's test sees the tau the chunks before it left.  Called warp-uniformly.
 template <bool kExclude>
 __device__ __forceinline__ void filter_row_half(const float (&acc)[64], int rh, int32_t pos0, float bmax_scaled,
-                                                uint32_t stage, int lane, int64_t u, const FilterParams& p,
+                                                uint32_t stage, int lane, int64_t u, const SweepParams& p,
                                                 int32_t& excl_next, RowState& r, const AdmitCtx& ctx) {
   float bf[2], tf[2];
   frag_rows(bmax_scaled, rh, lane, bf);
@@ -401,7 +340,7 @@ __device__ __forceinline__ void filter_row_half(const float (&acc)[64], int rh, 
 // lanes of row half rh; excluded positions are masked with the pre-pass cursor `pre_next`.  Called warp-uniformly.
 template <int kC, bool kExclude>
 __device__ __forceinline__ void warm_chunk(const float (&acc)[64], int rh, int32_t pos0, uint32_t stage, int lane,
-                                           int64_t u, const FilterParams& p, int32_t& pre_next, float (&g)[16]) {
+                                           int64_t u, const SweepParams& p, int32_t& pre_next, float (&g)[16]) {
   const bool own = (lane >> 4) == rh;
   stage_warp_chunk<kC>(acc, rh, stage, lane);
   if constexpr (kExclude) {
@@ -416,153 +355,56 @@ __device__ __forceinline__ void warm_chunk(const float (&acc)[64], int rh, int32
 }
 
 
-// kNKB: k-blocks of 64 per row (d_pad / 64).  kCluster: 1, or 2 = clusters of two CTAs that work on two different
-// 256-user groups over the SAME item tiles: each CTA fetches half of every tile and TMA-multicasts it into both CTAs'
-// shared memory, so the L2 -> SM stream of the item operand is halved.  kExclude: mask the items of each row's exclusion
-// list (p.excl_indptr / p.excl_pos) out of the candidate universe, see excl_mask_chunk.
+// Template parameters: see the sweep skeleton (filter_tc.cuh).
 template <int kNKB, int kCluster, bool kExclude = false>
 __global__ void __launch_bounds__(kTcThreads, 1)
 score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_constant__ CUtensorMap map_items,
                     const FilterParams p) {
-  uint8_t* smem = smem_base_1024();
-  const FilterLayout L = filter_layout(kNKB, p.n_stages);
-  const int n_slots = p.n_stages / kNKB;   // B tile slots
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
-  uint64_t* a_full = bars + 0;        // [user block]
-  uint64_t* b_full = bars + 2;
-  uint64_t* b_empty = bars + 2 + n_slots;
-  constexpr uint32_t kSlotBytes = kNKB * kBTileBytes;
-
+  const SweepParams& sweep = p.sweep;
+  const SweepCta cta = sweep_prologue<kNKB, kCluster>(sweep, kBufBytes, &map_users, &map_items);
   const int warp = threadIdx.x / 32;
   const int lane = threadIdx.x % 32;
-  // work unit = (group of kCluster user pairs, item split); CTA `crank` of the cluster takes pair kCluster * g + crank
-  const uint32_t crank = kCluster == 2 ? cluster_ctarank() : 0u;
-  const int n_groups = (p.n_user_pairs + kCluster - 1) / kCluster;
-  const int64_t n_work = static_cast<int64_t>(n_groups) * p.n_splits;
-  const int64_t w_first = blockIdx.x / kCluster, w_step = gridDim.x / kCluster;
-  constexpr uint16_t kClusterMask = (1u << kCluster) - 1u;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&map_items);
-    tma_prefetch_desc(&map_users);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < 2; ++i) mbar_init(a_full + i, 1);
-    for (int i = 0; i < n_slots; ++i) {
-      mbar_init(b_full + i, 1);
-      mbar_init(b_empty + i, 8 * kCluster);   // the consumer warps of all CTAs that received the tile
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  if (kCluster == 2) cluster_sync_all();   // the peer's barriers exist before anything is multicast to them
-
-  // register budget: the producer warpgroup (one issuing warp) needs few, the consumers hold 64 accumulators, a staged
-  // row and the admission state per thread (40 x 128 + 232 x 256 = 64,512 of the 65,536 registers)
-  if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
-    // ===================================== TMA producer ======================================
-    if (warp == 0) {   // warp-uniform control flow, one elected lane issues
-      int ts = 0;
-      uint32_t ts_phase = 0;
-      for (int64_t w = w_first; w < n_work; w += w_step) {
-        const int sp = static_cast<int>(w / n_groups);
-        const int t0 = sp * p.tiles_per_split;
-        const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
-        for (int t = t0; t < t1; ++t) {
-          if (kCluster == 2)
-            mbar_wait_cluster(b_empty + ts, ts_phase ^ 1);
-          else
-            mbar_wait(b_empty + ts, ts_phase ^ 1);
-          if (elect_one()) {
-            mbar_arrive_expect_tx(b_full + ts, kSlotBytes);
-#pragma unroll
-            for (int kb = 0; kb < kNKB; ++kb) {
-              if (kCluster == 2)   // this CTA's half of the tile rows (box = 64 rows), delivered to both CTAs
-                tma_load_2d_multicast(smem + L.b_off + ts * kSlotBytes + kb * kBTileBytes + crank * (kBTileBytes / 2),
-                                      &map_items, b_full + ts, kb * kKBlock,
-                                      t * kBlockN + static_cast<int>(crank) * (kBlockN / 2), kClusterMask, kEvictLast);
-              else
-                tma_load_2d(smem + L.b_off + ts * kSlotBytes + kb * kBTileBytes, &map_items, b_full + ts,
-                            kb * kKBlock, t * kBlockN, kEvictLast);
-            }
-          }
-          __syncwarp();
-          if (++ts == n_slots) {
-            ts = 0;
-            ts_phase ^= 1;
-          }
-        }
-      }
-    }
+  if (sweep_split_registers(warp)) {
+    if (warp == 0) sweep_producer<kNKB, kCluster>(sweep, cta, &map_items);
   } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
     // ================================ consumers: wgmma + admission ================================
     const int group = warp / 4 - 1;
     const int row = filter_owned_row(warp % 4, lane);   // row inside the user block
     const float kNegInf = -__int_as_float(0x7f800000);
     const uint32_t buf_row_addr =   // group g owns user block g of the pair
-        smem_u32(smem + L.buf_off) + static_cast<uint32_t>((group * kBlockM + row) * kBufEntries * 8);
-    const uint32_t stage = smem_u32(smem + L.acc_off) + static_cast<uint32_t>(warp - 4) * kWarpStageBytes;
-    const uint32_t a_base = smem_u32(smem + L.a_off) + group * kNKB * kATileBytes;
-    const uint32_t b_base = smem_u32(smem + L.b_off);
-    const float max_item_norm = __ldg(p.item_stats + 0);
-    const float item_scale = fmaxf(__ldg(p.item_stats + 1), 1e-38f);
-    const float max_item_bias = __ldg(p.item_stats + 2);
-    const AdmitCtx ctx = {p.item_bias, p.item_perm, p.item_id_offset, static_cast<int32_t>(p.n_items), p.k};
+        smem_u32(cta.smem + cta.L.extra_off) + static_cast<uint32_t>((group * kBlockM + row) * kBufEntries * 8);
+    const uint32_t stage = smem_u32(cta.smem + cta.L.acc_off) + static_cast<uint32_t>(warp - 4) * kWarpStageBytes;
+    const uint32_t a_base = smem_u32(cta.smem + cta.L.a_off) + group * kNKB * kATileBytes;
+    const uint32_t b_base = smem_u32(cta.smem + cta.L.b_off);
+    const float max_item_norm = __ldg(sweep.item_stats + 0);
+    const float item_scale = fmaxf(__ldg(sweep.item_stats + 1), 1e-38f);
+    const float max_item_bias = __ldg(sweep.item_stats + 2);
+    const AdmitCtx ctx = {sweep.item_bias, sweep.item_perm, sweep.item_id_offset, static_cast<int32_t>(sweep.n_items),
+                          sweep.k};
     int ts = 0;
     uint32_t ts_phase = 0, witer = 0;
     float acc[64];
 
-    for (int64_t w = w_first; w < n_work; w += w_step) {
-      const int up = static_cast<int>(w % n_groups) * kCluster + static_cast<int>(crank);
-      const int sp = static_cast<int>(w / n_groups);
-      const int t0 = sp * p.tiles_per_split;
-      const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
-      const int64_t ublock_row0 = (static_cast<int64_t>(up) * 2 + group) * kBlockM;
-      const int64_t u = ublock_row0 + row;
-      const bool u_ok = u < p.n_users;
-      const float su = u_ok ? __ldg(p.user_scale + u) : 1.0f;
-      const float ubias = (u_ok && p.user_bias != nullptr) ? __ldg(p.user_bias + u) : 0.0f;
-      const float unorm = u_ok ? __ldg(p.user_norm + u) : 0.0f;
+    for (int64_t w = cta.w_first; w < cta.n_work; w += cta.w_step) {
+      const SweepUnit wu = sweep_unit<kCluster>(sweep, cta, w, group, row);
+      const int64_t u = wu.u;
       RowState rs;
       rs.buf = buf_row_addr;
       rs.cnt = rs.n_res = rs.n_ovf = 0;
       rs.tau = rs.theta = rs.drop_max = kNegInf;
-      rs.ubias = ubias;
-      rs.c = su * item_scale;          // powers of two: exact
-      rs.inv_c = 1.0f / rs.c;
-      // error bound of one approximate score: operand rounding + the fp32 rounding of the two bias adds
-      rs.m3 = kThetaMargins * (kMarginFactor * unorm * max_item_norm + kBiasUlps * (fabsf(ubias) + max_item_bias));
-      int32_t excl_next = 0x7fffffff;   // kExclude: next excluded processing position >= the current chunk
-      if constexpr (kExclude) {
-        if (u_ok && t1 > t0) excl_next = excl_next_at(p.excl_indptr, p.excl_pos, u, t0 * kBlockN);
-      }
+      int32_t excl_next = sweep_row_start<kExclude>(rs, sweep, wu, max_item_norm, item_scale, max_item_bias);
+      sweep_load_user_block<kNKB>(cta, &map_users, wu, group, warp, lane, witer);
 
-      if (t1 > t0) {
-        // this group's user block (hi half, fp16; rows past n_users arrive as zeros) goes to shared memory.  Every
-        // wgmma of the previous unit has completed in all four warps once they pass this barrier.
-        named_barrier_sync(1 + group, kConsumerThreads);
-        if (warp % 4 == 0 && lane == 0) {
-          mbar_arrive_expect_tx(a_full + group, kNKB * kATileBytes);
-#pragma unroll
-          for (int kb = 0; kb < kNKB; ++kb)
-            tma_load_2d(smem + L.a_off + (group * kNKB + kb) * kATileBytes, &map_users, a_full + group, kb * kKBlock,
-                        static_cast<int32_t>(ublock_row0), kEvictFirst);
-        }
-        mbar_wait(a_full + group, witer & 1);
-        ++witer;
-      }
-
-      float bmax_next = t1 > t0 ? __ldg(p.block_bias_max + t0) : 0.0f;
-      for (int t = t0; t < t1; ++t) {
+      float bmax_next = wu.t1 > wu.t0 ? __ldg(sweep.block_bias_max + wu.t0) : 0.0f;
+      for (int t = wu.t0; t < wu.t1; ++t) {
         const float bmax_scaled = bmax_next * rs.inv_c;
-        if (t + 1 < t1) bmax_next = __ldg(p.block_bias_max + t + 1);   // in flight while this tile is filtered
-        mbar_wait(b_full + ts, ts_phase);
-        const uint32_t b_slot = b_base + ts * kSlotBytes;
+        if (t + 1 < wu.t1) bmax_next = __ldg(sweep.block_bias_max + t + 1);   // in flight while this tile is filtered
+        mbar_wait(cta.b_full + ts, ts_phase);
+        const uint32_t b_slot = b_base + ts * (kNKB * kBTileBytes);
         const int32_t pos0 = t * kBlockN;
-        if (t == t0 && p.block_bias_min != nullptr) {
-          const float bmin = __ldg(p.block_bias_min + t0);   // the same for the whole CTA: warp-uniform branch
+        if (t == wu.t0 && p.block_bias_min != nullptr) {
+          const float bmin = __ldg(p.block_bias_min + wu.t0);   // the same for the whole CTA: warp-uniform branch
           if (bmin > kNegInf) {
             float g[16];
             // the tile is filtered again below: the pre-pass masks with a copy of the cursor
@@ -570,16 +412,16 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
 #pragma unroll
             for (int rh = 0; rh < 2; ++rh) {   // each lane's row is in one row half: its 16 groups come from that one
               filter_mma_rows<kNKB>(acc, a_base, b_slot, rh);
-              warm_chunk<0, kExclude>(acc, rh, pos0, stage, lane, u, p, pre_next, g);
-              warm_chunk<1, kExclude>(acc, rh, pos0, stage, lane, u, p, pre_next, g);
-              warm_chunk<2, kExclude>(acc, rh, pos0, stage, lane, u, p, pre_next, g);
-              warm_chunk<3, kExclude>(acc, rh, pos0, stage, lane, u, p, pre_next, g);
+              warm_chunk<0, kExclude>(acc, rh, pos0, stage, lane, u, sweep, pre_next, g);
+              warm_chunk<1, kExclude>(acc, rh, pos0, stage, lane, u, sweep, pre_next, g);
+              warm_chunk<2, kExclude>(acc, rh, pos0, stage, lane, u, sweep, pre_next, g);
+              warm_chunk<3, kExclude>(acc, rh, pos0, stage, lane, u, sweep, pre_next, g);
             }
             sort16_desc(g);
             float a_k = g[0];
 #pragma unroll
-            for (int i = 1; i < 16; ++i) a_k = (i < p.k) ? g[i] : a_k;   // g[k - 1]: the k-th largest group maximum
-            const float th0 = (fmaf(a_k, rs.c, ubias) + bmin) - rs.m3;
+            for (int i = 1; i < 16; ++i) a_k = (i < sweep.k) ? g[i] : a_k;   // g[k - 1]: the k-th largest group maximum
+            const float th0 = (fmaf(a_k, rs.c, rs.ubias) + bmin) - rs.m3;
             if (th0 == th0) {   // not NaN (infinite biases / margins): otherwise the sweep starts from -inf as before
               rs.theta = th0;
               set_tau(rs);
@@ -589,31 +431,18 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
 #pragma unroll 1
         for (int rh = 0; rh < 2; ++rh) {
           filter_mma_rows<kNKB>(acc, a_base, b_slot, rh);
-          if (rh == 1) {   // the tile's last MMAs of this warp are complete: release the B slot in every CTA that got it
-            __syncwarp();
-            if (lane == 0) {
-              if (kCluster == 2) {
-#pragma unroll
-                for (uint32_t r = 0; r < kCluster; ++r) mbar_arrive_cluster(b_empty + ts, r);
-              } else {
-                mbar_arrive(b_empty + ts);
-              }
-            }
-          }
+          if (rh == 1) sweep_release_slot<kCluster>(cta, ts, lane);   // the tile's last MMAs of this warp are complete
           // kExclude: one vote per row half.  Only a row half in which some owner's next excluded position lies runs
           // the exclusion test of every chunk; every other one (all of them with empty lists) runs the exclusion-free
           // code, which decides exactly as the exclusion test would there.
           bool excl_rh = false;
           if constexpr (kExclude) excl_rh = __any_sync(0xffffffffu, (lane >> 4) == rh && excl_next < pos0 + kBlockN);
           if (excl_rh)
-            filter_row_half<kExclude>(acc, rh, pos0, bmax_scaled, stage, lane, u, p, excl_next, rs, ctx);
+            filter_row_half<kExclude>(acc, rh, pos0, bmax_scaled, stage, lane, u, sweep, excl_next, rs, ctx);
           else
-            filter_row_half<false>(acc, rh, pos0, bmax_scaled, stage, lane, u, p, excl_next, rs, ctx);
+            filter_row_half<false>(acc, rh, pos0, bmax_scaled, stage, lane, u, sweep, excl_next, rs, ctx);
         }
-        if (++ts == n_slots) {
-          ts = 0;
-          ts_phase ^= 1;
-        }
+        sweep_ring_advance(ts, ts_phase, cta.n_slots);
         // A compaction waits one L2 round trip for the biases / item ids of its new entries -- during which, in the
         // middle of a tile, the warp's 32 rows stand still.  So rows whose buffer is filling up are compacted HERE, at
         // the end of the tile, where the round trip overlaps the other warpgroup's MMAs.  The mid-tile path remains for
@@ -627,8 +456,8 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
 
       // end of the item range: final compaction of every row of this warp, then emit the survivors
       compact_rows(0xffffffffu, lane, rs, ctx);
-      if (u_ok) {
-        const int64_t base = u * p.n_splits + sp;
+      if (wu.u_ok) {
+        const int64_t base = u * sweep.n_splits + wu.sp;
         float* os = p.cand_score + base * kKeepMax;
         int32_t* oi = p.cand_item + base * kKeepMax;
         for (int e = 0; e < kKeepMax; ++e) {
@@ -638,10 +467,7 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
           os[e] = s;
           oi[e] = id;
         }
-        // every excluded item has an approximate score <= this; a NaN (inf - inf with infinite biases) must not read
-        // as "nothing was excluded": +inf makes the certificate fail and the row goes through the exact kernel
-        const bool th_nan = rs.theta != rs.theta || rs.drop_max != rs.drop_max;
-        p.row_theta[base] = th_nan ? __int_as_float(0x7f800000) : fmaxf(rs.theta, rs.drop_max);
+        sweep_store_theta(sweep, base, rs);
       }
       __syncwarp();
     }
@@ -780,50 +606,27 @@ int exclusion_positions(const int32_t* item_perm, int64_t n_items, int32_t* inv_
   return TRK_OK;
 }
 
+// (the kernel of one instantiation, for launch_sweep)
+template <int kNKB, int kCluster, bool kExclude>
+struct FilterKernel {
+  static constexpr auto fn = score_filter_kernel<kNKB, kCluster, kExclude>;
+};
+
 int score_filter_f16(const void* user_split, const float* user_scale, const float* user_bias,
                      const float* user_norm, const void* item_hi, const float* item_stats, const float* item_bias,
                      const float* block_bias_max, const float* block_bias_min, const int32_t* item_perm,
                      int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k, int32_t n_splits,
                      int32_t item_id_offset, float* cand_score, int32_t* cand_item, float* row_theta,
                      const int32_t* excl_indptr, const int32_t* excl_pos, cudaStream_t stream) {
-  TRK_CHECK_ARG(user_split && user_scale && user_norm && item_hi && item_stats && item_bias && block_bias_max,
-                "score_filter: null input");
-  TRK_CHECK_ARG((excl_indptr == nullptr) == (excl_pos == nullptr), "score_filter: excl_indptr and excl_pos go together");
   TRK_CHECK_ARG(cand_score && cand_item && row_theta, "score_filter: null output");
-  TRK_CHECK_ARG(n_users >= 1 && n_items >= 1 && n_splits >= 1, "score_filter: empty shape");
-  TRK_CHECK_ARG(n_users < (1ll << 31) && n_items < (1ll << 31) - 512, "score_filter: shape exceeds int32 indexing");
-  if (d_pad != 64 && d_pad != 128) {
-    set_error("score_filter: d_pad=%d not supported (64 or 128)", d_pad);
-    return TRK_ERR_UNSUPPORTED;
-  }
   if (k < 1 || k > kFilterMaxK) {
     set_error("score_filter: k=%d outside [1, %d]", k, kFilterMaxK);
     return TRK_ERR_UNSUPPORTED;
   }
-  TRK_CHECK_ARG(reinterpret_cast<uintptr_t>(user_split) % 16 == 0 && reinterpret_cast<uintptr_t>(item_hi) % 16 == 0 &&
-                    reinterpret_cast<uintptr_t>(item_bias) % 16 == 0,
-                "score_filter: operands must be 16-byte aligned");
+  TRK_CHECK_ARG(reinterpret_cast<uintptr_t>(item_bias) % 16 == 0, "score_filter: operands must be 16-byte aligned");
 
   FilterParams p;
-  p.user_split = static_cast<const __half*>(user_split);
-  p.d_pad = d_pad;
-  p.user_scale = user_scale;
-  p.user_bias = user_bias;
-  p.user_norm = user_norm;
-  p.item_bias = item_bias;
-  p.block_bias_max = block_bias_max;
   p.block_bias_min = block_bias_min;
-  p.item_perm = item_perm;
-  p.item_stats = item_stats;
-  p.n_users = n_users;
-  p.n_items = n_items;
-  p.n_kblocks = d_pad / kKBlock;
-  p.k = k;
-  p.n_tiles = static_cast<int32_t>(ceil_div(n_items, kBlockN));
-  p.n_splits = n_splits;
-  p.tiles_per_split = static_cast<int32_t>(ceil_div(p.n_tiles, n_splits));
-  p.n_user_pairs = static_cast<int32_t>(ceil_div(n_users, 2 * kBlockM));
-  p.item_id_offset = item_id_offset;
   // Tile-end compaction trigger.  TRK_FILTER_TILE_END_TRIGGER (probe knob) sets it; kBufEntries or more turns the
   // tile-end pass off (no buffer holds more than kBufEntries entries).
   p.tile_end_trigger = 26;
@@ -834,90 +637,9 @@ int score_filter_f16(const void* user_split, const float* user_scale, const floa
   }
   p.cand_score = cand_score;
   p.cand_item = cand_item;
-  p.row_theta = row_theta;
-  p.excl_indptr = excl_indptr;
-  p.excl_pos = excl_pos;
-  const bool excl = excl_indptr != nullptr;
-  CUtensorMap map_users, map_items;
-  int rc;
-  p.n_stages = 0;
-  for (int s = kMaxStages; s >= 2; --s)
-    if (s % p.n_kblocks == 0 && filter_layout(p.n_kblocks, s).total + kSmemAlignSlack <= kSmemLimit) {
-      p.n_stages = s;
-      break;
-    }
-  TRK_CHECK_ARG(p.n_stages >= 2 * p.n_kblocks, "score_filter: shared memory budget exceeded");
-  const uint32_t smem_bytes = filter_layout(p.n_kblocks, p.n_stages).total + kSmemAlignSlack;
-
-  // Launch form: clusters of two CTAs sharing every item tile through TMA multicast (default when the device can keep
-  // (almost) all SMs busy with 2-CTA clusters), else independent CTAs.  TRK_FILTER_CLUSTER=1|2 forces one.
-  int cluster = 2;
-  {
-    const char* env = getenv("TRK_FILTER_CLUSTER");
-    if (env != nullptr && (atoi(env) == 1 || atoi(env) == 2)) cluster = atoi(env);
-  }
-  auto kernel2 = excl ? (p.n_kblocks == 2 ? score_filter_kernel<2, 2, true> : score_filter_kernel<1, 2, true>)
-                     : (p.n_kblocks == 2 ? score_filter_kernel<2, 2> : score_filter_kernel<1, 2>);
-  auto kernel1 = excl ? (p.n_kblocks == 2 ? score_filter_kernel<2, 1, true> : score_filter_kernel<1, 1, true>)
-                     : (p.n_kblocks == 2 ? score_filter_kernel<2, 1> : score_filter_kernel<1, 1>);
-  cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[1];
-  int max_clusters = 0;
-  if (cluster == 2) {
-    TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel2, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    cfg.gridDim = dim3(2);
-    cfg.blockDim = dim3(kTcThreads);
-    cfg.dynamicSmemBytes = smem_bytes;
-    cfg.stream = stream;
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    // the answer depends on (device, kernel, shared memory) only: asked once per device and kernel variant
-    // (n_kblocks x exclusion)
-    static int cached_clusters[64][4];
-    static bool cached_valid[64][4];
-    int device = 0;
-    TRK_CHECK_CUDA(cudaGetDevice(&device));
-    const int variant = (p.n_kblocks == 2 ? 1 : 0) + (excl ? 2 : 0);
-    if (device >= 0 && device < 64 && cached_valid[device][variant]) {
-      max_clusters = cached_clusters[device][variant];
-    } else {
-      if (cudaOccupancyMaxActiveClusters(&max_clusters, kernel2, &cfg) != cudaSuccess) {
-        (void)cudaGetLastError();
-        max_clusters = 0;
-      }
-      if (device >= 0 && device < 64) {
-        cached_clusters[device][variant] = max_clusters;
-        cached_valid[device][variant] = true;
-      }
-    }
-    const char* env = getenv("TRK_FILTER_CLUSTER");
-    if (max_clusters * 2 < sm_count() - 8 && env == nullptr) cluster = 1;   // too many SMs would sit idle
-    if (max_clusters < 1) cluster = 1;
-  }
-  // fp16 operands, boxes of one k-block: the items [n_items, d_pad] (each CTA of a cluster fetches half of a tile) and
-  // the hi half of the split user rows [n_users, 2 d_pad]
-  rc = encode_tiled_2d(&map_items, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, item_hi, d_pad, n_items, 2 * d_pad, kKBlock,
-                       kBlockN / cluster, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
-  if (rc != TRK_OK) return rc;
-  rc = encode_tiled_2d(&map_users, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, user_split, d_pad, n_users, 4 * d_pad, kKBlock,
-                       kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
-  if (rc != TRK_OK) return rc;
-  if (cluster == 2) {
-    const int64_t n_work = ceil_div(static_cast<int64_t>(p.n_user_pairs), 2) * n_splits;
-    const int n_clusters = static_cast<int>(n_work < max_clusters ? n_work : max_clusters);
-    cfg.gridDim = dim3(static_cast<unsigned>(2 * n_clusters));
-    TRK_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel2, map_users, map_items, p));
-  } else {
-    TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel1, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    const int grid = capped_grid(static_cast<int64_t>(p.n_user_pairs) * n_splits, 1);
-    kernel1<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, p);
-  }
-  TRK_CHECK_LAUNCH();
-  return TRK_OK;
+  return launch_sweep<FilterKernel>("score_filter", p, kBufBytes, user_split, user_scale, user_bias, user_norm, item_hi,
+                                    item_stats, item_bias, block_bias_max, item_perm, n_users, n_items, d_pad, k,
+                                    n_splits, item_id_offset, row_theta, excl_indptr, excl_pos, stream);
 }
 
 }  // namespace trk

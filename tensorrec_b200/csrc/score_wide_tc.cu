@@ -1,7 +1,7 @@
-// Wide form of the one-pass tensor-core filter (score_filter_tc.cu, DESIGN §3.3): the same warp-specialised CTA, the
-// same fp16 "hi" operands in descending-bias order, the same register fast path on the wgmma fragments and the same
-// per-warp staging of flagged chunks -- but every user row keeps its candidates in a list in GLOBAL memory, so k is not
-// bounded by a 32-entry shared-memory buffer: 32 < k <= kWideMaxK.
+// Wide form of the one-pass tensor-core filter (score_filter_tc.cu, DESIGN §3.3): the same sweep skeleton
+// (filter_tc.cuh), the same fp16 "hi" operands in descending-bias order, the same register fast path on the wgmma
+// fragments and the same per-warp staging of flagged chunks -- but every user row keeps its candidates in a list in
+// GLOBAL memory, so k is not bounded by a 32-entry shared-memory buffer: 32 < k <= kWideMaxK.
 //
 // Per (row, item split) the list holds up to `cap` = 2 keep entries, keep = k + max(k / 2, 32) rounded up to 32.  The
 // owner lane appends (raw accumulator, processing position) on the rare admission path; when a row's list could not
@@ -19,8 +19,6 @@
 // Warm start: none.  The sweep starts at theta = -inf and the first compaction sets the threshold.  That costs every
 // row `cap` appends at the start of each work unit -- a handful of tiles out of the ~8K of a 1M-item sweep -- and keeps
 // the certificate argument of §3 word for word: theta only ever comes from admitted (eligible) items.
-#include <stdlib.h>
-
 #include "filter_tc.cuh"
 
 namespace trk {
@@ -30,44 +28,13 @@ constexpr int kWideMaxK = 1024;
 __host__ __device__ inline int wide_keep(int k) { return static_cast<int>(round_up(k + (k / 2 > 32 ? k / 2 : 32), 32)); }
 
 struct WideParams {
-  const float* user_scale;
-  const float* user_bias;      // may be null
-  const float* user_norm;      // |u|_2 per user
-  const float* item_bias;      // [padded items] in processing order, padding = -inf
-  const float* block_bias_max; // max item bias of every block of 128 processing positions
-  const int32_t* item_perm;    // processing position -> local item index, or null = identity
-  const float* item_stats;     // [0] = max_j |i_j|_2, [1] = global item scale, [2] = max_j |bias_j|
-  int64_t n_users;
-  int64_t n_items;
-  int32_t n_stages;
-  int32_t k;
+  SweepParams sweep;
   int32_t keep;                // entries a compaction keeps at most
   int32_t cap;                 // list capacity per (row, split): 2 keep
-  int32_t n_splits;
-  int32_t tiles_per_split;
-  int32_t n_tiles;
-  int32_t n_user_pairs;
-  int32_t item_id_offset;
   float* list_score;           // [n_users, n_splits, cap] approximate scores
   int32_t* list_item;          // [n_users, n_splits, cap] global item ids
   int32_t* list_count;         // [n_users, n_splits] entries of each list (<= keep at the end)
-  float* row_theta;            // [n_users, n_splits] max(theta, drop_max) (certified by select_wide_kernel)
-  const int32_t* excl_indptr;  // exclusion lists as processing positions (kExclude), see score_filter_tc.cu
-  const int32_t* excl_pos;
 };
-
-struct WideLayout {
-  uint32_t a_off, b_off, acc_off, bar_off, total;
-};
-__host__ __device__ inline WideLayout wide_layout(int n_kblocks, int n_stages) {
-  WideLayout L;
-  L.a_off = 0;
-  L.b_off = L.a_off + 2u * static_cast<uint32_t>(n_kblocks) * kATileBytes;
-  L.acc_off = L.b_off + static_cast<uint32_t>(n_stages) * kBTileBytes;
-  L.bar_off = L.acc_off + 2u * kAccStageBytes;
-  L.total = L.bar_off + 512u;
-  return L;
-}
 
 // Admission state of the row a consumer lane owns (filter_owned_row); the list itself is in global memory.
 struct WideRow {
@@ -254,7 +221,7 @@ __device__ __forceinline__ void wide_chunk(const float (&acc0)[32], const float 
   if (!__any_sync(0xffffffffu, flag)) return;
   stage_warp_chunk<kC>(acc0, acc1, stage, lane);
   if constexpr (kExclude) {
-    if (excl_next < base + 32) excl_next = excl_mask_chunk(p.excl_indptr, p.excl_pos, u, base, stage, lane);
+    if (excl_next < base + 32) excl_next = excl_mask_chunk(p.sweep.excl_indptr, p.sweep.excl_pos, u, base, stage, lane);
   }
   uint32_t v[32];
   load_staged_row(stage, lane, v);
@@ -262,176 +229,75 @@ __device__ __forceinline__ void wide_chunk(const float (&acc0)[32], const float 
   wide_32(v, base, bmax_scaled, lane, r, ctx, p.keep, p.cap, hist);
 }
 
-// Template parameters as score_filter_kernel's.
+// Template parameters: see the sweep skeleton (filter_tc.cuh).
 template <int kNKB, int kCluster, bool kExclude>
 __global__ void __launch_bounds__(kTcThreads, 1)
 score_wide_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_constant__ CUtensorMap map_items,
                   const WideParams p) {
-  uint8_t* smem = smem_base_1024();
-  const WideLayout L = wide_layout(kNKB, p.n_stages);
-  const int n_slots = p.n_stages / kNKB;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
-  uint64_t* a_full = bars + 0;
-  uint64_t* b_full = bars + 2;
-  uint64_t* b_empty = bars + 2 + n_slots;
-  constexpr uint32_t kSlotBytes = kNKB * kBTileBytes;
-
+  const SweepParams& sweep = p.sweep;
+  const SweepCta cta = sweep_prologue<kNKB, kCluster>(sweep, 0u, &map_users, &map_items);
   const int warp = threadIdx.x / 32;
   const int lane = threadIdx.x % 32;
-  const uint32_t crank = kCluster == 2 ? cluster_ctarank() : 0u;
-  const int n_groups = (p.n_user_pairs + kCluster - 1) / kCluster;
-  const int64_t n_work = static_cast<int64_t>(n_groups) * p.n_splits;
-  const int64_t w_first = blockIdx.x / kCluster, w_step = gridDim.x / kCluster;
-  constexpr uint16_t kClusterMask = (1u << kCluster) - 1u;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&map_items);
-    tma_prefetch_desc(&map_users);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < 2; ++i) mbar_init(a_full + i, 1);
-    for (int i = 0; i < n_slots; ++i) {
-      mbar_init(b_full + i, 1);
-      mbar_init(b_empty + i, 8 * kCluster);
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  if (kCluster == 2) cluster_sync_all();
-
-  if (warp < 4) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
-    // ===================================== TMA producer ======================================
-    if (warp == 0) {
-      int ts = 0;
-      uint32_t ts_phase = 0;
-      for (int64_t w = w_first; w < n_work; w += w_step) {
-        const int sp = static_cast<int>(w / n_groups);
-        const int t0 = sp * p.tiles_per_split;
-        const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
-        for (int t = t0; t < t1; ++t) {
-          if (kCluster == 2)
-            mbar_wait_cluster(b_empty + ts, ts_phase ^ 1);
-          else
-            mbar_wait(b_empty + ts, ts_phase ^ 1);
-          if (elect_one()) {
-            mbar_arrive_expect_tx(b_full + ts, kSlotBytes);
-#pragma unroll
-            for (int kb = 0; kb < kNKB; ++kb) {
-              if (kCluster == 2)
-                tma_load_2d_multicast(smem + L.b_off + ts * kSlotBytes + kb * kBTileBytes + crank * (kBTileBytes / 2),
-                                      &map_items, b_full + ts, kb * kKBlock,
-                                      t * kBlockN + static_cast<int>(crank) * (kBlockN / 2), kClusterMask, kEvictLast);
-              else
-                tma_load_2d(smem + L.b_off + ts * kSlotBytes + kb * kBTileBytes, &map_items, b_full + ts,
-                            kb * kKBlock, t * kBlockN, kEvictLast);
-            }
-          }
-          __syncwarp();
-          if (++ts == n_slots) {
-            ts = 0;
-            ts_phase ^= 1;
-          }
-        }
-      }
-    }
+  if (sweep_split_registers(warp)) {
+    if (warp == 0) sweep_producer<kNKB, kCluster>(sweep, cta, &map_items);
   } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
     // ================================ consumers: wgmma + admission ================================
     const int group = warp / 4 - 1;
     const int row = filter_owned_row(warp % 4, lane);
     const float kNegInf = -__int_as_float(0x7f800000);
-    const uint32_t stage = smem_u32(smem + L.acc_off) + static_cast<uint32_t>(warp - 4) * kWarpStageBytes;
-    uint32_t* hist = reinterpret_cast<uint32_t*>(smem + L.acc_off + static_cast<uint32_t>(warp - 4) * kWarpStageBytes);
-    const uint32_t a_base = smem_u32(smem + L.a_off) + group * kNKB * kATileBytes;
-    const uint32_t b_base = smem_u32(smem + L.b_off);
-    const float max_item_norm = __ldg(p.item_stats + 0);
-    const float item_scale = fmaxf(__ldg(p.item_stats + 1), 1e-38f);
-    const float max_item_bias = __ldg(p.item_stats + 2);
-    const AdmitCtx ctx = {p.item_bias, p.item_perm, p.item_id_offset, static_cast<int32_t>(p.n_items), p.k};
+    const uint32_t stage = smem_u32(cta.smem + cta.L.acc_off) + static_cast<uint32_t>(warp - 4) * kWarpStageBytes;
+    uint32_t* hist =
+        reinterpret_cast<uint32_t*>(cta.smem + cta.L.acc_off + static_cast<uint32_t>(warp - 4) * kWarpStageBytes);
+    const uint32_t a_base = smem_u32(cta.smem + cta.L.a_off) + group * kNKB * kATileBytes;
+    const uint32_t b_base = smem_u32(cta.smem + cta.L.b_off);
+    const float max_item_norm = __ldg(sweep.item_stats + 0);
+    const float item_scale = fmaxf(__ldg(sweep.item_stats + 1), 1e-38f);
+    const float max_item_bias = __ldg(sweep.item_stats + 2);
+    const AdmitCtx ctx = {sweep.item_bias, sweep.item_perm, sweep.item_id_offset, static_cast<int32_t>(sweep.n_items),
+                          sweep.k};
     int ts = 0;
     uint32_t ts_phase = 0, witer = 0;
     float acc0[32], acc1[32];
 
-    for (int64_t w = w_first; w < n_work; w += w_step) {
-      const int up = static_cast<int>(w % n_groups) * kCluster + static_cast<int>(crank);
-      const int sp = static_cast<int>(w / n_groups);
-      const int t0 = sp * p.tiles_per_split;
-      const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
-      const int64_t ublock_row0 = (static_cast<int64_t>(up) * 2 + group) * kBlockM;
-      const int64_t u = ublock_row0 + row;
-      const bool u_ok = u < p.n_users;
-      const float su = u_ok ? __ldg(p.user_scale + u) : 1.0f;
-      const float ubias = (u_ok && p.user_bias != nullptr) ? __ldg(p.user_bias + u) : 0.0f;
-      const float unorm = u_ok ? __ldg(p.user_norm + u) : 0.0f;
-      const int64_t list = u_ok ? (u * p.n_splits + sp) : 0;
+    for (int64_t w = cta.w_first; w < cta.n_work; w += cta.w_step) {
+      const SweepUnit wu = sweep_unit<kCluster>(sweep, cta, w, group, row);
+      const int64_t u = wu.u;
+      const int64_t list = wu.u_ok ? (u * sweep.n_splits + wu.sp) : 0;
       WideRow rs;
       rs.ls = p.list_score + list * p.cap;
       rs.li = p.list_item + list * p.cap;
       rs.cnt = rs.n_res = rs.n_ovf = 0;
       rs.theta = rs.drop_max = kNegInf;
-      rs.tau = u_ok ? kNegInf : __int_as_float(0x7f800000);   // rows past n_users admit nothing (they have no list)
-      rs.ubias = ubias;
-      rs.c = su * item_scale;
-      rs.inv_c = 1.0f / rs.c;
-      rs.m3 = kThetaMargins * (kMarginFactor * unorm * max_item_norm + kBiasUlps * (fabsf(ubias) + max_item_bias));
-      int32_t excl_next = 0x7fffffff;
-      if constexpr (kExclude) {
-        if (u_ok && t1 > t0) excl_next = excl_next_at(p.excl_indptr, p.excl_pos, u, t0 * kBlockN);
-      }
+      rs.tau = wu.u_ok ? kNegInf : __int_as_float(0x7f800000);   // rows past n_users admit nothing (they have no list)
+      int32_t excl_next = sweep_row_start<kExclude>(rs, sweep, wu, max_item_norm, item_scale, max_item_bias);
+      sweep_load_user_block<kNKB>(cta, &map_users, wu, group, warp, lane, witer);
 
-      if (t1 > t0) {
-        named_barrier_sync(1 + group, kConsumerThreads);
-        if (warp % 4 == 0 && lane == 0) {
-          mbar_arrive_expect_tx(a_full + group, kNKB * kATileBytes);
-#pragma unroll
-          for (int kb = 0; kb < kNKB; ++kb)
-            tma_load_2d(smem + L.a_off + (group * kNKB + kb) * kATileBytes, &map_users, a_full + group, kb * kKBlock,
-                        static_cast<int32_t>(ublock_row0), kEvictFirst);
-        }
-        mbar_wait(a_full + group, witer & 1);
-        ++witer;
-      }
-
-      float bmax_next = t1 > t0 ? __ldg(p.block_bias_max + t0) : 0.0f;
-      for (int t = t0; t < t1; ++t) {
+      float bmax_next = wu.t1 > wu.t0 ? __ldg(sweep.block_bias_max + wu.t0) : 0.0f;
+      for (int t = wu.t0; t < wu.t1; ++t) {
         const float bmax_scaled = bmax_next * rs.inv_c;
-        if (t + 1 < t1) bmax_next = __ldg(p.block_bias_max + t + 1);
-        mbar_wait(b_full + ts, ts_phase);
-        const uint32_t b_slot = b_base + ts * kSlotBytes;
+        if (t + 1 < wu.t1) bmax_next = __ldg(sweep.block_bias_max + t + 1);
+        mbar_wait(cta.b_full + ts, ts_phase);
+        const uint32_t b_slot = b_base + ts * (kNKB * kBTileBytes);
         const int32_t pos0 = t * kBlockN;
 #pragma unroll 1
         for (int h = 0; h < 2; ++h) {
           filter_mma_half<kNKB>(acc0, acc1, a_base, b_slot, h);
-          if (h == 1) {
-            __syncwarp();
-            if (lane == 0) {
-              if (kCluster == 2) {
-#pragma unroll
-                for (uint32_t r = 0; r < kCluster; ++r) mbar_arrive_cluster(b_empty + ts, r);
-              } else {
-                mbar_arrive(b_empty + ts);
-              }
-            }
-          }
+          if (h == 1) sweep_release_slot<kCluster>(cta, ts, lane);
           const float amax0 = chunk_row_max<0>(acc0, acc1, lane), amax1 = chunk_row_max<1>(acc0, acc1, lane);
           wide_chunk<0, kExclude>(acc0, acc1, amax0, pos0 + h * 64, bmax_scaled, stage, lane, u, p, excl_next, rs, ctx,
                                   hist);
           wide_chunk<1, kExclude>(acc0, acc1, amax1, pos0 + h * 64 + 32, bmax_scaled, stage, lane, u, p, excl_next, rs,
                                   ctx, hist);
         }
-        if (++ts == n_slots) {
-          ts = 0;
-          ts_phase ^= 1;
-        }
+        sweep_ring_advance(ts, ts_phase, cta.n_slots);
       }
 
       // end of the item range: one last compaction of every row (resolves the raw entries, count <= keep)
-      wide_compact_rows(__ballot_sync(0xffffffffu, u_ok), lane, rs, ctx, p.keep, hist);
-      if (u_ok) {
+      wide_compact_rows(__ballot_sync(0xffffffffu, wu.u_ok), lane, rs, ctx, p.keep, hist);
+      if (wu.u_ok) {
         p.list_count[list] = rs.cnt;
-        const bool th_nan = rs.theta != rs.theta || rs.drop_max != rs.drop_max;
-        p.row_theta[list] = th_nan ? __int_as_float(0x7f800000) : fmaxf(rs.theta, rs.drop_max);
+        sweep_store_theta(sweep, list, rs);
       }
       __syncwarp();
     }
@@ -447,114 +313,32 @@ score_wide_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_co
 int score_wide_max_k() { return kWideMaxK; }
 int score_wide_list_capacity(int32_t k) { return 2 * wide_keep(k); }
 
+template <int kNKB, int kCluster, bool kExclude>
+struct WideKernel {
+  static constexpr auto fn = score_wide_kernel<kNKB, kCluster, kExclude>;
+};
+
 int score_wide_f16(const void* user_split, const float* user_scale, const float* user_bias, const float* user_norm,
                    const void* item_hi, const float* item_stats, const float* item_bias, const float* block_bias_max,
                    const int32_t* item_perm, int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k,
                    int32_t n_splits, int32_t item_id_offset, float* list_score, int32_t* list_item,
                    int32_t* list_count, float* row_theta, const int32_t* excl_indptr, const int32_t* excl_pos,
                    cudaStream_t stream) {
-  TRK_CHECK_ARG(user_split && user_scale && user_norm && item_hi && item_stats && item_bias && block_bias_max,
-                "score_wide: null input");
-  TRK_CHECK_ARG((excl_indptr == nullptr) == (excl_pos == nullptr), "score_wide: excl_indptr and excl_pos go together");
   TRK_CHECK_ARG(list_score && list_item && list_count && row_theta, "score_wide: null output");
-  TRK_CHECK_ARG(n_users >= 1 && n_items >= 1 && n_splits >= 1, "score_wide: empty shape");
-  TRK_CHECK_ARG(n_users < (1ll << 31) && n_items < (1ll << 31) - 512, "score_wide: shape exceeds int32 indexing");
-  if (d_pad != 64 && d_pad != 128) {
-    set_error("score_wide: d_pad=%d not supported (64 or 128)", d_pad);
-    return TRK_ERR_UNSUPPORTED;
-  }
   if (k < 1 || k > kWideMaxK) {
     set_error("score_wide: k=%d outside [1, %d]", k, kWideMaxK);
     return TRK_ERR_UNSUPPORTED;
   }
-  TRK_CHECK_ARG(reinterpret_cast<uintptr_t>(user_split) % 16 == 0 && reinterpret_cast<uintptr_t>(item_hi) % 16 == 0,
-                "score_wide: operands must be 16-byte aligned");
 
   WideParams p;
-  p.user_scale = user_scale;
-  p.user_bias = user_bias;
-  p.user_norm = user_norm;
-  p.item_bias = item_bias;
-  p.block_bias_max = block_bias_max;
-  p.item_perm = item_perm;
-  p.item_stats = item_stats;
-  p.n_users = n_users;
-  p.n_items = n_items;
-  p.k = k;
   p.keep = wide_keep(k);
   p.cap = 2 * p.keep;
-  p.n_tiles = static_cast<int32_t>(ceil_div(n_items, kBlockN));
-  p.n_splits = n_splits;
-  p.tiles_per_split = static_cast<int32_t>(ceil_div(p.n_tiles, n_splits));
-  p.n_user_pairs = static_cast<int32_t>(ceil_div(n_users, 2 * kBlockM));
-  p.item_id_offset = item_id_offset;
   p.list_score = list_score;
   p.list_item = list_item;
   p.list_count = list_count;
-  p.row_theta = row_theta;
-  p.excl_indptr = excl_indptr;
-  p.excl_pos = excl_pos;
-  const bool excl = excl_indptr != nullptr;
-  const int n_kblocks = d_pad / kKBlock;
-  p.n_stages = 0;
-  for (int s = kMaxStages; s >= 2; --s)
-    if (s % n_kblocks == 0 && wide_layout(n_kblocks, s).total + kSmemAlignSlack <= kSmemLimit) {
-      p.n_stages = s;
-      break;
-    }
-  TRK_CHECK_ARG(p.n_stages >= 2 * n_kblocks, "score_wide: shared memory budget exceeded");
-  const uint32_t smem_bytes = wide_layout(n_kblocks, p.n_stages).total + kSmemAlignSlack;
-
-  // launch form as score_filter_f16: 2-CTA clusters sharing every item tile when the device can keep (almost) all SMs
-  // busy with them, else independent CTAs; TRK_FILTER_CLUSTER=1|2 forces one
-  int cluster = 2;
-  const char* env = getenv("TRK_FILTER_CLUSTER");
-  if (env != nullptr && (atoi(env) == 1 || atoi(env) == 2)) cluster = atoi(env);
-  auto kernel2 = excl ? (n_kblocks == 2 ? score_wide_kernel<2, 2, true> : score_wide_kernel<1, 2, true>)
-                      : (n_kblocks == 2 ? score_wide_kernel<2, 2, false> : score_wide_kernel<1, 2, false>);
-  auto kernel1 = excl ? (n_kblocks == 2 ? score_wide_kernel<2, 1, true> : score_wide_kernel<1, 1, true>)
-                      : (n_kblocks == 2 ? score_wide_kernel<2, 1, false> : score_wide_kernel<1, 1, false>);
-  cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[1];
-  int max_clusters = 0;
-  if (cluster == 2) {
-    TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel2, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    cfg.gridDim = dim3(2);
-    cfg.blockDim = dim3(kTcThreads);
-    cfg.dynamicSmemBytes = smem_bytes;
-    cfg.stream = stream;
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    if (cudaOccupancyMaxActiveClusters(&max_clusters, kernel2, &cfg) != cudaSuccess) {
-      (void)cudaGetLastError();
-      max_clusters = 0;
-    }
-    if (max_clusters * 2 < sm_count() - 8 && env == nullptr) cluster = 1;
-    if (max_clusters < 1) cluster = 1;
-  }
-  CUtensorMap map_users, map_items;
-  int rc = encode_tiled_2d(&map_items, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, item_hi, d_pad, n_items, 2 * d_pad, kKBlock,
-                           kBlockN / cluster, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
-  if (rc != TRK_OK) return rc;
-  rc = encode_tiled_2d(&map_users, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, user_split, d_pad, n_users, 4 * d_pad, kKBlock,
-                       kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
-  if (rc != TRK_OK) return rc;
-  if (cluster == 2) {
-    const int64_t n_work = ceil_div(static_cast<int64_t>(p.n_user_pairs), 2) * n_splits;
-    const int n_clusters = static_cast<int>(n_work < max_clusters ? n_work : max_clusters);
-    cfg.gridDim = dim3(static_cast<unsigned>(2 * n_clusters));
-    TRK_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel2, map_users, map_items, p));
-  } else {
-    TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel1, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    const int grid = capped_grid(static_cast<int64_t>(p.n_user_pairs) * n_splits, 1);
-    kernel1<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, p);
-  }
-  TRK_CHECK_LAUNCH();
-  return TRK_OK;
+  return launch_sweep<WideKernel>("score_wide", p, 0u, user_split, user_scale, user_bias, user_norm, item_hi,
+                                  item_stats, item_bias, block_bias_max, item_perm, n_users, n_items, d_pad, k,
+                                  n_splits, item_id_offset, row_theta, excl_indptr, excl_pos, stream);
 }
 
 }  // namespace trk
