@@ -42,24 +42,30 @@ def _stale(target, deps):
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build(force=False, verbose=False):
+def build(force=False, verbose=False, defines=(), out_dir=None):
+    """Builds the library; returns its path.  `defines` (e.g. ['TRK_FILTER_CYCLES']) are passed to every translation
+    unit as -D flags; such a build belongs in its own `out_dir` (objects and library), which leaves the in-tree build
+    alone."""
     nvcc = find_nvcc()
+    obj_dir = out_dir or HERE
+    lib_path = os.path.join(out_dir, 'libtensorrec_b200.so') if out_dir else LIB_PATH
+    dflags = ['-D' + d for d in defines]
     objs = []
     for src in SOURCES:
         src_path = os.path.join(HERE, src)
-        obj = os.path.join(HERE, src.replace('.cu', '.o'))
+        obj = os.path.join(obj_dir, src.replace('.cu', '.o'))
         objs.append(obj)
         if force or _stale(obj, [src_path] + HEADERS):
-            cmd = [nvcc] + NVCC_FLAGS + (['-Xptxas', '-v'] if verbose else []) + ['-c', src_path, '-o', obj]
+            cmd = [nvcc] + NVCC_FLAGS + dflags + (['-Xptxas', '-v'] if verbose else []) + ['-c', src_path, '-o', obj]
             if verbose:
                 print(' '.join(cmd), flush=True)
             subprocess.run(cmd, check=True)
-    if force or _stale(LIB_PATH, objs):
-        cmd = [nvcc, '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', LIB_PATH] + objs
+    if force or _stale(lib_path, objs):
+        cmd = [nvcc, '-shared', '-gencode', 'arch=compute_90a,code=sm_90a', '-o', lib_path] + objs
         if verbose:
             print(' '.join(cmd), flush=True)
         subprocess.run(cmd, check=True)
-    return LIB_PATH
+    return lib_path
 
 
 if __name__ == '__main__':

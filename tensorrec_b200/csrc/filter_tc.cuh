@@ -189,9 +189,14 @@ __device__ __forceinline__ void sweep_ring_advance(int& ts, uint32_t& ts_phase, 
 }
 
 // Warp 0: every tile of every work unit of this CTA into the ring, warp-uniform control flow, one elected lane issues.
+// (TRK_FILTER_CYCLES builds: `empty_wait`, if given, accumulates the clocks spent waiting for a free slot.)
 template <int kNKB, int kCluster>
 __device__ __forceinline__ void sweep_producer(const SweepParams& p, const SweepCta& cta,
-                                               const CUtensorMap* map_items) {
+                                               const CUtensorMap* map_items
+#ifdef TRK_FILTER_CYCLES
+                                               , unsigned long long* empty_wait = nullptr
+#endif
+) {
   constexpr uint32_t kSlotBytes = kNKB * kBTileBytes;
   constexpr uint16_t kClusterMask = (1u << kCluster) - 1u;
   uint8_t* const ring = cta.smem + cta.L.b_off;
@@ -200,10 +205,16 @@ __device__ __forceinline__ void sweep_producer(const SweepParams& p, const Sweep
   for (int64_t w = cta.w_first; w < cta.n_work; w += cta.w_step) {
     const SweepUnit wu = sweep_unit<kCluster>(p, cta, w, 0, 0);
     for (int t = wu.t0; t < wu.t1; ++t) {
+#ifdef TRK_FILTER_CYCLES
+      const long long c0 = clock64();
+#endif
       if (kCluster == 2)
         mbar_wait_cluster(cta.b_empty + ts, ts_phase ^ 1);
       else
         mbar_wait(cta.b_empty + ts, ts_phase ^ 1);
+#ifdef TRK_FILTER_CYCLES
+      if (empty_wait != nullptr) *empty_wait += clock64() - c0;
+#endif
       if (elect_one()) {
         mbar_arrive_expect_tx(cta.b_full + ts, kSlotBytes);
 #pragma unroll

@@ -52,6 +52,25 @@ struct FilterParams {
   int32_t* cand_item;          // [n_users, n_splits, kKeepMax] global ids (sentinel INT32_MAX)
 };
 
+// Cycle accounting, compiled only with -DTRK_FILTER_CYCLES (scripts/filter_cycles.py builds such a library; the
+// shipped one has none of it).  Lane 0 of every consumer warp sums clock64() deltas per category in registers, the
+// producer warp its waits for a free B slot; each warp adds its sums to g_filter_cycles when it leaves the kernel and
+// trk_debug_filter_cycles copies them out.  kCycRowHalves holds the whole admission epilogue of the row halves, of
+// which kCycSlow is the staged path and kCycCompactMid the compactions inside it.
+#ifdef TRK_FILTER_CYCLES
+enum FilterCycle {
+  kCycBFull, kCycMma, kCycRowHalves, kCycSlow, kCycCompactMid, kCycCompactTileEnd, kCycCompactFinal, kCycOutput,
+  kCycRelease, kCycUnitStart, kCycWarm, kCycConsumer, kCycConsumerWarps, kCycProducerEmpty, kCycProducer,
+  kCycProducerWarps, kNumCycles
+};
+__device__ unsigned long long g_filter_cycles[kNumCycles];
+#define TRK_CYC_START(t) const long long t = clock64()
+#define TRK_CYC_ADD(sum, t) (sum) += static_cast<unsigned long long>(clock64() - (t))
+#else
+#define TRK_CYC_START(t)
+#define TRK_CYC_ADD(sum, t)
+#endif
+
 __device__ __forceinline__ void f_sts64(uint32_t addr, float s, int32_t id) {
   asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(__float_as_uint(s)), "r"(id) : "memory");
 }
@@ -74,6 +93,9 @@ struct RowState {
   float drop_max;   // best score a compaction dropped
   // row constants: the margin 2.25 m, the user bias, c = user scale x global item scale (a power of two) and 1 / c
   float m3, ubias, c, inv_c;
+#ifdef TRK_FILTER_CYCLES
+  unsigned long long cyc_slow, cyc_compact_mid;
+#endif
 };
 
 
@@ -203,7 +225,9 @@ __device__ __forceinline__ void admit_16(const uint32_t* acc, bool hit, int32_t 
   }
   __syncwarp();   // earlier appends of every lane are visible to the lanes that may now compact its row
   const unsigned need = __ballot_sync(0xffffffffu, r.cnt + __popc(pass) > kBufEntries);
+  TRK_CYC_START(c0);
   compact_rows(need, lane, r, ctx);
+  TRK_CYC_ADD(r.cyc_compact_mid, c0);
   if (pass != 0 && r.n_ovf < kGiveUpOverflows) {   // (a row that has just given up appends nothing more)   // cnt + popc(pass) <= kBufEntries holds here (a compaction leaves at most kKeepMax = 16)
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
@@ -311,6 +335,7 @@ __device__ __forceinline__ void filter_chunk(const float (&acc)[64], int rh, int
   bool flag = chunk_frag_pass<kC>(acc, bf, tf);   // == the h0 || h1 of filter_32 over the quad
   if constexpr (kExclude) flag = flag || (own && excl_next < base + 32);
   if (!__any_sync(0xffffffffu, flag)) return;
+  TRK_CYC_START(c0);
   stage_warp_chunk<kC>(acc, rh, stage, lane);
   if constexpr (kExclude) {
     if (own && excl_next < base + 32) excl_next = excl_mask_chunk(p.excl_indptr, p.excl_pos, u, base, stage, lane);
@@ -319,10 +344,15 @@ __device__ __forceinline__ void filter_chunk(const float (&acc)[64], int rh, int
   load_staged_row(stage, lane, v);
   filter_32(v, own, base, bmax_scaled, lane, r, ctx);
   frag_rows(r.tau, rh, lane, tf);
+  TRK_CYC_ADD(r.cyc_slow, c0);
 }
 
 // The four chunks of row half rh, processing positions [pos0, pos0 + 128): every row's columns in ascending order, and
-// a chunk's test sees the tau the chunks before it left.  Called warp-uniformly.
+// a chunk's test sees the tau the chunks before it left.  Only a slow path changes tau, so while no chunk has taken
+// one the four tests are independent: ONE vote on all four of them first (four independent FMNMX trees instead of four
+// vote-and-branch steps in a row) ends the usual row half, in which no row passes, with exactly the decision of the
+// four chunk votes.  Otherwise the chunks run one after the other as before.  (The exclusion code runs only on row
+// halves where some owner's next excluded position lies, whose chunks are staged anyway.)  Called warp-uniformly.
 template <bool kExclude>
 __device__ __forceinline__ void filter_row_half(const float (&acc)[64], int rh, int32_t pos0, float bmax_scaled,
                                                 uint32_t stage, int lane, int64_t u, const SweepParams& p,
@@ -330,6 +360,11 @@ __device__ __forceinline__ void filter_row_half(const float (&acc)[64], int rh, 
   float bf[2], tf[2];
   frag_rows(bmax_scaled, rh, lane, bf);
   frag_rows(r.tau, rh, lane, tf);
+  if constexpr (!kExclude) {
+    const bool any = chunk_frag_pass<0>(acc, bf, tf) | chunk_frag_pass<1>(acc, bf, tf) |
+                     chunk_frag_pass<2>(acc, bf, tf) | chunk_frag_pass<3>(acc, bf, tf);
+    if (!__any_sync(0xffffffffu, any)) return;
+  }
   filter_chunk<0, kExclude>(acc, rh, pos0, bmax_scaled, bf, tf, stage, lane, u, p, excl_next, r, ctx);
   filter_chunk<1, kExclude>(acc, rh, pos0 + 32, bmax_scaled, bf, tf, stage, lane, u, p, excl_next, r, ctx);
   filter_chunk<2, kExclude>(acc, rh, pos0 + 64, bmax_scaled, bf, tf, stage, lane, u, p, excl_next, r, ctx);
@@ -365,8 +400,20 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
   const int warp = threadIdx.x / 32;
   const int lane = threadIdx.x % 32;
 
+#ifdef TRK_FILTER_CYCLES
+  unsigned long long cyc[kNumCycles] = {};
+  TRK_CYC_START(c_all);
+#endif
   if (sweep_split_registers(warp)) {
+#ifdef TRK_FILTER_CYCLES
+    if (warp == 0) {
+      sweep_producer<kNKB, kCluster>(sweep, cta, &map_items, &cyc[kCycProducerEmpty]);
+      TRK_CYC_ADD(cyc[kCycProducer], c_all);
+      cyc[kCycProducerWarps] = 1;
+    }
+#else
     if (warp == 0) sweep_producer<kNKB, kCluster>(sweep, cta, &map_items);
+#endif
   } else {
     // ================================ consumers: wgmma + admission ================================
     const int group = warp / 4 - 1;
@@ -389,20 +436,28 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
     for (int64_t w = cta.w_first; w < cta.n_work; w += cta.w_step) {
       const SweepUnit wu = sweep_unit<kCluster>(sweep, cta, w, group, row);
       const int64_t u = wu.u;
+      TRK_CYC_START(c_unit);
       RowState rs;
       rs.buf = buf_row_addr;
       rs.cnt = rs.n_res = rs.n_ovf = 0;
       rs.tau = rs.theta = rs.drop_max = kNegInf;
+#ifdef TRK_FILTER_CYCLES
+      rs.cyc_slow = rs.cyc_compact_mid = 0;
+#endif
       int32_t excl_next = sweep_row_start<kExclude>(rs, sweep, wu, max_item_norm, item_scale, max_item_bias);
       sweep_load_user_block<kNKB>(cta, &map_users, wu, group, warp, lane, witer);
+      TRK_CYC_ADD(cyc[kCycUnitStart], c_unit);
 
       float bmax_next = wu.t1 > wu.t0 ? __ldg(sweep.block_bias_max + wu.t0) : 0.0f;
       for (int t = wu.t0; t < wu.t1; ++t) {
         const float bmax_scaled = bmax_next * rs.inv_c;
         if (t + 1 < wu.t1) bmax_next = __ldg(sweep.block_bias_max + t + 1);   // in flight while this tile is filtered
+        TRK_CYC_START(c_full);
         mbar_wait(cta.b_full + ts, ts_phase);
+        TRK_CYC_ADD(cyc[kCycBFull], c_full);
         const uint32_t b_slot = b_base + ts * (kNKB * kBTileBytes);
         const int32_t pos0 = t * kBlockN;
+        TRK_CYC_START(c_warm);
         if (t == wu.t0 && p.block_bias_min != nullptr) {
           const float bmin = __ldg(p.block_bias_min + wu.t0);   // the same for the whole CTA: warp-uniform branch
           if (bmin > kNegInf) {
@@ -428,10 +483,16 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
             }
           }
         }
+        TRK_CYC_ADD(cyc[kCycWarm], c_warm);
 #pragma unroll 1
         for (int rh = 0; rh < 2; ++rh) {
+          TRK_CYC_START(c_mma);
           filter_mma_rows<kNKB>(acc, a_base, b_slot, rh);
+          TRK_CYC_ADD(cyc[kCycMma], c_mma);
+          TRK_CYC_START(c_rel);
           if (rh == 1) sweep_release_slot<kCluster>(cta, ts, lane);   // the tile's last MMAs of this warp are complete
+          TRK_CYC_ADD(cyc[kCycRelease], c_rel);
+          TRK_CYC_START(c_rh);
           // kExclude: one vote per row half.  Only a row half in which some owner's next excluded position lies runs
           // the exclusion test of every chunk; every other one (all of them with empty lists) runs the exclusion-free
           // code, which decides exactly as the exclusion test would there.
@@ -441,6 +502,7 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
             filter_row_half<kExclude>(acc, rh, pos0, bmax_scaled, stage, lane, u, sweep, excl_next, rs, ctx);
           else
             filter_row_half<false>(acc, rh, pos0, bmax_scaled, stage, lane, u, sweep, excl_next, rs, ctx);
+          TRK_CYC_ADD(cyc[kCycRowHalves], c_rh);
         }
         sweep_ring_advance(ts, ts_phase, cta.n_slots);
         // A compaction waits one L2 round trip for the biases / item ids of its new entries -- during which, in the
@@ -449,13 +511,18 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
         // a row that overflows inside a tile.  (Measured on an H100 80GB HBM3 at 400 W, against a build without this
         // pass: 1M-item sweep 1570 -> 1560 ms, 125K-item shard 186.0 -> 183.6 ms.)
         {
+          TRK_CYC_START(c_te);
           const unsigned early = __ballot_sync(0xffffffffu, rs.cnt > p.tile_end_trigger);
           compact_rows(early, lane, rs, ctx);
+          TRK_CYC_ADD(cyc[kCycCompactTileEnd], c_te);
         }
       }
 
       // end of the item range: final compaction of every row of this warp, then emit the survivors
+      TRK_CYC_START(c_fin);
       compact_rows(0xffffffffu, lane, rs, ctx);
+      TRK_CYC_ADD(cyc[kCycCompactFinal], c_fin);
+      TRK_CYC_START(c_out);
       if (wu.u_ok) {
         const int64_t base = u * sweep.n_splits + wu.sp;
         float* os = p.cand_score + base * kKeepMax;
@@ -470,9 +537,25 @@ score_filter_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_
         sweep_store_theta(sweep, base, rs);
       }
       __syncwarp();
+      TRK_CYC_ADD(cyc[kCycOutput], c_out);
+#ifdef TRK_FILTER_CYCLES
+      cyc[kCycSlow] += rs.cyc_slow;
+      cyc[kCycCompactMid] += rs.cyc_compact_mid;
+#endif
     }
+#ifdef TRK_FILTER_CYCLES
+    TRK_CYC_ADD(cyc[kCycConsumer], c_all);
+    cyc[kCycConsumerWarps] = 1;
+#endif
   }
 
+#ifdef TRK_FILTER_CYCLES
+  if (lane == 0) {
+#pragma unroll
+    for (int i = 0; i < kNumCycles; ++i)
+      if (cyc[i] != 0) atomicAdd(g_filter_cycles + i, cyc[i]);
+  }
+#endif
   __syncthreads();
   if (kCluster == 2) cluster_sync_all();   // no CTA leaves while its peer may still multicast into it or arrive on it
 }
@@ -565,6 +648,19 @@ __global__ void exclusion_keys_kernel(const int32_t* __restrict__ indptr, const 
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
+#ifdef TRK_FILTER_CYCLES
+// Copies the cycle sums of every filter launch since the last call (categories in FilterCycle order) to `out` and
+// zeroes them.  Returns the number of categories.
+extern "C" int trk_debug_filter_cycles(unsigned long long* out, int n) {
+  if (out == nullptr || n < kNumCycles) return -kNumCycles;
+  if (cudaDeviceSynchronize() != cudaSuccess) return 0;
+  if (cudaMemcpyFromSymbol(out, g_filter_cycles, sizeof(g_filter_cycles)) != cudaSuccess) return 0;
+  const unsigned long long zero[kNumCycles] = {};
+  if (cudaMemcpyToSymbol(g_filter_cycles, zero, sizeof(zero)) != cudaSuccess) return 0;
+  return kNumCycles;
+}
+#endif
+
 int score_filter_max_k() { return kFilterMaxK; }
 int score_filter_list_width() { return kKeepMax; }
 
