@@ -361,6 +361,35 @@ int trk_score_topk_euclid_f16x3(const void* user_split, const float* user_scale,
                                 const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
                                 const float* user_half_sqnorm, const float* item_half_sqnorm, void* stream);
 
+/* Mixtures of tastes, with or without attention (collapse_mixture_of_tastes, tensorrec/recommendation_graphs.py:85-109,
+ * then bias_prediction_dense, :41), dot / cosine prediction (cosine: operands pre-normalised by K1), on the same
+ * tensor-core kernels.  Every user has n_ops operand rows: u_0 .. u_{T-1} and, with attention != 0, a_0 .. a_{T-1}
+ * (n_ops = T or 2T), stacked as user_split [n_ops, n_users, 2 d_pad] (16-byte aligned) with user_scale
+ * [n_ops, n_users]; every dot product is the 3-pass split product.  Per (user, item), left to right, each product and
+ * sum rounded on its own:
+ *   p_t = u_t . i;   no attention:  pred = max_t p_t;
+ *   attention:  a_t = a_t . i,  m = max_t a_t,  e_t = expf(a_t - m),  s = sum_t e_t (taste order),
+ *               pred = sum_t p_t * (e_t / s) (taste order);
+ *   out = (pred + user_bias[u]) + item_bias[i]
+ * (exact for integer-valued representations without attention, and with attention when every pair's weights are
+ * one-hot).  user_bias [n_users] may be NULL; item_meta as for trk_score_dense_f16x3.
+ *   trk_score_dense_tastes_f16x3  out[n_users, n_items] (row stride out_row_stride).
+ *   trk_score_topk_tastes_f16x3   cand_score / cand_item [n_users, n_splits, k] as trk_score_topk_f16x3_excl;
+ *                                 excl_indptr / excl_ids / excl_row_map may all be NULL (no exclusion).
+ * Constraints: d_pad in {64, 128}; n_tastes >= 1 and 2 <= n_ops <= 64 (T <= 64 without attention, T <= 32 with it;
+ * larger n_ops returns TRK_ERR_UNSUPPORTED); top-k: 1 <= k <= trk_score_topk_max_k(d_pad).  A user block holds
+ * 2 * floor(64 / n_ops) users. */
+int trk_score_dense_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                 int32_t n_tastes, int32_t attention, const void* item_split, const float* item_meta,
+                                 int64_t n_users, int64_t n_items, int32_t d_pad, float* out, int64_t out_row_stride,
+                                 void* stream);
+int trk_score_topk_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                int32_t n_tastes, int32_t attention, const void* item_split, const float* item_meta,
+                                int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k, int32_t n_splits,
+                                int32_t item_id_offset, float* cand_score, int32_t* cand_item,
+                                const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
+                                void* stream);
+
 /* Merges n_lists candidate lists per user (each sorted by (score desc, id asc), k_in entries) into the global
  * top k_out per user, same order.  Lists are the n_splits of one GPU and/or the shards received from the other GPUs
  * (item-axis sharding; the exchange itself is one NCCL all-to-all done by the host layer, SURVEY 8e).

@@ -49,6 +49,10 @@ SIGNATURES = {
                                                     _c_p, _c_p, _c_p]),
     'trk_score_topk_euclid_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_p, _c_i64, _c_i64, _c_i32, _c_i32, _c_i32,
                                                    _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p]),
+    'trk_score_dense_tastes_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i32, _c_i32, _c_p, _c_p, _c_i64, _c_i64,
+                                                    _c_i32, _c_p, _c_i64, _c_p]),
+    'trk_score_topk_tastes_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i32, _c_i32, _c_p, _c_p, _c_i64, _c_i64, _c_i32,
+                                                   _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p]),
     'trk_topk_merge': (ctypes.c_int, [_c_p, _c_p, _c_i64, _c_i32, _c_i32, _c_i32, _c_i64, _c_i64, _c_p, _c_p, _c_i64,
                                       _c_p, _c_i32, _c_p]),
     'trk_score_filter_max_k': (ctypes.c_int, []),

@@ -36,8 +36,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-int encode_tiled_2d(CUtensorMap* map, CUtensorMapDataType type, const void* base, uint64_t cols, uint64_t rows,
-                    uint64_t row_bytes, uint32_t box_cols, uint32_t box_rows, CUtensorMapL2promotion l2_promotion) {
+static EncodeTiledFn encode_tiled_fn() {
   static EncodeTiledFn encode = nullptr;   // the library links no driver: the entry point is looked up at run time
   if (encode == nullptr) {
     void* ptr = nullptr;
@@ -46,10 +45,35 @@ int encode_tiled_2d(CUtensorMap* map, CUtensorMapDataType type, const void* base
         qres == cudaDriverEntryPointSuccess)
       encode = reinterpret_cast<EncodeTiledFn>(ptr);
   }
-  if (encode == nullptr) {
-    set_error("cuTensorMapEncodeTiled is not available from the CUDA driver");
+  if (encode == nullptr) set_error("cuTensorMapEncodeTiled is not available from the CUDA driver");
+  return encode;
+}
+
+int encode_tiled_3d(CUtensorMap* map, CUtensorMapDataType type, const void* base, uint64_t cols, uint64_t rows,
+                    uint64_t planes, uint64_t row_bytes, uint64_t plane_bytes, uint32_t box_cols, uint32_t box_rows,
+                    uint32_t box_planes, CUtensorMapL2promotion l2_promotion) {
+  const EncodeTiledFn encode = encode_tiled_fn();
+  if (encode == nullptr) return TRK_ERR_CUDA;
+  const cuuint64_t dims[3] = {cols, rows, planes};
+  const cuuint64_t strides[2] = {row_bytes, plane_bytes};
+  const cuuint32_t box[3] = {box_cols, box_rows, box_planes};
+  const cuuint32_t elem_strides[3] = {1, 1, 1};
+  const CUresult r = encode(map, type, 3, const_cast<void*>(base), dims, strides, box, elem_strides,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, l2_promotion,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled failed with CUresult %d (planes=%llu rows=%llu cols=%llu)", static_cast<int>(r),
+              static_cast<unsigned long long>(planes), static_cast<unsigned long long>(rows),
+              static_cast<unsigned long long>(cols));
     return TRK_ERR_CUDA;
   }
+  return TRK_OK;
+}
+
+int encode_tiled_2d(CUtensorMap* map, CUtensorMapDataType type, const void* base, uint64_t cols, uint64_t rows,
+                    uint64_t row_bytes, uint32_t box_cols, uint32_t box_rows, CUtensorMapL2promotion l2_promotion) {
+  const EncodeTiledFn encode = encode_tiled_fn();
+  if (encode == nullptr) return TRK_ERR_CUDA;
   const cuuint64_t dims[2] = {cols, rows};
   const cuuint64_t strides[1] = {row_bytes};
   const cuuint32_t box[2] = {box_cols, box_rows};
@@ -83,6 +107,11 @@ int score_topk_f16x3(const void*, const float*, const float*, const void*, const
                      const int32_t*, const float*, const float*, cudaStream_t);
 int score_dense_f16x3(const void*, const float*, const float*, const void*, const float*, int64_t, int64_t, int32_t,
                       float*, int64_t, const float*, const float*, cudaStream_t);
+int score_topk_tastes_f16x3(const void*, const float*, const float*, int32_t, int32_t, const void*, const float*,
+                            int64_t, int64_t, int32_t, int32_t, int32_t, int32_t, float*, int32_t*, const int32_t*,
+                            const int32_t*, const int32_t*, cudaStream_t);
+int score_dense_tastes_f16x3(const void*, const float*, const float*, int32_t, int32_t, const void*, const float*,
+                             int64_t, int64_t, int32_t, float*, int64_t, cudaStream_t);
 int topk_merge(const float*, const int32_t*, int64_t, int32_t, int32_t, int32_t, int64_t, int64_t, float*, int32_t*,
                int64_t, const int32_t*, int32_t, cudaStream_t);
 int score_filter_max_k();
@@ -238,6 +267,25 @@ int trk_score_dense_euclid_f16x3(const void* user_split, const float* user_scale
                 "trk_score_dense_euclid_f16x3: null squared norms");
   return trk::score_dense_f16x3(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad,
                                 out, out_row_stride, user_half_sqnorm, item_half_sqnorm, trk::as_stream(stream));
+}
+
+int trk_score_dense_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                 int32_t n_tastes, int32_t attention, const void* item_split, const float* item_meta,
+                                 int64_t n_users, int64_t n_items, int32_t d_pad, float* out, int64_t out_row_stride,
+                                 void* stream) {
+  return trk::score_dense_tastes_f16x3(user_split, user_scale, user_bias, n_tastes, attention, item_split, item_meta,
+                                       n_users, n_items, d_pad, out, out_row_stride, trk::as_stream(stream));
+}
+
+int trk_score_topk_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                int32_t n_tastes, int32_t attention, const void* item_split, const float* item_meta,
+                                int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k, int32_t n_splits,
+                                int32_t item_id_offset, float* cand_score, int32_t* cand_item,
+                                const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
+                                void* stream) {
+  return trk::score_topk_tastes_f16x3(user_split, user_scale, user_bias, n_tastes, attention, item_split, item_meta,
+                                      n_users, n_items, d_pad, k, n_splits, item_id_offset, cand_score, cand_item,
+                                      excl_indptr, excl_ids, excl_row_map, trk::as_stream(stream));
 }
 
 int trk_topk_merge(const float* cand_score, const int32_t* cand_item, int64_t n_users, int32_t n_lists,

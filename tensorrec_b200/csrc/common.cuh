@@ -51,6 +51,13 @@ int capped_grid(int64_t blocks, int per_sm);
 int encode_tiled_2d(CUtensorMap* map, CUtensorMapDataType type, const void* base, uint64_t cols, uint64_t rows,
                     uint64_t row_bytes, uint32_t box_cols, uint32_t box_rows, CUtensorMapL2promotion l2_promotion);
 
+// Encodes a 3-D tensor map with the 128-byte swizzle: `planes` planes of `rows` rows of `cols` elements, rows
+// row_bytes apart and planes plane_bytes apart, loaded in boxes of box_cols x box_rows x box_planes.  A box lands in
+// shared memory as box_planes x box_rows consecutive rows (plane-major), swizzled as a 2-D box of that many rows.
+int encode_tiled_3d(CUtensorMap* map, CUtensorMapDataType type, const void* base, uint64_t cols, uint64_t rows,
+                    uint64_t planes, uint64_t row_bytes, uint64_t plane_bytes, uint32_t box_cols, uint32_t box_rows,
+                    uint32_t box_planes, CUtensorMapL2promotion l2_promotion);
+
 constexpr int kWarp = 32;
 constexpr int kSMsH100 = 132;
 
@@ -146,6 +153,17 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       :
       : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
         "l"(cache_hint)
+      : "memory");
+}
+// 3-D tiled load (see encode_tiled_3d), completion counted in bytes on `bar`.  c0 = innermost coordinate.
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int32_t c0,
+                                            int32_t c1, int32_t c2, uint64_t cache_hint) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
+      " [%0], [%1, {%3, %4, %5}], [%2], %6;"
+      :
+      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
+        "r"(c2), "l"(cache_hint)
       : "memory");
 }
 // 1-D bulk copy global -> shared (16-byte aligned, size a multiple of 16), completion counted in bytes on `bar`

@@ -71,6 +71,19 @@ struct TcEuclid {
   const float* item_half_sqnorm;
 };
 
+// Mixtures of tastes (kTastes instantiations): every user has n_ops operand rows -- u_0 .. u_{T-1} and, with attention,
+// a_0 .. a_{T-1} -- stacked as [n_ops, n_users, 2 d_pad] with scales [n_ops, n_users].  A consumer warpgroup's 64
+// accumulator rows hold per_wg = 64 / n_ops users x n_ops operands (row j * per_wg + q = operand j of user q; rows at
+// or beyond n_ops * per_wg are never loaded nor read), so a user block is 2 per_wg users and all operands of a (user,
+// item) pair come out of one tile's MMAs.  Also a kernel parameter of its own, for the same reason as TcExcl.
+struct TcTastes {
+  int32_t n_ops;
+  int32_t n_tastes;
+  int32_t per_wg;
+};
+constexpr int kTastesMax = 1;         // pred = max_t u_t . i        (recommendation_graphs.py:107)
+constexpr int kTastesAttention = 2;   // pred = sum_t softmax_t(a_t . i) u_t . i   (:96-103)
+
 // shared-memory carve-up (offsets from a 1024-byte aligned base)
 struct SmemLayout {
   uint32_t a_off, b_off, list_score_off, list_item_off, acc_off, bar_off, total;
@@ -163,6 +176,72 @@ __device__ __forceinline__ float score_chunk_as(uint32_t (&r)[32], const float2*
   else return score_chunk(r, meta, su, ubias);
 }
 
+// The taste collapse of one staged chunk (kTastes): columns [32 c, 32 c + 32) of both 64-column halves of the tile,
+// in the warpgroup's staging tile (stage = acc_stage, rows as in TcTastes).  Every (column half, user, column) element
+// is collapsed by one thread -- all 128 of the warpgroup share the work, lane = column -- and its final score replaces
+// operand row 0 of its user; the element reads and writes only its own user's rows in its own column.  Reference
+// order (collapse_mixture_of_tastes, recommendation_graphs.py:85-109, then bias_prediction_dense, :41), every
+// product and sum rounded on its own (no contraction):
+//   p_j = acc_j * (scale_i * scale_j)  (powers of two: exact);
+//   max:        pred = max_t p_t;
+//   attention:  m = max_t a_t,  e_t = expf(a_t - m),  s = sum_t e_t,  pred = sum_t p_t * (e_t / s)  (taste order);
+//   score = (pred + ub) + ib.
+// With attention, e_t is parked in a_t's staging row between the two passes.
+template <int kTastes>
+__device__ __forceinline__ void collapse_chunk(float* stage, int wt, int c, const float2* meta, const TcParams& p,
+                                               const TcTastes z, int64_t u0) {
+  const int lane = wt % 32;
+  const int n_tastes = z.n_tastes;
+  for (int e = wt / 32; e < 2 * z.per_wg; e += kConsumerThreads / 32) {   // warp-uniform: one (half, user) per warp
+    const int h = e / z.per_wg;
+    const int q = e - h * z.per_wg;
+    const int64_t u = u0 + q;
+    const bool u_ok = u < p.n_users;
+    const float2 m = meta[h * 64 + c * 32 + lane];
+    float* col = stage + (h * kWgRows + q) * kStageStride + lane;   // operand j at col[j * per_wg * kStageStride]
+    const int64_t op_stride = z.per_wg * kStageStride;
+    float pred;
+    if constexpr (kTastes == kTastesMax) {
+      pred = -__int_as_float(0x7f800000);
+      for (int t = 0; t < n_tastes; ++t) {
+        const float su = u_ok ? __ldg(p.user_scale + t * p.n_users + u) : 0.0f;
+        pred = fmaxf(pred, __fmul_rn(col[t * op_stride], m.x * su));
+      }
+    } else {
+      float amax = -__int_as_float(0x7f800000);
+      for (int t = 0; t < n_tastes; ++t) {
+        const float sa = u_ok ? __ldg(p.user_scale + (n_tastes + t) * p.n_users + u) : 0.0f;
+        const float a = __fmul_rn(col[(n_tastes + t) * op_stride], m.x * sa);
+        col[(n_tastes + t) * op_stride] = a;
+        amax = fmaxf(amax, a);
+      }
+      float sum = 0.0f;
+      for (int t = 0; t < n_tastes; ++t) {
+        const float ex = expf(__fsub_rn(col[(n_tastes + t) * op_stride], amax));
+        col[(n_tastes + t) * op_stride] = ex;
+        sum = t == 0 ? ex : __fadd_rn(sum, ex);
+      }
+      pred = 0.0f;
+      for (int t = 0; t < n_tastes; ++t) {
+        const float su = u_ok ? __ldg(p.user_scale + t * p.n_users + u) : 0.0f;
+        const float pt = __fmul_rn(col[t * op_stride], m.x * su);
+        const float w = __fdiv_rn(col[(n_tastes + t) * op_stride], sum);
+        pred = t == 0 ? __fmul_rn(pt, w) : __fadd_rn(pred, __fmul_rn(pt, w));
+      }
+    }
+    const float ub = (u_ok && p.user_bias != nullptr) ? __ldg(p.user_bias + u) : 0.0f;
+    col[0] = __fadd_rn(__fadd_rn(pred, ub), m.y);
+  }
+}
+
+// Chunk maximum of final scores (kTastes: collapse_chunk formed them).
+__device__ __forceinline__ float chunk_max(const uint32_t (&r)[32]) {
+  float cmax = -__int_as_float(0x7f800000);
+#pragma unroll
+  for (int j = 0; j < 32; ++j) cmax = fmaxf(cmax, __uint_as_float(r[j]));
+  return cmax;
+}
+
 // Exclusion (kExclude): the final scores of the chunk's columns [base, base + 32) named in list row `xr` become -inf
 // (never inserted: the compare is strict and the lists start at -inf).  A select per register, not r[dynamic index],
 // which would put r[] into local memory; the FINAL score is masked, not the accumulator (a zero scale would turn -inf into
@@ -200,13 +279,15 @@ struct ExclCursor<false> {};
 // One 32-column chunk of one user row: final scores, then (top-k mode) the row's listed columns masked (kExclude) and
 // the rare inserts, or (dense mode) the store.  `x` is taken by value: a reference bound to the kernel parameter
 // changes the generated code of the instantiations without exclusion.  kEuclid: the Euclidean score (ihsq = the tile's
-// item norms, usq = the row's |u|^2).
-template <bool kDense, bool kExclude, bool kEuclid>
+// item norms, usq = the row's |u|^2).  kTastes: r[] already holds final scores.
+template <bool kDense, bool kExclude, bool kEuclid, int kTastes = 0>
 __device__ __forceinline__ void process_chunk(uint32_t (&r)[32], int c, int t, int32_t id0, const float2* meta,
                                               const float* ihsq, float su, float usq, float ubias, float& thr,
                                               float* ls, int32_t* li, const TcParams& p, int64_t u, bool u_ok,
                                               const TcExcl x, ExclCursor<kExclude>& xc) {
-  float cmax = score_chunk_as<kEuclid>(r, meta + c * 32, ihsq + c * 32, su, usq, ubias);
+  float cmax;
+  if constexpr (kTastes != 0) cmax = chunk_max(r);
+  else cmax = score_chunk_as<kEuclid>(r, meta + c * 32, ihsq + c * 32, su, usq, ubias);
   if constexpr (!kDense) {
     if constexpr (kExclude) {
       const int32_t base = t * kBlockN + c * 32;   // local id of the chunk's first column
@@ -263,10 +344,14 @@ __device__ __forceinline__ void store_chunk_tma(const uint32_t (&r)[32], uint32_
 
 // kNKB = d_pad / 64 k-blocks per operand half.  kExclude (top-k mode): columns named in the row's exclusion list are
 // left out of the top-k (excl_mask_scores).  kEuclid: Euclidean similarity (score_chunk_euclid) in either mode.
-template <bool kDense, int kNKB, bool kExclude = false, bool kEuclid = false>
+// kTastes (kTastesMax / kTastesAttention): a mixture of tastes collapsed per (user, item) (collapse_chunk); map_users
+// is then the 3-D map of the stacked operand, a user block holds 2 z.per_wg users, and in dense mode map_out's box
+// is 32 columns x z.per_wg rows.
+template <bool kDense, int kNKB, bool kExclude = false, bool kEuclid = false, int kTastes = 0>
 __global__ void __launch_bounds__(kTcThreads, 1)
 score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_constant__ CUtensorMap map_items,
-                const __grid_constant__ CUtensorMap map_out, const TcParams p, const TcExcl x, const TcEuclid e) {
+                const __grid_constant__ CUtensorMap map_out, const TcParams p, const TcExcl x, const TcEuclid e,
+                const TcTastes z) {
   uint8_t* smem = smem_base_1024();
   const SmemLayout L = make_layout(p.n_kblocks, p.n_stages, kDense ? 0 : p.k, kDense && p.tma_store != 0);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
@@ -316,7 +401,18 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
         const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
         if (t1 <= t0 || ub >= live_blocks) continue;
         mbar_wait(a_empty, (witer & 1) ^ 1);  // the MMAs of the previous work item no longer read A
-        if (elect_one()) {
+        if constexpr (kTastes != 0) {
+          // one box of n_ops x per_wg rows per warpgroup half and k-block; a half without users is not loaded
+          const int32_t u0 = ub * 2 * z.per_wg;
+          const int n_halves = u0 + z.per_wg < p.n_users ? 2 : 1;
+          if (elect_one()) {
+            mbar_arrive_expect_tx(a_full, n_kb2 * n_halves * z.n_ops * z.per_wg * (kKBlock * 2));
+            for (int kb = 0; kb < n_kb2; ++kb)
+              for (int h = 0; h < n_halves; ++h)
+                tma_load_3d(smem + L.a_off + kb * kATileBytes + h * (kWgRows * 128), &map_users, a_full, kb * kKBlock,
+                            u0 + h * z.per_wg, 0, kEvictFirst);
+          }
+        } else if (elect_one()) {
           mbar_arrive_expect_tx(a_full, n_kb2 * kATileBytes);
           for (int kb = 0; kb < n_kb2; ++kb)
             tma_load_2d(smem + L.a_off + kb * kATileBytes, &map_users, a_full, kb * kKBlock, ub * kBlockM,
@@ -366,10 +462,12 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
       const int t0 = sp * p.tiles_per_split;
       const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
       if (ub >= live_blocks) continue;   // (an empty split still emits its sentinel candidates)
-      const int64_t u = static_cast<int64_t>(ub) * kBlockM + row;
-      const bool u_ok = u < p.n_users;
-      const float su = u_ok ? __ldg(p.user_scale + u) : 0.0f;
-      const float ubias = (u_ok && p.user_bias != nullptr) ? __ldg(p.user_bias + u) : 0.0f;
+      // kTastes: this warpgroup's users start at u0; the thread of row q < per_wg owns user u0 + q, later rows own none
+      const int64_t u0 = kTastes != 0 ? static_cast<int64_t>(ub) * 2 * z.per_wg + g * z.per_wg : 0;
+      const int64_t u = kTastes != 0 ? u0 + wt % kWgRows : static_cast<int64_t>(ub) * kBlockM + row;
+      const bool u_ok = u < p.n_users && (kTastes == 0 || wt % kWgRows < z.per_wg);
+      const float su = (kTastes == 0 && u_ok) ? __ldg(p.user_scale + u) : 0.0f;
+      const float ubias = (kTastes == 0 && u_ok && p.user_bias != nullptr) ? __ldg(p.user_bias + u) : 0.0f;
       float usq = 0.0f;   // kEuclid: |u|^2 (rows at or beyond n_users read nothing)
       if constexpr (kEuclid) usq = u_ok ? -2.0f * __ldg(e.user_half_sqnorm + u) : 0.0f;
       float thr = kNegInf;
@@ -433,19 +531,31 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
             acc_stage[((col / 64) * kWgRows + wgmma_acc_row(wt, i)) * kStageStride + col % 32] = acc[i];
           }
           named_barrier_sync(1 + g, kConsumerThreads);
+          if constexpr (kTastes != 0) {   // row q of each half now holds user q's final scores
+            collapse_chunk<kTastes>(acc_stage, wt, c, meta, p, z, u0);
+            named_barrier_sync(1 + g, kConsumerThreads);
+          }
           uint32_t r[32];
           const float* src = acc_stage + (half * kWgRows + wt % kWgRows) * kStageStride;
 #pragma unroll
           for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(src[j]);
           const int chunk = half * 2 + c;
           if (kDense && p.tma_store) {
-            score_chunk_as<kEuclid>(r, meta + chunk * 32, ihsq + chunk * 32, su, usq, ubias);
-            store_chunk_tma(r, stage_base + (n_stored & 1) * kStoreTileBytes, lane, &map_out, t * kBlockN + chunk * 32,
-                            ub * kBlockM + g * kWgRows + (warp % 2) * 32);
-            ++n_stored;
-          } else {
-            process_chunk<kDense, kExclude, kEuclid>(r, chunk, t, id0, meta, ihsq, su, usq, ubias, thr, ls, li, p, u,
-                                                     u_ok, x, xc);
+            if constexpr (kTastes != 0) {   // the users are rows 0 .. per_wg - 1 (<= 32): the first warp of each half
+              if (warp % 2 == 0) {
+                store_chunk_tma(r, stage_base + (n_stored & 1) * kStoreTileBytes, lane, &map_out,
+                                t * kBlockN + chunk * 32, static_cast<int32_t>(u0));
+                ++n_stored;
+              }
+            } else {
+              score_chunk_as<kEuclid>(r, meta + chunk * 32, ihsq + chunk * 32, su, usq, ubias);
+              store_chunk_tma(r, stage_base + (n_stored & 1) * kStoreTileBytes, lane, &map_out,
+                              t * kBlockN + chunk * 32, ub * kBlockM + g * kWgRows + (warp % 2) * 32);
+              ++n_stored;
+            }
+          } else if (kTastes == 0 || wt % kWgRows < z.per_wg) {
+            process_chunk<kDense, kExclude, kEuclid, kTastes>(r, chunk, t, id0, meta, ihsq, su, usq, ubias, thr, ls, li,
+                                                              p, u, u_ok, x, xc);
           }
         }
       }
@@ -507,7 +617,8 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
                      int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset, float* cand_score,
                      int32_t* cand_item, float* dense_out, int64_t dense_stride, const int32_t* n_users_live,
                      const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
-                     const float* user_half_sqnorm, const float* item_half_sqnorm, cudaStream_t stream) {
+                     const float* user_half_sqnorm, const float* item_half_sqnorm, int32_t n_tastes,
+                     int32_t attention, cudaStream_t stream) {
   TRK_CHECK_ARG(user_split && user_scale && item_split && item_meta, "score_tc: null operand");
   TRK_CHECK_ARG((user_half_sqnorm == nullptr) == (item_half_sqnorm == nullptr),
                 "score_tc: user_half_sqnorm and item_half_sqnorm go together");
@@ -534,6 +645,22 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
   TRK_CHECK_ARG(n_splits >= 1, "score_tc: n_splits < 1");
   TRK_CHECK_ARG((excl_indptr == nullptr) == (excl_ids == nullptr) && (excl_indptr != nullptr || excl_row_map == nullptr),
                 "score_topk: excl_indptr and excl_ids go together (excl_row_map needs both)");
+  // n_tastes != 0: a mixture of tastes on the stacked operand [n_ops, n_users, 2 d_pad] (TcTastes)
+  const bool tastes = n_tastes != 0;
+  TcTastes z = {0, 0, 0};
+  if (tastes) {
+    // (one operand row per user is the plain kernel: per_wg would exceed the 32 rows of a dense store tile)
+    TRK_CHECK_ARG(n_tastes >= 2 || (n_tastes == 1 && attention), "score_tastes: n_tastes=%d needs n_tastes >= 2 or attention",
+                  n_tastes);
+    TRK_CHECK_ARG(!euclid && n_users_live == nullptr, "score_tastes: no Euclidean form and no live-row count");
+    const int n_ops = n_tastes <= 64 ? (attention ? 2 : 1) * n_tastes : 65;
+    if (n_ops > kWgRows) {
+      set_error("score_tastes: %d operand rows per user (n_tastes=%d%s) exceed %d", n_ops, n_tastes,
+                attention ? ", attention" : "", kWgRows);
+      return TRK_ERR_UNSUPPORTED;
+    }
+    z = {n_ops, n_tastes, kWgRows / n_ops};
+  }
 
   TcParams p;
   p.user_scale = user_scale;
@@ -546,7 +673,7 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
   p.n_tiles = static_cast<int32_t>(ceil_div(n_items, kBlockN));
   p.n_splits = n_splits;
   p.tiles_per_split = static_cast<int32_t>(ceil_div(p.n_tiles, n_splits));
-  p.n_user_blocks = static_cast<int32_t>(ceil_div(n_users, kBlockM));
+  p.n_user_blocks = static_cast<int32_t>(ceil_div(n_users, tastes ? 2 * z.per_wg : kBlockM));
   p.item_id_offset = item_id_offset;
   p.cand_score = cand_score;
   p.cand_item = cand_item;
@@ -560,9 +687,13 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
   TRK_CHECK_ARG(p.n_stages >= 2, "score_tc: shared memory budget exceeded (d_pad=%d k=%d)", d_pad, k);
 
   // operands: [rows, 2 d_pad] fp16 (hi | lo), boxes of one k-block x one tile
+  // (tastes: the stacked operand, boxes of one k-block x per_wg users x n_ops operands = one warpgroup's rows)
   CUtensorMap map_users, map_items;
-  int rc = encode_tiled_2d(&map_users, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, user_split, 2 * d_pad, n_users, 4 * d_pad,
-                           kKBlock, kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  int rc = tastes ? encode_tiled_3d(&map_users, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, user_split, 2 * d_pad, n_users, z.n_ops,
+                                    4 * d_pad, 4 * d_pad * n_users, kKBlock, z.per_wg, z.n_ops,
+                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B)
+                  : encode_tiled_2d(&map_users, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, user_split, 2 * d_pad, n_users,
+                                    4 * d_pad, kKBlock, kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   if (rc != TRK_OK) return rc;
   rc = encode_tiled_2d(&map_items, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, item_split, 2 * d_pad, n_items, 4 * d_pad, kKBlock,
                        kBlockN, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
@@ -571,7 +702,7 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
   CUtensorMap map_out = map_items;   // placeholder when the TMA store path is off
   if (p.tma_store) {
     rc = encode_tiled_2d(&map_out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, dense_out, n_items, n_users, 4 * dense_stride, 32,
-                         32, CU_TENSOR_MAP_L2_PROMOTION_NONE);
+                         tastes ? z.per_wg : 32, CU_TENSOR_MAP_L2_PROMOTION_NONE);
     if (rc != TRK_OK) return rc;
   }
   const uint32_t smem_bytes = make_layout(p.n_kblocks, p.n_stages, p.k, p.tma_store != 0).total + kSmemAlignSlack;
@@ -589,9 +720,29 @@ static int launch_tc(const void* user_split, const float* user_scale, const floa
       kernel = p.n_kblocks == 2 ? score_tc_kernel<false, 2, false, true> : score_tc_kernel<false, 1, false, true>;
     }
   }
+  if (tastes) {
+    const bool att = attention != 0;
+    const bool two = p.n_kblocks == 2;
+    if constexpr (kDense) {
+      kernel = att ? (two ? score_tc_kernel<true, 2, false, false, kTastesAttention>
+                          : score_tc_kernel<true, 1, false, false, kTastesAttention>)
+                   : (two ? score_tc_kernel<true, 2, false, false, kTastesMax>
+                          : score_tc_kernel<true, 1, false, false, kTastesMax>);
+    } else if (excl_indptr != nullptr) {
+      kernel = att ? (two ? score_tc_kernel<false, 2, true, false, kTastesAttention>
+                          : score_tc_kernel<false, 1, true, false, kTastesAttention>)
+                   : (two ? score_tc_kernel<false, 2, true, false, kTastesMax>
+                          : score_tc_kernel<false, 1, true, false, kTastesMax>);
+    } else {
+      kernel = att ? (two ? score_tc_kernel<false, 2, false, false, kTastesAttention>
+                          : score_tc_kernel<false, 1, false, false, kTastesAttention>)
+                   : (two ? score_tc_kernel<false, 2, false, false, kTastesMax>
+                          : score_tc_kernel<false, 1, false, false, kTastesMax>);
+    }
+  }
   TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
   const int grid = capped_grid(static_cast<int64_t>(p.n_user_blocks) * n_splits, 1);
-  kernel<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, map_out, p, x, e);
+  kernel<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, map_out, p, x, e, z);
   TRK_CHECK_LAUNCH();
   return TRK_OK;
 }
@@ -604,22 +755,49 @@ int score_topk_f16x3(const void* user_split, const float* user_scale, const floa
                      const float* item_half_sqnorm, cudaStream_t stream) {
   return launch_tc<false>(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k,
                           n_splits, item_id_offset, cand_score, cand_item, nullptr, 0, n_users_live, excl_indptr,
-                          excl_ids, excl_row_map, user_half_sqnorm, item_half_sqnorm, stream);
+                          excl_ids, excl_row_map, user_half_sqnorm, item_half_sqnorm, 0, 0, stream);
+}
+
+// Item splits of a dense launch over n_ub user blocks: enough that every SM gets work when there are few user blocks.
+static int32_t dense_splits(int64_t n_ub, int64_t n_items) {
+  const int64_t n_tiles = ceil_div(n_items, kBlockN);
+  int64_t splits = ceil_div(2 * static_cast<int64_t>(sm_count()), n_ub);
+  if (splits > n_tiles) splits = n_tiles;
+  if (splits < 1) splits = 1;
+  return static_cast<int32_t>(splits);
 }
 
 int score_dense_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
                       const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
                       int32_t d_pad, float* out, int64_t out_row_stride, const float* user_half_sqnorm,
                       const float* item_half_sqnorm, cudaStream_t stream) {
-  // split the item axis so that every SM gets work even when there are few user blocks
-  const int64_t n_ub = ceil_div(n_users, kBlockM);
-  const int64_t n_tiles = ceil_div(n_items, kBlockN);
-  int64_t splits = ceil_div(2 * static_cast<int64_t>(sm_count()), n_ub);
-  if (splits > n_tiles) splits = n_tiles;
-  if (splits < 1) splits = 1;
   return launch_tc<true>(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, 0,
-                         static_cast<int32_t>(splits), 0, nullptr, nullptr, out, out_row_stride, nullptr, nullptr,
-                         nullptr, nullptr, user_half_sqnorm, item_half_sqnorm, stream);
+                         dense_splits(ceil_div(n_users, kBlockM), n_items), 0, nullptr, nullptr, out, out_row_stride,
+                         nullptr, nullptr, nullptr, nullptr, user_half_sqnorm, item_half_sqnorm, 0, 0, stream);
+}
+
+int score_topk_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                            int32_t n_tastes, int32_t attention, const void* item_split, const float* item_meta,
+                            int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k, int32_t n_splits,
+                            int32_t item_id_offset, float* cand_score, int32_t* cand_item, const int32_t* excl_indptr,
+                            const int32_t* excl_ids, const int32_t* excl_row_map, cudaStream_t stream) {
+  TRK_CHECK_ARG(n_tastes >= 1, "score_tastes: n_tastes=%d < 1", n_tastes);
+  return launch_tc<false>(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k,
+                          n_splits, item_id_offset, cand_score, cand_item, nullptr, 0, nullptr, excl_indptr, excl_ids,
+                          excl_row_map, nullptr, nullptr, n_tastes, attention, stream);
+}
+
+int score_dense_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                             int32_t n_tastes, int32_t attention, const void* item_split, const float* item_meta,
+                             int64_t n_users, int64_t n_items, int32_t d_pad, float* out, int64_t out_row_stride,
+                             cudaStream_t stream) {
+  TRK_CHECK_ARG(n_tastes >= 1, "score_tastes: n_tastes=%d < 1", n_tastes);
+  const int64_t n_ops = (attention ? 2 : 1) * static_cast<int64_t>(n_tastes);
+  const int64_t users_per_block = n_ops <= kWgRows ? 2 * (kWgRows / n_ops) : kBlockM;   // (launch_tc rejects the rest)
+  return launch_tc<true>(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, 0,
+                         dense_splits(ceil_div(n_users, users_per_block), n_items), 0, nullptr, nullptr, out,
+                         out_row_stride, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, n_tastes, attention,
+                         stream);
 }
 
 }  // namespace trk

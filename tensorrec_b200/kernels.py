@@ -117,11 +117,14 @@ class DeviceCSR(object):
 K1_MAX_WIDTH = 512      # widest row one K1 launch covers (256 when the width is not a multiple of 4)
 
 
-def gather_reduce(csr, weights, n_normalize=0, want_f32=True, split_d_pad=None, want_norm=False, stats=None):
+def gather_reduce(csr, weights, n_normalize=0, want_f32=True, split_d_pad=None, want_norm=False, stats=None,
+                  split_out=None):
     """K1.  Returns (repr_f32 or None, split or None, scale or None[, norm]).
 
     want_norm: also return the row norms (upper bounds) formed in K1's epilogue; stats: float32[3] that receives the
-    max norm / max row scale (zeroed by the call).  Both feed the filter form of the fused top-k."""
+    max norm / max row scale (zeroed by the call).  Both feed the filter form of the fused top-k.
+    split_out: (split [rows, 2 split_d_pad] fp16, scale [rows] f32) contiguous tensors -- e.g. one operand's slice of a
+    stacked mixture-of-tastes operand -- that K1 writes instead of new ones."""
     lib = require_cuda()
     rows, n_features = csr.shape
     d = int(weights.shape[1])
@@ -135,8 +138,11 @@ def gather_reduce(csr, weights, n_normalize=0, want_f32=True, split_d_pad=None, 
     d_pad = 0
     if split_d_pad is not None:
         d_pad = int(split_d_pad)
-        split = torch.empty((rows, 2 * d_pad), dtype=torch.float16, device=dev)
-        scale = torch.empty((rows,), dtype=torch.float32, device=dev)
+        if split_out is not None:
+            split, scale = split_out
+        else:
+            split = torch.empty((rows, 2 * d_pad), dtype=torch.float16, device=dev)
+            scale = torch.empty((rows,), dtype=torch.float32, device=dev)
     if want_norm:
         norm = torch.empty((rows,), dtype=torch.float32, device=dev)
     rc = lib.trk_csr_gather_reduce_f32(_p(csr.indptr), _p(csr.col), _p(csr.val), _p(weights), rows, n_features, d,
@@ -173,12 +179,16 @@ def _l2_normalize_rows_any_width_(x):
     return x
 
 
-def split_f32(repr_f32, n_normalize=0, d_pad=None):
+def split_f32(repr_f32, n_normalize=0, d_pad=None, out=None):
+    """out: (split, scale) tensors to write, as gather_reduce's split_out."""
     lib = require_cuda()
     rows, d = repr_f32.shape
     d_pad = d_pad_for(d) if d_pad is None else int(d_pad)
-    split = torch.empty((rows, 2 * d_pad), dtype=torch.float16, device=repr_f32.device)
-    scale = torch.empty((rows,), dtype=torch.float32, device=repr_f32.device)
+    if out is not None:
+        split, scale = out
+    else:
+        split = torch.empty((rows, 2 * d_pad), dtype=torch.float16, device=repr_f32.device)
+        scale = torch.empty((rows,), dtype=torch.float32, device=repr_f32.device)
     rc = lib.trk_split_f32_to_f16x2(_p(repr_f32), rows, d, int(n_normalize), _p(split), d_pad, _p(scale), _stream())
     _lib.check(rc, 'trk_split_f32_to_f16x2')
     return split, scale
@@ -314,6 +324,67 @@ def score_dense_tc(user_split, user_scale, user_bias, item_split, item_meta, n_u
         name, extra = 'trk_score_dense_euclid_f16x3', (_p(sqnorms[0]), _p(sqnorms[1]))
     rc = getattr(lib, name)(*args, *extra, _stream())
     _lib.check(rc, name)
+    return out
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# mixtures of tastes on the tensor-core kernels: every user's n_ops operand rows (u_0 .. u_{T-1}, then a_0 .. a_{T-1}
+# with attention) stacked as [n_ops, U, 2 d_pad]; the kernel collapses the tastes per (user, item)
+# ---------------------------------------------------------------------------------------------------------------
+TASTES_MAX_OPS = 64      # operand rows per user the kernel holds: one consumer warpgroup's accumulator rows
+
+
+def tastes_n_ops(n_tastes, attention):
+    return int(n_tastes) * (2 if attention else 1)
+
+
+def tastes_plan(n_tastes, attention):
+    """Block layout of the taste-collapsing kernel: (users per warpgroup P, users per 128-row block 2P, accumulator
+    rows used per warpgroup n_ops * P, out of 64).  None when n_ops is outside [2, TASTES_MAX_OPS]."""
+    n_ops = tastes_n_ops(n_tastes, attention)
+    if n_ops < 2 or n_ops > TASTES_MAX_OPS:
+        return None
+    per_wg = TASTES_MAX_OPS // n_ops
+    return per_wg, 2 * per_wg, n_ops * per_wg
+
+
+def score_topk_tastes(users, items, meta, n_tastes, attention, k, n_splits=None, item_id_offset=0, excl=None,
+                      excl_row_map=None):
+    """The fused top-k of a mixture of tastes (users: stacked SideOperands).  Returns (cand_score, cand_item)
+    [U, n_splits, k]."""
+    lib = require_cuda()
+    n_users = users.n_rows
+    if n_splits is None:
+        n_splits = default_splits(n_users, items.n_rows)
+    dev = users.split.device
+    cand_score = torch.empty((n_users, n_splits, k), dtype=torch.float32, device=dev)
+    cand_item = torch.empty((n_users, n_splits, k), dtype=torch.int32, device=dev)
+    ex = (None, None, None) if excl is None else (_p(excl.indptr), _p(excl.ids), _p(excl_row_map))
+    rc = lib.trk_score_topk_tastes_f16x3(_p(users.split), _p(users.scale), _p(users.bias), int(n_tastes),
+                                         1 if attention else 0, _p(items.split), _p(meta), n_users, items.n_rows,
+                                         int(users.d_pad), int(k), int(n_splits), int(item_id_offset), _p(cand_score),
+                                         _p(cand_item), *ex, _stream())
+    _lib.check(rc, 'trk_score_topk_tastes_f16x3')
+    return cand_score, cand_item
+
+
+def topk_tastes(users, items, n_tastes, attention, k, n_splits=None, item_id_offset=0, excl=None, out=None):
+    """Fused top-k of a mixture of tastes + merge -> PackedTopK [U, k]."""
+    meta = pack_item_meta(items.scale, items.bias, items.n_rows)
+    cs, ci = score_topk_tastes(users, items, meta, n_tastes, attention, k, n_splits=n_splits,
+                               item_id_offset=item_id_offset, excl=excl)
+    return topk_merge(cs, ci, k, out=out)
+
+
+def score_dense_tastes(users, item_split, item_meta, n_items, n_tastes, attention, out=None):
+    """Dense scores [U, n_items] of a mixture of tastes (users: stacked SideOperands)."""
+    lib = require_cuda()
+    if out is None:
+        out = torch.empty((users.n_rows, n_items), dtype=torch.float32, device=users.split.device)
+    rc = lib.trk_score_dense_tastes_f16x3(_p(users.split), _p(users.scale), _p(users.bias), int(n_tastes),
+                                          1 if attention else 0, _p(item_split), _p(item_meta), users.n_rows, n_items,
+                                          int(users.d_pad), _p(out), out.stride(0), _stream())
+    _lib.check(rc, 'trk_score_dense_tastes_f16x3')
     return out
 
 

@@ -62,9 +62,13 @@ WIDE_MIN_ITEMS = 4096
 # items.  The fused route was faster at every measured catalogue size, from 1024 items up (see README, "Euclidean
 # models"); smaller catalogues stay on dense scoring and ranking.
 EUCLIDEAN_MIN_ITEMS = 1024
+# Mixture-of-tastes models with an attention graph take the taste-collapsing exact kernel for k <= 32 on catalogues of
+# at least ATTENTION_MIN_ITEMS items (see README, "Mixtures of tastes and attention").
+ATTENTION_MIN_ITEMS = 1024
 
 
-def topk_route(k, n_items, model_ok, single_taste, filter_max_k, exact_max_k, sharded=False, euclidean=False):
+def topk_route(k, n_items, model_ok, single_taste, filter_max_k, exact_max_k, sharded=False, euclidean=False,
+               attention=False):
     """The route of a top-k call -- 'filter', 'exact3', 'wide' or 'dense+rank' -- from k, the catalogue size and the
     model alone.  model_ok: the tensor-core kernels evaluate the model (built-in dot / cosine prediction, or any
     built-in similar-items graph, no attention, d_pad <= 128); single_taste: one taste (the wide route has no
@@ -73,13 +77,15 @@ def topk_route(k, n_items, model_ok, single_taste, filter_max_k, exact_max_k, sh
     rank's shard size does not decide the wide route.  TOPK_PATH='exact' means "no filter": k > exact_max_k then
     goes to dense+rank.  euclidean: a Euclidean user x item model (model_ok from _euclidean_tensor_ok), which has no
     filter or wide form: 'exact3' for k <= exact_max_k on catalogues of at least EUCLIDEAN_MIN_ITEMS items (any shard
-    size in a sharded call), 'dense+rank' otherwise."""
+    size in a sharded call), 'dense+rank' otherwise.  attention: a mixture of tastes with an attention graph (model_ok
+    from _tastes_tensor_ok), whose softmax has no filter or wide form either: the same rule with ATTENTION_MIN_ITEMS."""
     if not model_ok:
         return 'dense+rank'
-    if euclidean:
+    if euclidean or attention:
         if k > exact_max_k or n_items == 0:
             return 'dense+rank'
-        return 'exact3' if sharded or n_items >= EUCLIDEAN_MIN_ITEMS else 'dense+rank'
+        min_items = ATTENTION_MIN_ITEMS if attention else EUCLIDEAN_MIN_ITEMS
+        return 'exact3' if sharded or n_items >= min_items else 'dense+rank'
     if k <= exact_max_k:
         if n_items == 0:
             return 'dense+rank'
@@ -555,13 +561,15 @@ class TensorRec(object):
                 side, sparse_input.shape[1], n_features))
 
     def _represent(self, graph, sparse_input, n_features, node_name_ending, device, extra_normalize=0,
-                   want_f32=True, split_d_pad=None, want_norm=False, stats=None):
-        """One representation on the device: (repr_f32 | None, split | None, scale | None[, norm])."""
+                   want_f32=True, split_d_pad=None, want_norm=False, stats=None, split_out=None):
+        """One representation on the device: (repr_f32 | None, split | None, scale | None[, norm]).  split_out:
+        (split, scale) tensors the split operand is written to."""
         if type(graph) in _BUILTIN_REPR:
             weights = self._var(LinearRepresentationGraph.weight_name(node_name_ending), device)
             n_norm = (1 if graph.b200_kind == 'normalized_linear' else 0) + extra_normalize
             return kernels.gather_reduce(sparse_input.device_csr(device), weights, n_normalize=n_norm,
-                                         want_f32=want_f32, split_d_pad=split_d_pad, want_norm=want_norm, stats=stats)
+                                         want_f32=want_f32, split_d_pad=split_d_pad, want_norm=want_norm, stats=stats,
+                                         split_out=split_out)
         # user-defined / non-linear plugin: run its own forward on the device, then hand the dense rows to the kernels
         with torch.no_grad(), variable_scope(self._variables), name_scope(node_name_ending):
             for k in list(self._variables):
@@ -574,7 +582,7 @@ class TensorRec(object):
             kernels.l2_normalize_rows_(dense)
         split = scale = None
         if split_d_pad is not None:
-            split, scale = kernels.split_f32(dense, n_normalize=0, d_pad=split_d_pad)
+            split, scale = kernels.split_f32(dense, n_normalize=0, d_pad=split_d_pad, out=split_out)
         if stats is not None:
             stats.zero_()
         if want_norm or stats is not None:
@@ -604,6 +612,34 @@ class TensorRec(object):
         one taste only -- _score_plan checks that)."""
         return (SCORE_PATH != 'exact' and type(self.prediction_graph_factory) is EuclideanSimilarityPredictionGraph
                 and self.attention_graph_factory is None and kernels.d_pad_for(self.n_components) <= 128)
+
+    def _tastes_tensor_ok(self):
+        """Can the taste-collapsing tensor-core kernels evaluate this mixture of tastes?  Built-in dot or cosine
+        prediction, n_tastes >= 2 within the kernel's operand rows (T <= 64, T <= 32 with attention), any attention
+        graph or none, d_pad <= 128."""
+        return (SCORE_PATH != 'exact'
+                and type(self.prediction_graph_factory) in (DotProductPredictionGraph, CosineSimilarityPredictionGraph)
+                and self.n_tastes >= 2
+                and kernels.tastes_plan(self.n_tastes, self.attention_graph_factory is not None) is not None
+                and kernels.d_pad_for(self.n_components) <= 128)
+
+    def _taste_operands(self, block_in, device):
+        """The users of a mixture of tastes as kernels.SideOperands whose split is the stacked operand [n_ops, U,
+        2 d_pad] (u_0 .. u_{T-1}, then a_0 .. a_{T-1} with attention) and scale [n_ops, U]; K1 writes every operand
+        straight into its slice, normalised as the CUDA-core path normalises it."""
+        extra = 1 if type(self.prediction_graph_factory) is CosineSimilarityPredictionGraph else 0
+        d_pad = kernels.d_pad_for(self.n_components)
+        rows = block_in.shape[0]
+        ops = [(self.user_repr_graph_factory, 'user_{}'.format(t)) for t in range(self.n_tastes)]
+        if self.attention_graph_factory is not None:
+            ops += [(self.attention_graph_factory, 'attn_{}'.format(t)) for t in range(self.n_tastes)]
+        split = torch.empty((len(ops), rows, 2 * d_pad), dtype=torch.float16, device=device)
+        scale = torch.empty((len(ops), rows), dtype=torch.float32, device=device)
+        for j, (graph, name) in enumerate(ops):
+            self._represent(graph, block_in, self.n_user_features, name, device, extra, want_f32=False,
+                            split_d_pad=d_pad, split_out=(split[j], scale[j]))
+        bias = self._projected_biases(block_in, 'feature_biases_user', device) if self.biased else None
+        return kernels.SideOperands(None, split, scale, bias, rows, self.n_components, d_pad)
 
     def _side_operands(self, side, sparse_in, device, for_filter=False, taste=0):
         """One side ('user' or 'item') as kernels.SideOperands: split-fp16 operand + scale, projected biases and -- for
@@ -636,6 +672,15 @@ class TensorRec(object):
         model allows, the exact CUDA-core kernel (tastes, attention, wide rows) or the plugin's own dense form
         otherwise."""
         n_items = item_in.shape[0]
+        if self._tastes_tensor_ok():      # (checked first: SCORE_PATH='tensor' accepts these models)
+            items = self._side_operands('item', item_in, device)
+            meta = kernels.pack_item_meta(items.scale, items.bias, n_items)
+            attention = self.attention_graph_factory is not None
+
+            def score(block_in, out=None):
+                return kernels.score_dense_tastes(self._taste_operands(block_in, device), items.split, meta, n_items,
+                                                  self.n_tastes, attention, out=out)
+            return score
         euclidean = self.n_tastes == 1 and self._euclidean_tensor_ok()
         if euclidean or self._tensor_path_ok():
             items = self._side_operands('item', item_in, device)
@@ -835,7 +880,8 @@ class TensorRec(object):
         32 < k <= WIDE_MAX_K on catalogues of at least WIDE_MIN_ITEMS items runs on the wide form of the filter (each
         user's candidates in a list in device memory, rows the certificate rejects scored dense and ranked); the default
         user blocks then keep those lists within PREDICT_BLOCK_BYTES.  Euclidean models run k <= 32 on the exact kernel
-        (catalogues of at least EUCLIDEAN_MIN_ITEMS items) and larger k on dense+rank with tensor-core scoring.
+        (catalogues of at least EUCLIDEAN_MIN_ITEMS items) and larger k on dense+rank with tensor-core scoring; so do
+        mixtures of tastes with an attention graph (ATTENTION_MIN_ITEMS), on the taste-collapsing kernel.
         last_topk_info['path'] names the route (topk_route).
 
         exclude: None, or a scipy sparse matrix (any format) with n_users rows whose column index is the GLOBAL item id
@@ -874,12 +920,17 @@ class TensorRec(object):
                 return None
             return kernels.exclusion_host_csr(exclude, item_id_offset, n_items, u0, u1)
 
+        attention = self.attention_graph_factory is not None
         euclidean = self._euclidean_tensor_ok()      # (checked first: SCORE_PATH='tensor' accepts these models)
-        model_ok = euclidean or self._tensor_path_ok(allow_tastes=True)
+        if attention:
+            model_ok = self._tastes_tensor_ok()
+        else:
+            model_ok = euclidean or self._tensor_path_ok(allow_tastes=True)
         d_pad = kernels.d_pad_for(self.n_components)
         limits = (kernels.filter_max_k(), kernels.topk_max_k(d_pad)) if model_ok else (0, 0)
         path = topk_route(k, n_items, model_ok, self.n_tastes == 1, *limits,
-                          sharded=item_id_offset != 0 or gather_group is not None, euclidean=euclidean)
+                          sharded=item_id_offset != 0 or gather_group is not None, euclidean=euclidean,
+                          attention=attention)
         fused = path != 'dense+rank'
         use_filter = path == 'filter'
         wide = path == 'wide'
@@ -919,6 +970,11 @@ class TensorRec(object):
                                              host_excl), [(None, 0)]
             # every taste sweep of the block uses the same lists (an item is excluded for every taste)
             excl = None if host_excl is None else kernels.DeviceExclusion.upload(*host_excl, device=device)
+            if attention:
+                # the softmax mixes the tastes: one sweep of the taste-collapsing kernel, no device-side fallback
+                users = self._taste_operands(block_in, device)
+                return kernels.topk_tastes(users, items, self.n_tastes, True, k, item_id_offset=item_id_offset,
+                                           excl=excl), [(None, 0)]
             if self.n_tastes == 1:
                 top, cnt, cap = run_taste(block_in, 0, force_exact, excl)
                 return top, [(cnt, cap)]
