@@ -704,13 +704,15 @@ class FilterItems(object):
                                                                        perm=self.perm, want_min=True)
 
 
-def filter_and_rescore(users, items, fitems, user_norm, k, n_splits=None, item_id_offset=0, out=None, excl=None):
-    """(PackedTopK [U, k], flags [U]) -- flags mark users the certificate did not cover."""
-    _, ci, theta = score_filter(users.split, users.scale, users.bias, user_norm, fitems.hi, fitems.stats,
-                                fitems.bias_pad, fitems.block_max, fitems.perm, users.n_rows, items.n_rows,
-                                users.d_pad, k, n_splits=n_splits, item_id_offset=item_id_offset,
-                                block_bias_min=fitems.block_min, excl=excl)
-    return rescore_topk(users, items, ci, theta, user_norm, fitems.stats, k, item_id_offset=item_id_offset, out=out)
+def _filter_inputs(users, items, fitems, excl):
+    """What both filter forms read besides the operands: (user row norms, FilterItems), each formed here when the
+    caller has none, and -- with exclusion lists -- their positions in fitems' processing order."""
+    user_norm = users.norm if users.norm is not None else operand_stats(users.split, users.scale, users.d_pad)
+    if fitems is None:
+        fitems = FilterItems(items)
+    if excl is not None and excl.pos is None:
+        exclusion_positions(excl, fitems.perm, items.n_rows)
+    return user_norm, fitems
 
 
 def fallback_capacity(n_users):
@@ -728,6 +730,31 @@ def _ptr_at(t, index):
     return ctypes.c_void_p(t.data_ptr() + index * t.element_size())
 
 
+def _gather_flagged_rows(users, bad, counters, capacity, small=None):
+    """Compacts the indices of the rows of `users` with bad != 0 into idx on the device (at most `capacity`;
+    counters[0] = how many were flagged) and gathers those rows' operands.  Returns (idx, SideOperands of `capacity`
+    rows whose first min(flagged, capacity) are filled; `small`: the bound of trk_gather_operand_rows' small tier).
+    small=None: the count is read back first (one synchronisation) and exactly the flagged rows are gathered -- None
+    when there are none."""
+    lib = require_cuda()
+    dev = users.split.device
+    idx = torch.empty((capacity,), dtype=torch.int32, device=dev)
+    rc = lib.trk_select_flagged_rows(_p(bad), users.n_rows, _p(idx), capacity, _p(counters), _stream())
+    _lib.check(rc, 'trk_select_flagged_rows')
+    rows = capacity
+    if small is None:
+        rows = small = int(counters[0].item())
+        if rows == 0:
+            return idx, None
+    split = torch.empty((rows, 2 * users.d_pad), dtype=torch.float16, device=dev)
+    scale = torch.empty((rows,), dtype=torch.float32, device=dev)
+    bias = None if users.bias is None else torch.empty((rows,), dtype=torch.float32, device=dev)
+    rc = lib.trk_gather_operand_rows(_p(idx), _p(counters), rows, small, _p(users.split), _p(users.scale),
+                                     _p(users.bias), int(users.d_pad), _p(split), _p(scale), _p(bias), _stream())
+    _lib.check(rc, 'trk_gather_operand_rows')
+    return idx, SideOperands(None, split, scale, bias, rows, users.d, users.d_pad)
+
+
 def rerun_uncertified(users, items, bad, top, k, item_id_offset=0, excl=None):
     """Users flagged by the certificate go through the exact kernel WITHOUT a host round trip: the flagged rows are
     compacted on the device, their operands gathered into a fixed-capacity buffer, the exact kernel runs over that buffer
@@ -737,21 +764,10 @@ def rerun_uncertified(users, items, bad, top, k, item_id_offset=0, excl=None):
     Returns (counters, capacity); counters[0] = flagged rows, > capacity means overflow (the caller checks it at its
     next synchronisation).  excl: the exclusion lists of the users; the gathered rows read them through idx."""
     lib = require_cuda()
-    dev = users.split.device
     cap = fallback_capacity(users.n_rows)
     small = min(cap, FALLBACK_SMALL_ROWS)
-    idx = torch.empty((cap,), dtype=torch.int32, device=dev)
-    counters = torch.empty((4,), dtype=torch.int32, device=dev)
-    rc = lib.trk_select_flagged_rows(_p(bad), users.n_rows, _p(idx), cap, _p(counters), _stream())
-    _lib.check(rc, 'trk_select_flagged_rows')
-    sub_split = torch.empty((cap, 2 * users.d_pad), dtype=torch.float16, device=dev)
-    sub_scale = torch.empty((cap,), dtype=torch.float32, device=dev)
-    sub_bias = None if users.bias is None else torch.empty((cap,), dtype=torch.float32, device=dev)
-    rc = lib.trk_gather_operand_rows(_p(idx), _p(counters), cap, small, _p(users.split), _p(users.scale),
-                                     _p(users.bias), int(users.d_pad), _p(sub_split), _p(sub_scale), _p(sub_bias),
-                                     _stream())
-    _lib.check(rc, 'trk_gather_operand_rows')
-    sub = SideOperands(None, sub_split, sub_scale, sub_bias, cap, users.d, users.d_pad)
+    counters = torch.empty((4,), dtype=torch.int32, device=users.split.device)
+    idx, sub = _gather_flagged_rows(users, bad, counters, cap, small=small)
     tiers = [(sub.rows(0, small), small, 2, default_splits(2 * TILE_USERS, items.n_rows))]
     if cap > small:
         tiers.append((sub, cap, 3, None))
@@ -770,13 +786,12 @@ def topk_filter(users, items, k, n_splits=None, item_id_offset=0, fitems=None, e
     (buffer overflow under massive ties, bound violated) are re-run through the exact kernel on the device.
     excl: DeviceExclusion of the users (its positions are formed here for fitems' processing order if missing).
     Returns (PackedTopK, counters device int32[2], capacity)."""
-    user_norm = users.norm if users.norm is not None else operand_stats(users.split, users.scale, users.d_pad)
-    if fitems is None:
-        fitems = FilterItems(items)
-    if excl is not None and excl.pos is None:
-        exclusion_positions(excl, fitems.perm, items.n_rows)
-    top, bad = filter_and_rescore(users, items, fitems, user_norm, k, n_splits=n_splits, item_id_offset=item_id_offset,
-                                  excl=excl)
+    user_norm, fitems = _filter_inputs(users, items, fitems, excl)
+    _, ci, theta = score_filter(users.split, users.scale, users.bias, user_norm, fitems.hi, fitems.stats,
+                                fitems.bias_pad, fitems.block_max, fitems.perm, users.n_rows, items.n_rows,
+                                users.d_pad, k, n_splits=n_splits, item_id_offset=item_id_offset,
+                                block_bias_min=fitems.block_min, excl=excl)
+    top, bad = rescore_topk(users, items, ci, theta, user_norm, fitems.stats, k, item_id_offset=item_id_offset)
     counters, cap = rerun_uncertified(users, items, bad, top, k, item_id_offset=item_id_offset, excl=excl)
     return top, counters, cap
 
@@ -891,24 +906,13 @@ def rerun_flagged_dense(users, items, bad, top, k, item_id_offset=0, excl=None, 
     Returns the device counters (counters[0] = rows)."""
     lib = require_cuda()
     dev = users.split.device
-    n = users.n_rows
-    idx = torch.empty((max(n, 1),), dtype=torch.int32, device=dev)
     counters = torch.zeros((4,), dtype=torch.int32, device=dev)
-    if n == 0:
+    if users.n_rows == 0:
         return counters
-    rc = lib.trk_select_flagged_rows(_p(bad), n, _p(idx), n, _p(counters), _stream())
-    _lib.check(rc, 'trk_select_flagged_rows')
-    n_bad = int(counters[0].item())
-    if n_bad == 0:
+    idx, sub = _gather_flagged_rows(users, bad, counters, users.n_rows)
+    if sub is None:
         return counters
-    sub_split = torch.empty((n_bad, 2 * users.d_pad), dtype=torch.float16, device=dev)
-    sub_scale = torch.empty((n_bad,), dtype=torch.float32, device=dev)
-    sub_bias = None if users.bias is None else torch.empty((n_bad,), dtype=torch.float32, device=dev)
-    rc = lib.trk_gather_operand_rows(_p(idx), _p(counters), n_bad, n_bad, _p(users.split), _p(users.scale),
-                                     _p(users.bias), int(users.d_pad), _p(sub_split), _p(sub_scale), _p(sub_bias),
-                                     _stream())
-    _lib.check(rc, 'trk_gather_operand_rows')
-    sub = SideOperands(None, sub_split, sub_scale, sub_bias, n_bad, users.d, users.d_pad)
+    n_bad = sub.n_rows
     meta = pack_item_meta(items.scale, items.bias, items.n_rows)
     cand = torch.empty((n_bad, k), dtype=torch.int32, device=dev)
     step = dense_rank_rows(items.n_rows, block_bytes)
@@ -934,11 +938,7 @@ def topk_wide(users, items, k, n_splits=None, item_id_offset=0, fitems=None, exc
     re-scoring + selection + certificate (trk_select_wide_topk), and the rows the certificate rejects scored dense and
     ranked (rerun_flagged_dense).  Returns (PackedTopK, counters device int32[4], capacity); counters[0] = rows that
     took the dense fallback (every flagged row fits: capacity = the number of rows)."""
-    user_norm = users.norm if users.norm is not None else operand_stats(users.split, users.scale, users.d_pad)
-    if fitems is None:
-        fitems = FilterItems(items)
-    if excl is not None and excl.pos is None:
-        exclusion_positions(excl, fitems.perm, items.n_rows)
+    user_norm, fitems = _filter_inputs(users, items, fitems, excl)
     if n_splits is None:
         n_splits = wide_splits(users.n_rows, items.n_rows, k)
     cand, count, theta = score_wide(users, user_norm, fitems, items.n_rows, k, n_splits,
@@ -951,6 +951,21 @@ def topk_wide(users, items, k, n_splits=None, item_id_offset=0, fitems=None, exc
     counters = rerun_flagged_dense(users, items, bad, top, k, item_id_offset=item_id_offset, excl=excl,
                                    euclidean=euclidean, block_bytes=block_bytes)
     return top, counters, users.n_rows
+
+
+def topk_fused(path, users, items, k, fitems=None, excl=None, item_id_offset=0, item_hsq=None, euclidean=False,
+               block_bytes=4 << 30):
+    """The fused top-k of one route of topk_route: 'filter' (topk_filter), 'exact3' (topk_exact, with item_hsq) or
+    'wide' (topk_wide, with euclidean and block_bytes).  Returns (PackedTopK [U, k], device counters of the rows the
+    certificate rejected | None, capacity of the device-side fallback)."""
+    if path == 'filter':
+        return topk_filter(users, items, k, item_id_offset=item_id_offset, fitems=fitems, excl=excl)
+    if path == 'wide':
+        return topk_wide(users, items, k, item_id_offset=item_id_offset, fitems=fitems, excl=excl, euclidean=euclidean,
+                         block_bytes=block_bytes)
+    if path == 'exact3':
+        return topk_exact(users, items, k, item_id_offset=item_id_offset, excl=excl, item_hsq=item_hsq), None, 0
+    raise ValueError('%r is not a fused top-k route' % (path,))
 
 
 # ---------------------------------------------------------------------------------------------------------------

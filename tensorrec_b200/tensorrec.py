@@ -914,31 +914,20 @@ class TensorRec(object):
             return TopK(np.zeros((0, k), np.int32), np.zeros((0, k), np.float32))
         from . import distributed
 
-        def block_exclusion(u0, u1):
-            """-> host lists (indptr, ids) of user rows [u0, u1) over this shard's items, or None"""
-            if exclude is None:
-                return None
-            return kernels.exclusion_host_csr(exclude, item_id_offset, n_items, u0, u1)
-
         attention = self.attention_graph_factory is not None
         euclidean = self._euclidean_tensor_ok()      # (checked first: SCORE_PATH='tensor' accepts these models)
         if attention:
             model_ok = self._tastes_tensor_ok()
         else:
             model_ok = euclidean or self._tensor_path_ok(allow_tastes=True)
-        d_pad = kernels.d_pad_for(self.n_components)
-        limits = (kernels.filter_max_k(), kernels.topk_max_k(d_pad)) if model_ok else (0, 0)
-        path = topk_route(k, n_items, model_ok, self.n_tastes == 1, *limits,
-                          sharded=item_id_offset != 0 or gather_group is not None, euclidean=euclidean,
-                          attention=attention)
-        fused = path != 'dense+rank'
-        use_filter = path == 'filter'
-        wide = path == 'wide'
-        info = self.last_topk_info = {'path': path, 'fallback_rows': 0}
+        path = self._topk_path(k, n_items, model_ok, self.n_tastes == 1,
+                               sharded=item_id_offset != 0 or gather_group is not None, euclidean=euclidean,
+                               attention=attention)
         items = fitems = item_hsq = None
-        if fused and n_items > 0:
-            items = self._side_operands('item', item_in, device, for_filter=use_filter or wide)
-            if use_filter or wide:
+        if path != 'dense+rank' and n_items > 0:
+            one_pass = path in ('filter', 'wide')
+            items = self._side_operands('item', item_in, device, for_filter=one_pass)
+            if one_pass:
                 fitems = kernels.FilterItems(items)
             if euclidean:
                 item_hsq = kernels.item_half_sqnorm(items)
@@ -947,43 +936,25 @@ class TensorRec(object):
             user_batch_size = self._topk_block_rows(path, n_users, n_items, k, gather_group, device)
         blocks = self._user_blocks(user_in, n_items, user_batch_size)
 
-        def run_taste(block_in, taste, force_exact, excl):
-            if wide and n_items == 0:     # an empty item shard: no candidates, but the same calls as the other ranks
-                return kernels.empty_topk(block_in.shape[0], k, device), torch.zeros((4,), dtype=torch.int32,
-                                                                                     device=device), 0
-            users = self._side_operands('user', block_in, device, for_filter=(use_filter or wide) and not force_exact,
-                                        taste=taste)
-            if wide:
-                return kernels.topk_wide(users, items, k, item_id_offset=item_id_offset, fitems=fitems, excl=excl,
-                                         block_bytes=self.PREDICT_BLOCK_BYTES)
-            if use_filter and not force_exact:
-                return kernels.topk_filter(users, items, k, item_id_offset=item_id_offset, fitems=fitems, excl=excl)
-            return kernels.topk_exact(users, items, k, item_id_offset=item_id_offset, excl=excl,
-                                      item_hsq=item_hsq), None, 0
-
-        def run_block(block_in, u0, u1, force_exact=False):
-            """-> (PackedTopK of the block, [(device counters | None, capacity)] of its sweeps)"""
-            host_excl = block_exclusion(u0, u1)
-            if not fused:
-                return self._topk_from_dense(block_in.shape[0], n_items, k, item_id_offset, device,
-                                             lambda: self._predict_device(block_in, item_in, device),
-                                             host_excl), [(None, 0)]
-            # every taste sweep of the block uses the same lists (an item is excluded for every taste)
-            excl = None if host_excl is None else kernels.DeviceExclusion.upload(*host_excl, device=device)
+        def sweeps(block_in, u0, u1, route, excl):
             if attention:
                 # the softmax mixes the tastes: one sweep of the taste-collapsing kernel, no device-side fallback
                 users = self._taste_operands(block_in, device)
                 return kernels.topk_tastes(users, items, self.n_tastes, True, k, item_id_offset=item_id_offset,
                                            excl=excl), [(None, 0)]
-            if self.n_tastes == 1:
-                top, cnt, cap = run_taste(block_in, 0, force_exact, excl)
-                return top, [(cnt, cap)]
             # mixture of tastes (no attention): prediction = max over tastes (recommendation_graphs.py:107), so the top-k
             # lies in the union of the per-taste top-k lists: one fused sweep per taste, then a de-duplicating merge
-            per_taste = [run_taste(block_in, t, force_exact, excl) for t in range(self.n_tastes)]
-            stacked = torch.stack([top.buf for top, _, _ in per_taste]).contiguous()          # [T, U_block, 2k]
-            merged = kernels.topk_merge_received(stacked, block_in.shape[0], self.n_tastes, k, dedup=True)
-            return merged, [(cnt, cap) for _, cnt, cap in per_taste]
+            per_taste = []
+            for t in range(self.n_tastes):
+                users = self._side_operands('user', block_in, device, for_filter=route != 'exact3', taste=t)
+                per_taste.append(kernels.topk_fused(route, users, items, k, fitems=fitems, excl=excl,
+                                                    item_id_offset=item_id_offset, item_hsq=item_hsq,
+                                                    block_bytes=self.PREDICT_BLOCK_BYTES))
+            top = per_taste[0][0]
+            if self.n_tastes > 1:
+                stacked = torch.stack([sweep[0].buf for sweep in per_taste]).contiguous()       # [T, U_block, 2k]
+                top = kernels.topk_merge_received(stacked, block_in.shape[0], self.n_tastes, k, dedup=True)
+            return top, [(cnt, cap) for _, cnt, cap in per_taste]
 
         def exchange(top, u0, u1):
             if gather_group is None:
@@ -993,17 +964,36 @@ class TensorRec(object):
                 return distributed.all_gather_rows(merged, u1 - u0, gather_group), np.arange(u0, u1)
             return merged, np.arange(u0 + lo, u0 + hi)
 
-        results, rows = self._run_topk_blocks(blocks, run_block, exchange, info, gather_group, device)
-        info['user_rows'] = rows[0] if len(rows) == 1 else np.concatenate(rows)
+        results, rows = self._run_topk_blocks(path, k, blocks, n_items, item_id_offset, exclude, sweeps,
+                                              lambda block_in, u0, u1: self._predict_device(block_in, item_in, device),
+                                              exchange, gather_group)
+        self.last_topk_info['user_rows'] = rows[0] if len(rows) == 1 else np.concatenate(rows)
         return self._topk_result(results, to_host)
 
-    @staticmethod
-    def _run_topk_blocks(blocks, run_block, exchange, info, gather_group=None, device=None):
-        """The block loop of the fused top-k: run_block(block_in, r0, r1, force_exact=False) -> (PackedTopK, [(device
-        counters | None, capacity)] of its sweeps) for every (r0, r1, block_in) of `blocks`, exchange(top, r0, r1) ->
-        (top, result rows).  Then one synchronisation for the whole call: how many rows the certificate rejected per
-        sweep (device counters, summed into info['fallback_rows']); a block with more rejected rows than the device-side
-        fallback holds is re-run through the exact kernel.  Returns (the PackedTopK of every block, its result rows)."""
+    def _run_topk_blocks(self, path, k, blocks, n_items, item_id_offset, exclude, fused, dense_scores, exchange,
+                         gather_group=None):
+        """The block loop of a top-k call on `path`, for every (r0, r1, block_in) of `blocks`.  exclude: None, or a CSR
+        matrix of excluded (row, GLOBAL item id) pairs; a block's lists over the items [item_id_offset, item_id_offset +
+        n_items) are uploaded once for all its sweeps.  The block's top-k: on dense+rank from dense_scores(block_in, r0,
+        r1) -> its float32 [r1 - r0, n_items] scores on the device, on a fused route fused(block_in, r0, r1, route,
+        excl) -> (PackedTopK, [(device counters | None, capacity)] of its sweeps) (kernels.topk_fused); then
+        exchange(top, r0, r1) -> (top, result rows).  Then one synchronisation for the whole call: how many rows the
+        certificate rejected per sweep (device counters, summed into last_topk_info['fallback_rows']); a block with more
+        rejected rows than the device-side fallback holds is re-run through the exact kernel.  Returns (the PackedTopK
+        of every block, its result rows)."""
+        info = self.last_topk_info
+        device = self._cuda_device()
+
+        def run_block(block_in, r0, r1, force_exact=False):
+            excl = None if exclude is None else kernels.DeviceExclusion.upload(
+                *kernels.exclusion_host_csr(exclude, item_id_offset, n_items, r0, r1), device=device)
+            if path == 'dense+rank':
+                return self._topk_from_dense(r1 - r0, n_items, k, item_id_offset, device,
+                                             lambda: dense_scores(block_in, r0, r1), excl), [(None, 0)]
+            if path == 'wide' and n_items == 0:     # an empty item shard: no candidates, the calls of the other ranks
+                return kernels.empty_topk(r1 - r0, k, device), [(torch.zeros((4,), dtype=torch.int32, device=device), 0)]
+            return fused(block_in, r0, r1, 'exact3' if force_exact and path == 'filter' else path, excl)
+
         results, counters, rows = [], [], []
         for (r0, r1, block_in) in blocks:
             top, sweeps = run_block(block_in, r0, r1)
@@ -1062,19 +1052,24 @@ class TensorRec(object):
             rows = distributed.common_block_rows(rows, gather_group, device)
         return rows
 
-    def _topk_from_dense(self, n_users, n_items, k, item_id_offset, device, score, host_excl=None):
+    def _topk_path(self, k, n_items, model_ok, single_taste, **route):
+        """The route of a top-k call: topk_route(...) with the k limits of this model's kernels.  Starts
+        last_topk_info."""
+        d_pad = kernels.d_pad_for(self.n_components)
+        limits = (kernels.filter_max_k(), kernels.topk_max_k(d_pad)) if model_ok else (0, 0)
+        path = topk_route(k, n_items, model_ok, single_taste, *limits, **route)
+        self.last_topk_info = {'path': path, 'fallback_rows': 0}
+        return path
+
+    def _topk_from_dense(self, n_users, n_items, k, item_id_offset, device, score, excl=None):
         """Any model the fused kernel does not cover: dense scores -> exact full ranks -> the rank <= k entries.
-        score() -> the float32 [n_users, n_items] scores of the rows on the device.  host_excl: exclusion lists (indptr,
-        local ids) of the rows -- those scores become -inf before the ranking and those entries are never emitted (their
-        slots keep the sentinel)."""
+        score() -> the float32 [n_users, n_items] scores of the rows on the device.  excl: the rows' DeviceExclusion
+        -- those scores become -inf before the ranking and those entries are never emitted (their slots keep the
+        sentinel)."""
         if n_items == 0:
             return kernels.empty_topk(n_users, k, device)
-        ex_rows = ex_cols = None
-        if host_excl is not None:
-            indptr, ids = host_excl
-            ex_rows = torch.from_numpy(np.repeat(np.arange(n_users, dtype=np.int64), np.diff(indptr))).to(device)
-            ex_cols = torch.from_numpy(ids.astype(np.int64)).to(device)
-        return kernels.topk_from_scores(score(), k, item_id_offset, ex_rows, ex_cols)
+        ex = (None, None) if excl is None else kernels.exclusion_pairs(excl, torch.arange(n_users, device=device))
+        return kernels.topk_from_scores(score(), k, item_id_offset, *ex)
 
     def predict_similar_items(self, item_features, item_ids, n_similar):
         """tensorrec/tensorrec.py:666-703: for each id, the n_similar (item_id, score) pairs of highest prediction
@@ -1161,12 +1156,8 @@ class TensorRec(object):
                     and d_pad <= 128)
         if SCORE_PATH == 'tensor' and not model_ok:
             raise RuntimeError('TENSORREC_B200_SCORE_PATH=tensor but this model cannot use the tensor-core kernel')
-        limits = (kernels.filter_max_k(), kernels.topk_max_k(d_pad)) if model_ok else (0, 0)
-        path = topk_route(n, n_items, model_ok, True, *limits)
+        path = self._topk_path(n, n_items, model_ok, True)
         fused = path != 'dense+rank'
-        use_filter = path == 'filter'
-        wide = path == 'wide'
-        info = self.last_topk_info = {'path': path, 'fallback_rows': 0}
         if n_queries == 0:
             return TopK(np.zeros((0, n), np.int32), np.zeros((0, n), np.float32))
         ids_dev = None if ids is None else torch.from_numpy(ids).to(device)
@@ -1178,10 +1169,11 @@ class TensorRec(object):
             return t[q0:q1] if ids_dev is None else t.index_select(0, ids_dev[q0:q1])
 
         extra = 1 if kind == 'cosine' else 0
+        sweep = dense_scores = None
         if fused:
             # the item operand once: split fp16 + scale (+ row norms and statistics for the filter), no projected biases;
             # Euclidean: bias -1/2 |i|^2.  The queries are rows of this same operand.
-            one_pass = use_filter or wide
+            one_pass = path in ('filter', 'wide')
             stats = torch.empty((3,), dtype=torch.float32, device=device) if one_pass else None
             out = self._represent(self.item_repr_graph_factory, item_in, self.n_item_features, 'item', device, extra,
                                   want_f32=False, split_d_pad=d_pad, want_norm=one_pass, stats=stats)
@@ -1190,14 +1182,17 @@ class TensorRec(object):
             items = kernels.SideOperands(None, split, scale, bias, n_items, self.n_components, d_pad, stats=stats)
             fitems = kernels.FilterItems(items) if one_pass else None
 
-            def query_rows(q0, q1):
-                return kernels.SideOperands(None, take(split, q0, q1), take(scale, q0, q1), take(bias, q0, q1), q1 - q0,
-                                            self.n_components, d_pad, norm=take(norm, q0, q1))
+            def sweep(_, q0, q1, route, excl):
+                queries = kernels.SideOperands(None, take(split, q0, q1), take(scale, q0, q1), take(bias, q0, q1),
+                                               q1 - q0, self.n_components, d_pad, norm=take(norm, q0, q1))
+                top, cnt, cap = kernels.topk_fused(route, queries, items, n, fitems=fitems, excl=excl,
+                                                   euclidean=euclidean, block_bytes=self.PREDICT_BLOCK_BYTES)
+                return top, [(cnt, cap)]
         else:
             item_repr = self._represent(self.item_repr_graph_factory, item_in, self.n_item_features, 'item', device,
                                         extra)[0]
 
-            def dense_scores(q0, q1):
+            def dense_scores(_, q0, q1):
                 gathered = take(item_repr, q0, q1).contiguous()
                 if kind is not None:
                     return kernels.score_exact(gathered, item_repr, mode=1 if euclidean else 0)
@@ -1206,29 +1201,14 @@ class TensorRec(object):
                                                                      tf_item_representation=item_repr)
                 return sims.to(torch.float32).contiguous()
 
-        def run_block(_, q0, q1, force_exact=False):
-            host_excl = None if mask is None else kernels.exclusion_host_csr(mask, 0, n_items, q0, q1)
-            if not fused:
-                return self._topk_from_dense(q1 - q0, n_items, n, 0, device, lambda: dense_scores(q0, q1),
-                                             host_excl), [(None, 0)]
-            excl = None if host_excl is None else kernels.DeviceExclusion.upload(*host_excl, device=device)
-            queries = query_rows(q0, q1)
-            if wide:
-                top, cnt, cap = kernels.topk_wide(queries, items, n, fitems=fitems, excl=excl, euclidean=euclidean,
-                                                  block_bytes=self.PREDICT_BLOCK_BYTES)
-                return top, [(cnt, cap)]
-            if use_filter and not force_exact:
-                top, cnt, cap = kernels.topk_filter(queries, items, n, fitems=fitems, excl=excl)
-                return top, [(cnt, cap)]
-            return kernels.topk_exact(queries, items, n, excl=excl), [(None, 0)]
-
         if item_batch_size is not None:
             step = max(1, int(item_batch_size))
         else:
             step = self._topk_block_rows(path, n_queries, n_items, n)
         blocks = [(q0, min(n_queries, q0 + step), None) for q0 in range(0, n_queries, step)]
-        results, _ = self._run_topk_blocks(blocks, run_block, lambda top, q0, q1: (top, None), info)
-        if fused and euclidean and not wide:     # (the wide route maps its survivors in the selection kernel)
+        results, _ = self._run_topk_blocks(path, n, blocks, n_items, 0, mask, sweep, dense_scores,
+                                           lambda top, q0, q1: (top, None))
+        if fused and euclidean and path != 'wide':     # (the wide route maps its survivors in the selection kernel)
             for top in results:
                 kernels.topk_euclidean_finish(top)
         return self._topk_result(results, to_host)
