@@ -406,6 +406,18 @@ int trk_topk_merge(const float* cand_score, const int32_t* cand_item, int64_t n_
                    int32_t k_in, int32_t k_out, int64_t user_stride, int64_t list_stride, float* out_score,
                    int32_t* out_item, int64_t out_row_stride, const int32_t* n_users_live, int32_t dedup, void* stream);
 
+/* De-duplicating merge of TWO lists per row for any 1 <= k <= 1024 (trk_score_wide_max_k): the top-k of a mixture of
+ * tastes on the wide route folds the per-taste lists one at a time, R_t = R_{t-1} (+) L_t (DESIGN §3.6).  Entry j of
+ * row u of list A is (a_score, a_item)[u * a_row_stride + j], of B and of the result likewise with their own strides
+ * (a PackedTopK [n_rows, 2k] buffer: *_score = the row base, *_item = *_score + k, stride 2k).  Both lists are sorted
+ * by (score desc, id asc) with real ids unique within a list, padded with sentinels (-inf, INT32_MAX); a row may be
+ * all sentinels.  Row u of the result = the k best entries of A_u united with B_u, every real id once at the higher of
+ * its scores (an id with equal scores in both lists keeps one copy), in the same order, padded with sentinels.
+ * Sentinels are never entries.  The output must not overlap A or B.  Deterministic. */
+int trk_topk_merge_dedup_pair(const float* a_score, const int32_t* a_item, int64_t a_row_stride, const float* b_score,
+                              const int32_t* b_item, int64_t b_row_stride, int64_t n_rows, int32_t k, float* out_score,
+                              int32_t* out_item, int64_t out_row_stride, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------
  * The sampled-rank training step (SURVEY 8 row f1): everything of one Adam step of
  * LinearRepresentationGraph x DotProductPredictionGraph x WMRBLossGraph / BalancedWMRBLossGraph that is not a

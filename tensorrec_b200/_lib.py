@@ -55,6 +55,8 @@ SIGNATURES = {
                                                    _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p]),
     'trk_topk_merge': (ctypes.c_int, [_c_p, _c_p, _c_i64, _c_i32, _c_i32, _c_i32, _c_i64, _c_i64, _c_p, _c_p, _c_i64,
                                       _c_p, _c_i32, _c_p]),
+    'trk_topk_merge_dedup_pair': (ctypes.c_int, [_c_p, _c_p, _c_i64, _c_p, _c_p, _c_i64, _c_i64, _c_i32, _c_p, _c_p,
+                                                 _c_i64, _c_p]),
     'trk_score_filter_max_k': (ctypes.c_int, []),
     'trk_score_filter_list_width': (ctypes.c_int, []),
     'trk_operand_stats': (ctypes.c_int, [_c_p, _c_p, _c_i64, _c_i32, _c_p, _c_p, _c_p]),

@@ -114,6 +114,8 @@ int score_dense_tastes_f16x3(const void*, const float*, const float*, int32_t, i
                              int64_t, int64_t, int32_t, float*, int64_t, cudaStream_t);
 int topk_merge(const float*, const int32_t*, int64_t, int32_t, int32_t, int32_t, int64_t, int64_t, float*, int32_t*,
                int64_t, const int32_t*, int32_t, cudaStream_t);
+int topk_merge_dedup_pair(const float*, const int32_t*, int64_t, const float*, const int32_t*, int64_t, int64_t,
+                          int32_t, float*, int32_t*, int64_t, cudaStream_t);
 int score_filter_max_k();
 int score_filter_list_width();
 int operand_stats(const void*, const float*, int64_t, int32_t, float*, float*, cudaStream_t);
@@ -293,6 +295,13 @@ int trk_topk_merge(const float* cand_score, const int32_t* cand_item, int64_t n_
                    int32_t* out_item, int64_t out_row_stride, const int32_t* n_users_live, int32_t dedup, void* stream) {
   return trk::topk_merge(cand_score, cand_item, n_users, n_lists, k_in, k_out, user_stride, list_stride, out_score,
                          out_item, out_row_stride, n_users_live, dedup, trk::as_stream(stream));
+}
+
+int trk_topk_merge_dedup_pair(const float* a_score, const int32_t* a_item, int64_t a_row_stride, const float* b_score,
+                              const int32_t* b_item, int64_t b_row_stride, int64_t n_rows, int32_t k, float* out_score,
+                              int32_t* out_item, int64_t out_row_stride, void* stream) {
+  return trk::topk_merge_dedup_pair(a_score, a_item, a_row_stride, b_score, b_item, b_row_stride, n_rows, k, out_score,
+                                    out_item, out_row_stride, trk::as_stream(stream));
 }
 
 int trk_score_filter_max_k(void) { return trk::score_filter_max_k(); }

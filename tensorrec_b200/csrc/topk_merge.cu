@@ -106,4 +106,153 @@ int topk_merge(const float* cand_score, const int32_t* cand_item, int64_t n_user
   return TRK_OK;
 }
 
+// De-duplicating merge of two sorted lists per row for any k <= kPairMaxK (DESIGN §3.6): the fold of the per-taste
+// top-k lists of a mixture-of-tastes model on the wide route, where k is too large for topk_merge_kernel's one id per
+// lane.  One CTA per row, both lists in shared memory:
+//   1. A's real ids go into an open-addressing table of A positions (ids are unique within a list, so what a probe
+//      finds does not depend on the order of the insertions);
+//   2. every real id of B is looked up; of a duplicate pair the copy with the lower score is dropped, A's on a tie;
+//   3. the survivor flags of A and B are scanned into exclusive prefix counts;
+//   4. a survivor lands at (survivors of its own list before it) + (survivors of the other list ordered before it):
+//      the second term is a binary search of the other list for the first entry not before it, then a prefix count.
+//      Survivors have distinct ids, hence a strict order, so the positions are a permutation of [0, survivors);
+//   5. positions below k are written and the slots from the survivor count on get the sentinel.
+// Integer and float compares only: the result does not depend on thread scheduling.
+constexpr int kPairThreads = 256;
+constexpr int kPairMaxK = 1024;
+
+// exclusive prefix sum of v[0, n) in place, v[n] = the total, by the whole CTA; ends with a barrier
+__device__ __forceinline__ void block_exclusive_scan(int* v, int n, int* warp_total) {
+  const int lane = threadIdx.x % 32, warp = threadIdx.x / 32;
+  const int per = (n + blockDim.x - 1) / blockDim.x;
+  const int lo = min(n, static_cast<int>(threadIdx.x) * per), hi = min(n, lo + per);
+  int sum = 0;
+  for (int i = lo; i < hi; ++i) sum += v[i];
+  int incl = sum;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += t;
+  }
+  if (lane == 31) warp_total[warp] = incl;
+  __syncthreads();
+  int run = incl - sum;
+  for (int w = 0; w < warp; ++w) run += warp_total[w];
+  for (int i = lo; i < hi; ++i) {
+    const int x = v[i];
+    v[i] = run;
+    run += x;
+  }
+  if (threadIdx.x == blockDim.x - 1) v[n] = run;
+  __syncthreads();
+}
+
+// first position j of the sorted list (s, id)[0, n) whose entry is not ordered before (xs, xi)
+__device__ __forceinline__ int count_before(const float* s, const int32_t* id, int n, float xs, int32_t xi) {
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int mid = (lo + hi) / 2;
+    if (cand_better(s[mid], id[mid], xs, xi)) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+__device__ __forceinline__ uint32_t pair_hash(int32_t id, int table_bits) {
+  return (static_cast<uint32_t>(id) * 0x9e3779b1u) >> (32 - table_bits);
+}
+
+__global__ void __launch_bounds__(kPairThreads)
+topk_merge_dedup_pair_kernel(const float* __restrict__ a_score, const int32_t* __restrict__ a_item, int64_t a_stride,
+                             const float* __restrict__ b_score, const int32_t* __restrict__ b_item, int64_t b_stride,
+                             int k, int table_bits, float* __restrict__ out_score, int32_t* __restrict__ out_item,
+                             int64_t out_stride) {
+  extern __shared__ int32_t pair_smem[];
+  __shared__ int warp_total[kPairThreads / 32];
+  float* as = reinterpret_cast<float*>(pair_smem);
+  int32_t* ai = pair_smem + k;
+  float* bs = reinterpret_cast<float*>(pair_smem + 2 * k);
+  int32_t* bi = pair_smem + 3 * k;
+  int* pa = pair_smem + 4 * k;        // A's survivor flags, then their exclusive prefix counts ([k + 1])
+  int* pb = pa + k + 1;               // the same for B
+  int* table = pb + k + 1;            // A position per slot, -1 = empty ([1 << table_bits])
+  const int table_size = 1 << table_bits;
+  const uint32_t mask = table_size - 1;
+  const int64_t u = blockIdx.x;
+  const float kNegInf = -__int_as_float(0x7f800000);
+
+  for (int t = threadIdx.x; t < k; t += blockDim.x) {
+    as[t] = __ldg(a_score + u * a_stride + t);
+    ai[t] = __ldg(a_item + u * a_stride + t);
+    bs[t] = __ldg(b_score + u * b_stride + t);
+    bi[t] = __ldg(b_item + u * b_stride + t);
+    pa[t] = ai[t] != 0x7fffffff ? 1 : 0;
+  }
+  for (int t = threadIdx.x; t < table_size; t += blockDim.x) table[t] = -1;
+  __syncthreads();
+  for (int i = threadIdx.x; i < k; i += blockDim.x) {
+    if (ai[i] == 0x7fffffff) continue;
+    uint32_t h = pair_hash(ai[i], table_bits);
+    while (atomicCAS(table + h, -1, i) != -1) h = (h + 1) & mask;
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < k; j += blockDim.x) {
+    const int32_t id = bi[j];
+    int keep = id != 0x7fffffff ? 1 : 0;
+    if (keep) {
+      for (uint32_t h = pair_hash(id, table_bits);; h = (h + 1) & mask) {
+        const int i = table[h];
+        if (i < 0) break;
+        if (ai[i] == id) {        // the only copy of this id in A: exactly one thread writes pa[i]
+          if (bs[j] > as[i]) pa[i] = 0;
+          else keep = 0;
+          break;
+        }
+      }
+    }
+    pb[j] = keep;
+  }
+  __syncthreads();
+  block_exclusive_scan(pa, k, warp_total);
+  block_exclusive_scan(pb, k, warp_total);
+
+  for (int t = threadIdx.x; t < 2 * k; t += blockDim.x) {
+    const bool from_a = t < k;
+    const int j = from_a ? t : t - k;
+    const int* own = from_a ? pa : pb;
+    if (own[j + 1] == own[j]) continue;       // dropped duplicate or sentinel
+    const float s = from_a ? as[j] : bs[j];
+    const int32_t id = from_a ? ai[j] : bi[j];
+    const int other = from_a ? pb[count_before(bs, bi, k, s, id)] : pa[count_before(as, ai, k, s, id)];
+    const int pos = own[j] + other;
+    if (pos < k) {
+      out_score[u * out_stride + pos] = s;
+      out_item[u * out_stride + pos] = id;
+    }
+  }
+  for (int r = pa[k] + pb[k] + threadIdx.x; r < k; r += blockDim.x) {
+    out_score[u * out_stride + r] = kNegInf;
+    out_item[u * out_stride + r] = 0x7fffffff;
+  }
+}
+
+int topk_merge_dedup_pair(const float* a_score, const int32_t* a_item, int64_t a_row_stride, const float* b_score,
+                          const int32_t* b_item, int64_t b_row_stride, int64_t n_rows, int32_t k, float* out_score,
+                          int32_t* out_item, int64_t out_row_stride, cudaStream_t stream) {
+  TRK_CHECK_ARG(a_score && a_item && b_score && b_item && out_score && out_item, "topk_merge_dedup_pair: null pointer");
+  TRK_CHECK_ARG(n_rows >= 0 && n_rows <= 0x7fffffff, "topk_merge_dedup_pair: n_rows=%lld",
+                static_cast<long long>(n_rows));
+  TRK_CHECK_ARG(k >= 1 && k <= kPairMaxK, "topk_merge_dedup_pair: k=%d outside [1, %d]", k, kPairMaxK);
+  TRK_CHECK_ARG(a_row_stride >= k && b_row_stride >= k && out_row_stride >= k, "topk_merge_dedup_pair: bad strides");
+  if (n_rows == 0) return TRK_OK;
+  int table_bits = 6;
+  while ((1 << table_bits) < 2 * k) ++table_bits;        // load factor <= 1/2
+  const size_t smem = (4 * static_cast<size_t>(k) + 2 * (k + 1) + (size_t{1} << table_bits)) * sizeof(int32_t);
+  topk_merge_dedup_pair_kernel<<<static_cast<unsigned>(n_rows), kPairThreads, smem, stream>>>(
+      a_score, a_item, a_row_stride, b_score, b_item, b_row_stride, k, table_bits, out_score, out_item,
+      out_row_stride);
+  TRK_CHECK_LAUNCH();
+  return TRK_OK;
+}
+
 }  // namespace trk

@@ -452,6 +452,23 @@ def topk_merge_received(recv, n_users, n_lists, k, dedup=False):
     return out
 
 
+def topk_merge_dedup(a, b, out=None):
+    """Two PackedTopK [U, k] of the same users -> PackedTopK [U, k]: the top-k of their union with every item once, at
+    its higher score (trk_topk_merge_dedup_pair, any k <= wide_max_k()).  The fold of the per-taste lists of a mixture
+    of tastes on the wide route; `out` must be a third buffer."""
+    lib = require_cuda()
+    if a.k != b.k or a.n_users != b.n_users:
+        raise ValueError('topk_merge_dedup: lists of [%d, %d] and [%d, %d]' % (a.n_users, a.k, b.n_users, b.k))
+    if out is None:
+        out = PackedTopK(a.n_users, a.k, a.buf.device)
+    if a.n_users == 0:
+        return out
+    rc = lib.trk_topk_merge_dedup_pair(a.score_ptr(), a.item_ptr(), 2 * a.k, b.score_ptr(), b.item_ptr(), 2 * b.k,
+                                       a.n_users, a.k, out.score_ptr(), out.item_ptr(), 2 * out.k, _stream())
+    _lib.check(rc, 'trk_topk_merge_dedup_pair')
+    return out
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # filter form of the fused top-k: 1 tensor pass + exact fp32 re-scoring of the survivors
 # ---------------------------------------------------------------------------------------------------------------

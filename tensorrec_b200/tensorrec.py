@@ -68,17 +68,20 @@ ATTENTION_MIN_ITEMS = 1024
 
 
 def topk_route(k, n_items, model_ok, single_taste, filter_max_k, exact_max_k, sharded=False, euclidean=False,
-               attention=False):
+               attention=False, merge_max_k=32):
     """The route of a top-k call -- 'filter', 'exact3', 'wide' or 'dense+rank' -- from k, the catalogue size and the
     model alone.  model_ok: the tensor-core kernels evaluate the model (built-in dot / cosine prediction, or any
-    built-in similar-items graph, no attention, d_pad <= 128); single_taste: one taste (the wide route has no
-    de-duplicating merge); filter_max_k / exact_max_k: the k limits of the filter and of the exact 3-pass kernel.
+    built-in similar-items graph, no attention, d_pad <= 128); single_taste: one taste; filter_max_k / exact_max_k:
+    the k limits of the filter and of the exact 3-pass kernel; merge_max_k: the largest k whose per-taste lists the
+    caller can merge with de-duplication (32: trk_topk_merge alone; WIDE_MAX_K: with trk_topk_merge_dedup_pair on the
+    wide route), so a mixture of tastes takes the wide route under the one-taste conditions when k <= merge_max_k.
     sharded: an item-sharded call, where every rank must take the same route (the exchange is collective), so a
     rank's shard size does not decide the wide route.  TOPK_PATH='exact' means "no filter": k > exact_max_k then
     goes to dense+rank.  euclidean: a Euclidean user x item model (model_ok from _euclidean_tensor_ok), which has no
     filter or wide form: 'exact3' for k <= exact_max_k on catalogues of at least EUCLIDEAN_MIN_ITEMS items (any shard
     size in a sharded call), 'dense+rank' otherwise.  attention: a mixture of tastes with an attention graph (model_ok
-    from _tastes_tensor_ok), whose softmax has no filter or wide form either: the same rule with ATTENTION_MIN_ITEMS."""
+    from _tastes_tensor_ok), whose softmax has no filter or wide form either: the same rule with ATTENTION_MIN_ITEMS.
+    merge_max_k does not apply to either."""
     if not model_ok:
         return 'dense+rank'
     if euclidean or attention:
@@ -90,7 +93,7 @@ def topk_route(k, n_items, model_ok, single_taste, filter_max_k, exact_max_k, sh
         if n_items == 0:
             return 'dense+rank'
         return 'filter' if TOPK_PATH != 'exact' and k <= filter_max_k else 'exact3'
-    if TOPK_PATH == 'exact' or not single_taste or k > WIDE_MAX_K:
+    if TOPK_PATH == 'exact' or k > WIDE_MAX_K or (not single_taste and k > merge_max_k):
         return 'dense+rank'
     return 'wide' if sharded or n_items >= WIDE_MIN_ITEMS else 'dense+rank'
 
@@ -596,7 +599,9 @@ class TensorRec(object):
 
     def _tensor_path_ok(self, allow_tastes=False):
         """Can the tensor-core kernels evaluate this model?  allow_tastes: the fused top-k also covers n_tastes > 1 without
-        attention (one sweep per taste, then a de-duplicating merge: the prediction is the maximum over the tastes)."""
+        attention (one sweep per taste, then a de-duplicating merge: the prediction is the maximum over the tastes) --
+        for k <= 32 one merge of all the per-taste lists, on the wide route a pairwise fold of each taste's list into
+        the running result (DESIGN §3.6)."""
         if SCORE_PATH == 'exact':
             return False
         ok = (type(self.prediction_graph_factory) in (DotProductPredictionGraph, CosineSimilarityPredictionGraph)
@@ -879,7 +884,10 @@ class TensorRec(object):
         user_batch_size: users are processed in blocks of this many rows (bounds device memory at 10M+ users).
         32 < k <= WIDE_MAX_K on catalogues of at least WIDE_MIN_ITEMS items runs on the wide form of the filter (each
         user's candidates in a list in device memory, rows the certificate rejects scored dense and ranked); the default
-        user blocks then keep those lists within PREDICT_BLOCK_BYTES.  Euclidean models run k <= 32 on the exact kernel
+        user blocks then keep those lists within PREDICT_BLOCK_BYTES.  A mixture of tastes without attention takes the
+        same routes as one taste: one sweep per taste, and on the wide route each taste's top-k folded into the running
+        result by a de-duplicating merge (last_topk_info['fallback_rows'] sums the tastes' fallback rows).  Euclidean
+        models run k <= 32 on the exact kernel
         (catalogues of at least EUCLIDEAN_MIN_ITEMS items) and larger k on dense+rank with tensor-core scoring; so do
         mixtures of tastes with an attention graph (ATTENTION_MIN_ITEMS), on the taste-collapsing kernel.
         last_topk_info['path'] names the route (topk_route).
@@ -933,7 +941,8 @@ class TensorRec(object):
                 item_hsq = kernels.item_half_sqnorm(items)
 
         if user_batch_size is None:
-            user_batch_size = self._topk_block_rows(path, n_users, n_items, k, gather_group, device)
+            user_batch_size = self._topk_block_rows(path, n_users, n_items, k, gather_group, device,
+                                                    n_tastes=self.n_tastes)
         blocks = self._user_blocks(user_in, n_items, user_batch_size)
 
         def sweeps(block_in, u0, u1, route, excl):
@@ -943,18 +952,27 @@ class TensorRec(object):
                 return kernels.topk_tastes(users, items, self.n_tastes, True, k, item_id_offset=item_id_offset,
                                            excl=excl), [(None, 0)]
             # mixture of tastes (no attention): prediction = max over tastes (recommendation_graphs.py:107), so the top-k
-            # lies in the union of the per-taste top-k lists: one fused sweep per taste, then a de-duplicating merge
-            per_taste = []
+            # lies in the union of the per-taste top-k lists: one fused sweep per taste, then a de-duplicating merge.
+            # The wide route folds each taste's list into the running result right after its sweep (DESIGN §3.6), so a
+            # block holds three lists of k entries per row whatever the number of tastes.
+            tops, counters, spare = [], [], None
             for t in range(self.n_tastes):
                 users = self._side_operands('user', block_in, device, for_filter=route != 'exact3', taste=t)
-                per_taste.append(kernels.topk_fused(route, users, items, k, fitems=fitems, excl=excl,
-                                                    item_id_offset=item_id_offset, item_hsq=item_hsq,
-                                                    block_bytes=self.PREDICT_BLOCK_BYTES))
-            top = per_taste[0][0]
-            if self.n_tastes > 1:
-                stacked = torch.stack([sweep[0].buf for sweep in per_taste]).contiguous()       # [T, U_block, 2k]
+                taste_top, cnt, cap = kernels.topk_fused(route, users, items, k, fitems=fitems, excl=excl,
+                                                         item_id_offset=item_id_offset, item_hsq=item_hsq,
+                                                         block_bytes=self.PREDICT_BLOCK_BYTES)
+                counters.append((cnt, cap))
+                if route == 'wide' and tops:
+                    spare = kernels.topk_merge_dedup(tops[0], taste_top, out=spare)
+                    tops[0], spare = spare, tops[0]
+                else:
+                    tops.append(taste_top)
+                del users, taste_top
+            top = tops[0]
+            if len(tops) > 1:
+                stacked = torch.stack([t.buf for t in tops]).contiguous()       # [T, U_block, 2k]
                 top = kernels.topk_merge_received(stacked, block_in.shape[0], self.n_tastes, k, dedup=True)
-            return top, [(cnt, cap) for _, cnt, cap in per_taste]
+            return top, counters
 
         def exchange(top, u0, u1):
             if gather_group is None:
@@ -1033,15 +1051,19 @@ class TensorRec(object):
             return TopK(top_i, top_s)
         return TopK(*kernels.to_host(top_i, top_s))
 
-    def _topk_block_rows(self, path, n_rows, n_items, k, gather_group=None, device=None):
+    def _topk_block_rows(self, path, n_rows, n_items, k, gather_group=None, device=None, n_tastes=1):
         """Default rows per block of a top-k call: every row at once on the k <= 32 fused routes; on dense+rank as many
         as keep the dense scores, ranks and selection masks within PREDICT_BLOCK_BYTES; on the wide route as many as
-        keep the candidate lists within PREDICT_BLOCK_BYTES at one item split per row.  (A block splits the items only
-        when it has fewer user blocks than the device has SMs; its rows x splits then stay below ~3 x 128 x the SM count,
-        about 1.2 GB of lists at k = 1024 on an H100.)  In a sharded call (gather_group) every rank takes the smallest
-        of the ranks' choices: each block ends in the collective exchange, so all ranks must cut the same blocks."""
+        keep the candidate lists within PREDICT_BLOCK_BYTES at one item split per row, and with n_tastes > 1 (a user x item
+        call of a mixture of tastes) the running, per-taste and merged PackedTopK of the pairwise fold (3 x 8k bytes per
+        row) as well.  (A block splits the items only when it has fewer user blocks than the device has SMs; its rows x
+        splits then stay below ~3 x 128 x the SM count, about 1.2 GB of lists at k = 1024 on an H100.)  In a sharded call
+        (gather_group) every rank takes the smallest of the ranks' choices: each block ends in the collective exchange,
+        so all ranks must cut the same blocks."""
         if path == 'wide':
             per_row = 8 * kernels.wide_list_capacity(k)
+            if n_tastes > 1:
+                per_row += 3 * 8 * k
             rows = max(2 * kernels.TILE_USERS, self.PREDICT_BLOCK_BYTES // per_row // 256 * 256)
         elif path == 'dense+rank':
             rows = kernels.dense_rank_rows(n_items, self.PREDICT_BLOCK_BYTES)
@@ -1053,11 +1075,11 @@ class TensorRec(object):
         return rows
 
     def _topk_path(self, k, n_items, model_ok, single_taste, **route):
-        """The route of a top-k call: topk_route(...) with the k limits of this model's kernels.  Starts
-        last_topk_info."""
+        """The route of a top-k call: topk_route(...) with the k limits of this model's kernels (the per-taste lists of
+        the wide route merge pairwise, up to WIDE_MAX_K).  Starts last_topk_info."""
         d_pad = kernels.d_pad_for(self.n_components)
         limits = (kernels.filter_max_k(), kernels.topk_max_k(d_pad)) if model_ok else (0, 0)
-        path = topk_route(k, n_items, model_ok, single_taste, *limits, **route)
+        path = topk_route(k, n_items, model_ok, single_taste, *limits, merge_max_k=WIDE_MAX_K, **route)
         self.last_topk_info = {'path': path, 'fallback_rows': 0}
         return path
 
