@@ -102,16 +102,6 @@ size_t rank_full_workspace_bytes(int64_t, int64_t);
 int rank_full(const float*, int32_t*, int64_t, int64_t, void*, size_t, cudaStream_t);
 int order_from_ranks(const int32_t*, int64_t, int32_t*, cudaStream_t);
 int score_topk_max_k(int32_t);
-int score_topk_f16x3(const void*, const float*, const float*, const void*, const float*, int64_t, int64_t, int32_t,
-                     int32_t, int32_t, int32_t, float*, int32_t*, const int32_t*, const int32_t*, const int32_t*,
-                     const int32_t*, const float*, const float*, cudaStream_t);
-int score_dense_f16x3(const void*, const float*, const float*, const void*, const float*, int64_t, int64_t, int32_t,
-                      float*, int64_t, const float*, const float*, cudaStream_t);
-int score_topk_tastes_f16x3(const void*, const float*, const float*, int32_t, int32_t, const void*, const float*,
-                            int64_t, int64_t, int32_t, int32_t, int32_t, int32_t, float*, int32_t*, const int32_t*,
-                            const int32_t*, const int32_t*, cudaStream_t);
-int score_dense_tastes_f16x3(const void*, const float*, const float*, int32_t, int32_t, const void*, const float*,
-                             int64_t, int64_t, int32_t, float*, int64_t, cudaStream_t);
 int topk_merge(const float*, const int32_t*, int64_t, int32_t, int32_t, int32_t, int64_t, int64_t, float*, int32_t*,
                int64_t, const int32_t*, int32_t, cudaStream_t);
 int topk_merge_dedup_pair(const float*, const int32_t*, int64_t, const float*, const int32_t*, int64_t, int64_t,
@@ -225,9 +215,9 @@ int trk_score_topk_f16x3(const void* user_split, const float* user_scale, const 
                          const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
                          int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset, float* cand_score,
                          int32_t* cand_item, const int32_t* n_users_live, void* stream) {
-  return trk::score_topk_f16x3(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k,
-                               n_splits, item_id_offset, cand_score, cand_item, n_users_live, nullptr, nullptr, nullptr,
-                               nullptr, nullptr, trk::as_stream(stream));
+  return trk::score_tc({user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k, n_splits,
+                        item_id_offset, cand_score, cand_item, n_users_live},
+                       trk::as_stream(stream));
 }
 
 int trk_score_topk_f16x3_excl(const void* user_split, const float* user_scale, const float* user_bias,
@@ -236,9 +226,9 @@ int trk_score_topk_f16x3_excl(const void* user_split, const float* user_scale, c
                               int32_t* cand_item, const int32_t* n_users_live, const int32_t* excl_indptr,
                               const int32_t* excl_ids, const int32_t* excl_row_map, void* stream) {
   TRK_CHECK_ARG(excl_indptr != nullptr && excl_ids != nullptr, "trk_score_topk_f16x3_excl: null exclusion list");
-  return trk::score_topk_f16x3(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k,
-                               n_splits, item_id_offset, cand_score, cand_item, n_users_live, excl_indptr, excl_ids,
-                               excl_row_map, nullptr, nullptr, trk::as_stream(stream));
+  return trk::score_tc({user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k, n_splits,
+                        item_id_offset, cand_score, cand_item, n_users_live, excl_indptr, excl_ids, excl_row_map},
+                       trk::as_stream(stream));
 }
 
 int trk_score_topk_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
@@ -249,16 +239,20 @@ int trk_score_topk_euclid_f16x3(const void* user_split, const float* user_scale,
                                 const float* item_half_sqnorm, void* stream) {
   TRK_CHECK_ARG(user_half_sqnorm != nullptr && item_half_sqnorm != nullptr,
                 "trk_score_topk_euclid_f16x3: null squared norms");
-  return trk::score_topk_f16x3(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k,
-                               n_splits, item_id_offset, cand_score, cand_item, n_users_live, excl_indptr, excl_ids,
-                               excl_row_map, user_half_sqnorm, item_half_sqnorm, trk::as_stream(stream));
+  return trk::score_tc({user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k, n_splits,
+                        item_id_offset, cand_score, cand_item, n_users_live, excl_indptr, excl_ids, excl_row_map,
+                        user_half_sqnorm, item_half_sqnorm},
+                       trk::as_stream(stream));
 }
 
 int trk_score_dense_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
                           const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
                           int32_t d_pad, float* out, int64_t out_row_stride, void* stream) {
-  return trk::score_dense_f16x3(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad,
-                                out, out_row_stride, nullptr, nullptr, trk::as_stream(stream));
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad};
+  a.dense = true;
+  a.dense_out = out;
+  a.dense_stride = out_row_stride;
+  return trk::score_tc(a, trk::as_stream(stream));
 }
 
 int trk_score_dense_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
@@ -267,16 +261,27 @@ int trk_score_dense_euclid_f16x3(const void* user_split, const float* user_scale
                                  const float* item_half_sqnorm, void* stream) {
   TRK_CHECK_ARG(user_half_sqnorm != nullptr && item_half_sqnorm != nullptr,
                 "trk_score_dense_euclid_f16x3: null squared norms");
-  return trk::score_dense_f16x3(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad,
-                                out, out_row_stride, user_half_sqnorm, item_half_sqnorm, trk::as_stream(stream));
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad};
+  a.user_half_sqnorm = user_half_sqnorm;
+  a.item_half_sqnorm = item_half_sqnorm;
+  a.dense = true;
+  a.dense_out = out;
+  a.dense_stride = out_row_stride;
+  return trk::score_tc(a, trk::as_stream(stream));
 }
 
 int trk_score_dense_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
                                  int32_t n_tastes, int32_t attention, const void* item_split, const float* item_meta,
                                  int64_t n_users, int64_t n_items, int32_t d_pad, float* out, int64_t out_row_stride,
                                  void* stream) {
-  return trk::score_dense_tastes_f16x3(user_split, user_scale, user_bias, n_tastes, attention, item_split, item_meta,
-                                       n_users, n_items, d_pad, out, out_row_stride, trk::as_stream(stream));
+  TRK_CHECK_ARG(n_tastes >= 1, "score_tastes: n_tastes=%d < 1", n_tastes);
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad};
+  a.dense = true;
+  a.dense_out = out;
+  a.dense_stride = out_row_stride;
+  a.n_tastes = n_tastes;
+  a.attention = attention;
+  return trk::score_tc(a, trk::as_stream(stream));
 }
 
 int trk_score_topk_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
@@ -285,9 +290,15 @@ int trk_score_topk_tastes_f16x3(const void* user_split, const float* user_scale,
                                 int32_t item_id_offset, float* cand_score, int32_t* cand_item,
                                 const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
                                 void* stream) {
-  return trk::score_topk_tastes_f16x3(user_split, user_scale, user_bias, n_tastes, attention, item_split, item_meta,
-                                      n_users, n_items, d_pad, k, n_splits, item_id_offset, cand_score, cand_item,
-                                      excl_indptr, excl_ids, excl_row_map, trk::as_stream(stream));
+  TRK_CHECK_ARG(n_tastes >= 1, "score_tastes: n_tastes=%d < 1", n_tastes);
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k, n_splits,
+                        item_id_offset, cand_score, cand_item};
+  a.excl_indptr = excl_indptr;
+  a.excl_ids = excl_ids;
+  a.excl_row_map = excl_row_map;
+  a.n_tastes = n_tastes;
+  a.attention = attention;
+  return trk::score_tc(a, trk::as_stream(stream));
 }
 
 int trk_topk_merge(const float* cand_score, const int32_t* cand_item, int64_t n_users, int32_t n_lists,

@@ -58,6 +58,38 @@ int encode_tiled_3d(CUtensorMap* map, CUtensorMapDataType type, const void* base
                     uint64_t planes, uint64_t row_bytes, uint64_t plane_bytes, uint32_t box_cols, uint32_t box_rows,
                     uint32_t box_planes, CUtensorMapL2promotion l2_promotion);
 
+// Host arguments of score_tc (score_topk_tc.cu), which validates them and launches the exact tensor-core kernel behind
+// every trk_score_{topk,dense}* entry point.  The fields up to item_half_sqnorm are the arguments of
+// trk_score_topk_euclid_f16x3, in its order.  The score form follows from the fields that are set: n_tastes != 0 is a
+// mixture of tastes (attention != 0: with attention), the two norms are Euclidean similarity, neither is dot / cosine.
+struct ScoreTcArgs {
+  const void* user_split = nullptr;
+  const float* user_scale = nullptr;
+  const float* user_bias = nullptr;   // may be null
+  const void* item_split = nullptr;
+  const float* item_meta = nullptr;
+  int64_t n_users = 0;
+  int64_t n_items = 0;
+  int32_t d_pad = 0;
+  int32_t k = 0;                      // top-k mode: k, n_splits .. n_users_live and the exclusion lists
+  int32_t n_splits = 0;
+  int32_t item_id_offset = 0;
+  float* cand_score = nullptr;
+  int32_t* cand_item = nullptr;
+  const int32_t* n_users_live = nullptr;
+  const int32_t* excl_indptr = nullptr;
+  const int32_t* excl_ids = nullptr;
+  const int32_t* excl_row_map = nullptr;
+  const float* user_half_sqnorm = nullptr;
+  const float* item_half_sqnorm = nullptr;
+  bool dense = false;                 // dense mode: the score matrix to dense_out instead of top-k candidates
+  float* dense_out = nullptr;
+  int64_t dense_stride = 0;
+  int32_t n_tastes = 0;
+  int32_t attention = 0;
+};
+int score_tc(const ScoreTcArgs& a, cudaStream_t stream);
+
 constexpr int kWarp = 32;
 constexpr int kSMsH100 = 132;
 

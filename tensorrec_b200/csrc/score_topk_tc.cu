@@ -20,6 +20,10 @@
 //                 list's current k-th best, rare insert into the sorted list in shared memory.  The two half-lists of
 //                 a row are merged at the end of the item range.  Items are visited in ascending id order and the
 //                 compare is strict, so equal scores keep the lower item id first -- tf.nn.top_k's order.
+//
+// Score forms (ScoreForm, one template parameter; DESIGN.md §3.7): dot / cosine as above, Euclidean similarity (§3.4),
+// and mixtures of tastes collapsed by a max or by attention (§3.5).  score_tc is the one host entry point behind every
+// trk_score_{topk,dense}* function: it validates the arguments and launches one of the 24 instantiations.
 #include "common.cuh"
 
 namespace trk {
@@ -61,7 +65,16 @@ struct TcExcl {
   const int32_t* row_map;
 };
 
-// Euclidean similarity (kEuclid instantiations): -1/2 |row|^2 of every user row [n_users] and item column, as
+// The score form of an instantiation: what the epilogue makes of a (user, item) tile's accumulators.
+enum ScoreForm {
+  kFormDot,               // dot / cosine (score_chunk)
+  kFormEuclid,            // Euclidean similarity (score_chunk_euclid, TcEuclid)
+  kFormTastesMax,         // pred = max_t u_t . i        (recommendation_graphs.py:107; collapse_chunk, TcTastes)
+  kFormTastesAttention,   // pred = sum_t softmax_t(a_t . i) u_t . i   (:96-103)
+};
+__host__ __device__ constexpr bool is_tastes(ScoreForm f) { return f == kFormTastesMax || f == kFormTastesAttention; }
+
+// Euclidean similarity (kFormEuclid): -1/2 |row|^2 of every user row [n_users] and item column, as
 // operand_half_sqnorm_kernel (similar_items.cu) computes them from the split operands -- the norms see exactly the values
 // the dot product sees.  The epilogue reads item norms for whole 128-column tiles, so item_half_sqnorm holds
 // n_items_padded256 entries, 0 beyond n_items (finite: the meta's -inf bias still gives those columns -inf).  Also a
@@ -71,7 +84,7 @@ struct TcEuclid {
   const float* item_half_sqnorm;
 };
 
-// Mixtures of tastes (kTastes instantiations): every user has n_ops operand rows -- u_0 .. u_{T-1} and, with attention,
+// Mixtures of tastes (the tastes forms): every user has n_ops operand rows -- u_0 .. u_{T-1} and, with attention,
 // a_0 .. a_{T-1} -- stacked as [n_ops, n_users, 2 d_pad] with scales [n_ops, n_users].  A consumer warpgroup's 64
 // accumulator rows hold per_wg = 64 / n_ops users x n_ops operands (row j * per_wg + q = operand j of user q; rows at
 // or beyond n_ops * per_wg are never loaded nor read), so a user block is 2 per_wg users and all operands of a (user,
@@ -81,8 +94,6 @@ struct TcTastes {
   int32_t n_tastes;
   int32_t per_wg;
 };
-constexpr int kTastesMax = 1;         // pred = max_t u_t . i        (recommendation_graphs.py:107)
-constexpr int kTastesAttention = 2;   // pred = sum_t softmax_t(a_t . i) u_t . i   (:96-103)
 
 // shared-memory carve-up (offsets from a 1024-byte aligned base)
 struct SmemLayout {
@@ -168,15 +179,7 @@ __device__ __forceinline__ float score_chunk_euclid(uint32_t (&r)[32], const flo
   return cmax;
 }
 
-// Final scores of one 32-column chunk, dot / cosine or Euclidean.
-template <bool kEuclid>
-__device__ __forceinline__ float score_chunk_as(uint32_t (&r)[32], const float2* meta, const float* ihsq, float su,
-                                                float usq, float ubias) {
-  if constexpr (kEuclid) return score_chunk_euclid(r, meta, ihsq, su, usq, ubias);
-  else return score_chunk(r, meta, su, ubias);
-}
-
-// The taste collapse of one staged chunk (kTastes): columns [32 c, 32 c + 32) of both 64-column halves of the tile,
+// The taste collapse of one staged chunk: columns [32 c, 32 c + 32) of both 64-column halves of the tile,
 // in the warpgroup's staging tile (stage = acc_stage, rows as in TcTastes).  Every (column half, user, column) element
 // is collapsed by one thread -- all 128 of the warpgroup share the work, lane = column -- and its final score replaces
 // operand row 0 of its user; the element reads and writes only its own user's rows in its own column.  Reference
@@ -187,7 +190,7 @@ __device__ __forceinline__ float score_chunk_as(uint32_t (&r)[32], const float2*
 //   attention:  m = max_t a_t,  e_t = expf(a_t - m),  s = sum_t e_t,  pred = sum_t p_t * (e_t / s)  (taste order);
 //   score = (pred + ub) + ib.
 // With attention, e_t is parked in a_t's staging row between the two passes.
-template <int kTastes>
+template <ScoreForm kForm>
 __device__ __forceinline__ void collapse_chunk(float* stage, int wt, int c, const float2* meta, const TcParams& p,
                                                const TcTastes z, int64_t u0) {
   const int lane = wt % 32;
@@ -201,7 +204,7 @@ __device__ __forceinline__ void collapse_chunk(float* stage, int wt, int c, cons
     float* col = stage + (h * kWgRows + q) * kStageStride + lane;   // operand j at col[j * per_wg * kStageStride]
     const int64_t op_stride = z.per_wg * kStageStride;
     float pred;
-    if constexpr (kTastes == kTastesMax) {
+    if constexpr (kForm == kFormTastesMax) {
       pred = -__int_as_float(0x7f800000);
       for (int t = 0; t < n_tastes; ++t) {
         const float su = u_ok ? __ldg(p.user_scale + t * p.n_users + u) : 0.0f;
@@ -234,12 +237,22 @@ __device__ __forceinline__ void collapse_chunk(float* stage, int wt, int c, cons
   }
 }
 
-// Chunk maximum of final scores (kTastes: collapse_chunk formed them).
+// Chunk maximum of final scores (tastes forms: collapse_chunk formed them).
 __device__ __forceinline__ float chunk_max(const uint32_t (&r)[32]) {
   float cmax = -__int_as_float(0x7f800000);
 #pragma unroll
   for (int j = 0; j < 32; ++j) cmax = fmaxf(cmax, __uint_as_float(r[j]));
   return cmax;
+}
+
+// Final scores of one 32-column chunk of one user row in form kForm, and their maximum.  Dot / Euclidean: r[] holds
+// raw accumulators (ihsq = the chunk's item norms, usq = the row's |u|^2); tastes: r[] already holds final scores.
+template <ScoreForm kForm>
+__device__ __forceinline__ float score_chunk_as(uint32_t (&r)[32], const float2* meta, const float* ihsq, float su,
+                                                float usq, float ubias) {
+  if constexpr (is_tastes(kForm)) return chunk_max(r);
+  else if constexpr (kForm == kFormEuclid) return score_chunk_euclid(r, meta, ihsq, su, usq, ubias);
+  else return score_chunk(r, meta, su, ubias);
 }
 
 // Exclusion (kExclude): the final scores of the chunk's columns [base, base + 32) named in list row `xr` become -inf
@@ -278,16 +291,13 @@ struct ExclCursor<false> {};
 
 // One 32-column chunk of one user row: final scores, then (top-k mode) the row's listed columns masked (kExclude) and
 // the rare inserts, or (dense mode) the store.  `x` is taken by value: a reference bound to the kernel parameter
-// changes the generated code of the instantiations without exclusion.  kEuclid: the Euclidean score (ihsq = the tile's
-// item norms, usq = the row's |u|^2).  kTastes: r[] already holds final scores.
-template <bool kDense, bool kExclude, bool kEuclid, int kTastes = 0>
+// changes the generated code of the instantiations without exclusion.  ihsq = the tile's item norms (kFormEuclid).
+template <bool kDense, bool kExclude, ScoreForm kForm>
 __device__ __forceinline__ void process_chunk(uint32_t (&r)[32], int c, int t, int32_t id0, const float2* meta,
                                               const float* ihsq, float su, float usq, float ubias, float& thr,
                                               float* ls, int32_t* li, const TcParams& p, int64_t u, bool u_ok,
                                               const TcExcl x, ExclCursor<kExclude>& xc) {
-  float cmax;
-  if constexpr (kTastes != 0) cmax = chunk_max(r);
-  else cmax = score_chunk_as<kEuclid>(r, meta + c * 32, ihsq + c * 32, su, usq, ubias);
+  float cmax = score_chunk_as<kForm>(r, meta + c * 32, ihsq + c * 32, su, usq, ubias);
   if constexpr (!kDense) {
     if constexpr (kExclude) {
       const int32_t base = t * kBlockN + c * 32;   // local id of the chunk's first column
@@ -343,11 +353,10 @@ __device__ __forceinline__ void store_chunk_tma(const uint32_t (&r)[32], uint32_
 }
 
 // kNKB = d_pad / 64 k-blocks per operand half.  kExclude (top-k mode): columns named in the row's exclusion list are
-// left out of the top-k (excl_mask_scores).  kEuclid: Euclidean similarity (score_chunk_euclid) in either mode.
-// kTastes (kTastesMax / kTastesAttention): a mixture of tastes collapsed per (user, item) (collapse_chunk); map_users
-// is then the 3-D map of the stacked operand, a user block holds 2 z.per_wg users, and in dense mode map_out's box
-// is 32 columns x z.per_wg rows.
-template <bool kDense, int kNKB, bool kExclude = false, bool kEuclid = false, int kTastes = 0>
+// left out of the top-k (excl_mask_scores).  kForm: the score form, in either mode.  The tastes forms collapse a
+// mixture of tastes per (user, item) (collapse_chunk); map_users is then the 3-D map of the stacked operand, a user
+// block holds 2 z.per_wg users, and in dense mode map_out's box is 32 columns x z.per_wg rows.
+template <bool kDense, int kNKB, bool kExclude, ScoreForm kForm>
 __global__ void __launch_bounds__(kTcThreads, 1)
 score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_constant__ CUtensorMap map_items,
                 const __grid_constant__ CUtensorMap map_out, const TcParams p, const TcExcl x, const TcEuclid e,
@@ -401,7 +410,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
         const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
         if (t1 <= t0 || ub >= live_blocks) continue;
         mbar_wait(a_empty, (witer & 1) ^ 1);  // the MMAs of the previous work item no longer read A
-        if constexpr (kTastes != 0) {
+        if constexpr (is_tastes(kForm)) {
           // one box of n_ops x per_wg rows per warpgroup half and k-block; a half without users is not loaded
           const int32_t u0 = ub * 2 * z.per_wg;
           const int n_halves = u0 + z.per_wg < p.n_users ? 2 : 1;
@@ -462,14 +471,14 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
       const int t0 = sp * p.tiles_per_split;
       const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
       if (ub >= live_blocks) continue;   // (an empty split still emits its sentinel candidates)
-      // kTastes: this warpgroup's users start at u0; the thread of row q < per_wg owns user u0 + q, later rows own none
-      const int64_t u0 = kTastes != 0 ? static_cast<int64_t>(ub) * 2 * z.per_wg + g * z.per_wg : 0;
-      const int64_t u = kTastes != 0 ? u0 + wt % kWgRows : static_cast<int64_t>(ub) * kBlockM + row;
-      const bool u_ok = u < p.n_users && (kTastes == 0 || wt % kWgRows < z.per_wg);
-      const float su = (kTastes == 0 && u_ok) ? __ldg(p.user_scale + u) : 0.0f;
-      const float ubias = (kTastes == 0 && u_ok && p.user_bias != nullptr) ? __ldg(p.user_bias + u) : 0.0f;
-      float usq = 0.0f;   // kEuclid: |u|^2 (rows at or beyond n_users read nothing)
-      if constexpr (kEuclid) usq = u_ok ? -2.0f * __ldg(e.user_half_sqnorm + u) : 0.0f;
+      // tastes: this warpgroup's users start at u0; the thread of row q < per_wg owns user u0 + q, later rows own none
+      const int64_t u0 = is_tastes(kForm) ? static_cast<int64_t>(ub) * 2 * z.per_wg + g * z.per_wg : 0;
+      const int64_t u = is_tastes(kForm) ? u0 + wt % kWgRows : static_cast<int64_t>(ub) * kBlockM + row;
+      const bool u_ok = u < p.n_users && (!is_tastes(kForm) || wt % kWgRows < z.per_wg);
+      const float su = (!is_tastes(kForm) && u_ok) ? __ldg(p.user_scale + u) : 0.0f;
+      const float ubias = (!is_tastes(kForm) && u_ok && p.user_bias != nullptr) ? __ldg(p.user_bias + u) : 0.0f;
+      float usq = 0.0f;   // kFormEuclid: |u|^2 (rows at or beyond n_users read nothing)
+      if constexpr (kForm == kFormEuclid) usq = u_ok ? -2.0f * __ldg(e.user_half_sqnorm + u) : 0.0f;
       float thr = kNegInf;
       // kExclude: this row's list row and the first listed id >= the current chunk.  Rows of a gathered launch beyond
       // *n_users_live have no map entry and are discarded by the caller: they exclude nothing.
@@ -519,7 +528,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
         // ---- epilogue: two rounds, each stages columns [32 c, 32 c + 32) of both 64-column halves ----
         const int32_t id0 = p.item_id_offset + t * kBlockN;
         const float2* meta = p.item_meta + static_cast<int64_t>(t) * kBlockN;
-        const float* ihsq = kEuclid ? e.item_half_sqnorm + static_cast<int64_t>(t) * kBlockN : nullptr;
+        const float* ihsq = kForm == kFormEuclid ? e.item_half_sqnorm + static_cast<int64_t>(t) * kBlockN : nullptr;
 #pragma unroll
         for (int c = 0; c < 2; ++c) {
           named_barrier_sync(1 + g, kConsumerThreads);   // the previous round's rows have been read
@@ -531,8 +540,8 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
             acc_stage[((col / 64) * kWgRows + wgmma_acc_row(wt, i)) * kStageStride + col % 32] = acc[i];
           }
           named_barrier_sync(1 + g, kConsumerThreads);
-          if constexpr (kTastes != 0) {   // row q of each half now holds user q's final scores
-            collapse_chunk<kTastes>(acc_stage, wt, c, meta, p, z, u0);
+          if constexpr (is_tastes(kForm)) {   // row q of each half now holds user q's final scores
+            collapse_chunk<kForm>(acc_stage, wt, c, meta, p, z, u0);
             named_barrier_sync(1 + g, kConsumerThreads);
           }
           uint32_t r[32];
@@ -541,21 +550,21 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
           for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(src[j]);
           const int chunk = half * 2 + c;
           if (kDense && p.tma_store) {
-            if constexpr (kTastes != 0) {   // the users are rows 0 .. per_wg - 1 (<= 32): the first warp of each half
+            if constexpr (is_tastes(kForm)) {   // users are rows 0 .. per_wg - 1 (<= 32): the first warp of each half
               if (warp % 2 == 0) {
                 store_chunk_tma(r, stage_base + (n_stored & 1) * kStoreTileBytes, lane, &map_out,
                                 t * kBlockN + chunk * 32, static_cast<int32_t>(u0));
                 ++n_stored;
               }
             } else {
-              score_chunk_as<kEuclid>(r, meta + chunk * 32, ihsq + chunk * 32, su, usq, ubias);
+              score_chunk_as<kForm>(r, meta + chunk * 32, ihsq + chunk * 32, su, usq, ubias);
               store_chunk_tma(r, stage_base + (n_stored & 1) * kStoreTileBytes, lane, &map_out,
                               t * kBlockN + chunk * 32, ub * kBlockM + g * kWgRows + (warp % 2) * 32);
               ++n_stored;
             }
-          } else if (kTastes == 0 || wt % kWgRows < z.per_wg) {
-            process_chunk<kDense, kExclude, kEuclid, kTastes>(r, chunk, t, id0, meta, ihsq, su, usq, ubias, thr, ls, li,
-                                                              p, u, u_ok, x, xc);
+          } else if (!is_tastes(kForm) || wt % kWgRows < z.per_wg) {
+            process_chunk<kDense, kExclude, kForm>(r, chunk, t, id0, meta, ihsq, su, usq, ubias, thr, ls, li, p, u,
+                                                   u_ok, x, xc);
           }
         }
       }
@@ -611,153 +620,6 @@ int score_topk_max_k(int32_t d_pad) {
   return kMaxK;
 }
 
-template <bool kDense>
-static int launch_tc(const void* user_split, const float* user_scale, const float* user_bias,
-                     const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
-                     int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset, float* cand_score,
-                     int32_t* cand_item, float* dense_out, int64_t dense_stride, const int32_t* n_users_live,
-                     const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
-                     const float* user_half_sqnorm, const float* item_half_sqnorm, int32_t n_tastes,
-                     int32_t attention, cudaStream_t stream) {
-  TRK_CHECK_ARG(user_split && user_scale && item_split && item_meta, "score_tc: null operand");
-  TRK_CHECK_ARG((user_half_sqnorm == nullptr) == (item_half_sqnorm == nullptr),
-                "score_tc: user_half_sqnorm and item_half_sqnorm go together");
-  TRK_CHECK_ARG(reinterpret_cast<uintptr_t>(item_half_sqnorm) % 16 == 0, "score_tc: item_half_sqnorm must be 16-byte aligned");
-  const bool euclid = user_half_sqnorm != nullptr;
-  TRK_CHECK_ARG(n_users >= 1 && n_items >= 1, "score_tc: empty shape");
-  TRK_CHECK_ARG(n_users < (1ll << 31) && n_items < (1ll << 31) - 512, "score_tc: shape exceeds int32 indexing");
-  if (d_pad != 64 && d_pad != 128) {
-    set_error("score_tc: d_pad=%d not supported by the tensor-core kernel (64 or 128)", d_pad);
-    return TRK_ERR_UNSUPPORTED;
-  }
-  TRK_CHECK_ARG(reinterpret_cast<uintptr_t>(user_split) % 16 == 0 && reinterpret_cast<uintptr_t>(item_split) % 16 == 0 &&
-                    reinterpret_cast<uintptr_t>(item_meta) % 16 == 0,
-                "score_tc: operands must be 16-byte aligned");
-  if (!kDense) {
-    TRK_CHECK_ARG(cand_score && cand_item, "score_topk: null output");
-    if (k < 1 || k > kMaxK) {
-      set_error("score_topk: k=%d outside [1, %d]", k, kMaxK);
-      return TRK_ERR_UNSUPPORTED;
-    }
-  } else {
-    TRK_CHECK_ARG(dense_out && dense_stride >= n_items, "score_dense: bad output");
-  }
-  TRK_CHECK_ARG(n_splits >= 1, "score_tc: n_splits < 1");
-  TRK_CHECK_ARG((excl_indptr == nullptr) == (excl_ids == nullptr) && (excl_indptr != nullptr || excl_row_map == nullptr),
-                "score_topk: excl_indptr and excl_ids go together (excl_row_map needs both)");
-  // n_tastes != 0: a mixture of tastes on the stacked operand [n_ops, n_users, 2 d_pad] (TcTastes)
-  const bool tastes = n_tastes != 0;
-  TcTastes z = {0, 0, 0};
-  if (tastes) {
-    // (one operand row per user is the plain kernel: per_wg would exceed the 32 rows of a dense store tile)
-    TRK_CHECK_ARG(n_tastes >= 2 || (n_tastes == 1 && attention), "score_tastes: n_tastes=%d needs n_tastes >= 2 or attention",
-                  n_tastes);
-    TRK_CHECK_ARG(!euclid && n_users_live == nullptr, "score_tastes: no Euclidean form and no live-row count");
-    const int n_ops = n_tastes <= 64 ? (attention ? 2 : 1) * n_tastes : 65;
-    if (n_ops > kWgRows) {
-      set_error("score_tastes: %d operand rows per user (n_tastes=%d%s) exceed %d", n_ops, n_tastes,
-                attention ? ", attention" : "", kWgRows);
-      return TRK_ERR_UNSUPPORTED;
-    }
-    z = {n_ops, n_tastes, kWgRows / n_ops};
-  }
-
-  TcParams p;
-  p.user_scale = user_scale;
-  p.user_bias = user_bias;
-  p.item_meta = reinterpret_cast<const float2*>(item_meta);
-  p.n_users = n_users;
-  p.n_items = n_items;
-  p.n_kblocks = d_pad / kKBlock;
-  p.k = kDense ? 0 : k;
-  p.n_tiles = static_cast<int32_t>(ceil_div(n_items, kBlockN));
-  p.n_splits = n_splits;
-  p.tiles_per_split = static_cast<int32_t>(ceil_div(p.n_tiles, n_splits));
-  p.n_user_blocks = static_cast<int32_t>(ceil_div(n_users, tastes ? 2 * z.per_wg : kBlockM));
-  p.item_id_offset = item_id_offset;
-  p.cand_score = cand_score;
-  p.cand_item = cand_item;
-  p.dense_out = dense_out;
-  p.dense_stride = dense_stride;
-  p.n_users_live = n_users_live;
-  const TcExcl x = {excl_indptr, excl_ids, excl_row_map};
-  const TcEuclid e = {user_half_sqnorm, item_half_sqnorm};
-  p.tma_store = (kDense && dense_stride % 4 == 0 && reinterpret_cast<uintptr_t>(dense_out) % 16 == 0) ? 1 : 0;
-  p.n_stages = pick_stages(p.n_kblocks, p.k, p.tma_store != 0);
-  TRK_CHECK_ARG(p.n_stages >= 2, "score_tc: shared memory budget exceeded (d_pad=%d k=%d)", d_pad, k);
-
-  // operands: [rows, 2 d_pad] fp16 (hi | lo), boxes of one k-block x one tile
-  // (tastes: the stacked operand, boxes of one k-block x per_wg users x n_ops operands = one warpgroup's rows)
-  CUtensorMap map_users, map_items;
-  int rc = tastes ? encode_tiled_3d(&map_users, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, user_split, 2 * d_pad, n_users, z.n_ops,
-                                    4 * d_pad, 4 * d_pad * n_users, kKBlock, z.per_wg, z.n_ops,
-                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B)
-                  : encode_tiled_2d(&map_users, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, user_split, 2 * d_pad, n_users,
-                                    4 * d_pad, kKBlock, kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
-  if (rc != TRK_OK) return rc;
-  rc = encode_tiled_2d(&map_items, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, item_split, 2 * d_pad, n_items, 4 * d_pad, kKBlock,
-                       kBlockN, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
-  if (rc != TRK_OK) return rc;
-
-  CUtensorMap map_out = map_items;   // placeholder when the TMA store path is off
-  if (p.tma_store) {
-    rc = encode_tiled_2d(&map_out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, dense_out, n_items, n_users, 4 * dense_stride, 32,
-                         tastes ? z.per_wg : 32, CU_TENSOR_MAP_L2_PROMOTION_NONE);
-    if (rc != TRK_OK) return rc;
-  }
-  const uint32_t smem_bytes = make_layout(p.n_kblocks, p.n_stages, p.k, p.tma_store != 0).total + kSmemAlignSlack;
-  decltype(&score_tc_kernel<kDense, 1>) kernel = nullptr;
-  if constexpr (!kDense) {
-    if (excl_indptr != nullptr) kernel = p.n_kblocks == 2 ? score_tc_kernel<false, 2, true> : score_tc_kernel<false, 1, true>;
-  }
-  if (kernel == nullptr) kernel = p.n_kblocks == 2 ? score_tc_kernel<kDense, 2> : score_tc_kernel<kDense, 1>;
-  if (euclid) {
-    if constexpr (kDense) {
-      kernel = p.n_kblocks == 2 ? score_tc_kernel<true, 2, false, true> : score_tc_kernel<true, 1, false, true>;
-    } else if (excl_indptr != nullptr) {
-      kernel = p.n_kblocks == 2 ? score_tc_kernel<false, 2, true, true> : score_tc_kernel<false, 1, true, true>;
-    } else {
-      kernel = p.n_kblocks == 2 ? score_tc_kernel<false, 2, false, true> : score_tc_kernel<false, 1, false, true>;
-    }
-  }
-  if (tastes) {
-    const bool att = attention != 0;
-    const bool two = p.n_kblocks == 2;
-    if constexpr (kDense) {
-      kernel = att ? (two ? score_tc_kernel<true, 2, false, false, kTastesAttention>
-                          : score_tc_kernel<true, 1, false, false, kTastesAttention>)
-                   : (two ? score_tc_kernel<true, 2, false, false, kTastesMax>
-                          : score_tc_kernel<true, 1, false, false, kTastesMax>);
-    } else if (excl_indptr != nullptr) {
-      kernel = att ? (two ? score_tc_kernel<false, 2, true, false, kTastesAttention>
-                          : score_tc_kernel<false, 1, true, false, kTastesAttention>)
-                   : (two ? score_tc_kernel<false, 2, true, false, kTastesMax>
-                          : score_tc_kernel<false, 1, true, false, kTastesMax>);
-    } else {
-      kernel = att ? (two ? score_tc_kernel<false, 2, false, false, kTastesAttention>
-                          : score_tc_kernel<false, 1, false, false, kTastesAttention>)
-                   : (two ? score_tc_kernel<false, 2, false, false, kTastesMax>
-                          : score_tc_kernel<false, 1, false, false, kTastesMax>);
-    }
-  }
-  TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-  const int grid = capped_grid(static_cast<int64_t>(p.n_user_blocks) * n_splits, 1);
-  kernel<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, map_out, p, x, e, z);
-  TRK_CHECK_LAUNCH();
-  return TRK_OK;
-}
-
-int score_topk_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
-                     const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
-                     int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset, float* cand_score,
-                     int32_t* cand_item, const int32_t* n_users_live, const int32_t* excl_indptr,
-                     const int32_t* excl_ids, const int32_t* excl_row_map, const float* user_half_sqnorm,
-                     const float* item_half_sqnorm, cudaStream_t stream) {
-  return launch_tc<false>(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k,
-                          n_splits, item_id_offset, cand_score, cand_item, nullptr, 0, n_users_live, excl_indptr,
-                          excl_ids, excl_row_map, user_half_sqnorm, item_half_sqnorm, 0, 0, stream);
-}
-
 // Item splits of a dense launch over n_ub user blocks: enough that every SM gets work when there are few user blocks.
 static int32_t dense_splits(int64_t n_ub, int64_t n_items) {
   const int64_t n_tiles = ceil_div(n_items, kBlockN);
@@ -767,37 +629,121 @@ static int32_t dense_splits(int64_t n_ub, int64_t n_items) {
   return static_cast<int32_t>(splits);
 }
 
-int score_dense_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
-                      const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
-                      int32_t d_pad, float* out, int64_t out_row_stride, const float* user_half_sqnorm,
-                      const float* item_half_sqnorm, cudaStream_t stream) {
-  return launch_tc<true>(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, 0,
-                         dense_splits(ceil_div(n_users, kBlockM), n_items), 0, nullptr, nullptr, out, out_row_stride,
-                         nullptr, nullptr, nullptr, nullptr, user_half_sqnorm, item_half_sqnorm, 0, 0, stream);
-}
+// (the kernels of one instantiation, for score_tc: fn[d_pad / 64 - 1])
+using TcKernelFn = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, TcParams, TcExcl, TcEuclid, TcTastes);
+template <bool kDense, bool kExclude, ScoreForm kForm>
+struct TcKernel {
+  static constexpr TcKernelFn fn[2] = {score_tc_kernel<kDense, 1, kExclude, kForm>,
+                                       score_tc_kernel<kDense, 2, kExclude, kForm>};
+};
 
-int score_topk_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
-                            int32_t n_tastes, int32_t attention, const void* item_split, const float* item_meta,
-                            int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k, int32_t n_splits,
-                            int32_t item_id_offset, float* cand_score, int32_t* cand_item, const int32_t* excl_indptr,
-                            const int32_t* excl_ids, const int32_t* excl_row_map, cudaStream_t stream) {
-  TRK_CHECK_ARG(n_tastes >= 1, "score_tastes: n_tastes=%d < 1", n_tastes);
-  return launch_tc<false>(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k,
-                          n_splits, item_id_offset, cand_score, cand_item, nullptr, 0, nullptr, excl_indptr, excl_ids,
-                          excl_row_map, nullptr, nullptr, n_tastes, attention, stream);
-}
+int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
+  TRK_CHECK_ARG(a.user_split && a.user_scale && a.item_split && a.item_meta, "score_tc: null operand");
+  TRK_CHECK_ARG((a.user_half_sqnorm == nullptr) == (a.item_half_sqnorm == nullptr),
+                "score_tc: user_half_sqnorm and item_half_sqnorm go together");
+  TRK_CHECK_ARG(reinterpret_cast<uintptr_t>(a.item_half_sqnorm) % 16 == 0,
+                "score_tc: item_half_sqnorm must be 16-byte aligned");
+  const bool euclid = a.user_half_sqnorm != nullptr;
+  TRK_CHECK_ARG(a.n_users >= 1 && a.n_items >= 1, "score_tc: empty shape");
+  TRK_CHECK_ARG(a.n_users < (1ll << 31) && a.n_items < (1ll << 31) - 512, "score_tc: shape exceeds int32 indexing");
+  if (a.d_pad != 64 && a.d_pad != 128) {
+    set_error("score_tc: d_pad=%d not supported by the tensor-core kernel (64 or 128)", a.d_pad);
+    return TRK_ERR_UNSUPPORTED;
+  }
+  TRK_CHECK_ARG(reinterpret_cast<uintptr_t>(a.user_split) % 16 == 0 &&
+                    reinterpret_cast<uintptr_t>(a.item_split) % 16 == 0 &&
+                    reinterpret_cast<uintptr_t>(a.item_meta) % 16 == 0,
+                "score_tc: operands must be 16-byte aligned");
+  if (!a.dense) {
+    TRK_CHECK_ARG(a.cand_score && a.cand_item, "score_topk: null output");
+    if (a.k < 1 || a.k > kMaxK) {
+      set_error("score_topk: k=%d outside [1, %d]", a.k, kMaxK);
+      return TRK_ERR_UNSUPPORTED;
+    }
+    TRK_CHECK_ARG(a.n_splits >= 1, "score_tc: n_splits < 1");
+  } else {
+    TRK_CHECK_ARG(a.dense_out && a.dense_stride >= a.n_items, "score_dense: bad output");
+  }
+  TRK_CHECK_ARG((a.excl_indptr == nullptr) == (a.excl_ids == nullptr) &&
+                    (a.excl_indptr != nullptr || a.excl_row_map == nullptr),
+                "score_topk: excl_indptr and excl_ids go together (excl_row_map needs both)");
+  // n_tastes != 0: a mixture of tastes on the stacked operand [n_ops, n_users, 2 d_pad] (TcTastes)
+  const bool tastes = a.n_tastes != 0;
+  TcTastes z = {0, 0, 0};
+  if (tastes) {
+    // (one operand row per user is the plain kernel: per_wg would exceed the 32 rows of a dense store tile)
+    TRK_CHECK_ARG(a.n_tastes >= 2 || (a.n_tastes == 1 && a.attention),
+                  "score_tastes: n_tastes=%d needs n_tastes >= 2 or attention", a.n_tastes);
+    TRK_CHECK_ARG(!euclid && a.n_users_live == nullptr, "score_tastes: no Euclidean form and no live-row count");
+    const int n_ops = a.n_tastes <= 64 ? (a.attention ? 2 : 1) * a.n_tastes : 65;
+    if (n_ops > kWgRows) {
+      set_error("score_tastes: %d operand rows per user (n_tastes=%d%s) exceed %d", n_ops, a.n_tastes,
+                a.attention ? ", attention" : "", kWgRows);
+      return TRK_ERR_UNSUPPORTED;
+    }
+    z = {n_ops, a.n_tastes, kWgRows / n_ops};
+  }
+  const ScoreForm form = tastes ? (a.attention ? kFormTastesAttention : kFormTastesMax)
+                                : (euclid ? kFormEuclid : kFormDot);
 
-int score_dense_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
-                             int32_t n_tastes, int32_t attention, const void* item_split, const float* item_meta,
-                             int64_t n_users, int64_t n_items, int32_t d_pad, float* out, int64_t out_row_stride,
-                             cudaStream_t stream) {
-  TRK_CHECK_ARG(n_tastes >= 1, "score_tastes: n_tastes=%d < 1", n_tastes);
-  const int64_t n_ops = (attention ? 2 : 1) * static_cast<int64_t>(n_tastes);
-  const int64_t users_per_block = n_ops <= kWgRows ? 2 * (kWgRows / n_ops) : kBlockM;   // (launch_tc rejects the rest)
-  return launch_tc<true>(user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, 0,
-                         dense_splits(ceil_div(n_users, users_per_block), n_items), 0, nullptr, nullptr, out,
-                         out_row_stride, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, n_tastes, attention,
-                         stream);
+  TcParams p;
+  p.user_scale = a.user_scale;
+  p.user_bias = a.user_bias;
+  p.item_meta = reinterpret_cast<const float2*>(a.item_meta);
+  p.n_users = a.n_users;
+  p.n_items = a.n_items;
+  p.n_kblocks = a.d_pad / kKBlock;
+  p.k = a.dense ? 0 : a.k;
+  p.n_tiles = static_cast<int32_t>(ceil_div(a.n_items, kBlockN));
+  p.n_user_blocks = static_cast<int32_t>(ceil_div(a.n_users, tastes ? 2 * z.per_wg : kBlockM));
+  p.n_splits = a.dense ? dense_splits(p.n_user_blocks, a.n_items) : a.n_splits;
+  p.tiles_per_split = static_cast<int32_t>(ceil_div(p.n_tiles, p.n_splits));
+  p.item_id_offset = a.item_id_offset;
+  p.cand_score = a.cand_score;
+  p.cand_item = a.cand_item;
+  p.dense_out = a.dense_out;
+  p.dense_stride = a.dense_stride;
+  p.n_users_live = a.n_users_live;
+  const TcExcl x = {a.excl_indptr, a.excl_ids, a.excl_row_map};
+  const TcEuclid e = {a.user_half_sqnorm, a.item_half_sqnorm};
+  p.tma_store = (a.dense && a.dense_stride % 4 == 0 && reinterpret_cast<uintptr_t>(a.dense_out) % 16 == 0) ? 1 : 0;
+  p.n_stages = pick_stages(p.n_kblocks, p.k, p.tma_store != 0);
+  TRK_CHECK_ARG(p.n_stages >= 2, "score_tc: shared memory budget exceeded (d_pad=%d k=%d)", a.d_pad, p.k);
+
+  // operands: [rows, 2 d_pad] fp16 (hi | lo), boxes of one k-block x one tile
+  // (tastes: the stacked operand, boxes of one k-block x per_wg users x n_ops operands = one warpgroup's rows)
+  CUtensorMap map_users, map_items;
+  int rc = tastes ? encode_tiled_3d(&map_users, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, a.user_split, 2 * a.d_pad, a.n_users,
+                                    z.n_ops, 4 * a.d_pad, 4 * a.d_pad * a.n_users, kKBlock, z.per_wg, z.n_ops,
+                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B)
+                  : encode_tiled_2d(&map_users, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, a.user_split, 2 * a.d_pad, a.n_users,
+                                    4 * a.d_pad, kKBlock, kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  if (rc != TRK_OK) return rc;
+  rc = encode_tiled_2d(&map_items, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, a.item_split, 2 * a.d_pad, a.n_items, 4 * a.d_pad,
+                       kKBlock, kBlockN, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  if (rc != TRK_OK) return rc;
+
+  CUtensorMap map_out = map_items;   // placeholder when the TMA store path is off
+  if (p.tma_store) {
+    rc = encode_tiled_2d(&map_out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, a.dense_out, a.n_items, a.n_users,
+                         4 * a.dense_stride, 32, tastes ? z.per_wg : 32, CU_TENSOR_MAP_L2_PROMOTION_NONE);
+    if (rc != TRK_OK) return rc;
+  }
+  const uint32_t smem_bytes = make_layout(p.n_kblocks, p.n_stages, p.k, p.tma_store != 0).total + kSmemAlignSlack;
+  // every instantiation: [dense | top-k | top-k with exclusion][form][d_pad / 64 - 1]
+  static constexpr const TcKernelFn* kKernels[3][4] = {
+      {TcKernel<true, false, kFormDot>::fn, TcKernel<true, false, kFormEuclid>::fn,
+       TcKernel<true, false, kFormTastesMax>::fn, TcKernel<true, false, kFormTastesAttention>::fn},
+      {TcKernel<false, false, kFormDot>::fn, TcKernel<false, false, kFormEuclid>::fn,
+       TcKernel<false, false, kFormTastesMax>::fn, TcKernel<false, false, kFormTastesAttention>::fn},
+      {TcKernel<false, true, kFormDot>::fn, TcKernel<false, true, kFormEuclid>::fn,
+       TcKernel<false, true, kFormTastesMax>::fn, TcKernel<false, true, kFormTastesAttention>::fn}};
+  const TcKernelFn kernel = kKernels[a.dense ? 0 : a.excl_indptr != nullptr ? 2 : 1][form][p.n_kblocks - 1];
+  TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+  const int grid = capped_grid(static_cast<int64_t>(p.n_user_blocks) * p.n_splits, 1);
+  kernel<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, map_out, p, x, e, z);
+  TRK_CHECK_LAUNCH();
+  return TRK_OK;
 }
 
 }  // namespace trk
