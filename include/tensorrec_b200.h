@@ -390,6 +390,42 @@ int trk_score_topk_tastes_f16x3(const void* user_split, const float* user_scale,
                                 const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
                                 void* stream);
 
+/* Wide top-k of the Euclidean and attention forms on the exact kernel: 1 <= k <= 1024, every score final and exact
+ * (the same epilogue as trk_score_topk_euclid_f16x3 / trk_score_topk_tastes_f16x3), so no certificate, re-scoring or
+ * fallback.  Every (user, item split, column half) keeps a list in global memory of
+ * trk_score_topk_wide_list_capacity(k) entries (0 for k outside [1, 1024]); a warp compacts a full list to exactly its
+ * top k by (score desc, id asc).
+ *   trk_score_topk_wide_euclid_f16x3  the arguments of trk_score_topk_euclid_f16x3 with cand_score / cand_item
+ *                                     replaced by list_score / list_item [n_users, n_splits, 2, capacity] (scratch
+ *                                     while the kernel runs; on return entries [0, list_count) hold (final score,
+ *                                     global item id), unsorted) and list_count [n_users, n_splits, 2] (<= k).
+ *   trk_score_topk_wide_tastes_f16x3  the same for trk_score_topk_tastes_f16x3; attention != 0 (a mixture of tastes
+ *                                     without attention returns TRK_ERR_UNSUPPORTED: the wide filter serves it).
+ *                                     Only the users own lists: [n_users, n_splits, 2, capacity].
+ *   trk_select_topk_lists             per row: the n_lists lists of list_width entries (list l of row r at
+ *                                     (r * n_lists + l) * list_width, list_count[r * n_lists + l] <= k entries) sorted
+ *                                     by (score desc, id asc); the first k go to out_score / out_item (row stride
+ *                                     out_row_stride), sentinels (-inf, INT32_MAX) where there are fewer.  For the
+ *                                     lists above, n_lists = 2 n_splits and list_width = the capacity.
+ *                                     n_lists * k <= 16384. */
+int trk_score_topk_wide_list_capacity(int32_t k);
+int trk_score_topk_wide_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                     const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
+                                     int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset,
+                                     float* list_score, int32_t* list_item, int32_t* list_count,
+                                     const int32_t* n_users_live, const int32_t* excl_indptr, const int32_t* excl_ids,
+                                     const int32_t* excl_row_map, const float* user_half_sqnorm,
+                                     const float* item_half_sqnorm, void* stream);
+int trk_score_topk_wide_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                     int32_t n_tastes, int32_t attention, const void* item_split,
+                                     const float* item_meta, int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k,
+                                     int32_t n_splits, int32_t item_id_offset, float* list_score, int32_t* list_item,
+                                     int32_t* list_count, const int32_t* excl_indptr, const int32_t* excl_ids,
+                                     const int32_t* excl_row_map, void* stream);
+int trk_select_topk_lists(const float* list_score, const int32_t* list_item, const int32_t* list_count,
+                          int64_t n_rows, int32_t n_lists, int32_t list_width, int32_t k, float* out_score,
+                          int32_t* out_item, int64_t out_row_stride, void* stream);
+
 /* Merges n_lists candidate lists per user (each sorted by (score desc, id asc), k_in entries) into the global
  * top k_out per user, same order.  Lists are the n_splits of one GPU and/or the shards received from the other GPUs
  * (item-axis sharding; the exchange itself is one NCCL all-to-all done by the host layer, SURVEY 8e).

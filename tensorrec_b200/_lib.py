@@ -53,6 +53,15 @@ SIGNATURES = {
                                                     _c_i32, _c_p, _c_i64, _c_p]),
     'trk_score_topk_tastes_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i32, _c_i32, _c_p, _c_p, _c_i64, _c_i64, _c_i32,
                                                    _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p]),
+    'trk_score_topk_wide_list_capacity': (ctypes.c_int, [_c_i32]),
+    'trk_score_topk_wide_euclid_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_p, _c_i64, _c_i64, _c_i32, _c_i32,
+                                                        _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p,
+                                                        _c_p, _c_p]),
+    'trk_score_topk_wide_tastes_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i32, _c_i32, _c_p, _c_p, _c_i64, _c_i64,
+                                                        _c_i32, _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p,
+                                                        _c_p, _c_p]),
+    'trk_select_topk_lists': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i64, _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_i64,
+                                             _c_p]),
     'trk_topk_merge': (ctypes.c_int, [_c_p, _c_p, _c_i64, _c_i32, _c_i32, _c_i32, _c_i64, _c_i64, _c_p, _c_p, _c_i64,
                                       _c_p, _c_i32, _c_p]),
     'trk_topk_merge_dedup_pair': (ctypes.c_int, [_c_p, _c_p, _c_i64, _c_p, _c_p, _c_i64, _c_i64, _c_i32, _c_p, _c_p,

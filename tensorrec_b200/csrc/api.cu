@@ -106,6 +106,9 @@ int topk_merge(const float*, const int32_t*, int64_t, int32_t, int32_t, int32_t,
                int64_t, const int32_t*, int32_t, cudaStream_t);
 int topk_merge_dedup_pair(const float*, const int32_t*, int64_t, const float*, const int32_t*, int64_t, int64_t,
                           int32_t, float*, int32_t*, int64_t, cudaStream_t);
+int score_topk_wide_list_capacity(int32_t);
+int select_topk_lists(const float*, const int32_t*, const int32_t*, int64_t, int32_t, int32_t, int32_t, float*,
+                      int32_t*, int64_t, cudaStream_t);
 int score_filter_max_k();
 int score_filter_list_width();
 int operand_stats(const void*, const float*, int64_t, int32_t, float*, float*, cudaStream_t);
@@ -299,6 +302,51 @@ int trk_score_topk_tastes_f16x3(const void* user_split, const float* user_scale,
   a.n_tastes = n_tastes;
   a.attention = attention;
   return trk::score_tc(a, trk::as_stream(stream));
+}
+
+int trk_score_topk_wide_list_capacity(int32_t k) { return trk::score_topk_wide_list_capacity(k); }
+
+int trk_score_topk_wide_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                     const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
+                                     int32_t d_pad, int32_t k, int32_t n_splits, int32_t item_id_offset,
+                                     float* list_score, int32_t* list_item, int32_t* list_count,
+                                     const int32_t* n_users_live, const int32_t* excl_indptr, const int32_t* excl_ids,
+                                     const int32_t* excl_row_map, const float* user_half_sqnorm,
+                                     const float* item_half_sqnorm, void* stream) {
+  TRK_CHECK_ARG(user_half_sqnorm != nullptr && item_half_sqnorm != nullptr,
+                "trk_score_topk_wide_euclid_f16x3: null squared norms");
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k, n_splits,
+                        item_id_offset, list_score, list_item, n_users_live, excl_indptr, excl_ids, excl_row_map,
+                        user_half_sqnorm, item_half_sqnorm};
+  a.wide = true;
+  a.list_count = list_count;
+  return trk::score_tc(a, trk::as_stream(stream));
+}
+
+int trk_score_topk_wide_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                     int32_t n_tastes, int32_t attention, const void* item_split,
+                                     const float* item_meta, int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k,
+                                     int32_t n_splits, int32_t item_id_offset, float* list_score, int32_t* list_item,
+                                     int32_t* list_count, const int32_t* excl_indptr, const int32_t* excl_ids,
+                                     const int32_t* excl_row_map, void* stream) {
+  TRK_CHECK_ARG(n_tastes >= 1, "score_tastes: n_tastes=%d < 1", n_tastes);
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k, n_splits,
+                        item_id_offset, list_score, list_item};
+  a.excl_indptr = excl_indptr;
+  a.excl_ids = excl_ids;
+  a.excl_row_map = excl_row_map;
+  a.n_tastes = n_tastes;
+  a.attention = attention;
+  a.wide = true;
+  a.list_count = list_count;
+  return trk::score_tc(a, trk::as_stream(stream));
+}
+
+int trk_select_topk_lists(const float* list_score, const int32_t* list_item, const int32_t* list_count,
+                          int64_t n_rows, int32_t n_lists, int32_t list_width, int32_t k, float* out_score,
+                          int32_t* out_item, int64_t out_row_stride, void* stream) {
+  return trk::select_topk_lists(list_score, list_item, list_count, n_rows, n_lists, list_width, k, out_score, out_item,
+                                out_row_stride, trk::as_stream(stream));
 }
 
 int trk_topk_merge(const float* cand_score, const int32_t* cand_item, int64_t n_users, int32_t n_lists,

@@ -83,6 +83,8 @@ struct ScoreTcArgs {
   const float* user_half_sqnorm = nullptr;
   const float* item_half_sqnorm = nullptr;
   bool dense = false;                 // dense mode: the score matrix to dense_out instead of top-k candidates
+  bool wide = false;                  // wide mode: cand_score / cand_item are the lists [n_users, n_splits, 2, cap]
+  int32_t* list_count = nullptr;      // wide mode: [n_users, n_splits, 2] entries of each list
   float* dense_out = nullptr;
   int64_t dense_stride = 0;
   int32_t n_tastes = 0;
@@ -355,6 +357,68 @@ __device__ __forceinline__ void warp_sort_desc(float& s, int32_t& id, int lane) 
       }
     }
   }
+}
+
+// order-preserving keys of the wide form's selections: a > b  <=>  key(a) > key(b) for non-NaN floats
+__device__ __forceinline__ uint32_t wide_key(float s) {
+  const uint32_t u = __float_as_uint(s);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float wide_unkey(uint32_t key) {
+  return __uint_as_float((key & 0x80000000u) ? (key & 0x7fffffffu) : ~key);
+}
+
+// The key of the rank-th largest (1-based) real entry (id != INT32_MAX) of the list ls / li [0, n) in global memory;
+// the list holds at least `rank` real entries.  4 passes of 8 bits; `hist` = 256 words of the warp's shared-memory
+// scratch.  Called warp-uniformly.  (The compactions of the wide filter, score_wide_tc.cu, and of the exact kernel's
+// wide mode, score_topk_tc.cu.)
+__device__ __forceinline__ uint32_t wide_select(const float* ls, const int32_t* li, int n, int rank, uint32_t* hist,
+                                                int lane) {
+  uint32_t prefix = 0, mask = 0;
+#pragma unroll 1
+  for (int shift = 24; shift >= 0; shift -= 8) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) hist[8 * lane + j] = 0u;
+    __syncwarp();
+    for (int i = lane; i < n; i += 32) {
+      const uint32_t key = wide_key(ls[i]);
+      if (li[i] != 0x7fffffff && (key & mask) == prefix) atomicAdd(hist + ((key >> shift) & 255u), 1u);
+    }
+    __syncwarp();
+    uint32_t c8[8], local = 0;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      c8[j] = hist[8 * lane + j];
+      local += c8[j];
+    }
+    uint32_t incl = local;   // entries in the bins of lanes >= lane
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t t = __shfl_down_sync(0xffffffffu, incl, o);
+      if (lane + o < 32) incl += t;
+    }
+    const uint32_t above = incl - local;
+    const uint32_t r = static_cast<uint32_t>(rank);
+    const int src = __ffs(__ballot_sync(0xffffffffu, above < r && r <= incl)) - 1;
+    int bin = 0;
+    uint32_t rest = 0, acc = above;
+    bool found = false;
+#pragma unroll
+    for (int j = 7; j >= 0; --j) {
+      if (!found && acc + c8[j] >= r) {
+        bin = 8 * lane + j;
+        rest = r - acc;
+        found = true;
+      }
+      acc += c8[j];
+    }
+    bin = __shfl_sync(0xffffffffu, bin, src);
+    rank = static_cast<int>(__shfl_sync(0xffffffffu, rest, src));
+    prefix |= static_cast<uint32_t>(bin) << shift;
+    mask |= 255u << shift;
+    __syncwarp();   // every lane has read the histogram before the next pass clears it
+  }
+  return prefix;
 }
 
 // four consecutive elements of a split row (hi | lo halves, d_pad apart) as fp32 values hi + lo; zeros past d_pad

@@ -530,15 +530,6 @@ __device__ __forceinline__ void filter_mma_half(float (&acc0)[32], float (&acc1)
   wgmma_wait<0>();
 }
 
-// order-preserving keys of the wide form's selections: a > b  <=>  key(a) > key(b) for non-NaN floats
-__device__ __forceinline__ uint32_t wide_key(float s) {
-  const uint32_t u = __float_as_uint(s);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float wide_unkey(uint32_t key) {
-  return __uint_as_float((key & 0x80000000u) ? (key & 0x7fffffffu) : ~key);
-}
-
 // ---- host: the launcher of both forms -------------------------------------------------------------------------------
 // Checks the arguments both C entry points take (messages prefixed with `name`), fills p.sweep, picks the stage count
 // and the launch form, encodes the two tensor maps and launches Kernel<d_pad / 64, cluster, exclusion>::fn.  The

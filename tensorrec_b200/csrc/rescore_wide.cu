@@ -143,6 +143,56 @@ select_wide_kernel(const __half* __restrict__ user_split, const float* __restric
   }
 }
 
+// The exact kernel's wide mode (score_topk_tc.cu, DESIGN §3.8) leaves per row n_lists lists of FINAL scores, at most
+// k entries each (list_count): select_lists_kernel sorts their union by (score desc, id asc) and writes the first k,
+// sentinels (-inf, INT32_MAX) where there are fewer -- no re-scoring, no certificate.  Slot l * k + e holds entry e of
+// list l.  One CTA per row.
+__global__ void __launch_bounds__(kSelectThreads)
+select_lists_kernel(const float* __restrict__ list_score, const int32_t* __restrict__ list_item,
+                    const int32_t* __restrict__ list_count, int n_lists, int list_width, int k, int n_slots,
+                    float* __restrict__ out_score, int32_t* __restrict__ out_item, int64_t out_stride) {
+  extern __shared__ uint64_t keys[];
+  const int64_t u = blockIdx.x;
+  const float kNegInf = -__int_as_float(0x7f800000);
+  for (int t = threadIdx.x; t < n_slots; t += blockDim.x) {
+    uint64_t key = select_key(kNegInf, 0x7fffffff);
+    const int l = t / k;
+    if (l < n_lists && t - l * k < __ldg(list_count + u * n_lists + l)) {
+      const int64_t at = (u * n_lists + l) * list_width + (t - l * k);
+      key = select_key(__ldg(list_score + at), __ldg(list_item + at));
+    }
+    keys[t] = key;
+  }
+  block_sort_keys(keys, n_slots);
+  for (int j = threadIdx.x; j < k; j += blockDim.x) {
+    const uint64_t key = keys[j];
+    const int32_t id = static_cast<int32_t>(static_cast<uint32_t>(key));
+    out_score[u * out_stride + j] = id != 0x7fffffff ? select_key_score(key) : kNegInf;
+    out_item[u * out_stride + j] = id;
+  }
+}
+
+int select_topk_lists(const float* list_score, const int32_t* list_item, const int32_t* list_count, int64_t n_rows,
+                      int32_t n_lists, int32_t list_width, int32_t k, float* out_score, int32_t* out_item,
+                      int64_t out_row_stride, cudaStream_t stream) {
+  TRK_CHECK_ARG(list_score && list_item && list_count, "select_topk_lists: null input");
+  TRK_CHECK_ARG(out_score && out_item, "select_topk_lists: null output");
+  TRK_CHECK_ARG(n_rows >= 0 && n_lists >= 1 && k >= 1 && list_width >= k, "select_topk_lists: bad sizes");
+  TRK_CHECK_ARG(out_row_stride >= k, "select_topk_lists: out_row_stride < k");
+  int n_slots = 64;
+  while (n_slots < static_cast<int64_t>(n_lists) * k && n_slots <= kSelectMaxSlots) n_slots *= 2;
+  TRK_CHECK_ARG(n_slots <= kSelectMaxSlots, "select_topk_lists: n_lists x k = %lld entries per row exceed %d",
+                static_cast<long long>(n_lists) * k, kSelectMaxSlots);
+  if (n_rows == 0) return TRK_OK;
+  const size_t smem = static_cast<size_t>(n_slots) * sizeof(uint64_t);
+  TRK_CHECK_CUDA(cudaFuncSetAttribute(select_lists_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      static_cast<int>(smem)));
+  select_lists_kernel<<<static_cast<unsigned>(n_rows), kSelectThreads, smem, stream>>>(
+      list_score, list_item, list_count, n_lists, list_width, k, n_slots, out_score, out_item, out_row_stride);
+  TRK_CHECK_LAUNCH();
+  return TRK_OK;
+}
+
 int select_wide_topk(const void* user_split, const float* user_scale, const void* item_split, const float* item_scale,
                      const float* user_bias, const float* item_bias, const int32_t* cand_item, int64_t cand_row_stride,
                      int32_t n_lists, int32_t list_width, const int32_t* list_count, const float* row_theta,

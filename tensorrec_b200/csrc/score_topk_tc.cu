@@ -22,8 +22,10 @@
 //                 compare is strict, so equal scores keep the lower item id first -- tf.nn.top_k's order.
 //
 // Score forms (ScoreForm, one template parameter; DESIGN.md §3.7): dot / cosine as above, Euclidean similarity (§3.4),
-// and mixtures of tastes collapsed by a max or by attention (§3.5).  score_tc is the one host entry point behind every
-// trk_score_{topk,dense}* function: it validates the arguments and launches one of the 24 instantiations.
+// and mixtures of tastes collapsed by a max or by attention (§3.5).  Modes (TcMode): the dense matrix, the top-k above
+// (k <= 32), or the wide top-k (k <= 1024, DESIGN.md §3.8), where every (row, column half) keeps its list in global
+// memory and a warp compacts a full list to its exact top k.  score_tc is the one host entry point behind every
+// trk_score_{topk,dense}* function: it validates the arguments and launches one of the 32 instantiations.
 #include "common.cuh"
 
 namespace trk {
@@ -32,6 +34,17 @@ constexpr int kWgRows = 64;           // user rows per consumer warpgroup
 constexpr int kStageStride = 33;      // fp32 per staged row (32 columns + 1: conflict-free row reads)
 constexpr uint32_t kAccStageBytes = 2u * kWgRows * kStageStride * 4u;   // per warpgroup: 2 halves x 64 rows x 32 cols
 constexpr int kMaxK = 32;
+constexpr int kExactWideMaxK = 1024;   // wide mode
+
+// What the kernel makes of the scores: the dense matrix, a sorted top-k list per (row, column half) in shared memory
+// (k <= kMaxK), or an unsorted list per (row, column half) in global memory (k <= kExactWideMaxK).
+enum TcMode { kModeDense, kModeTopk, kModeWide };
+
+// Wide mode: a list keeps at most k entries between compactions and holds exact_wide_cap(k) = 2 keep, keep = k rounded
+// up to 32, so a compacted list always has room for one whole chunk of 32 columns (DESIGN.md §3.8).
+__host__ __device__ constexpr int exact_wide_keep(int k) { return static_cast<int>(round_up(k, 32)); }
+__host__ __device__ constexpr int exact_wide_cap(int k) { return 2 * exact_wide_keep(k); }
+constexpr uint32_t kWideScratchBytes = 8u * 256u * 4u;   // wide mode: a 256-bin histogram per consumer warp
 
 struct TcParams {
   const float* user_scale;
@@ -95,17 +108,27 @@ struct TcTastes {
   int32_t per_wg;
 };
 
-// shared-memory carve-up (offsets from a 1024-byte aligned base)
+// Wide mode (kModeWide): the lists live in global memory, [n_users, n_splits, 2, exact_wide_cap(k)] scores and ids
+// (list (u, split, column half)) plus [n_users, n_splits, 2] counts.  A kernel parameter of its own, for the same reason
+// as TcExcl.
+struct TcWide {
+  int32_t* list_count;
+};
+
+// shared-memory carve-up (offsets from a 1024-byte aligned base); the list region holds the top-k lists, the dense
+// mode's TMA store tiles or the wide mode's histograms
 struct SmemLayout {
   uint32_t a_off, b_off, list_score_off, list_item_off, acc_off, bar_off, total;
 };
 constexpr uint32_t kStoreTileBytes = 32 * 32 * 4;   // one warp's 32 rows x 32 columns of fp32 scores
-__host__ __device__ inline SmemLayout make_layout(int n_kblocks, int n_stages, int k, bool dense_staging = false) {
+__host__ __device__ inline SmemLayout make_layout(int n_kblocks, int n_stages, int k, bool dense_staging = false,
+                                                  bool wide = false) {
   SmemLayout L;
   L.a_off = 0;
   L.b_off = L.a_off + 2u * n_kblocks * kATileBytes;
   L.list_score_off = L.b_off + static_cast<uint32_t>(n_stages) * kBTileBytes;
-  L.list_item_off = L.list_score_off + (dense_staging ? 16u * kStoreTileBytes : 2u * k * kBlockM * 4u);
+  L.list_item_off = L.list_score_off + (dense_staging ? 16u * kStoreTileBytes
+                                                      : wide ? kWideScratchBytes : 2u * k * kBlockM * 4u);
   L.acc_off = L.list_item_off + (dense_staging ? 0u : 2u * k * kBlockM * 4u);
   L.bar_off = L.acc_off + 2u * kAccStageBytes;
   L.total = L.bar_off + 512u;
@@ -327,6 +350,124 @@ __device__ __forceinline__ void process_chunk(uint32_t (&r)[32], int c, int t, i
   }
 }
 
+// ---- wide mode (DESIGN.md §3.8) ----
+// Each thread's list holds (final score, item id) entries in ascending id order: items arrive in ascending id order and
+// a compaction is stable.  An item enters when its score is > thr, the k-th best score the list has kept so far: an
+// item whose score equals it has a larger id than the k kept entries that rank ahead of it, so it cannot be in the
+// list's top k.  -inf never enters.
+
+// Warp-cooperative compaction of lane src's list (ls / li, cnt > k entries) to exactly its top k by (score desc,
+// id asc): the k-th best key by a radix select, every entry above it, and the first entries equal to it -- the lowest
+// ids -- up to k.  Returns the k-th best score on every lane.  Called warp-uniformly.
+__device__ __forceinline__ float exact_wide_compact(int src, int lane, float* ls_own, int32_t* li_own, int cnt_own,
+                                                    int k, uint32_t* hist) {
+  const int n = __shfl_sync(0xffffffffu, cnt_own, src);
+  float* ls = reinterpret_cast<float*>(__shfl_sync(0xffffffffu, reinterpret_cast<unsigned long long>(ls_own), src));
+  int32_t* li =
+      reinterpret_cast<int32_t*>(__shfl_sync(0xffffffffu, reinterpret_cast<unsigned long long>(li_own), src));
+  __syncwarp();   // the owner's appends are visible to every lane
+  const uint32_t kth = wide_select(ls, li, n, k, hist, lane);
+  int n_gt = 0;
+  for (int i = lane; i < n; i += 32) n_gt += wide_key(ls[i]) > kth ? 1 : 0;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) n_gt += __shfl_xor_sync(0xffffffffu, n_gt, o);
+  const int n_eq = k - n_gt;   // entries equal to the k-th best that are kept
+  const uint32_t below = (1u << lane) - 1u;
+  int n_keep = 0, eq_seen = 0;
+  for (int i0 = 0; i0 < n; i0 += 32) {
+    const int i = i0 + lane;
+    float s = 0.0f;
+    int32_t id = 0;
+    uint32_t key = 0;
+    if (i < n) {
+      s = ls[i];
+      id = li[i];
+      key = wide_key(s);
+    }
+    const unsigned eq = __ballot_sync(0xffffffffu, i < n && key == kth);
+    const bool kp = i < n && (key > kth || (key == kth && eq_seen + __popc(eq & below) < n_eq));
+    const unsigned b = __ballot_sync(0xffffffffu, kp);   // every lane has read its entry of this round
+    if (kp) {
+      const int dst = n_keep + __popc(b & below);   // <= i: never an entry not yet read
+      ls[dst] = s;
+      li[dst] = id;
+    }
+    n_keep += __popc(b);
+    eq_seen += __popc(eq);
+    __syncwarp();
+  }
+  return wide_unkey(kth);
+}
+
+// Per-row state of the wide mode (empty in the other modes): the list's entry count and its index (u, split, half).
+template <bool kOn>
+struct WideCursor {
+  int cnt = 0;
+  int64_t list = 0;
+};
+template <>
+struct WideCursor<false> {};
+
+// The histogram of consumer warp `warp` in the list region of shared memory (wide mode).
+__device__ __forceinline__ uint32_t* wide_hist(uint8_t* list_region, int warp) {
+  return reinterpret_cast<uint32_t*>(list_region) + (warp - 4) * 256;
+}
+
+// The columns of a chunk of final scores that enter a list with threshold thr (bit j: column j).
+__device__ __forceinline__ uint32_t exact_wide_admit(const uint32_t (&r)[32], float thr) {
+  uint32_t mask = 0;
+#pragma unroll
+  for (int j = 0; j < 32; ++j) mask |= (__uint_as_float(r[j]) > thr ? 1u : 0u) << j;
+  return mask;
+}
+
+// Compacts the lists of the lanes in `rows` (each to its top k) and lowers their counts to k.  Warp-uniform.
+__device__ __forceinline__ void exact_wide_compact_rows(unsigned rows, int lane, float* ls, int32_t* li, int& cnt,
+                                                        float& thr, int k, uint32_t* hist) {
+  while (rows != 0u) {
+    const int src = __ffs(rows) - 1;
+    rows &= rows - 1u;
+    const float kth = exact_wide_compact(src, lane, ls, li, cnt, k, hist);
+    if (lane == src) {
+      thr = kth;
+      cnt = k;
+    }
+  }
+  __syncwarp();
+}
+
+// One 32-column chunk of the lane's row in wide mode: final scores, the row's listed columns masked (kExclude), then
+// the admitted columns appended to the lane's list; lists that could not take them are compacted first.  Lanes without
+// a list (owner false) admit nothing.  Warp-uniform.
+template <bool kExclude, ScoreForm kForm>
+__device__ __forceinline__ void wide_chunk(uint32_t (&r)[32], int c, int t, int32_t id0, const float2* meta,
+                                           const float* ihsq, float su, float usq, float ubias, float& thr, float* ls,
+                                           int32_t* li, int& cnt, int k, bool owner, const TcExcl x,
+                                           ExclCursor<kExclude>& xc, int lane, uint32_t* hist) {
+  float cmax = score_chunk_as<kForm>(r, meta + c * 32, ihsq + c * 32, su, usq, ubias);
+  if constexpr (kExclude) {
+    const int32_t base = t * kBlockN + c * 32;
+    if (xc.next < base + 32) cmax = excl_mask_scores(r, x, xc.row, base, xc.next);
+  }
+  uint32_t mask = (owner && cmax > thr) ? exact_wide_admit(r, thr) : 0u;
+  const unsigned full = __ballot_sync(0xffffffffu, cnt + __popc(mask) > exact_wide_cap(k));
+  if (full != 0u) {
+    exact_wide_compact_rows(full, lane, ls, li, cnt, thr, k, hist);
+    if (mask != 0u) mask = exact_wide_admit(r, thr);
+  }
+  if (mask != 0u) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      if ((mask >> j) & 1u) {
+        const int e = cnt + __popc(mask & ((1u << j) - 1u));
+        ls[e] = __uint_as_float(r[j]);
+        li[e] = id0 + c * 32 + j;
+      }
+    }
+    cnt += __popc(mask);
+  }
+}
+
 // Dense mode, TMA path: the warp's 32 rows x 32 columns go to a 128B-swizzled staging tile in shared memory and
 // leave as ONE cp.async.bulk.tensor store (full 128-byte lines per row, rows / columns beyond the matrix clipped by the
 // tensor map).  Direct stores from the row-per-thread layout write 16 bytes per lane to 32 different rows.
@@ -352,17 +493,20 @@ __device__ __forceinline__ void store_chunk_tma(const uint32_t (&r)[32], uint32_
   }
 }
 
-// kNKB = d_pad / 64 k-blocks per operand half.  kExclude (top-k mode): columns named in the row's exclusion list are
+// kMode: dense, top-k or wide (TcMode).  kNKB = d_pad / 64 k-blocks per operand half.  kExclude (top-k modes): columns named in the row's exclusion list are
 // left out of the top-k (excl_mask_scores).  kForm: the score form, in either mode.  The tastes forms collapse a
 // mixture of tastes per (user, item) (collapse_chunk); map_users is then the 3-D map of the stacked operand, a user
 // block holds 2 z.per_wg users, and in dense mode map_out's box is 32 columns x z.per_wg rows.
-template <bool kDense, int kNKB, bool kExclude, ScoreForm kForm>
+template <TcMode kMode, int kNKB, bool kExclude, ScoreForm kForm>
 __global__ void __launch_bounds__(kTcThreads, 1)
 score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_constant__ CUtensorMap map_items,
                 const __grid_constant__ CUtensorMap map_out, const TcParams p, const TcExcl x, const TcEuclid e,
-                const TcTastes z) {
+                const TcTastes z, const TcWide wl) {
+  constexpr bool kDense = kMode == kModeDense;
+  constexpr bool kWide = kMode == kModeWide;
   uint8_t* smem = smem_base_1024();
-  const SmemLayout L = make_layout(p.n_kblocks, p.n_stages, kDense ? 0 : p.k, kDense && p.tma_store != 0);
+  const SmemLayout L =
+      make_layout(p.n_kblocks, p.n_stages, kMode == kModeTopk ? p.k : 0, kDense && p.tma_store != 0, kWide);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
   uint64_t* a_full = bars + 0;
   uint64_t* a_empty = bars + 1;
@@ -489,11 +633,17 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
           xc.next = excl_next_at(x.indptr, x.ids, xc.row, t0 * kBlockN);
         }
       }
-      if constexpr (!kDense) {
+      if constexpr (kMode == kModeTopk) {
         for (int j = 0; j < p.k; ++j) {
           ls[j * kBlockM] = kNegInf;
           li[j * kBlockM] = 0x7fffffff;
         }
+      }
+      WideCursor<kWide> wc;   // wide mode: this thread's list (u, split, column half) in global memory, empty
+      if constexpr (kWide) {
+        wc.list = u_ok ? (u * p.n_splits + sp) * 2 + half : 0;
+        ls = p.cand_score + wc.list * exact_wide_cap(p.k);
+        li = p.cand_item + wc.list * exact_wide_cap(p.k);
       }
       if (t1 > t0) {
         mbar_wait(a_full, witer & 1);
@@ -562,6 +712,9 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
                               t * kBlockN + chunk * 32, ub * kBlockM + g * kWgRows + (warp % 2) * 32);
               ++n_stored;
             }
+          } else if constexpr (kWide) {   // every lane: the compactions are warp-cooperative
+            wide_chunk<kExclude, kForm>(r, chunk, t, id0, meta, ihsq, su, usq, ubias, thr, ls, li, wc.cnt, p.k, u_ok, x,
+                                        xc, lane, wide_hist(smem + L.list_score_off, warp));
           } else if (!is_tastes(kForm) || wt % kWgRows < z.per_wg) {
             process_chunk<kDense, kExclude, kForm>(r, chunk, t, id0, meta, ihsq, su, usq, ubias, thr, ls, li, p, u,
                                                    u_ok, x, xc);
@@ -571,7 +724,12 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
       __syncwarp();
       if (t1 > t0 && lane == 0) mbar_arrive(a_empty);   // this warp's MMAs of the work item are complete
 
-      if constexpr (!kDense) {
+      if constexpr (kWide) {
+        // the end of the item range: every list to at most k entries, and its count
+        exact_wide_compact_rows(__ballot_sync(0xffffffffu, wc.cnt > p.k), lane, ls, li, wc.cnt, thr, p.k,
+                                wide_hist(smem + L.list_score_off, warp));
+        if (u_ok) wl.list_count[wc.list] = wc.cnt;
+      } else if constexpr (!kDense) {
         // both halves have finished the item range: merge the two lists of each row and emit the candidates
         named_barrier_sync(1 + g, kConsumerThreads);
         if (half == 0 && u_ok) {
@@ -607,9 +765,9 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
 // ---------------------------------------------------------------------------------------------------------
 namespace {
 
-int pick_stages(int n_kblocks, int k, bool dense_staging) {
+int pick_stages(int n_kblocks, int k, bool dense_staging, bool wide) {
   for (int s = kMaxStages; s >= 2; --s)
-    if (make_layout(n_kblocks, s, k, dense_staging).total + kSmemAlignSlack <= kSmemLimit) return s;
+    if (make_layout(n_kblocks, s, k, dense_staging, wide).total + kSmemAlignSlack <= kSmemLimit) return s;
   return 0;
 }
 
@@ -619,6 +777,8 @@ int score_topk_max_k(int32_t d_pad) {
   if (d_pad != 64 && d_pad != 128) return 0;
   return kMaxK;
 }
+
+int score_topk_wide_list_capacity(int32_t k) { return k >= 1 && k <= kExactWideMaxK ? exact_wide_cap(k) : 0; }
 
 // Item splits of a dense launch over n_ub user blocks: enough that every SM gets work when there are few user blocks.
 static int32_t dense_splits(int64_t n_ub, int64_t n_items) {
@@ -630,11 +790,11 @@ static int32_t dense_splits(int64_t n_ub, int64_t n_items) {
 }
 
 // (the kernels of one instantiation, for score_tc: fn[d_pad / 64 - 1])
-using TcKernelFn = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, TcParams, TcExcl, TcEuclid, TcTastes);
-template <bool kDense, bool kExclude, ScoreForm kForm>
+using TcKernelFn = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, TcParams, TcExcl, TcEuclid, TcTastes, TcWide);
+template <TcMode kMode, bool kExclude, ScoreForm kForm>
 struct TcKernel {
-  static constexpr TcKernelFn fn[2] = {score_tc_kernel<kDense, 1, kExclude, kForm>,
-                                       score_tc_kernel<kDense, 2, kExclude, kForm>};
+  static constexpr TcKernelFn fn[2] = {score_tc_kernel<kMode, 1, kExclude, kForm>,
+                                       score_tc_kernel<kMode, 2, kExclude, kForm>};
 };
 
 int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
@@ -655,9 +815,10 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
                     reinterpret_cast<uintptr_t>(a.item_meta) % 16 == 0,
                 "score_tc: operands must be 16-byte aligned");
   if (!a.dense) {
-    TRK_CHECK_ARG(a.cand_score && a.cand_item, "score_topk: null output");
-    if (a.k < 1 || a.k > kMaxK) {
-      set_error("score_topk: k=%d outside [1, %d]", a.k, kMaxK);
+    TRK_CHECK_ARG(a.cand_score && a.cand_item && (!a.wide || a.list_count), "score_topk: null output");
+    const int max_k = a.wide ? kExactWideMaxK : kMaxK;
+    if (a.k < 1 || a.k > max_k) {
+      set_error("score_topk: k=%d outside [1, %d]", a.k, max_k);
       return TRK_ERR_UNSUPPORTED;
     }
     TRK_CHECK_ARG(a.n_splits >= 1, "score_tc: n_splits < 1");
@@ -685,6 +846,22 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
   }
   const ScoreForm form = tastes ? (a.attention ? kFormTastesAttention : kFormTastesMax)
                                 : (euclid ? kFormEuclid : kFormDot);
+  // every instantiation: [dense | top-k | top-k with exclusion | wide | wide with exclusion][form][d_pad / 64 - 1]
+  // (the wide mode exists for the forms without a wide filter: Euclidean similarity and attention)
+  static constexpr const TcKernelFn* kKernels[5][4] = {
+      {TcKernel<kModeDense, false, kFormDot>::fn, TcKernel<kModeDense, false, kFormEuclid>::fn,
+       TcKernel<kModeDense, false, kFormTastesMax>::fn, TcKernel<kModeDense, false, kFormTastesAttention>::fn},
+      {TcKernel<kModeTopk, false, kFormDot>::fn, TcKernel<kModeTopk, false, kFormEuclid>::fn,
+       TcKernel<kModeTopk, false, kFormTastesMax>::fn, TcKernel<kModeTopk, false, kFormTastesAttention>::fn},
+      {TcKernel<kModeTopk, true, kFormDot>::fn, TcKernel<kModeTopk, true, kFormEuclid>::fn,
+       TcKernel<kModeTopk, true, kFormTastesMax>::fn, TcKernel<kModeTopk, true, kFormTastesAttention>::fn},
+      {nullptr, TcKernel<kModeWide, false, kFormEuclid>::fn, nullptr, TcKernel<kModeWide, false, kFormTastesAttention>::fn},
+      {nullptr, TcKernel<kModeWide, true, kFormEuclid>::fn, nullptr, TcKernel<kModeWide, true, kFormTastesAttention>::fn}};
+  const int mode_row = a.dense ? 0 : (a.wide ? 3 : 1) + (a.excl_indptr != nullptr ? 1 : 0);
+  if (kKernels[mode_row][form] == nullptr) {
+    set_error("score_topk_wide: the wide mode serves the Euclidean and attention forms only");
+    return TRK_ERR_UNSUPPORTED;
+  }
 
   TcParams p;
   p.user_scale = a.user_scale;
@@ -707,7 +884,8 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
   const TcExcl x = {a.excl_indptr, a.excl_ids, a.excl_row_map};
   const TcEuclid e = {a.user_half_sqnorm, a.item_half_sqnorm};
   p.tma_store = (a.dense && a.dense_stride % 4 == 0 && reinterpret_cast<uintptr_t>(a.dense_out) % 16 == 0) ? 1 : 0;
-  p.n_stages = pick_stages(p.n_kblocks, p.k, p.tma_store != 0);
+  const int list_k = a.wide ? 0 : p.k;   // k of the shared-memory lists (the wide mode keeps its lists in global memory)
+  p.n_stages = pick_stages(p.n_kblocks, list_k, p.tma_store != 0, a.wide);
   TRK_CHECK_ARG(p.n_stages >= 2, "score_tc: shared memory budget exceeded (d_pad=%d k=%d)", a.d_pad, p.k);
 
   // operands: [rows, 2 d_pad] fp16 (hi | lo), boxes of one k-block x one tile
@@ -729,19 +907,13 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
                          4 * a.dense_stride, 32, tastes ? z.per_wg : 32, CU_TENSOR_MAP_L2_PROMOTION_NONE);
     if (rc != TRK_OK) return rc;
   }
-  const uint32_t smem_bytes = make_layout(p.n_kblocks, p.n_stages, p.k, p.tma_store != 0).total + kSmemAlignSlack;
-  // every instantiation: [dense | top-k | top-k with exclusion][form][d_pad / 64 - 1]
-  static constexpr const TcKernelFn* kKernels[3][4] = {
-      {TcKernel<true, false, kFormDot>::fn, TcKernel<true, false, kFormEuclid>::fn,
-       TcKernel<true, false, kFormTastesMax>::fn, TcKernel<true, false, kFormTastesAttention>::fn},
-      {TcKernel<false, false, kFormDot>::fn, TcKernel<false, false, kFormEuclid>::fn,
-       TcKernel<false, false, kFormTastesMax>::fn, TcKernel<false, false, kFormTastesAttention>::fn},
-      {TcKernel<false, true, kFormDot>::fn, TcKernel<false, true, kFormEuclid>::fn,
-       TcKernel<false, true, kFormTastesMax>::fn, TcKernel<false, true, kFormTastesAttention>::fn}};
-  const TcKernelFn kernel = kKernels[a.dense ? 0 : a.excl_indptr != nullptr ? 2 : 1][form][p.n_kblocks - 1];
+  const uint32_t smem_bytes =
+      make_layout(p.n_kblocks, p.n_stages, list_k, p.tma_store != 0, a.wide).total + kSmemAlignSlack;
+  const TcKernelFn kernel = kKernels[mode_row][form][p.n_kblocks - 1];
   TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
   const int grid = capped_grid(static_cast<int64_t>(p.n_user_blocks) * p.n_splits, 1);
-  kernel<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, map_out, p, x, e, z);
+  const TcWide wl = {a.list_count};
+  kernel<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, map_out, p, x, e, z, wl);
   TRK_CHECK_LAUNCH();
   return TRK_OK;
 }

@@ -970,11 +970,88 @@ def topk_wide(users, items, k, n_splits=None, item_id_offset=0, fitems=None, exc
     return top, counters, users.n_rows
 
 
+# ---------------------------------------------------------------------------------------------------------------
+# wide mode of the exact kernel (k <= 1024, Euclidean and attention forms): every (user, item split, column half)
+# keeps its exact top k in a list in global memory, then one selection per row -- no certificate, no fallback
+# ---------------------------------------------------------------------------------------------------------------
+def exact_wide_list_capacity(k):
+    """Entries of one list of the exact kernel's wide mode (per user, item split and column half) for this k; 0 when k
+    is outside [1, 1024]."""
+    return int(require_cuda().trk_score_topk_wide_list_capacity(int(k)))
+
+
+def exact_wide_splits(n_users, n_items, k):
+    """default_splits, bounded so that a row's 2 n_splits lists fit one selection (2 n_splits keep <= WIDE_MAX_SLOTS,
+    keep = half the capacity)."""
+    return int(max(1, min(default_splits(n_users, n_items), WIDE_MAX_SLOTS // exact_wide_list_capacity(k))))
+
+
+def _exact_wide_lists(n_users, n_splits, k, device):
+    cap = exact_wide_list_capacity(k)
+    return (torch.empty((n_users, n_splits, 2, cap), dtype=torch.float32, device=device),
+            torch.empty((n_users, n_splits, 2, cap), dtype=torch.int32, device=device),
+            torch.empty((n_users, n_splits, 2), dtype=torch.int32, device=device))
+
+
+def select_topk_lists(list_s, list_i, count, k, out=None):
+    """Lists [U, n_splits, 2, capacity] with counts [U, n_splits, 2] (the wide mode's output) -> PackedTopK [U, k] in
+    (score desc, id asc) order, sentinels where a row has fewer than k entries (trk_select_topk_lists)."""
+    lib = require_cuda()
+    n_users, n_splits, _, cap = list_s.shape
+    if out is None:
+        out = PackedTopK(n_users, k, list_s.device)
+    rc = lib.trk_select_topk_lists(_p(list_s), _p(list_i), _p(count), n_users, 2 * n_splits, cap, int(k),
+                                   out.score_ptr(), out.item_ptr(), 2 * out.k, _stream())
+    _lib.check(rc, 'trk_select_topk_lists')
+    return out
+
+
+def topk_exact_wide(users, items, k, n_splits=None, item_id_offset=0, out=None, excl=None, excl_row_map=None,
+                    item_hsq=None):
+    """Top-k of a Euclidean model for any 1 <= k <= 1024 on the exact kernel's wide mode + trk_select_topk_lists ->
+    PackedTopK [U, k].  item_hsq: item_half_sqnorm(items), formed here when not given; the user norms come from
+    users.split, as in topk_exact."""
+    lib = require_cuda()
+    if n_splits is None:
+        n_splits = exact_wide_splits(users.n_rows, items.n_rows, k)
+    if item_hsq is None:
+        item_hsq = item_half_sqnorm(items)
+    meta = pack_item_meta(items.scale, items.bias, items.n_rows)
+    user_hsq = operand_half_sqnorm(users.split, users.scale, users.d_pad)
+    list_s, list_i, count = _exact_wide_lists(users.n_rows, n_splits, k, users.split.device)
+    ex = (None, None, None) if excl is None else (_p(excl.indptr), _p(excl.ids), _p(excl_row_map))
+    rc = lib.trk_score_topk_wide_euclid_f16x3(_p(users.split), _p(users.scale), _p(users.bias), _p(items.split),
+                                              _p(meta), users.n_rows, items.n_rows, int(users.d_pad), int(k),
+                                              int(n_splits), int(item_id_offset), _p(list_s), _p(list_i), _p(count),
+                                              None, *ex, _p(user_hsq), _p(item_hsq), _stream())
+    _lib.check(rc, 'trk_score_topk_wide_euclid_f16x3')
+    return select_topk_lists(list_s, list_i, count, k, out=out)
+
+
+def topk_tastes_wide(users, items, n_tastes, attention, k, n_splits=None, item_id_offset=0, excl=None, out=None):
+    """topk_tastes for any 1 <= k <= 1024 on the exact kernel's wide mode (attention only: a mixture of tastes without
+    attention takes the wide filter) -> PackedTopK [U, k]."""
+    lib = require_cuda()
+    n_users = users.n_rows
+    if n_splits is None:
+        n_splits = exact_wide_splits(n_users, items.n_rows, k)
+    meta = pack_item_meta(items.scale, items.bias, items.n_rows)
+    list_s, list_i, count = _exact_wide_lists(n_users, n_splits, k, users.split.device)
+    ex = (None, None, None) if excl is None else (_p(excl.indptr), _p(excl.ids), None)
+    rc = lib.trk_score_topk_wide_tastes_f16x3(_p(users.split), _p(users.scale), _p(users.bias), int(n_tastes),
+                                              1 if attention else 0, _p(items.split), _p(meta), n_users, items.n_rows,
+                                              int(users.d_pad), int(k), int(n_splits), int(item_id_offset), _p(list_s),
+                                              _p(list_i), _p(count), *ex, _stream())
+    _lib.check(rc, 'trk_score_topk_wide_tastes_f16x3')
+    return select_topk_lists(list_s, list_i, count, k, out=out)
+
+
 def topk_fused(path, users, items, k, fitems=None, excl=None, item_id_offset=0, item_hsq=None, euclidean=False,
                block_bytes=4 << 30):
-    """The fused top-k of one route of topk_route: 'filter' (topk_filter), 'exact3' (topk_exact, with item_hsq) or
-    'wide' (topk_wide, with euclidean and block_bytes).  Returns (PackedTopK [U, k], device counters of the rows the
-    certificate rejected | None, capacity of the device-side fallback)."""
+    """The fused top-k of one route of topk_route: 'filter' (topk_filter), 'exact3' (topk_exact, with item_hsq),
+    'exact3_wide' (topk_exact_wide, Euclidean, with item_hsq) or 'wide' (topk_wide, with euclidean and block_bytes).
+    Returns (PackedTopK [U, k], device counters of the rows the certificate rejected | None, capacity of the
+    device-side fallback)."""
     if path == 'filter':
         return topk_filter(users, items, k, item_id_offset=item_id_offset, fitems=fitems, excl=excl)
     if path == 'wide':
@@ -982,6 +1059,8 @@ def topk_fused(path, users, items, k, fitems=None, excl=None, item_id_offset=0, 
                          block_bytes=block_bytes)
     if path == 'exact3':
         return topk_exact(users, items, k, item_id_offset=item_id_offset, excl=excl, item_hsq=item_hsq), None, 0
+    if path == 'exact3_wide':
+        return topk_exact_wide(users, items, k, item_id_offset=item_id_offset, excl=excl, item_hsq=item_hsq), None, 0
     raise ValueError('%r is not a fused top-k route' % (path,))
 
 

@@ -65,11 +65,16 @@ EUCLIDEAN_MIN_ITEMS = 1024
 # Mixture-of-tastes models with an attention graph take the taste-collapsing exact kernel for k <= 32 on catalogues of
 # at least ATTENTION_MIN_ITEMS items (see README, "Mixtures of tastes and attention").
 ATTENTION_MIN_ITEMS = 1024
+# Euclidean and attention models take the exact kernel's wide mode for 32 < k <= WIDE_MAX_K on catalogues of at least
+# EXACT_WIDE_MIN_ITEMS items; below that, dense scoring and ranking (see README, "Large k for Euclidean and attention
+# models").
+EXACT_WIDE_MIN_ITEMS = 4096
 
 
 def topk_route(k, n_items, model_ok, single_taste, filter_max_k, exact_max_k, sharded=False, euclidean=False,
-               attention=False, merge_max_k=32):
-    """The route of a top-k call -- 'filter', 'exact3', 'wide' or 'dense+rank' -- from k, the catalogue size and the
+               attention=False, merge_max_k=32, exact_wide_max_k=0):
+    """The route of a top-k call -- 'filter', 'exact3', 'wide', 'exact3_wide' or 'dense+rank' -- from k, the catalogue
+    size and the
     model alone.  model_ok: the tensor-core kernels evaluate the model (built-in dot / cosine prediction, or any
     built-in similar-items graph, no attention, d_pad <= 128); single_taste: one taste; filter_max_k / exact_max_k:
     the k limits of the filter and of the exact 3-pass kernel; merge_max_k: the largest k whose per-taste lists the
@@ -81,12 +86,17 @@ def topk_route(k, n_items, model_ok, single_taste, filter_max_k, exact_max_k, sh
     filter or wide form: 'exact3' for k <= exact_max_k on catalogues of at least EUCLIDEAN_MIN_ITEMS items (any shard
     size in a sharded call), 'dense+rank' otherwise.  attention: a mixture of tastes with an attention graph (model_ok
     from _tastes_tensor_ok), whose softmax has no filter or wide form either: the same rule with ATTENTION_MIN_ITEMS.
-    merge_max_k does not apply to either."""
+    merge_max_k does not apply to either.  exact_wide_max_k: the largest k of the exact kernel's wide mode (0: none,
+    WIDE_MAX_K: trk_score_topk_wide_*); Euclidean and attention models with exact_max_k < k <= exact_wide_max_k take
+    'exact3_wide' on catalogues of at least EXACT_WIDE_MIN_ITEMS items (any shard size in a sharded call), with one
+    taste or several."""
     if not model_ok:
         return 'dense+rank'
     if euclidean or attention:
-        if k > exact_max_k or n_items == 0:
+        if n_items == 0 or k > max(exact_max_k, exact_wide_max_k):
             return 'dense+rank'
+        if k > exact_max_k:
+            return 'exact3_wide' if sharded or n_items >= EXACT_WIDE_MIN_ITEMS else 'dense+rank'
         min_items = ATTENTION_MIN_ITEMS if attention else EUCLIDEAN_MIN_ITEMS
         return 'exact3' if sharded or n_items >= min_items else 'dense+rank'
     if k <= exact_max_k:
@@ -888,8 +898,10 @@ class TensorRec(object):
         same routes as one taste: one sweep per taste, and on the wide route each taste's top-k folded into the running
         result by a de-duplicating merge (last_topk_info['fallback_rows'] sums the tastes' fallback rows).  Euclidean
         models run k <= 32 on the exact kernel
-        (catalogues of at least EUCLIDEAN_MIN_ITEMS items) and larger k on dense+rank with tensor-core scoring; so do
-        mixtures of tastes with an attention graph (ATTENTION_MIN_ITEMS), on the taste-collapsing kernel.
+        (catalogues of at least EUCLIDEAN_MIN_ITEMS items); so do mixtures of tastes with an attention graph
+        (ATTENTION_MIN_ITEMS), on the taste-collapsing kernel.  Both run 32 < k <= WIDE_MAX_K on the exact kernel's wide
+        mode on catalogues of at least EXACT_WIDE_MIN_ITEMS items (a Euclidean mixture of tastes: one sweep per taste,
+        folded as on the wide route), and otherwise on dense+rank with tensor-core scoring.
         last_topk_info['path'] names the route (topk_route).
 
         exclude: None, or a scipy sparse matrix (any format) with n_users rows whose column index is the GLOBAL item id
@@ -941,28 +953,31 @@ class TensorRec(object):
                 item_hsq = kernels.item_half_sqnorm(items)
 
         if user_batch_size is None:
+            # (an attention model collapses its tastes in one sweep: no per-taste fold to hold)
             user_batch_size = self._topk_block_rows(path, n_users, n_items, k, gather_group, device,
-                                                    n_tastes=self.n_tastes)
+                                                    n_tastes=1 if attention else self.n_tastes)
         blocks = self._user_blocks(user_in, n_items, user_batch_size)
 
         def sweeps(block_in, u0, u1, route, excl):
             if attention:
                 # the softmax mixes the tastes: one sweep of the taste-collapsing kernel, no device-side fallback
                 users = self._taste_operands(block_in, device)
-                return kernels.topk_tastes(users, items, self.n_tastes, True, k, item_id_offset=item_id_offset,
-                                           excl=excl), [(None, 0)]
+                topk = kernels.topk_tastes_wide if route == 'exact3_wide' else kernels.topk_tastes
+                return topk(users, items, self.n_tastes, True, k, item_id_offset=item_id_offset, excl=excl), [(None, 0)]
             # mixture of tastes (no attention): prediction = max over tastes (recommendation_graphs.py:107), so the top-k
             # lies in the union of the per-taste top-k lists: one fused sweep per taste, then a de-duplicating merge.
-            # The wide route folds each taste's list into the running result right after its sweep (DESIGN §3.6), so a
-            # block holds three lists of k entries per row whatever the number of tastes.
+            # The wide routes (the wide filter, and the exact kernel's wide mode for Euclidean models) fold each taste's
+            # list into the running result right after its sweep (DESIGN §3.6), so a block holds three lists of k
+            # entries per row whatever the number of tastes.
             tops, counters, spare = [], [], None
             for t in range(self.n_tastes):
-                users = self._side_operands('user', block_in, device, for_filter=route != 'exact3', taste=t)
+                users = self._side_operands('user', block_in, device, for_filter=route not in ('exact3', 'exact3_wide'),
+                                            taste=t)
                 taste_top, cnt, cap = kernels.topk_fused(route, users, items, k, fitems=fitems, excl=excl,
                                                          item_id_offset=item_id_offset, item_hsq=item_hsq,
                                                          block_bytes=self.PREDICT_BLOCK_BYTES)
                 counters.append((cnt, cap))
-                if route == 'wide' and tops:
+                if route in ('wide', 'exact3_wide') and tops:
                     spare = kernels.topk_merge_dedup(tops[0], taste_top, out=spare)
                     tops[0], spare = spare, tops[0]
                 else:
@@ -1053,15 +1068,19 @@ class TensorRec(object):
 
     def _topk_block_rows(self, path, n_rows, n_items, k, gather_group=None, device=None, n_tastes=1):
         """Default rows per block of a top-k call: every row at once on the k <= 32 fused routes; on dense+rank as many
-        as keep the dense scores, ranks and selection masks within PREDICT_BLOCK_BYTES; on the wide route as many as
-        keep the candidate lists within PREDICT_BLOCK_BYTES at one item split per row, and with n_tastes > 1 (a user x item
+        as keep the dense scores, ranks and selection masks within PREDICT_BLOCK_BYTES; on the wide routes ('wide',
+        'exact3_wide') as many as keep the lists within PREDICT_BLOCK_BYTES at one item split per row, and with
+        n_tastes > 1 (a user x item
         call of a mixture of tastes) the running, per-taste and merged PackedTopK of the pairwise fold (3 x 8k bytes per
         row) as well.  (A block splits the items only when it has fewer user blocks than the device has SMs; its rows x
         splits then stay below ~3 x 128 x the SM count, about 1.2 GB of lists at k = 1024 on an H100.)  In a sharded call
         (gather_group) every rank takes the smallest of the ranks' choices: each block ends in the collective exchange,
         so all ranks must cut the same blocks."""
-        if path == 'wide':
-            per_row = 8 * kernels.wide_list_capacity(k)
+        if path in ('wide', 'exact3_wide'):
+            if path == 'wide':
+                per_row = 8 * kernels.wide_list_capacity(k)
+            else:      # two lists per row (the column halves) and their counts
+                per_row = 2 * (8 * kernels.exact_wide_list_capacity(k) + 4)
             if n_tastes > 1:
                 per_row += 3 * 8 * k
             rows = max(2 * kernels.TILE_USERS, self.PREDICT_BLOCK_BYTES // per_row // 256 * 256)
@@ -1076,10 +1095,12 @@ class TensorRec(object):
 
     def _topk_path(self, k, n_items, model_ok, single_taste, **route):
         """The route of a top-k call: topk_route(...) with the k limits of this model's kernels (the per-taste lists of
-        the wide route merge pairwise, up to WIDE_MAX_K).  Starts last_topk_info."""
+        the wide routes merge pairwise, up to WIDE_MAX_K, the k limit of the exact kernel's wide mode too).  Starts
+        last_topk_info."""
         d_pad = kernels.d_pad_for(self.n_components)
         limits = (kernels.filter_max_k(), kernels.topk_max_k(d_pad)) if model_ok else (0, 0)
-        path = topk_route(k, n_items, model_ok, single_taste, *limits, merge_max_k=WIDE_MAX_K, **route)
+        path = topk_route(k, n_items, model_ok, single_taste, *limits, merge_max_k=WIDE_MAX_K,
+                          exact_wide_max_k=WIDE_MAX_K if model_ok else 0, **route)
         self.last_topk_info = {'path': path, 'fallback_rows': 0}
         return path
 
