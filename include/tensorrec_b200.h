@@ -426,6 +426,49 @@ int trk_select_topk_lists(const float* list_score, const int32_t* list_item, con
                           int64_t n_rows, int32_t n_lists, int32_t list_width, int32_t k, float* out_score,
                           int32_t* out_item, int64_t out_row_stride, void* stream);
 
+/* Counting mode of the exact kernel: the full rank of listed (user, item) pairs without the score matrix.  Every
+ * score is the one trk_score_dense_{f16x3, euclid_f16x3, tastes_f16x3} writes for the same users at the same rows
+ * (user row u of the call at accumulator row u mod 128, or u mod 2 floor(64 / n_ops) for a mixture of tastes): a
+ * caller that splits its users into several calls cuts them at multiples of that block for the ranks to equal the
+ * ranks of the dense scores bit for bit.  A column (s, id) outranks a pair (t, tid) when s > t, or s == t and
+ * id < tid (ids global: local id + item_id_offset); -0.0 == +0.0.  Pairs of user row u: [pair_indptr[u],
+ * pair_indptr[u + 1]) of pair_ids / pair_score / pair_count; block_pairs [ceil(n_users / block)] = the most pairs of a
+ * row of each user block (the block above).
+ *   pass = -1  capture: pair_ids = LOCAL item ids, ascending per row; pair_score[pair] = the pair's score (never
+ *              masked by the exclusion lists).  pair_count is not read (may be NULL).
+ *   pass >= 0  count: every row's pairs sorted by (score desc, id asc) -- pair_ids (LOCAL) and pair_score (from the
+ *              capture) in that order; pass p adds to pair_count[pair] (int32, zeroed by the caller before pass 0)
+ *              the number of columns outranking pair 32 p + j of its row, j < 32.  Columns listed in the row's
+ *              exclusion list (excl_indptr / excl_ids / excl_row_map as for trk_score_topk_f16x3_excl, or all NULL)
+ *              count as -inf; a pair never counts itself.  A row with n pairs needs passes 0 .. ceil(n / 32) - 1, and
+ *              user blocks whose block_pairs <= 32 p are skipped.
+ * After every pass: rank of a pair = 1 + pair_count (the rank among the row's non-excluded items plus the pair).  The
+ * counts add up over item splits and over item shards (integer adds: deterministic).
+ *   trk_score_count_f16x3         operands as trk_score_topk_f16x3 (dot / cosine).
+ *   trk_score_count_euclid_f16x3  plus the two norm arrays of trk_score_topk_euclid_f16x3 (Euclidean similarity).
+ *   trk_score_count_tastes_f16x3  operands as trk_score_topk_tastes_f16x3 (mixtures of tastes, attention or not).
+ * Constraints: d_pad in {64, 128}; n_splits >= 1; pass >= -1. */
+int trk_score_count_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                          const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
+                          int32_t d_pad, int32_t n_splits, int32_t item_id_offset, const int32_t* pair_indptr,
+                          const int32_t* pair_ids, float* pair_score, int32_t* pair_count,
+                          const int32_t* block_pairs, int32_t pass, const int32_t* excl_indptr,
+                          const int32_t* excl_ids, const int32_t* excl_row_map, void* stream);
+int trk_score_count_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                 const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
+                                 int32_t d_pad, int32_t n_splits, int32_t item_id_offset, const int32_t* pair_indptr,
+                                 const int32_t* pair_ids, float* pair_score, int32_t* pair_count,
+                                 const int32_t* block_pairs, int32_t pass, const int32_t* excl_indptr,
+                                 const int32_t* excl_ids, const int32_t* excl_row_map, const float* user_half_sqnorm,
+                                 const float* item_half_sqnorm, void* stream);
+int trk_score_count_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                 int32_t n_tastes, int32_t attention, const void* item_split, const float* item_meta,
+                                 int64_t n_users, int64_t n_items, int32_t d_pad, int32_t n_splits,
+                                 int32_t item_id_offset, const int32_t* pair_indptr, const int32_t* pair_ids,
+                                 float* pair_score, int32_t* pair_count, const int32_t* block_pairs, int32_t pass,
+                                 const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
+                                 void* stream);
+
 /* Merges n_lists candidate lists per user (each sorted by (score desc, id asc), k_in entries) into the global
  * top k_out per user, same order.  Lists are the n_splits of one GPU and/or the shards received from the other GPUs
  * (item-axis sharding; the exchange itself is one NCCL all-to-all done by the host layer, SURVEY 8e).

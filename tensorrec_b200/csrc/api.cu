@@ -342,6 +342,71 @@ int trk_score_topk_wide_tastes_f16x3(const void* user_split, const float* user_s
   return trk::score_tc(a, trk::as_stream(stream));
 }
 
+namespace {
+
+// the counting-mode fields of score_tc's arguments
+void set_count(trk::ScoreTcArgs& a, const int32_t* pair_indptr, const int32_t* pair_ids, float* pair_score,
+               int32_t* pair_count, const int32_t* block_pairs, int32_t pass, const int32_t* excl_indptr,
+               const int32_t* excl_ids, const int32_t* excl_row_map) {
+  a.count = true;
+  a.pair_indptr = pair_indptr;
+  a.pair_ids = pair_ids;
+  a.pair_score = pair_score;
+  a.pair_count = pair_count;
+  a.block_pairs = block_pairs;
+  a.pass = pass;
+  a.excl_indptr = excl_indptr;
+  a.excl_ids = excl_ids;
+  a.excl_row_map = excl_row_map;
+}
+
+}  // namespace
+
+int trk_score_count_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                          const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
+                          int32_t d_pad, int32_t n_splits, int32_t item_id_offset, const int32_t* pair_indptr,
+                          const int32_t* pair_ids, float* pair_score, int32_t* pair_count,
+                          const int32_t* block_pairs, int32_t pass, const int32_t* excl_indptr,
+                          const int32_t* excl_ids, const int32_t* excl_row_map, void* stream) {
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, 0, n_splits,
+                        item_id_offset};
+  set_count(a, pair_indptr, pair_ids, pair_score, pair_count, block_pairs, pass, excl_indptr, excl_ids, excl_row_map);
+  return trk::score_tc(a, trk::as_stream(stream));
+}
+
+int trk_score_count_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                 const void* item_split, const float* item_meta, int64_t n_users, int64_t n_items,
+                                 int32_t d_pad, int32_t n_splits, int32_t item_id_offset, const int32_t* pair_indptr,
+                                 const int32_t* pair_ids, float* pair_score, int32_t* pair_count,
+                                 const int32_t* block_pairs, int32_t pass, const int32_t* excl_indptr,
+                                 const int32_t* excl_ids, const int32_t* excl_row_map, const float* user_half_sqnorm,
+                                 const float* item_half_sqnorm, void* stream) {
+  TRK_CHECK_ARG(user_half_sqnorm != nullptr && item_half_sqnorm != nullptr,
+                "trk_score_count_euclid_f16x3: null squared norms");
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, 0, n_splits,
+                        item_id_offset};
+  set_count(a, pair_indptr, pair_ids, pair_score, pair_count, block_pairs, pass, excl_indptr, excl_ids, excl_row_map);
+  a.user_half_sqnorm = user_half_sqnorm;
+  a.item_half_sqnorm = item_half_sqnorm;
+  return trk::score_tc(a, trk::as_stream(stream));
+}
+
+int trk_score_count_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                 int32_t n_tastes, int32_t attention, const void* item_split, const float* item_meta,
+                                 int64_t n_users, int64_t n_items, int32_t d_pad, int32_t n_splits,
+                                 int32_t item_id_offset, const int32_t* pair_indptr, const int32_t* pair_ids,
+                                 float* pair_score, int32_t* pair_count, const int32_t* block_pairs, int32_t pass,
+                                 const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
+                                 void* stream) {
+  TRK_CHECK_ARG(n_tastes >= 1, "score_tastes: n_tastes=%d < 1", n_tastes);
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, 0, n_splits,
+                        item_id_offset};
+  set_count(a, pair_indptr, pair_ids, pair_score, pair_count, block_pairs, pass, excl_indptr, excl_ids, excl_row_map);
+  a.n_tastes = n_tastes;
+  a.attention = attention;
+  return trk::score_tc(a, trk::as_stream(stream));
+}
+
 int trk_select_topk_lists(const float* list_score, const int32_t* list_item, const int32_t* list_count,
                           int64_t n_rows, int32_t n_lists, int32_t list_width, int32_t k, float* out_score,
                           int32_t* out_item, int64_t out_row_stride, void* stream) {

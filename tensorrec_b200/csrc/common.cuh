@@ -59,7 +59,7 @@ int encode_tiled_3d(CUtensorMap* map, CUtensorMapDataType type, const void* base
                     uint32_t box_planes, CUtensorMapL2promotion l2_promotion);
 
 // Host arguments of score_tc (score_topk_tc.cu), which validates them and launches the exact tensor-core kernel behind
-// every trk_score_{topk,dense}* entry point.  The fields up to item_half_sqnorm are the arguments of
+// every trk_score_{topk,dense,count}* entry point.  The fields up to item_half_sqnorm are the arguments of
 // trk_score_topk_euclid_f16x3, in its order.  The score form follows from the fields that are set: n_tastes != 0 is a
 // mixture of tastes (attention != 0: with attention), the two norms are Euclidean similarity, neither is dot / cosine.
 struct ScoreTcArgs {
@@ -89,6 +89,13 @@ struct ScoreTcArgs {
   int64_t dense_stride = 0;
   int32_t n_tastes = 0;
   int32_t attention = 0;
+  bool count = false;                 // counting mode (TcCount): the listed pairs' scores (pass -1) or counts (pass >= 0)
+  const int32_t* pair_indptr = nullptr;
+  const int32_t* pair_ids = nullptr;
+  float* pair_score = nullptr;
+  int32_t* pair_count = nullptr;
+  const int32_t* block_pairs = nullptr;
+  int32_t pass = 0;
 };
 int score_tc(const ScoreTcArgs& a, cudaStream_t stream);
 

@@ -24,8 +24,10 @@
 // Score forms (ScoreForm, one template parameter; DESIGN.md §3.7): dot / cosine as above, Euclidean similarity (§3.4),
 // and mixtures of tastes collapsed by a max or by attention (§3.5).  Modes (TcMode): the dense matrix, the top-k above
 // (k <= 32), or the wide top-k (k <= 1024, DESIGN.md §3.8), where every (row, column half) keeps its list in global
-// memory and a warp compacts a full list to its exact top k.  score_tc is the one host entry point behind every
-// trk_score_{topk,dense}* function: it validates the arguments and launches one of the 32 instantiations.
+// memory and a warp compacts a full list to its exact top k, or the counting mode (DESIGN.md §3.9), which captures the
+// scores of listed (user, item) pairs and counts the columns that outrank each of them.  score_tc is the one host
+// entry point behind every trk_score_{topk,dense,count}* function: it validates the arguments and launches one of the
+// 40 instantiations.
 #include "common.cuh"
 
 namespace trk {
@@ -38,7 +40,7 @@ constexpr int kExactWideMaxK = 1024;   // wide mode
 
 // What the kernel makes of the scores: the dense matrix, a sorted top-k list per (row, column half) in shared memory
 // (k <= kMaxK), or an unsorted list per (row, column half) in global memory (k <= kExactWideMaxK).
-enum TcMode { kModeDense, kModeTopk, kModeWide };
+enum TcMode { kModeDense, kModeTopk, kModeWide, kModeCount };
 
 // Wide mode: a list keeps at most k entries between compactions and holds exact_wide_cap(k) = 2 keep, keep = k rounded
 // up to 32, so a compacted list always has room for one whole chunk of 32 columns (DESIGN.md §3.8).
@@ -114,6 +116,22 @@ struct TcTastes {
 struct TcWide {
   int32_t* list_count;
 };
+
+// Counting mode (kModeCount, DESIGN.md §3.9): listed (user row, item) pairs, the pairs of user row u at
+// [indptr[u], indptr[u + 1]).  pass < 0 (capture): ids = LOCAL item ids ascending per row, and the final unmasked score
+// of every pair goes to score[pair].  pass >= 0 (count): the row's pairs sorted by (score desc, id asc) -- ids and
+// score in that order -- and pass p adds to count[pair] how many columns outrank pair 32 p + j of the row (j < 32).
+// block_pairs [n_user_blocks]: the most pairs of a row of the block; user blocks with at most 32 max(p, 0) are
+// skipped.  A kernel parameter of its own, for the same reason as TcExcl.
+struct TcCount {
+  const int32_t* indptr;
+  const int32_t* ids;
+  float* score;
+  int32_t* count;
+  const int32_t* block_pairs;
+  int32_t pass;
+};
+constexpr int kCountTargets = 32;   // targets of a row per counting pass
 
 // shared-memory carve-up (offsets from a 1024-byte aligned base); the list region holds the top-k lists, the dense
 // mode's TMA store tiles or the wide mode's histograms
@@ -468,6 +486,97 @@ __device__ __forceinline__ void wide_chunk(uint32_t (&r)[32], int c, int t, int3
   }
 }
 
+// ---- counting mode (DESIGN.md §3.9) ----
+// A column (s, id) outranks a pair (t, tid) when s > t or (s == t and id < tid) (r_before): the rank order of
+// rank_full.  A pass's targets are a row's pairs 32 p .. 32 p + n - 1 in that order, staged in shared memory as [32][128]
+// (column = user row of the block) with (-inf, INT32_MAX) beyond n, which every column outranks.  A column that
+// outranks the lowest target outranks the suffix [lb, n) of the targets; it adds 1 to the row's bucket h[lb], and the
+// prefix sums of h at the end of the work item are the targets' counts.
+
+// Per-row state of the counting mode (empty in the other modes).  Capture: the row's pairs [lo, hi) and the first
+// listed id >= the current chunk.  Count: the pass's first pair lo, its n targets and the lowest of them (+inf: none).
+template <bool kOn>
+struct CountCursor {
+  int32_t lo = 0, hi = 0, n = 0;
+  int32_t next = 0x7fffffff;
+  float low_s = 0.0f;
+  int32_t low_id = 0;
+};
+template <>
+struct CountCursor<false> {};
+
+// Does user block ub hold a row with pairs in this pass (capture: any pair)?  The same test in both roles.
+__device__ __forceinline__ bool count_block_live(const TcCount& cn, int ub) {
+  return __ldg(cn.block_pairs + ub) > kCountTargets * max(cn.pass, 0);
+}
+
+// Capture: the final scores of the row's pairs among the chunk's columns [base, base + 32) go to cn.score.  The pairs'
+// columns become a bit mask, and an unrolled walk over the registers in column order stores the marked ones at
+// consecutive pair positions (the ids ascend and are distinct): every r[j] has a constant index, so r[] stays in
+// registers.  (A select of r[e - base] per pair was lowered to an indexed local-memory copy of r[] that every chunk of
+// every pass paid for.)
+__device__ __forceinline__ void capture_chunk(const uint32_t (&r)[32], const TcCount& cn, CountCursor<true>& cc,
+                                              int32_t base) {
+  int i = excl_lower_bound(cn.ids, cc.lo, cc.hi, base);
+  int pos = i;
+  int32_t e = i < cc.hi ? __ldg(cn.ids + i) : 0x7fffffff;
+  uint32_t mask = 0;
+  while (e < base + 32) {
+    mask |= 1u << (e - base);
+    ++i;
+    e = i < cc.hi ? __ldg(cn.ids + i) : 0x7fffffff;
+  }
+  cc.next = e;
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    if ((mask >> j) & 1u) {
+      cn.score[pos] = __uint_as_float(r[j]);
+      ++pos;
+    }
+  }
+}
+
+// Count: every column of the chunk (final scores, ids id0 ..) that outranks the lowest target adds 1 to h[lb], lb found
+// by a binary search over the 32 staged targets (ts / ti / h: this row's column, stride kBlockM).  Target 31 is
+// outranked whenever the lowest target is, so five steps find lb <= 31 exactly.
+__device__ __forceinline__ void count_chunk(const uint32_t (&r)[32], int32_t id0, const float* ts, const int32_t* ti,
+                                            int32_t* h, float low_s, int32_t low_id) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const float s = __uint_as_float(r[j]);
+    const int32_t id = id0 + j;
+    if (r_before(s, id, low_s, low_id)) {
+      int lb = 0;
+#pragma unroll
+      for (int step = 16; step > 0; step >>= 1) {
+        const int m = lb + step - 1;
+        if (!r_before(s, id, ts[m * kBlockM], ti[m * kBlockM])) lb += step;
+      }
+      h[lb * kBlockM] += 1;
+    }
+  }
+}
+
+// One 32-column chunk of one user row in counting mode: final scores, then the capture of the row's pairs (pass < 0)
+// or the row's excluded columns masked (kExclude, excl rows set) and the columns counted, unless the chunk's maximum
+// lies below the lowest target.
+template <bool kExclude, ScoreForm kForm>
+__device__ __forceinline__ void count_process_chunk(uint32_t (&r)[32], int c, int t, int32_t id0, const float2* meta,
+                                                    const float* ihsq, float su, float usq, float ubias, const TcExcl x,
+                                                    ExclCursor<kExclude>& xc, const TcCount cn, CountCursor<true>& cc,
+                                                    const float* ts, const int32_t* ti, int32_t* h) {
+  float cmax = score_chunk_as<kForm>(r, meta + c * 32, ihsq + c * 32, su, usq, ubias);
+  const int32_t base = t * kBlockN + c * 32;
+  if (cn.pass < 0) {
+    if (cc.next < base + 32) capture_chunk(r, cn, cc, base);
+    return;
+  }
+  if constexpr (kExclude) {
+    if (xc.next < base + 32) cmax = excl_mask_scores(r, x, xc.row, base, xc.next);
+  }
+  if (cmax >= cc.low_s) count_chunk(r, id0 + c * 32, ts, ti, h, cc.low_s, cc.low_id);
+}
+
 // Dense mode, TMA path: the warp's 32 rows x 32 columns go to a 128B-swizzled staging tile in shared memory and
 // leave as ONE cp.async.bulk.tensor store (full 128-byte lines per row, rows / columns beyond the matrix clipped by the
 // tensor map).  Direct stores from the row-per-thread layout write 16 bytes per lane to 32 different rows.
@@ -493,20 +602,23 @@ __device__ __forceinline__ void store_chunk_tma(const uint32_t (&r)[32], uint32_
   }
 }
 
-// kMode: dense, top-k or wide (TcMode).  kNKB = d_pad / 64 k-blocks per operand half.  kExclude (top-k modes): columns named in the row's exclusion list are
-// left out of the top-k (excl_mask_scores).  kForm: the score form, in either mode.  The tastes forms collapse a
+// kMode: dense, top-k, wide or count (TcMode).  kNKB = d_pad / 64 k-blocks per operand half.  kExclude (top-k modes): columns named in the row's exclusion list are
+// left out of the top-k (excl_mask_scores); the counting mode is always instantiated with it and excludes nothing when
+// x.indptr is null.  kForm: the score form, in every mode.  The tastes forms collapse a
 // mixture of tastes per (user, item) (collapse_chunk); map_users is then the 3-D map of the stacked operand, a user
 // block holds 2 z.per_wg users, and in dense mode map_out's box is 32 columns x z.per_wg rows.
 template <TcMode kMode, int kNKB, bool kExclude, ScoreForm kForm>
 __global__ void __launch_bounds__(kTcThreads, 1)
 score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_constant__ CUtensorMap map_items,
                 const __grid_constant__ CUtensorMap map_out, const TcParams p, const TcExcl x, const TcEuclid e,
-                const TcTastes z, const TcWide wl) {
+                const TcTastes z, const TcWide wl, const TcCount cn) {
   constexpr bool kDense = kMode == kModeDense;
   constexpr bool kWide = kMode == kModeWide;
+  constexpr bool kCount = kMode == kModeCount;
   uint8_t* smem = smem_base_1024();
-  const SmemLayout L =
-      make_layout(p.n_kblocks, p.n_stages, kMode == kModeTopk ? p.k : 0, kDense && p.tma_store != 0, kWide);
+  // (the counting mode stages its targets and buckets in the list region of k = kMaxK)
+  const SmemLayout L = make_layout(p.n_kblocks, p.n_stages, kMode == kModeTopk ? p.k : (kCount ? kMaxK : 0),
+                                   kDense && p.tma_store != 0, kWide);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
   uint64_t* a_full = bars + 0;
   uint64_t* a_empty = bars + 1;
@@ -552,7 +664,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
         const int sp = static_cast<int>(w % p.n_splits);
         const int t0 = sp * p.tiles_per_split;
         const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
-        if (t1 <= t0 || ub >= live_blocks) continue;
+        if (t1 <= t0 || ub >= live_blocks || (kCount && !count_block_live(cn, ub))) continue;
         mbar_wait(a_empty, (witer & 1) ^ 1);  // the MMAs of the previous work item no longer read A
         if constexpr (is_tastes(kForm)) {
           // one box of n_ops x per_wg rows per warpgroup half and k-block; a half without users is not loaded
@@ -614,7 +726,8 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
       const int sp = static_cast<int>(w % p.n_splits);
       const int t0 = sp * p.tiles_per_split;
       const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
-      if (ub >= live_blocks) continue;   // (an empty split still emits its sentinel candidates)
+      if (ub >= live_blocks || (kCount && !count_block_live(cn, ub)))
+        continue;   // (an empty split still emits its sentinel candidates)
       // tastes: this warpgroup's users start at u0; the thread of row q < per_wg owns user u0 + q, later rows own none
       const int64_t u0 = is_tastes(kForm) ? static_cast<int64_t>(ub) * 2 * z.per_wg + g * z.per_wg : 0;
       const int64_t u = is_tastes(kForm) ? u0 + wt % kWgRows : static_cast<int64_t>(ub) * kBlockM + row;
@@ -628,7 +741,8 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
       // *n_users_live have no map entry and are discarded by the caller: they exclude nothing.
       ExclCursor<kExclude> xc;
       if constexpr (kExclude) {
-        if (u_ok && t1 > t0 && (p.n_users_live == nullptr || u < __ldg(p.n_users_live))) {
+        if ((!kCount || (x.indptr != nullptr && cn.pass >= 0)) && u_ok && t1 > t0 &&
+            (p.n_users_live == nullptr || u < __ldg(p.n_users_live))) {
           xc.row = x.row_map != nullptr ? __ldg(x.row_map + u) : static_cast<int32_t>(u);
           xc.next = excl_next_at(x.indptr, x.ids, xc.row, t0 * kBlockN);
         }
@@ -637,6 +751,37 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
         for (int j = 0; j < p.k; ++j) {
           ls[j * kBlockM] = kNegInf;
           li[j * kBlockM] = 0x7fffffff;
+        }
+      }
+      // counting mode: this row's targets and this (row, column half)'s buckets in the list region
+      const float* cts = reinterpret_cast<const float*>(smem + L.list_score_off) + row;
+      const int32_t* cti = reinterpret_cast<const int32_t*>(smem + L.list_score_off + kCountTargets * kBlockM * 4) + row;
+      int32_t* ch = reinterpret_cast<int32_t*>(smem + L.list_item_off) + half * kCountTargets * kBlockM + row;
+      CountCursor<kCount> cc;
+      if constexpr (kCount) {
+        const int32_t lo = u_ok ? __ldg(cn.indptr + u) : 0;
+        const int32_t hi = u_ok ? __ldg(cn.indptr + u + 1) : 0;
+        if (cn.pass < 0) {
+          cc.lo = lo;
+          cc.hi = hi;
+          if (t1 > t0 && hi > lo) cc.next = excl_next_at(cn.indptr, cn.ids, u, t0 * kBlockN);
+        } else {
+          cc.lo = lo + kCountTargets * cn.pass;
+          cc.n = max(0, min(kCountTargets, hi - cc.lo));
+          cc.low_s = __int_as_float(0x7f800000);   // no targets: every chunk is skipped
+          if (cc.n > 0) {
+            cc.low_s = __ldg(cn.score + cc.lo + cc.n - 1);
+            cc.low_id = __ldg(cn.ids + cc.lo + cc.n - 1) + p.item_id_offset;
+          }
+          if (half == 0) {   // (read by both halves after the epilogue's first barrier)
+            float* ts = reinterpret_cast<float*>(smem + L.list_score_off) + row;
+            int32_t* ti = reinterpret_cast<int32_t*>(smem + L.list_score_off + kCountTargets * kBlockM * 4) + row;
+            for (int j = 0; j < kCountTargets; ++j) {
+              ts[j * kBlockM] = j < cc.n ? __ldg(cn.score + cc.lo + j) : kNegInf;
+              ti[j * kBlockM] = j < cc.n ? __ldg(cn.ids + cc.lo + j) + p.item_id_offset : 0x7fffffff;
+            }
+          }
+          for (int j = 0; j < kCountTargets; ++j) ch[j * kBlockM] = 0;
         }
       }
       WideCursor<kWide> wc;   // wide mode: this thread's list (u, split, column half) in global memory, empty
@@ -715,6 +860,10 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
           } else if constexpr (kWide) {   // every lane: the compactions are warp-cooperative
             wide_chunk<kExclude, kForm>(r, chunk, t, id0, meta, ihsq, su, usq, ubias, thr, ls, li, wc.cnt, p.k, u_ok, x,
                                         xc, lane, wide_hist(smem + L.list_score_off, warp));
+          } else if constexpr (kCount) {
+            if (!is_tastes(kForm) || wt % kWgRows < z.per_wg)
+              count_process_chunk<kExclude, kForm>(r, chunk, t, id0, meta, ihsq, su, usq, ubias, x, xc, cn, cc, cts,
+                                                   cti, ch);
           } else if (!is_tastes(kForm) || wt % kWgRows < z.per_wg) {
             process_chunk<kDense, kExclude, kForm>(r, chunk, t, id0, meta, ihsq, su, usq, ubias, thr, ls, li, p, u,
                                                    u_ok, x, xc);
@@ -729,6 +878,17 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
         exact_wide_compact_rows(__ballot_sync(0xffffffffu, wc.cnt > p.k), lane, ls, li, wc.cnt, thr, p.k,
                                 wide_hist(smem + L.list_score_off, warp));
         if (u_ok) wl.list_count[wc.list] = wc.cnt;
+      } else if constexpr (kCount) {
+        if (cn.pass >= 0) {
+          // every column of the work item is counted and the staged targets are read: the buckets' prefix sums are
+          // the counts of this (row, column half) over the split (integer adds: the total does not depend on order)
+          named_barrier_sync(1 + g, kConsumerThreads);
+          int32_t acc_count = 0;
+          for (int j = 0; j < cc.n; ++j) {
+            acc_count += ch[j * kBlockM];
+            if (acc_count != 0) atomicAdd(cn.count + cc.lo + j, acc_count);
+          }
+        }
       } else if constexpr (!kDense) {
         // both halves have finished the item range: merge the two lists of each row and emit the candidates
         named_barrier_sync(1 + g, kConsumerThreads);
@@ -790,7 +950,8 @@ static int32_t dense_splits(int64_t n_ub, int64_t n_items) {
 }
 
 // (the kernels of one instantiation, for score_tc: fn[d_pad / 64 - 1])
-using TcKernelFn = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, TcParams, TcExcl, TcEuclid, TcTastes, TcWide);
+using TcKernelFn = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, TcParams, TcExcl, TcEuclid, TcTastes, TcWide,
+                            TcCount);
 template <TcMode kMode, bool kExclude, ScoreForm kForm>
 struct TcKernel {
   static constexpr TcKernelFn fn[2] = {score_tc_kernel<kMode, 1, kExclude, kForm>,
@@ -814,7 +975,13 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
                     reinterpret_cast<uintptr_t>(a.item_split) % 16 == 0 &&
                     reinterpret_cast<uintptr_t>(a.item_meta) % 16 == 0,
                 "score_tc: operands must be 16-byte aligned");
-  if (!a.dense) {
+  if (a.count) {
+    TRK_CHECK_ARG(a.pair_indptr && a.pair_ids && a.pair_score && a.block_pairs, "score_count: null pair list");
+    TRK_CHECK_ARG(a.pass >= -1, "score_count: pass=%d < -1", a.pass);
+    TRK_CHECK_ARG(a.pass < 0 || a.pair_count, "score_count: null pair_count");
+    TRK_CHECK_ARG(a.n_users_live == nullptr, "score_count: no live-row count");
+    TRK_CHECK_ARG(a.n_splits >= 1, "score_tc: n_splits < 1");
+  } else if (!a.dense) {
     TRK_CHECK_ARG(a.cand_score && a.cand_item && (!a.wide || a.list_count), "score_topk: null output");
     const int max_k = a.wide ? kExactWideMaxK : kMaxK;
     if (a.k < 1 || a.k > max_k) {
@@ -846,9 +1013,10 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
   }
   const ScoreForm form = tastes ? (a.attention ? kFormTastesAttention : kFormTastesMax)
                                 : (euclid ? kFormEuclid : kFormDot);
-  // every instantiation: [dense | top-k | top-k with exclusion | wide | wide with exclusion][form][d_pad / 64 - 1]
-  // (the wide mode exists for the forms without a wide filter: Euclidean similarity and attention)
-  static constexpr const TcKernelFn* kKernels[5][4] = {
+  // every instantiation: [dense | top-k | top-k with exclusion | wide | wide with exclusion | count][form][d_pad / 64 - 1]
+  // (the wide mode exists for the forms without a wide filter: Euclidean similarity and attention; the counting mode
+  // takes its exclusion lists at run time)
+  static constexpr const TcKernelFn* kKernels[6][4] = {
       {TcKernel<kModeDense, false, kFormDot>::fn, TcKernel<kModeDense, false, kFormEuclid>::fn,
        TcKernel<kModeDense, false, kFormTastesMax>::fn, TcKernel<kModeDense, false, kFormTastesAttention>::fn},
       {TcKernel<kModeTopk, false, kFormDot>::fn, TcKernel<kModeTopk, false, kFormEuclid>::fn,
@@ -856,8 +1024,10 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
       {TcKernel<kModeTopk, true, kFormDot>::fn, TcKernel<kModeTopk, true, kFormEuclid>::fn,
        TcKernel<kModeTopk, true, kFormTastesMax>::fn, TcKernel<kModeTopk, true, kFormTastesAttention>::fn},
       {nullptr, TcKernel<kModeWide, false, kFormEuclid>::fn, nullptr, TcKernel<kModeWide, false, kFormTastesAttention>::fn},
-      {nullptr, TcKernel<kModeWide, true, kFormEuclid>::fn, nullptr, TcKernel<kModeWide, true, kFormTastesAttention>::fn}};
-  const int mode_row = a.dense ? 0 : (a.wide ? 3 : 1) + (a.excl_indptr != nullptr ? 1 : 0);
+      {nullptr, TcKernel<kModeWide, true, kFormEuclid>::fn, nullptr, TcKernel<kModeWide, true, kFormTastesAttention>::fn},
+      {TcKernel<kModeCount, true, kFormDot>::fn, TcKernel<kModeCount, true, kFormEuclid>::fn,
+       TcKernel<kModeCount, true, kFormTastesMax>::fn, TcKernel<kModeCount, true, kFormTastesAttention>::fn}};
+  const int mode_row = a.count ? 5 : a.dense ? 0 : (a.wide ? 3 : 1) + (a.excl_indptr != nullptr ? 1 : 0);
   if (kKernels[mode_row][form] == nullptr) {
     set_error("score_topk_wide: the wide mode serves the Euclidean and attention forms only");
     return TRK_ERR_UNSUPPORTED;
@@ -884,7 +1054,9 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
   const TcExcl x = {a.excl_indptr, a.excl_ids, a.excl_row_map};
   const TcEuclid e = {a.user_half_sqnorm, a.item_half_sqnorm};
   p.tma_store = (a.dense && a.dense_stride % 4 == 0 && reinterpret_cast<uintptr_t>(a.dense_out) % 16 == 0) ? 1 : 0;
-  const int list_k = a.wide ? 0 : p.k;   // k of the shared-memory lists (the wide mode keeps its lists in global memory)
+  // k of the shared-memory lists (the wide mode keeps its lists in global memory; the counting mode stages its targets
+  // and buckets in the region of kMaxK)
+  const int list_k = a.wide ? 0 : a.count ? kMaxK : p.k;
   p.n_stages = pick_stages(p.n_kblocks, list_k, p.tma_store != 0, a.wide);
   TRK_CHECK_ARG(p.n_stages >= 2, "score_tc: shared memory budget exceeded (d_pad=%d k=%d)", a.d_pad, p.k);
 
@@ -913,7 +1085,8 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
   TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
   const int grid = capped_grid(static_cast<int64_t>(p.n_user_blocks) * p.n_splits, 1);
   const TcWide wl = {a.list_count};
-  kernel<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, map_out, p, x, e, z, wl);
+  const TcCount cn = {a.pair_indptr, a.pair_ids, a.pair_score, a.pair_count, a.block_pairs, a.pass};
+  kernel<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, map_out, p, x, e, z, wl, cn);
   TRK_CHECK_LAUNCH();
   return TRK_OK;
 }

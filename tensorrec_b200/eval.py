@@ -2,7 +2,9 @@
 
 Consumers of the hot path, host-side numpy/scipy.  The reference builds `predicted_ranks * positive.A` dense
 (eval.py:22,48) and only ever tests `rank <= k` (eval.py:23,49,68-69); that is what makes the top-k output of
-predict_rank(k=...) sufficient: every function here accepts either the full int32 rank matrix or a TopK result."""
+predict_rank(k=...) sufficient: every function here accepts the full int32 rank matrix, a TopK result, or a scipy
+sparse rank matrix such as predict_rank_at returns -- the ranks of the test positives only, exact at any k (a positive
+without a stored rank raises ValueError).  fit_and_eval keeps the reference's full predict_rank."""
 import numpy as np
 import scipy.sparse as sp
 
@@ -10,8 +12,18 @@ import scipy.sparse as sp
 def _ranks_of_positives(predicted_ranks, positive):
     """csr matrix with the predicted rank of every positive test interaction (0 entries are not stored).
 
-    For a TopK input, positives outside the top-k get rank n_items + 1 (any value > k would do)."""
+    For a TopK input, positives outside the top-k get rank n_items + 1 (any value > k would do).  A scipy sparse input
+    (predict_rank_at) must hold a rank for every positive: a missing entry would read as rank 0, a hit at every k."""
     positive = sp.csr_matrix(positive)
+    if sp.issparse(predicted_ranks):
+        ranks = sp.csr_matrix(predicted_ranks)
+        if ranks.shape != positive.shape:
+            raise ValueError('the rank matrix has shape %s but the interactions have %s' % (ranks.shape, positive.shape))
+        stored = sp.csr_matrix(positive != 0).multiply(ranks != 0)
+        if stored.nnz != sp.csr_matrix(positive != 0).nnz:
+            raise ValueError('%d positive interactions have no stored rank (list them in the pairs of predict_rank_at)'
+                             % (sp.csr_matrix(positive != 0).nnz - stored.nnz))
+        return sp.csr_matrix(positive.multiply(ranks))
     if hasattr(predicted_ranks, 'items') and hasattr(predicted_ranks, 'scores'):       # TopK
         items = np.asarray(predicted_ranks.items)
         n_users, n_items = positive.shape

@@ -1126,3 +1126,111 @@ def exclusion_positions(excl, perm, n_items):
     _lib.check(rc, 'trk_exclusion_positions')
     excl.pos = (torch.sort(keys).values & 0xffffffff).to(torch.int32)
     return excl
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# counting mode of the exact kernel: the full ranks of listed (user, item) pairs without the score matrix
+# (DESIGN §3.9): one capture sweep for the pairs' scores, a sort of every row's pairs, then counting passes of up to
+# COUNT_TARGETS pairs per row
+# ---------------------------------------------------------------------------------------------------------------
+COUNT_TARGETS = 32          # pairs of a row per counting pass
+RANK_AT_BYTES_PER_PAIR = 48  # device bytes per listed pair: ids, scores and counts twice over, sort keys, permutation
+RANK_AT_TEMP_BYTES_PER_ELEMENT = 8   # dense+rank with exclusion: bytes per (pair, item) of a chunk's temporaries
+
+
+def pair_block_max(indptr, n_users, block_rows):
+    """The most pairs of a row in each kernel user block of block_rows rows (host, int32 [ceil(n_users / block_rows)])."""
+    per_row = np.zeros(-(-int(n_users) // block_rows) * block_rows, dtype=np.int64)
+    per_row[:n_users] = np.diff(np.asarray(indptr, dtype=np.int64))
+    return per_row.reshape(-1, block_rows).max(axis=1).astype(np.int32)
+
+
+def count_passes(max_row_pairs):
+    """Counting passes of a row with this many pairs."""
+    return -(-int(max_row_pairs) // COUNT_TARGETS)
+
+
+def rank_sort_order(score, pair_row):
+    """The permutation that orders the pairs of every row by (score desc, position asc); positions ascend with the item
+    id inside a row, so ties go to the lower id as in rank_full.  One stable sort of int64 keys (row << 32 | a key that
+    descends with the score); the scores get + 0.0 first so that -0.0 sorts with +0.0."""
+    bits = (score + 0.0).view(torch.int32).long()
+    ascending = torch.where(bits < 0, 0x7fffffff - (bits & 0x7fffffff), bits + 0x80000000)
+    return torch.sort((pair_row.long() << 32) | (0xffffffff - ascending), stable=True).indices
+
+
+def count_listed_pairs(users, items, meta, indptr, ids, block_rows, excl=None, item_hsq=None, tastes=None,
+                       n_splits=None):
+    """Counting mode of the exact kernel over the users of `users` (SideOperands; a mixture of tastes: the stacked
+    operand and tastes = (n_tastes, attention)).  indptr / ids: host int32 CSR of the listed pairs, ids LOCAL and
+    ascending per row; block_rows: the kernel's user block (128, or 2P for a mixture of tastes); excl: DeviceExclusion
+    of the same rows or None; item_hsq: item_half_sqnorm(items) for a Euclidean model.  Returns (int32 counts [nnz] on
+    the device in the order of ids -- rank = 1 + count --, passes)."""
+    lib = require_cuda()
+    dev = users.split.device
+    n_users, n_items = users.n_rows, items.n_rows
+    nnz = int(indptr[-1])
+    block_max = pair_block_max(indptr, n_users, block_rows)
+    passes = count_passes(block_max.max()) if block_max.size else 0
+    if nnz == 0:
+        return torch.zeros((0,), dtype=torch.int32, device=dev), 0
+    if n_splits is None:
+        n_splits = default_splits(n_users, n_items)
+    up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev, non_blocking=True)   # noqa: E731
+    d_indptr, d_ids, d_block_max = up(indptr), up(ids), up(block_max)
+    ex = (None, None, None) if excl is None else (_p(excl.indptr), _p(excl.ids), None)
+    user_hsq = None if item_hsq is None else operand_half_sqnorm(users.split, users.scale, users.d_pad)
+
+    def launch(pair_ids, pair_score, pair_count, pass_):
+        head = (_p(users.split), _p(users.scale), _p(users.bias))
+        lists = (_p(d_indptr), _p(pair_ids), _p(pair_score), _p(pair_count), _p(d_block_max), int(pass_)) + ex
+        shape = (n_users, n_items, int(users.d_pad), int(n_splits), 0)
+        if tastes is not None:
+            name = 'trk_score_count_tastes_f16x3'
+            args = head + (int(tastes[0]), 1 if tastes[1] else 0, _p(items.split), _p(meta)) + shape + lists
+        elif item_hsq is not None:
+            name = 'trk_score_count_euclid_f16x3'
+            args = head + (_p(items.split), _p(meta)) + shape + lists + (_p(user_hsq), _p(item_hsq))
+        else:
+            name = 'trk_score_count_f16x3'
+            args = head + (_p(items.split), _p(meta)) + shape + lists
+        _lib.check(getattr(lib, name)(*args, _stream()), name)
+
+    score = torch.empty((nnz,), dtype=torch.float32, device=dev)
+    launch(d_ids, score, None, -1)
+    pair_row = torch.repeat_interleave(torch.arange(n_users, device=dev), d_indptr[1:].long() - d_indptr[:-1].long())
+    order = rank_sort_order(score, pair_row)
+    sorted_ids, sorted_score = d_ids[order].contiguous(), score[order].contiguous()
+    del score, pair_row
+    counts = torch.zeros((nnz,), dtype=torch.int32, device=dev)
+    for p in range(passes):
+        launch(sorted_ids, sorted_score, counts, p)
+    out = torch.empty_like(counts)
+    out[order] = counts
+    return out, passes
+
+
+def rank_listed_from_scores(scores, pair_row, pair_col, excl=None, block_bytes=4 << 30):
+    """Ranks of listed pairs (long device tensors pair_row / pair_col) from a block's dense scores [rows, n_items]
+    (modified in place with excl).  Without excl: trk_rank_full, gathered.  With excl (DeviceExclusion of the rows):
+    1 + #{j != i, (row, j) not excluded: s_j > s_i or (s_j == s_i and j < i)}, the pair's own score counted against
+    the masked row, in chunks of pairs whose temporaries fit the part of block_bytes the scores leave free (at least
+    one pair per chunk).  Returns int32 ranks on the device."""
+    if excl is None:
+        return rank_full(scores)[pair_row, pair_col]
+    n_rows, n_items = scores.shape
+    target = scores[pair_row, pair_col]
+    ex_rows, ex_cols = exclusion_pairs(excl, torch.arange(n_rows, device=scores.device))
+    scores[ex_rows, ex_cols] = float('-inf')
+    cols = torch.arange(n_items, device=scores.device)
+    out = torch.empty((pair_row.numel(),), dtype=torch.int32, device=scores.device)
+    # per gathered element: its float32 score and at most three live bool masks (RANK_AT_TEMP_BYTES_PER_ELEMENT)
+    free = max(0, int(block_bytes) - 4 * scores.numel())
+    step = max(1, free // (RANK_AT_TEMP_BYTES_PER_ELEMENT * max(n_items, 1)))
+    for p0 in range(0, pair_row.numel(), step):
+        p1 = min(pair_row.numel(), p0 + step)
+        row = scores[pair_row[p0:p1]]
+        t = target[p0:p1, None]
+        ahead = (row > t).sum(dim=1) + ((row == t) & (cols[None, :] < pair_col[p0:p1, None])).sum(dim=1)
+        out[p0:p1] = (1 + ahead).to(torch.int32)
+    return out

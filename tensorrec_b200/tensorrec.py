@@ -69,6 +69,34 @@ ATTENTION_MIN_ITEMS = 1024
 # EXACT_WIDE_MIN_ITEMS items; below that, dense scoring and ranking (see README, "Large k for Euclidean and attention
 # models").
 EXACT_WIDE_MIN_ITEMS = 4096
+# predict_rank_at counts on the exact kernel's counting mode (route 'exact3_count') on catalogues of at least
+# RANK_AT_MIN_ITEMS items; below that, dense scoring and ranking of the user blocks (see README, "Ranks of listed
+# pairs").
+RANK_AT_MIN_ITEMS = 2048
+
+
+def rank_at_route(n_items, tensor_scored):
+    """The route of a predict_rank_at call: 'exact3_count' when predict() scores the model on the exact tensor-core
+    kernel (tensor_scored: TensorRec._tensor_score_form() is not None) and the catalogue has at least RANK_AT_MIN_ITEMS
+    items, 'dense+rank' otherwise."""
+    return 'exact3_count' if tensor_scored and n_items >= RANK_AT_MIN_ITEMS else 'dense+rank'
+
+
+def rank_at_blocks(indptr, unit, max_rows, max_pairs):
+    """User blocks [(u0, u1)] of a predict_rank_at call over the rows of the pair CSR indptr: every block starts at a
+    multiple of `unit` (the kernel's user block, so every user keeps its accumulator row), has at most max_rows rows (a
+    positive multiple of unit) and at most max_pairs pairs unless one unit alone holds more."""
+    n = len(indptr) - 1
+    indptr = np.asarray(indptr, dtype=np.int64)
+    blocks, u0 = [], 0
+    while u0 < n:
+        u1 = min(n, u0 + max_rows)
+        fit = int(np.searchsorted(indptr, indptr[u0] + max_pairs, side='right')) - 1   # last row end within max_pairs
+        if fit < u1:
+            u1 = min(n, max(u0 + unit, fit // unit * unit))
+        blocks.append((u0, u1))
+        u0 = u1
+    return blocks
 
 
 def topk_route(k, n_items, model_ok, single_taste, filter_max_k, exact_max_k, sharded=False, euclidean=False,
@@ -681,13 +709,23 @@ class TensorRec(object):
     def _tensor_operands(self, user_in, item_in, device):
         return self._side_operands('user', user_in, device), self._side_operands('item', item_in, device)
 
+    def _tensor_score_form(self):
+        """How _score_plan scores this model on the exact tensor-core kernel: 'tastes' (the taste-collapsing form),
+        'euclidean' or 'dot' (dot / cosine); None when it scores it otherwise."""
+        if self._tastes_tensor_ok():      # (checked first: SCORE_PATH='tensor' accepts these models)
+            return 'tastes'
+        if self.n_tastes == 1 and self._euclidean_tensor_ok():
+            return 'euclidean'
+        return 'dot' if self._tensor_path_ok() else None
+
     def _score_plan(self, item_in, device):
         """Item-side work of the dense prediction, done once per call: returns score(user_block_in, out=None) ->
         float32 [rows, n_items] on the device.  Tensor cores (split-product kernel, dot / cosine / Euclidean) when the
         model allows, the exact CUDA-core kernel (tastes, attention, wide rows) or the plugin's own dense form
         otherwise."""
         n_items = item_in.shape[0]
-        if self._tastes_tensor_ok():      # (checked first: SCORE_PATH='tensor' accepts these models)
+        form = self._tensor_score_form()
+        if form == 'tastes':
             items = self._side_operands('item', item_in, device)
             meta = kernels.pack_item_meta(items.scale, items.bias, n_items)
             attention = self.attention_graph_factory is not None
@@ -696,8 +734,8 @@ class TensorRec(object):
                 return kernels.score_dense_tastes(self._taste_operands(block_in, device), items.split, meta, n_items,
                                                   self.n_tastes, attention, out=out)
             return score
-        euclidean = self.n_tastes == 1 and self._euclidean_tensor_ok()
-        if euclidean or self._tensor_path_ok():
+        euclidean = form == 'euclidean'
+        if form is not None:
             items = self._side_operands('item', item_in, device)
             meta = kernels.pack_item_meta(items.scale, items.bias, n_items)
             item_hsq = kernels.item_half_sqnorm(items) if euclidean else None
@@ -879,6 +917,95 @@ class TensorRec(object):
         if scores.numel() == 0:
             return np.zeros(tuple(scores.shape), dtype=np.int32)
         return kernels.to_host(kernels.rank_full(scores))
+
+    def predict_rank_at(self, user_features, item_features, pairs, exclude=None, user_batch_size=None):
+        """The full rank of listed (user, item) pairs, without the [n_users, n_items] rank matrix: where each held-out
+        item ranks for its user (recall / precision / ndcg at any k, hit rate, MRR, mean rank; tensorrec_b200.eval
+        accepts the result).
+
+        pairs: a scipy sparse matrix [n_users, n_items]; the pair (u, i) is listed when pairs[u, i] != 0 after
+        duplicates are summed (explicit zeros list nothing).  Returns a scipy.sparse.csr_matrix of int32 [n_users,
+        n_items] with sorted indices and one stored entry per listed pair: predict_rank(user_features,
+        item_features)[u, i] = 1 + #{j: s_uj > s_ui} + #{j < i: s_uj == s_ui}, s the scores predict() returns, bit for
+        bit (-0.0 and +0.0 compare equal).  exclude (validated as predict_top_k's single-GPU exclude): the rank among
+        the items (u, j) not excluded plus the pair itself, 1 + #{j != i, (u, j) not excluded: s_uj > s_ui or (s_uj ==
+        s_ui and j < i)} -- a listed pair that is itself excluded is ranked by its own score against the eligible
+        items.  For a non-excluded pair of rank r <= k on an exact top-k route, predict_top_k(..., k,
+        exclude=exclude).items[u, r - 1] == i.
+
+        Users go in blocks that start at multiples of the kernel's user block (128 rows, or 2P for a mixture of tastes:
+        DESIGN §3.5), so user_batch_size is rounded down to a positive multiple of it.  last_rank_info['path'] names
+        the route (rank_at_route): 'exact3_count', the exact kernel's counting mode, or 'dense+rank', the scores of
+        predict() ranked per block; last_rank_info['passes'] = the counting passes of the largest block (ceil of a
+        row's most pairs / 32; 0 on dense+rank)."""
+        if self.tf_prediction is None:
+            raise ModelNotFitException(method='predict_rank_at')
+        user_in = self._single_input(user_features, 'user_features')
+        item_in = self._single_input(item_features, 'item_features')
+        n_users, n_items = user_in.shape[0], item_in.shape[0]
+        if not sp.issparse(pairs):
+            raise ValueError('pairs must be a scipy sparse matrix with one row per user and one column per item')
+        if tuple(pairs.shape) != (n_users, n_items):
+            raise ValueError('pairs has shape %s but there are %d users and %d items'
+                             % (tuple(pairs.shape), n_users, n_items))
+        if exclude is not None:      # validated before any device work (the k argument does not apply here)
+            exclude = _checked_exclude(exclude, n_users, n_items, 1, 0, False)
+        self._check_features(user_in, self.n_user_features, 'user')
+        self._check_features(item_in, self.n_item_features, 'item')
+        indptr, ids = kernels.exclusion_host_csr(pairs, 0, n_items)   # the listing rule is the exclusion rule
+        form = self._tensor_score_form()
+        path = rank_at_route(n_items, form is not None)
+        self.last_rank_info = {'path': path, 'passes': 0}
+        ranks = np.zeros(ids.shape[0], dtype=np.int32)
+        result = lambda: sp.csr_matrix((ranks, ids, indptr), shape=(n_users, n_items))   # noqa: E731
+        if ids.size == 0:
+            return result()
+        device = self._cuda_device()
+
+        attention = self.attention_graph_factory is not None
+        unit = kernels.tastes_plan(self.n_tastes, attention)[1] if form == 'tastes' else kernels.TILE_USERS
+        if path == 'exact3_count':
+            n_ops = kernels.tastes_n_ops(self.n_tastes, attention) if form == 'tastes' else 1
+            per_row = n_ops * (4 * kernels.d_pad_for(self.n_components) + 8) + 16
+        else:
+            per_row = kernels.DENSE_RANK_BYTES_PER_PAIR * n_items
+        max_rows = self.PREDICT_BLOCK_BYTES // per_row if user_batch_size is None else int(user_batch_size)
+        max_rows = max(unit, max_rows // unit * unit)
+        blocks = rank_at_blocks(indptr, unit, max_rows, self.PREDICT_BLOCK_BYTES // kernels.RANK_AT_BYTES_PER_PAIR)
+        csr = user_in.matrix if isinstance(user_in.matrix, sp.csr_matrix) else sp.csr_matrix(user_in.matrix)
+
+        if path == 'exact3_count':
+            items = self._side_operands('item', item_in, device)
+            meta = kernels.pack_item_meta(items.scale, items.bias, n_items)
+            item_hsq = kernels.item_half_sqnorm(items) if form == 'euclidean' else None
+        else:
+            score = self._score_plan(item_in, device)
+        parts = []
+        for u0, u1 in blocks:
+            p0, p1 = int(indptr[u0]), int(indptr[u1])
+            if p1 == p0:
+                continue
+            block_in = user_in if (u0, u1) == (0, n_users) else SparseInput(csr[u0:u1])
+            b_indptr, b_ids = (indptr[u0:u1 + 1] - p0).astype(np.int32), ids[p0:p1]
+            excl = None if exclude is None else kernels.DeviceExclusion.upload(
+                *kernels.exclusion_host_csr(exclude, 0, n_items, u0, u1), device=device)
+            if path == 'exact3_count':
+                if form == 'tastes':
+                    users, tastes = self._taste_operands(block_in, device), (self.n_tastes, attention)
+                else:
+                    users, tastes = self._side_operands('user', block_in, device), None
+                counts, passes = kernels.count_listed_pairs(users, items, meta, b_indptr, b_ids, unit, excl=excl,
+                                                            item_hsq=item_hsq, tastes=tastes)
+                self.last_rank_info['passes'] = max(self.last_rank_info['passes'], passes)
+                parts.append(counts + 1)
+                del users
+            else:
+                rows = torch.from_numpy(np.repeat(np.arange(u1 - u0), np.diff(b_indptr))).to(device)
+                cols = torch.from_numpy(b_ids.astype(np.int64)).to(device)
+                parts.append(kernels.rank_listed_from_scores(score(block_in), rows, cols, excl=excl,
+                                                             block_bytes=self.PREDICT_BLOCK_BYTES))
+        ranks = (torch.cat(parts) if len(parts) > 1 else parts[0]).cpu().numpy()
+        return result()
 
     def predict_top_k(self, user_features, item_features, k, item_id_offset=0, gather_group=None, to_host=True,
                       gather='all', user_batch_size=None, exclude=None):
