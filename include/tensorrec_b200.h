@@ -519,6 +519,21 @@ int trk_topk_merge_dedup_pair(const float* a_score, const int32_t* a_item, int64
  *                      first; the order of the floating-point additions is not fixed, as in tf.gather's GPU gradient).
  *                    Representations are fp32 or bf16 (repr_is_bf16; BASELINE config #4 allows bf16), arithmetic and
  *                    gradients fp32.  coef [nnz] is scratch.  Constraints: d % 4 == 0, d <= 512, n_sampled <= 2048.
+ * trk_wmrb_step_tastes
+ *                    the same step for every other form the fused path trains (DESIGN §3.10): n_tastes taste rows per user,
+ *                    with n_tastes attention rows after them when attention = 1, stacked as planes [n_rows, n_users, d]
+ *                    in user_rows (and d_user_rows, written); euclidean = 1 scores a pair -sqrt(max(|u - i|^2, 1e-16)),
+ *                    0 scores it u . i (cosine: the caller passes L2-normalised rows).  The prediction collapses the
+ *                    tastes' scores with max (ties split the gradient evenly, as tf.reduce_max) or, with attention, with
+ *                    sum_t softmax_t(a_t) score_t, a_t = score of attention row t for an interaction and of taste row t
+ *                    itself for a sampled item (tensorrec/tensorrec.py:367-372); then biases and loss as trk_wmrb_step.
+ *                    d_item_repr receives one red.global.add per pair, summed over the operand rows.  Constraints:
+ *                    d % 4 == 0 (pad with zero columns), d <= 512 for one taste and <= 128 for several, n_tastes <= 8
+ *                    (<= 4 and >= 2 with attention), n_sampled <= 2048; others return TRK_ERR_UNSUPPORTED.
+ * trk_l2_normalize_rows_step_f32
+ *                    row L2-normalisation N(x) = x rsqrt(max(|x|^2, 1e-12)), n_normalize (1 or 2) times, of raw rows
+ *                    x [rows, d <= 512]: out (if non-null) receives N^n(x); grad (if non-null) holds d loss / d N^n(x) and
+ *                    is replaced by d loss / d x (the Jacobian of each normalisation, tf.maximum's gradient rule).
  * trk_f32_to_bf16    round-to-nearest-even conversion of a representation for the bf16 form.
  * trk_adam_step_f32  tf.train.AdamOptimizer on (grad + l2 * w) (tensorrec/tensorrec.py:487-489):
  *                      m = b1 m + (1 - b1) g;  v = b2 v + (1 - b2) g^2;  w -= lr_t m / (sqrt(v) + epsilon),
@@ -532,6 +547,14 @@ int trk_wmrb_step(const void* user_repr, const void* item_repr, int32_t repr_is_
                   const float* inter_val, const float* item_weight_sum, const int32_t* samples, int64_t n_users,
                   int64_t n_items, int32_t d, int32_t n_sampled, float* loss, float* pred_serial, float* coef,
                   float* d_user_repr, float* d_user_bias, float* d_item_repr, float* d_item_bias, void* stream);
+int trk_wmrb_step_tastes(const void* user_rows, const void* item_repr, int32_t repr_is_bf16, int32_t n_tastes,
+                         int32_t attention, int32_t euclidean, const float* user_bias, const float* item_bias,
+                         const int32_t* inter_indptr, const int32_t* inter_item, const float* inter_val,
+                         const float* item_weight_sum, const int32_t* samples, int64_t n_users, int64_t n_items,
+                         int32_t d, int32_t n_sampled, float* loss, float* pred_serial, float* coef, float* d_user_rows,
+                         float* d_user_bias, float* d_item_repr, float* d_item_bias, void* stream);
+int trk_l2_normalize_rows_step_f32(const float* x, int64_t rows, int32_t d, int32_t n_normalize, float* out,
+                                   float* grad, void* stream);
 int trk_f32_to_bf16(const float* x, int64_t n, void* out, void* stream);
 int trk_adam_step_f32(float* w, const float* grad, float* m, float* v, int64_t n, float lr_t, float beta1, float beta2,
                       float epsilon, float l2, void* stream);

@@ -142,6 +142,10 @@ int sample_items(int64_t, int64_t, int32_t, int32_t, uint64_t, uint32_t, int32_t
 int wmrb_step(const void*, const void*, int32_t, const float*, const float*, const int32_t*, const int32_t*, const float*,
               const float*, const int32_t*, int64_t, int64_t, int32_t, int32_t, float*, float*, float*, float*, float*,
               float*, float*, cudaStream_t);
+int wmrb_step_tastes(const void*, const void*, int32_t, int32_t, int32_t, int32_t, const float*, const float*,
+                     const int32_t*, const int32_t*, const float*, const float*, const int32_t*, int64_t, int64_t, int32_t,
+                     int32_t, float*, float*, float*, float*, float*, float*, float*, cudaStream_t);
+int l2_normalize_rows_step(const float*, int64_t, int32_t, int32_t, float*, float*, cudaStream_t);
 int f32_to_bf16(const float*, int64_t, void*, cudaStream_t);
 int adam_step(float*, const float*, float*, float*, int64_t, float, float, float, float, float, cudaStream_t);
 uint64_t philox_u64_host(uint64_t, uint32_t, uint32_t, uint32_t);
@@ -578,6 +582,23 @@ int trk_wmrb_step(const void* user_repr, const void* item_repr, int32_t repr_is_
   return trk::wmrb_step(user_repr, item_repr, repr_is_bf16, user_bias, item_bias, inter_indptr, inter_item, inter_val,
                         item_weight_sum, samples, n_users, n_items, d, n_sampled, loss, pred_serial, coef, d_user_repr,
                         d_user_bias, d_item_repr, d_item_bias, trk::as_stream(stream));
+}
+
+int trk_wmrb_step_tastes(const void* user_rows, const void* item_repr, int32_t repr_is_bf16, int32_t n_tastes,
+                         int32_t attention, int32_t euclidean, const float* user_bias, const float* item_bias,
+                         const int32_t* inter_indptr, const int32_t* inter_item, const float* inter_val,
+                         const float* item_weight_sum, const int32_t* samples, int64_t n_users, int64_t n_items,
+                         int32_t d, int32_t n_sampled, float* loss, float* pred_serial, float* coef, float* d_user_rows,
+                         float* d_user_bias, float* d_item_repr, float* d_item_bias, void* stream) {
+  return trk::wmrb_step_tastes(user_rows, item_repr, repr_is_bf16, n_tastes, attention, euclidean, user_bias, item_bias,
+                               inter_indptr, inter_item, inter_val, item_weight_sum, samples, n_users, n_items, d,
+                               n_sampled, loss, pred_serial, coef, d_user_rows, d_user_bias, d_item_repr, d_item_bias,
+                               trk::as_stream(stream));
+}
+
+int trk_l2_normalize_rows_step_f32(const float* x, int64_t rows, int32_t d, int32_t n_normalize, float* out,
+                                   float* grad, void* stream) {
+  return trk::l2_normalize_rows_step(x, rows, d, n_normalize, out, grad, trk::as_stream(stream));
 }
 
 int trk_f32_to_bf16(const float* x, int64_t n, void* out, void* stream) {

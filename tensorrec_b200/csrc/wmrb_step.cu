@@ -15,6 +15,9 @@
 //                           backward                 d loss / d (user row, user bias) accumulated in registers and written
 //                                                    once per user; d loss / d (item rows, item biases) added with
 //                                                    red.global.add (the scatter-add of tf.gather's gradient);
+//                         The same kernel, templated on the pair form, the collapse and the taste count, trains cosine,
+//                         Euclidean, mixture-of-tastes and attention models (trk_wmrb_step_tastes; DESIGN §3.10), with
+//                         l2_normalize_rows_step_kernel normalising operands forward and backward;
 //   adam_step_kernel      tf.train.AdamOptimizer.minimize(basic_loss + alpha * sum l2_loss(w)) (tensorrec.py:487-489):
 //                         L2 term, moment updates and the parameter step in one pass over every weight.
 //
@@ -22,6 +25,8 @@
 // (csr_gather.cu) on the CSR of the features / of their transpose.  HBM-bound: the step gathers one item row per
 // (user, interaction or sample) pair, twice (the second time from L2).
 #include <cuda_bf16.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -148,10 +153,118 @@ struct WmrbParams {
 
 constexpr int kWmrbWarps = 4;
 
+// The forms of the step (trk_wmrb_step_tastes; trk_wmrb_step is the dot / single-taste form):
+//   pair      the scalar function of a pair's operand rows, evaluated as a "row form" f per (pair, operand row):
+//             kPairDot     f = u . i, score f (cosine: the same on rows the caller has L2-normalised);
+//             kPairEuclid  f = sum_k (u_k - i_k)^2, score -sqrt(max(f, 1e-16)) (prediction_graphs.py:102-117);
+//   collapse  over the tastes (recommendation_graphs.py:85-109): one taste; max_t score_t; or
+//             sum_t softmax_t(a_t) score_t with a_t the score of the attention row -- of the user row itself for the
+//             sampled items (tensorrec.py:367-372).
+constexpr int kPairDot = 0, kPairEuclid = 1;
+constexpr int kCollapseSingle = 0, kCollapseMax = 1, kCollapseAttention = 2;
+constexpr float kEuclidEps = 1e-16f;
+
+template <int kPair>
+__device__ __forceinline__ float pair_score(float f) {
+  if constexpr (kPair == kPairEuclid) return -sqrtf(fmaxf(f, kEuclidEps));
+  else return f;
+}
+
+// the prediction (without biases) of one pair from its row forms f[0, NT) (tastes) and f[NT, 2 NT) (attention rows of
+// an interaction; a sample has none)
+template <int kPair, int kCollapse, int NT, bool kSample, int NF>
+__device__ __forceinline__ float collapse_tastes(const float (&f)[NF]) {
+  if constexpr (kCollapse == kCollapseSingle) {
+    return pair_score<kPair>(f[0]);
+  } else if constexpr (kCollapse == kCollapseMax) {
+    float m = pair_score<kPair>(f[0]);
+#pragma unroll
+    for (int t = 1; t < NT; ++t) m = fmaxf(m, pair_score<kPair>(f[t]));
+    return m;
+  } else {
+    float s[NT], a[NT];
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
+      s[t] = pair_score<kPair>(f[t]);
+      a[t] = kSample ? s[t] : pair_score<kPair>(f[NT + t]);
+    }
+    float m = a[0];
+#pragma unroll
+    for (int t = 1; t < NT; ++t) m = fmaxf(m, a[t]);
+    float z = 0.0f;
+#pragma unroll
+    for (int t = 0; t < NT; ++t) z += expf(a[t] - m);
+    float out = 0.0f;
+#pragma unroll
+    for (int t = 0; t < NT; ++t) out += (expf(a[t] - m) / z) * s[t];
+    return out;
+  }
+}
+
+// c[r] = the coefficient of operand row r in the gradient of one pair whose prediction has gradient g:
+//   dot:    d u_r = c_r i,        d i += c_r u_r         (c_r = g d pred / d f_r)
+//   euclid: d u_r = c_r (i - u_r), d i += c_r (u_r - i)  (c_r = g d pred / d score_r / sqrt(f_r); 0 below the clamp,
+//                                                        where tf.maximum passes no gradient to f)
+// The max collapse splits g evenly among tied tastes (tf.reduce_max's gradient).
+template <int kPair, int kCollapse, int NT, bool kSample, int NF>
+__device__ __forceinline__ void taste_coefs(const float (&f)[NF], float g, float (&c)[NF]) {
+  float ds[NF];
+  if constexpr (kCollapse == kCollapseSingle) {
+    ds[0] = g;
+  } else if constexpr (kCollapse == kCollapseMax) {
+    float m = pair_score<kPair>(f[0]);
+#pragma unroll
+    for (int t = 1; t < NT; ++t) m = fmaxf(m, pair_score<kPair>(f[t]));
+    float n_max = 0.0f;
+#pragma unroll
+    for (int t = 0; t < NT; ++t) n_max += pair_score<kPair>(f[t]) == m ? 1.0f : 0.0f;
+    const float share = g / n_max;
+#pragma unroll
+    for (int t = 0; t < NT; ++t) ds[t] = pair_score<kPair>(f[t]) == m ? share : 0.0f;
+  } else {
+    float s[NT], a[NT], w[NT];
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
+      s[t] = pair_score<kPair>(f[t]);
+      a[t] = kSample ? s[t] : pair_score<kPair>(f[NT + t]);
+    }
+    float m = a[0];
+#pragma unroll
+    for (int t = 1; t < NT; ++t) m = fmaxf(m, a[t]);
+    float z = 0.0f;
+#pragma unroll
+    for (int t = 0; t < NT; ++t) z += expf(a[t] - m);
+    float pred = 0.0f;
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
+      w[t] = expf(a[t] - m) / z;
+      pred += w[t] * s[t];
+    }
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
+      const float da = g * w[t] * (s[t] - pred);    // d pred / d a_t = w_t (s_t - pred)
+      ds[t] = g * w[t];
+      if constexpr (kSample) ds[t] += da;           // a_t is s_t itself
+      else ds[NT + t] = da;
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < NF; ++r) {
+    if constexpr (kPair == kPairEuclid) c[r] = f[r] >= kEuclidEps ? ds[r] / sqrtf(f[r]) : 0.0f;
+    else c[r] = ds[r];
+  }
+}
+
 // CH: 128-column chunks per row (d <= 128 * CH, d a multiple of 4): lane l holds elements [4 (l + 32 c), +4) of chunk c.
-template <typename T, int CH>
+// NT tastes; the user operand is NR = NT (or 2 NT with attention: the attention rows follow the taste rows) planes
+// [n_users, d], plane r at user_repr + r * n_users * d, and so is d_user_repr.  The dot / single-taste form (kPlain) is
+// the step of trk_wmrb_step; the other forms recompute a pair's row forms in the backward pass (from the item row
+// gathered there anyway) instead of keeping NT values per sample.
+template <typename T, int CH, int kPair = kPairDot, int kCollapse = kCollapseSingle, int NT = 1>
 __global__ void __launch_bounds__(kWmrbWarps * 32)
 wmrb_step_kernel(const WmrbParams p) {
+  constexpr bool kPlain = kPair == kPairDot && kCollapse == kCollapseSingle;
+  constexpr int NR = kCollapse == kCollapseAttention ? 2 * NT : NT;
   extern __shared__ float s_wmrb[];
   const int lane = threadIdx.x % 32, wib = threadIdx.x / 32;
   float* sp = s_wmrb + wib * 2 * p.n_sampled;   // sample predictions of this warp's user
@@ -160,26 +273,49 @@ wmrb_step_kernel(const WmrbParams p) {
   const T* item_repr = static_cast<const T*>(p.item_repr);
   const int d = p.d, S = p.n_sampled;
   const int64_t n_warps = static_cast<int64_t>(gridDim.x) * kWmrbWarps;
+  const int64_t plane = p.n_users * d;
 
   for (int64_t u = static_cast<int64_t>(blockIdx.x) * kWmrbWarps + wib; u < p.n_users; u += n_warps) {
-    float uv[CH][4];
+    float uv[NR][CH][4];
 #pragma unroll
-    for (int c = 0; c < CH; ++c) {
-      const int e = 4 * (lane + 32 * c);
-      if (e < d) load4<T>(user_repr + u * d + e, uv[c]);
-      else uv[c][0] = uv[c][1] = uv[c][2] = uv[c][3] = 0.0f;
+    for (int r = 0; r < NR; ++r) {
+#pragma unroll
+      for (int c = 0; c < CH; ++c) {
+        const int e = 4 * (lane + 32 * c);
+        if (e < d) load4<T>(user_repr + r * plane + u * d + e, uv[r][c]);
+        else uv[r][c][0] = uv[r][c][1] = uv[r][c][2] = uv[r][c][3] = 0.0f;
+      }
     }
     const float ub = p.user_bias != nullptr ? __ldg(p.user_bias + u) : 0.0f;
     const int32_t* srow = p.samples + u * S;
     const int a = __ldg(p.inter_indptr + u), b = __ldg(p.inter_indptr + u + 1);
 
-    // prediction of (this user, item id): (sum_k u_k i_k + user bias) + item bias -- the order of
-    // bias_prediction_serial; the k-sum is a per-lane FMA chain + xor tree (deterministic)
-    auto predict4 = [&](const int32_t (&ids)[4], int n_valid, float (&out)[4]) {
-      float part[4];
+    // row forms of (this user's first NU operand rows, one 4-element chunk c of an item row): a per-lane FMA chain, then
+    // an xor tree (deterministic: the backward pass recomputes exactly the values of the forward pass)
+    auto row_part = [&](auto nu, int c, const float (&iv)[4], float (&part)[decltype(nu)::value]) {
+      constexpr int NU = decltype(nu)::value;
+#pragma unroll
+      for (int r = 0; r < NU; ++r)
+#pragma unroll
+        for (int w = 0; w < 4; ++w) {
+          if constexpr (kPair == kPairEuclid) {
+            const float diff = uv[r][c][w] - iv[w];
+            part[r] = fmaf(diff, diff, part[r]);
+          } else {
+            part[r] = fmaf(uv[r][c][w], iv[w], part[r]);
+          }
+        }
+    };
+
+    // prediction of (this user, item id): (collapse of the pair's scores + user bias) + item bias -- the order of
+    // bias_prediction_serial.  nu: the operand rows the pair uses (NT for a sample, NR for an interaction)
+    auto predict4 = [&](auto nu, const int32_t (&ids)[4], int n_valid, float (&out)[4]) {
+      constexpr int NU = decltype(nu)::value;
+      float part[4][NU];
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        part[q] = 0.0f;
+#pragma unroll
+        for (int r = 0; r < NU; ++r) part[q][r] = 0.0f;
         if (q < n_valid) {
 #pragma unroll
           for (int c = 0; c < CH; ++c) {
@@ -187,16 +323,17 @@ wmrb_step_kernel(const WmrbParams p) {
             if (e < d) {
               float iv[4];
               load4<T>(item_repr + static_cast<int64_t>(ids[q]) * d + e, iv);
-#pragma unroll
-              for (int w = 0; w < 4; ++w) part[q] = fmaf(uv[c][w], iv[w], part[q]);
+              row_part(nu, c, iv, part[q]);
             }
           }
         }
       }
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        const float dot = warp_sum(part[q]);
-        float s = dot;
+        float f[NU];
+#pragma unroll
+        for (int r = 0; r < NU; ++r) f[r] = warp_sum(part[q][r]);
+        float s = collapse_tastes<kPair, kCollapse, NT, NU == NT && NR != NT>(f);
         if (q < n_valid) {
           if (p.user_bias != nullptr) s = s + ub;
           if (p.item_bias != nullptr) s = s + __ldg(p.item_bias + ids[q]);
@@ -204,6 +341,8 @@ wmrb_step_kernel(const WmrbParams p) {
         out[q] = s;
       }
     };
+    using SampleRows = std::integral_constant<int, NT>;
+    using PairRows = std::integral_constant<int, NR>;
 
     // ---- forward 1: the sampled items ----
     for (int j0 = 0; j0 < S; j0 += 4) {
@@ -212,7 +351,7 @@ wmrb_step_kernel(const WmrbParams p) {
 #pragma unroll
       for (int q = 0; q < 4; ++q) ids[q] = q < nv ? __ldg(srow + j0 + q) : 0;
       float s[4];
-      predict4(ids, nv, s);
+      predict4(SampleRows{}, ids, nv, s);
       if (lane < nv) {
         sp[j0 + lane] = s[lane == 0 ? 0 : lane == 1 ? 1 : lane == 2 ? 2 : 3];
         gs[j0 + lane] = 0.0f;
@@ -227,7 +366,7 @@ wmrb_step_kernel(const WmrbParams p) {
 #pragma unroll
       for (int q = 0; q < 4; ++q) ids[q] = q < nv ? __ldg(p.inter_item + n0 + q) : 0;
       float pr[4];
-      predict4(ids, nv, pr);
+      predict4(PairRows{}, ids, nv, pr);
       for (int q = 0; q < nv; ++q) {      // warp-uniform
         const float val = __ldg(p.inter_val + n0 + q);
         float loss = 0.0f, coef = 0.0f;
@@ -264,15 +403,21 @@ wmrb_step_kernel(const WmrbParams p) {
     }
     __syncwarp();
 
-    // ---- backward: d/d user row in registers, d/d item rows by red.global.add ----
-    float du[CH][4];
+    // ---- backward: d/d user rows in registers, d/d item rows by red.global.add ----
+    float du[NR][CH][4];
 #pragma unroll
-    for (int c = 0; c < CH; ++c) du[c][0] = du[c][1] = du[c][2] = du[c][3] = 0.0f;
+    for (int r = 0; r < NR; ++r)
+#pragma unroll
+      for (int c = 0; c < CH; ++c) du[r][c][0] = du[r][c][1] = du[r][c][2] = du[r][c][3] = 0.0f;
     float dub = 0.0f;
+    float csum[NR];                   // euclid: sum over the pairs of c_r, the coefficient of -u_r in d u_r
+#pragma unroll
+    for (int r = 0; r < NR; ++r) csum[r] = 0.0f;
     // four pairs at a time: the item rows of all of them are requested before the first FMA (they were read by the
     // forward pass a moment ago: L1 / L2 hits); a pair whose coefficient is zero (inactive hinge) contributes exact
-    // zeros and is skipped (warp-uniform)
-    auto backward4 = [&](const int32_t (&ids)[4], const float (&g)[4]) {
+    // zeros and is skipped (warp-uniform).  Each pair's item gradient, summed over the operand rows, is one red.add.
+    auto backward4 = [&](auto nu, const int32_t (&ids)[4], const float (&g)[4]) {
+      constexpr int NU = decltype(nu)::value;
       float iv[4][CH][4];
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
@@ -287,15 +432,46 @@ wmrb_step_kernel(const WmrbParams p) {
       for (int q = 0; q < 4; ++q) {
         if (g[q] == 0.0f) continue;
         dub += g[q];
+        float cr[NU];
+        if constexpr (kPlain) {
+          cr[0] = g[q];
+        } else {
+          float part[NU];
+#pragma unroll
+          for (int r = 0; r < NU; ++r) part[r] = 0.0f;
+#pragma unroll
+          for (int c = 0; c < CH; ++c)
+            if (4 * (lane + 32 * c) < d) row_part(nu, c, iv[q][c], part);
+          float f[NU];
+#pragma unroll
+          for (int r = 0; r < NU; ++r) f[r] = warp_sum(part[r]);
+          taste_coefs<kPair, kCollapse, NT, NU == NT && NR != NT>(f, g[q], cr);
+        }
+        float cs = 0.0f;
+#pragma unroll
+        for (int r = 0; r < NU; ++r) cs += cr[r];
 #pragma unroll
         for (int c = 0; c < CH; ++c) {
           const int e = 4 * (lane + 32 * c);
           if (e < d) {
 #pragma unroll
-            for (int w = 0; w < 4; ++w) du[c][w] = fmaf(g[q], iv[q][c][w], du[c][w]);
-            red_add_v4(p.d_item_repr + static_cast<int64_t>(ids[q]) * d + e, g[q] * uv[c][0], g[q] * uv[c][1],
-                       g[q] * uv[c][2], g[q] * uv[c][3]);
+            for (int r = 0; r < NU; ++r)
+#pragma unroll
+              for (int w = 0; w < 4; ++w) du[r][c][w] = fmaf(cr[r], iv[q][c][w], du[r][c][w]);
+            float gi[4];
+#pragma unroll
+            for (int w = 0; w < 4; ++w) {
+              if constexpr (kPair == kPairEuclid) gi[w] = -cs * iv[q][c][w];
+              else gi[w] = cr[0] * uv[0][c][w];
+#pragma unroll
+              for (int r = kPair == kPairEuclid ? 0 : 1; r < NU; ++r) gi[w] = fmaf(cr[r], uv[r][c][w], gi[w]);
+            }
+            red_add_v4(p.d_item_repr + static_cast<int64_t>(ids[q]) * d + e, gi[0], gi[1], gi[2], gi[3]);
           }
+        }
+        if constexpr (kPair == kPairEuclid) {
+#pragma unroll
+          for (int r = 0; r < NU; ++r) csum[r] += cr[r];
         }
         if (lane == 0 && p.d_item_bias != nullptr) atomicAdd(p.d_item_bias + ids[q], g[q]);
       }
@@ -309,7 +485,7 @@ wmrb_step_kernel(const WmrbParams p) {
         ids[q] = ok ? __ldg(srow + j0 + q) : 0;
         g[q] = ok ? gs[j0 + q] : 0.0f;
       }
-      backward4(ids, g);
+      backward4(SampleRows{}, ids, g);
     }
     for (int n0 = a; n0 < b; n0 += 4) {
       int32_t ids[4];
@@ -322,16 +498,87 @@ wmrb_step_kernel(const WmrbParams p) {
         const float mine = (ok && lane == 0) ? p.coef[n0 + q] : 0.0f;
         g[q] = __shfl_sync(0xffffffffu, mine, 0);
       }
-      backward4(ids, g);
+      backward4(PairRows{}, ids, g);
     }
 #pragma unroll
-    for (int c = 0; c < CH; ++c) {
-      const int e = 4 * (lane + 32 * c);
-      if (e < d)
-        *reinterpret_cast<float4*>(p.d_user_repr + u * d + e) = make_float4(du[c][0], du[c][1], du[c][2], du[c][3]);
+    for (int r = 0; r < NR; ++r) {
+#pragma unroll
+      for (int c = 0; c < CH; ++c) {
+        const int e = 4 * (lane + 32 * c);
+        if (e < d) {
+          if constexpr (kPair == kPairEuclid) {
+#pragma unroll
+            for (int w = 0; w < 4; ++w) du[r][c][w] = fmaf(-csum[r], uv[r][c][w], du[r][c][w]);
+          }
+          *reinterpret_cast<float4*>(p.d_user_repr + r * plane + u * d + e) =
+              make_float4(du[r][c][0], du[r][c][1], du[r][c][2], du[r][c][3]);
+        }
+      }
     }
     if (lane == 0 && p.d_user_bias != nullptr) p.d_user_bias[u] = dub;
     __syncwarp();
+  }
+}
+
+// Row L2-normalisation of an operand of the step, forward and backward, from its raw rows x (K1's output, d <= 512):
+//   N(x) = x rsqrt(max(|x|^2, 1e-12))    (tf.nn.l2_normalize; representation_graphs.py:53-58, prediction_graphs.py:67-72)
+// applied n_normalize (1 or 2) times.  out (if non-null) receives N^n(x).  grad (if non-null) holds d loss / d N^n(x) and
+// is replaced by d loss / d x: through each normalisation, from the last, g <- s g - [|v|^2 >= 1e-12] s^3 (v . g) v with
+// v that normalisation's input and s its rsqrt (below the clamp tf.maximum passes nothing to |v|^2: g <- s g).
+// One warp per row; lane l holds elements l + 32 k.
+constexpr int kNormWarps = 8;
+__global__ void __launch_bounds__(kNormWarps * 32)
+l2_normalize_rows_step_kernel(const float* __restrict__ x, int64_t rows, int d, int n_normalize, float* __restrict__ out,
+                              float* __restrict__ grad) {
+  constexpr int K = 16;
+  const int lane = threadIdx.x % 32;
+  const int64_t n_warps = static_cast<int64_t>(gridDim.x) * kNormWarps;
+  for (int64_t row = static_cast<int64_t>(blockIdx.x) * kNormWarps + threadIdx.x / 32; row < rows; row += n_warps) {
+    float v[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) v[k] = lane + 32 * k < d ? x[row * d + lane + 32 * k] : 0.0f;
+    float scale[2];
+    bool clamped[2];
+    float y[K];
+#pragma unroll
+    for (int k = 0; k < K; ++k) y[k] = v[k];
+    for (int n = 0; n < n_normalize; ++n) {
+      float ss = 0.0f;
+#pragma unroll
+      for (int k = 0; k < K; ++k) ss = fmaf(y[k], y[k], ss);
+      ss = warp_sum(ss);
+      scale[n] = 1.0f / sqrtf(fmaxf(ss, 1e-12f));
+      clamped[n] = ss < 1e-12f;
+#pragma unroll
+      for (int k = 0; k < K; ++k) y[k] *= scale[n];
+    }
+    if (out != nullptr) {
+#pragma unroll
+      for (int k = 0; k < K; ++k)
+        if (lane + 32 * k < d) out[row * d + lane + 32 * k] = y[k];
+    }
+    if (grad != nullptr) {
+      float g[K];
+#pragma unroll
+      for (int k = 0; k < K; ++k) g[k] = lane + 32 * k < d ? grad[row * d + lane + 32 * k] : 0.0f;
+      for (int n = n_normalize - 1; n >= 0; --n) {
+        // the input of normalisation n: x, or N(x) for the second one
+        float in[K];
+#pragma unroll
+        for (int k = 0; k < K; ++k) in[k] = n == 0 ? v[k] : v[k] * scale[0];
+        float vg = 0.0f;
+#pragma unroll
+        for (int k = 0; k < K; ++k) vg = fmaf(in[k], g[k], vg);
+        vg = warp_sum(vg);
+        const float s = scale[n];
+        const float t = clamped[n] ? 0.0f : s * s * s * vg;
+#pragma unroll
+        for (int k = 0; k < K; ++k) g[k] = s * g[k] - t * in[k];
+      }
+#pragma unroll
+      for (int k = 0; k < K; ++k)
+        if (lane + 32 * k < d) grad[row * d + lane + 32 * k] = g[k];
+    }
   }
 }
 
@@ -389,24 +636,50 @@ int sample_items(int64_t n_users, int64_t n_items, int32_t n_sampled, int32_t re
   return TRK_OK;
 }
 
-template <typename T>
+template <typename T, int kPair = kPairDot, int kCollapse = kCollapseSingle, int NT = 1>
 static int launch_wmrb(const WmrbParams& p, cudaStream_t stream) {
   const int ch = static_cast<int>(ceil_div(p.d, 128));
   const size_t smem = static_cast<size_t>(kWmrbWarps) * 2 * p.n_sampled * sizeof(float);
   const int grid = capped_grid(ceil_div(p.n_users, kWmrbWarps), 16);
-#define TRK_WMRB_LAUNCH(CH)                                                                                   \
-  do {                                                                                                        \
-    if (smem > 48 * 1024)                                                                                     \
-      TRK_CHECK_CUDA(cudaFuncSetAttribute(wmrb_step_kernel<T, CH>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                          static_cast<int>(smem)));                                           \
-    wmrb_step_kernel<T, CH><<<grid, kWmrbWarps * 32, smem, stream>>>(p);                                      \
+#define TRK_WMRB_LAUNCH(CH)                                                                                             \
+  do {                                                                                                                  \
+    auto* kernel = wmrb_step_kernel<T, CH, kPair, kCollapse, NT>;                                                       \
+    if (smem > 48 * 1024)                                                                                               \
+      TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem))); \
+    kernel<<<grid, kWmrbWarps * 32, smem, stream>>>(p);                                                                 \
   } while (0)
-  if (ch == 1) TRK_WMRB_LAUNCH(1);
-  else if (ch == 2) TRK_WMRB_LAUNCH(2);
-  else TRK_WMRB_LAUNCH(4);
+  if constexpr (NT == 1) {
+    if (ch == 1) TRK_WMRB_LAUNCH(1);
+    else if (ch == 2) TRK_WMRB_LAUNCH(2);
+    else TRK_WMRB_LAUNCH(4);
+  } else {
+    TRK_WMRB_LAUNCH(1);    // mixtures of tastes: d <= 128
+  }
 #undef TRK_WMRB_LAUNCH
   TRK_CHECK_LAUNCH();
   return TRK_OK;
+}
+
+// the instantiation of (pair form, n_tastes, attention); the caller has checked the limits
+template <typename T, int kPair>
+static int launch_wmrb_form(const WmrbParams& p, int n_tastes, bool attention, cudaStream_t stream) {
+  if (n_tastes == 1) return launch_wmrb<T, kPair, kCollapseSingle, 1>(p, stream);
+  if (attention) {
+    switch (n_tastes) {
+      case 2: return launch_wmrb<T, kPair, kCollapseAttention, 2>(p, stream);
+      case 3: return launch_wmrb<T, kPair, kCollapseAttention, 3>(p, stream);
+      default: return launch_wmrb<T, kPair, kCollapseAttention, 4>(p, stream);
+    }
+  }
+  switch (n_tastes) {
+    case 2: return launch_wmrb<T, kPair, kCollapseMax, 2>(p, stream);
+    case 3: return launch_wmrb<T, kPair, kCollapseMax, 3>(p, stream);
+    case 4: return launch_wmrb<T, kPair, kCollapseMax, 4>(p, stream);
+    case 5: return launch_wmrb<T, kPair, kCollapseMax, 5>(p, stream);
+    case 6: return launch_wmrb<T, kPair, kCollapseMax, 6>(p, stream);
+    case 7: return launch_wmrb<T, kPair, kCollapseMax, 7>(p, stream);
+    default: return launch_wmrb<T, kPair, kCollapseMax, 8>(p, stream);
+  }
 }
 
 int wmrb_step(const void* user_repr, const void* item_repr, int32_t repr_is_bf16, const float* user_bias,
@@ -452,6 +725,77 @@ int wmrb_step(const void* user_repr, const void* item_repr, int32_t repr_is_bf16
   p.d_item_repr = d_item_repr;
   p.d_item_bias = d_item_bias;
   return repr_is_bf16 ? launch_wmrb<__nv_bfloat16>(p, stream) : launch_wmrb<float>(p, stream);
+}
+
+int wmrb_step_tastes(const void* user_rows, const void* item_repr, int32_t repr_is_bf16, int32_t n_tastes,
+                     int32_t attention, int32_t euclidean, const float* user_bias, const float* item_bias,
+                     const int32_t* inter_indptr, const int32_t* inter_item, const float* inter_val,
+                     const float* item_weight_sum, const int32_t* samples, int64_t n_users, int64_t n_items, int32_t d,
+                     int32_t n_sampled, float* loss, float* pred_serial, float* coef, float* d_user_rows,
+                     float* d_user_bias, float* d_item_repr, float* d_item_bias, cudaStream_t stream) {
+  TRK_CHECK_ARG(user_rows && item_repr && inter_indptr && samples, "wmrb_step_tastes: null input");
+  TRK_CHECK_ARG(loss && pred_serial && coef && d_user_rows && d_item_repr, "wmrb_step_tastes: null output");
+  TRK_CHECK_ARG((user_bias == nullptr) == (item_bias == nullptr), "wmrb_step_tastes: biases must be given together");
+  TRK_CHECK_ARG((user_bias == nullptr) == (d_user_bias == nullptr) && (item_bias == nullptr) == (d_item_bias == nullptr),
+                "wmrb_step_tastes: bias gradients must match the biases");
+  TRK_CHECK_ARG(n_users >= 0 && n_items >= 1 && n_items < (1ll << 31) && n_sampled >= 1 && n_tastes >= 1,
+                "wmrb_step_tastes: bad sizes");
+  TRK_CHECK_ARG((attention == 0 || attention == 1) && (euclidean == 0 || euclidean == 1),
+                "wmrb_step_tastes: attention and euclidean are flags");
+  const int max_d = n_tastes == 1 ? 512 : 128;
+  const int max_tastes = attention ? 4 : 8;
+  if (d < 4 || d % 4 != 0 || d > max_d || n_sampled > 2048 || n_tastes > max_tastes || (attention && n_tastes == 1)) {
+    set_error("wmrb_step_tastes: n_components=%d (multiple of 4, <= 512 for one taste, <= 128 for several) / "
+              "n_tastes=%d (<= 8, <= 4 with attention, attention needs >= 2) / n_sampled=%d (<= 2048) outside the fused "
+              "kernel", d, n_tastes, n_sampled);
+    return TRK_ERR_UNSUPPORTED;
+  }
+  TRK_CHECK_ARG(reinterpret_cast<uintptr_t>(user_rows) % 16 == 0 && reinterpret_cast<uintptr_t>(item_repr) % 16 == 0 &&
+                    reinterpret_cast<uintptr_t>(d_user_rows) % 16 == 0 && reinterpret_cast<uintptr_t>(d_item_repr) % 16 == 0,
+                "wmrb_step_tastes: rows must be 16-byte aligned");
+  if (n_users == 0) return TRK_OK;
+  WmrbParams p;
+  p.user_repr = user_rows;
+  p.item_repr = item_repr;
+  p.user_bias = user_bias;
+  p.item_bias = item_bias;
+  p.inter_indptr = inter_indptr;
+  p.inter_item = inter_item;
+  p.inter_val = inter_val;
+  p.item_weight_sum = item_weight_sum;
+  p.samples = samples;
+  p.n_users = n_users;
+  p.n_items = static_cast<int32_t>(n_items);
+  p.d = d;
+  p.n_sampled = n_sampled;
+  p.rank_scale = static_cast<float>(n_items) / static_cast<float>(n_sampled);
+  p.loss = loss;
+  p.pred_serial = pred_serial;
+  p.coef = coef;
+  p.d_user_repr = d_user_rows;
+  p.d_user_bias = d_user_bias;
+  p.d_item_repr = d_item_repr;
+  p.d_item_bias = d_item_bias;
+  const bool att = attention != 0;
+  if (repr_is_bf16)
+    return euclidean ? launch_wmrb_form<__nv_bfloat16, kPairEuclid>(p, n_tastes, att, stream)
+                     : launch_wmrb_form<__nv_bfloat16, kPairDot>(p, n_tastes, att, stream);
+  return euclidean ? launch_wmrb_form<float, kPairEuclid>(p, n_tastes, att, stream)
+                   : launch_wmrb_form<float, kPairDot>(p, n_tastes, att, stream);
+}
+
+int l2_normalize_rows_step(const float* x, int64_t rows, int32_t d, int32_t n_normalize, float* out, float* grad,
+                           cudaStream_t stream) {
+  TRK_CHECK_ARG(x && rows >= 0 && d >= 1 && (out || grad), "l2_normalize_rows_step: bad arguments");
+  if (d > 512 || n_normalize < 1 || n_normalize > 2) {
+    set_error("l2_normalize_rows_step: d=%d (<= 512) / n_normalize=%d (1 or 2) outside the kernel", d, n_normalize);
+    return TRK_ERR_UNSUPPORTED;
+  }
+  if (rows == 0) return TRK_OK;
+  l2_normalize_rows_step_kernel<<<capped_grid(ceil_div(rows, kNormWarps), 16), kNormWarps * 32, 0, stream>>>(
+      x, rows, d, n_normalize, out, grad);
+  TRK_CHECK_LAUNCH();
+  return TRK_OK;
 }
 
 int f32_to_bf16(const float* x, int64_t n, void* out, cudaStream_t stream) {

@@ -118,13 +118,14 @@ K1_MAX_WIDTH = 512      # widest row one K1 launch covers (256 when the width is
 
 
 def gather_reduce(csr, weights, n_normalize=0, want_f32=True, split_d_pad=None, want_norm=False, stats=None,
-                  split_out=None):
+                  split_out=None, out_f32=None):
     """K1.  Returns (repr_f32 or None, split or None, scale or None[, norm]).
 
     want_norm: also return the row norms (upper bounds) formed in K1's epilogue; stats: float32[3] that receives the
     max norm / max row scale (zeroed by the call).  Both feed the filter form of the fused top-k.
     split_out: (split [rows, 2 split_d_pad] fp16, scale [rows] f32) contiguous tensors -- e.g. one operand's slice of a
-    stacked mixture-of-tastes operand -- that K1 writes instead of new ones."""
+    stacked mixture-of-tastes operand -- that K1 writes instead of new ones.  out_f32: a contiguous float32 [rows, d]
+    tensor K1 writes the representation to instead of a new one (e.g. one plane of the training step's operand)."""
     lib = require_cuda()
     rows, n_features = csr.shape
     d = int(weights.shape[1])
@@ -133,7 +134,9 @@ def gather_reduce(csr, weights, n_normalize=0, want_f32=True, split_d_pad=None, 
     dev = weights.device
     if split_d_pad is None and not want_norm and stats is None and (d > K1_MAX_WIDTH or (d % 4 != 0 and d > 256)):
         return _gather_reduce_wide(csr, weights, n_normalize), None, None
-    out = torch.empty((rows, d), dtype=torch.float32, device=dev) if want_f32 else None
+    out = None
+    if want_f32:
+        out = torch.empty((rows, d), dtype=torch.float32, device=dev) if out_f32 is None else out_f32
     split = scale = norm = None
     d_pad = 0
     if split_d_pad is not None:

@@ -505,8 +505,7 @@ class TensorRec(object):
 
     def _fit_epochs(self, batches, epochs, learning_rate, alpha, batched_alpha, verbose, n_sampled_items, device):
         from . import train_kernels
-        on_kernels = device.type == 'cuda' and train_kernels.eligible(self) and \
-            (n_sampled_items is None or n_sampled_items <= 2048)
+        on_kernels = device.type == 'cuda' and train_kernels.step_plan(self, n_sampled_items) is not None
         for epoch in range(epochs):
             for batch, (int_in, uf_in, if_in) in enumerate(batches):
                 if uf_in.shape[1] != self.n_user_features or if_in.shape[1] != self.n_item_features:

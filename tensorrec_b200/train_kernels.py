@@ -13,8 +13,15 @@ WMRBLossGraph or BalancedWMRBLossGraph, one taste, no attention -- one Adam step
         trk_csr_project_biases_f32     on the transposed CSR: feature-bias gradients
         trk_adam_step_f32              L2 term + Adam moments + parameter step (tensorrec/tensorrec.py:487-489)
 
+The same step trains every other form step_plan() accepts (DESIGN §3.10): cosine and Euclidean prediction,
+NormalizedLinearRepresentationGraph users / items / attention, mixtures of tastes with max or attention collapse, and
+any n_components (zero-padded to a multiple of 4 inside the step).  There the user operand is NT taste planes (and NT
+attention planes) stacked for trk_wmrb_step_tastes, normalised rows come from trk_l2_normalize_rows_step_f32 forward
+and backward, and every weight gets its own K1^T and Adam pass.
+
 Every other model family trains through the torch-autograd mirror of the reference's graph functions
 (TensorRec._training_losses); TENSORREC_B200_TRAIN_PATH=torch forces that path."""
+import collections
 import ctypes
 import os
 
@@ -78,6 +85,82 @@ def eligible(model):
             and model.n_components % 4 == 0 and 4 <= model.n_components <= 512)
 
 
+MAX_SAMPLED = 2048                 # n_sampled_items the fused step covers
+MAX_D_ONE_TASTE = 512              # n_components with one taste
+MAX_D_TASTES = 128                 # n_components with several tastes
+MAX_TASTES = 8                     # n_tastes without attention
+MAX_TASTES_ATTENTION = 4           # n_tastes with attention
+
+# The form of the fused step that trains a model: pair 'dot' (dot and cosine) or 'euclidean'; how many times the user,
+# attention and item rows are L2-normalised (NormalizedLinearRepresentationGraph once, cosine once more); d_pad the
+# operand width (n_components rounded up to a multiple of 4).
+StepForm = collections.namedtuple('StepForm', ['pair', 'n_tastes', 'attention', 'normalize_user', 'normalize_attn',
+                                               'normalize_item', 'd_pad'])
+
+
+def step_plan(model, n_sampled_items=None):
+    """The StepForm of the fused training step for this model, or None when it trains on the torch path: a WMRB /
+    BalancedWMRB loss; dot, cosine or Euclidean prediction; Linear or NormalizedLinear user, item and attention graphs
+    (or no attention); n_components <= 512 for one taste, <= 128 with n_tastes <= 8 (<= 4 with attention);
+    n_sampled_items <= 2048."""
+    from .loss_graphs import WMRBLossGraph, BalancedWMRBLossGraph
+    from .prediction_graphs import (CosineSimilarityPredictionGraph, DotProductPredictionGraph,
+                                    EuclideanSimilarityPredictionGraph)
+    from .representation_graphs import LinearRepresentationGraph, NormalizedLinearRepresentationGraph
+    if TRAIN_PATH == 'torch' or type(model.loss_graph_factory) not in (WMRBLossGraph, BalancedWMRBLossGraph):
+        return None
+    pred = type(model.prediction_graph_factory)
+    if pred not in (DotProductPredictionGraph, CosineSimilarityPredictionGraph, EuclideanSimilarityPredictionGraph):
+        return None
+    linear = (LinearRepresentationGraph, NormalizedLinearRepresentationGraph)
+    attention = model.attention_graph_factory is not None
+    if type(model.user_repr_graph_factory) not in linear or type(model.item_repr_graph_factory) not in linear:
+        return None
+    if attention and type(model.attention_graph_factory) not in linear:
+        return None
+    d, nt = int(model.n_components), int(model.n_tastes)
+    if n_sampled_items is not None and n_sampled_items > MAX_SAMPLED:
+        return None
+    if nt == 1:
+        if attention or not 1 <= d <= MAX_D_ONE_TASTE:
+            return None
+    elif d > MAX_D_TASTES or nt > (MAX_TASTES_ATTENTION if attention else MAX_TASTES):
+        return None
+    cos = 1 if pred is CosineSimilarityPredictionGraph else 0
+
+    def n_norm(graph):
+        return (1 if type(graph) is NormalizedLinearRepresentationGraph else 0) + cos
+
+    return StepForm(pair='euclidean' if pred is EuclideanSimilarityPredictionGraph else 'dot', n_tastes=nt,
+                    attention=attention, normalize_user=n_norm(model.user_repr_graph_factory),
+                    normalize_attn=n_norm(model.attention_graph_factory) if attention else 0,
+                    normalize_item=n_norm(model.item_repr_graph_factory), d_pad=(d + 3) // 4 * 4)
+
+
+def _plain(form):
+    """The dot / one-taste / unnormalised / unpadded form: trk_wmrb_step."""
+    return (form.pair == 'dot' and form.n_tastes == 1 and form.normalize_user == 0 and form.normalize_item == 0)
+
+
+def check_step_inputs(interactions_shape, n_users, n_items, n_sampled_items, samples=None):
+    """Raises ValueError unless the interactions are (n_users, n_items) and the caller's samples, if any, are int32
+    [n_users, n_sampled_items] item ids in [0, n_items): the step's kernels index item rows with both, unchecked."""
+    if tuple(int(x) for x in interactions_shape) != (int(n_users), int(n_items)):
+        raise ValueError('interactions have shape {} but the feature matrices give {} users x {} items'.format(
+            tuple(interactions_shape), n_users, n_items))
+    if samples is None:
+        return
+    if samples.dtype not in (torch.int32, np.int32):
+        raise ValueError('samples must be int32, got {}'.format(samples.dtype))
+    if tuple(samples.shape) != (int(n_users), int(n_sampled_items)):
+        raise ValueError('samples have shape {} but the step needs ({}, {})'.format(tuple(samples.shape), n_users,
+                                                                                 n_sampled_items))
+    if samples.numel() if isinstance(samples, torch.Tensor) else samples.size:
+        lo, hi = int(samples.min()), int(samples.max())
+        if lo < 0 or hi >= n_items:
+            raise ValueError('samples hold item ids in [{}, {}] outside [0, {})'.format(lo, hi, n_items))
+
+
 class WmrbStep(object):
     """State of the kernel training path of one model: Adam moments per weight, the step counter of the sampler's
     stream and of Adam's bias correction."""
@@ -121,10 +204,14 @@ class WmrbStep(object):
                 return w * torch.rsqrt(torch.clamp((w * w).sum(dim=1, keepdim=True), min=1e-12))
             return init
 
-        names = ['linear_weights_item', 'linear_weights_user_0']      # creation order of the reference's graph
-        ws = {'linear_weights_item': self._weight('linear_weights_item', (n_item_features, d), normal_rows(n_item_features)),
-              'linear_weights_user_0': self._weight('linear_weights_user_0', (n_user_features, d),
-                                                    normal_rows(n_user_features))}
+        names = ['linear_weights_item']           # creation order of the reference's graph
+        for t in range(self.model.n_tastes):
+            names.append('linear_weights_user_{}'.format(t))
+            if self.model.attention_graph_factory is not None:
+                names.append('linear_weights_attn_{}'.format(t))
+        ws = {name: self._weight(name, (n_item_features if name == 'linear_weights_item' else n_user_features, d),
+                                 normal_rows(n_item_features if name == 'linear_weights_item' else n_user_features))
+              for name in names}
         if self.model.biased:         # recommendation_graphs.py:11: zeros
             for name, n in (('feature_biases_user', n_user_features), ('feature_biases_item', n_item_features)):
                 ws[name] = self._weight(name, (n, 1), lambda n=n: torch.zeros(n, 1, dtype=torch.float32))
@@ -138,18 +225,40 @@ class WmrbStep(object):
         n_positive_interactions * batched_alpha).  Returns the device tensors of the step (loss, pred_serial)."""
         lib = kernels.require_cuda()
         from .loss_graphs import BalancedWMRBLossGraph
-        dev, d = self.device, self.model.n_components
+        form = step_plan(self.model)
+        if form is None:
+            raise ValueError('the fused training step does not cover this model (train_kernels.step_plan)')
+        dev, d, dp = self.device, self.model.n_components, form.d_pad
         n_users, n_items = user_in.shape[0], item_in.shape[0]
+        check_step_inputs(interactions_in.shape, n_users, n_items, n_sampled_items, samples)
         ucsr, icsr = user_in.device_csr(dev), item_in.device_csr(dev)
         ucsr_t, icsr_t = user_in.device_csr_t(dev), item_in.device_csr_t(dev)
         inter = interactions_in.device_csr(dev)
         names, ws = self._weights(user_in.shape[1], item_in.shape[1])
-        w_user, w_item = ws['linear_weights_user_0'].detach(), ws['linear_weights_item'].detach()
+        # the user operand: taste planes, then attention planes, [n_rows, n_users, d_pad]
+        user_ops = [('linear_weights_user_{}'.format(t), form.normalize_user) for t in range(form.n_tastes)]
+        if form.attention:
+            user_ops += [('linear_weights_attn_{}'.format(t), form.normalize_attn) for t in range(form.n_tastes)]
+
+        def operand(csr, name, n_norm, out):
+            """K1 of one weight into `out` (normalised rows: K1's raw rows are kept for the backward pass)."""
+            w = ws[name].detach()
+            if dp != d:                # zero columns change no prediction, norm or gradient
+                w = torch.nn.functional.pad(w, (0, dp - d))
+            if n_norm == 0:
+                kernels.gather_reduce(csr, w, want_f32=True, out_f32=out)
+                return None
+            raw, _, _ = kernels.gather_reduce(csr, w, want_f32=True)
+            _lib.check(lib.trk_l2_normalize_rows_step_f32(_p(raw), raw.shape[0], dp, n_norm, _p(out), None, _stream()),
+                       'trk_l2_normalize_rows_step_f32')
+            return raw
 
         self._mark('start')
         # forward: representations and projected biases (K1)
-        user_repr, _, _ = kernels.gather_reduce(ucsr, w_user, want_f32=True)
-        item_repr, _, _ = kernels.gather_reduce(icsr, w_item, want_f32=True)
+        user_repr = torch.empty((len(user_ops), n_users, dp), dtype=torch.float32, device=dev)
+        item_repr = torch.empty((n_items, dp), dtype=torch.float32, device=dev)
+        item_raw = operand(icsr, 'linear_weights_item', form.normalize_item, item_repr)
+        user_raw = [operand(ucsr, name, n_norm, user_repr[r]) for r, (name, n_norm) in enumerate(user_ops)]
         ub = ib = None
         if self.model.biased:
             ub = kernels.project_biases(ucsr, ws['feature_biases_user'].detach().reshape(-1))
@@ -174,20 +283,36 @@ class WmrbStep(object):
         loss = torch.empty((nnz,), dtype=torch.float32, device=dev)
         pred = torch.empty((nnz,), dtype=torch.float32, device=dev)
         coef = torch.empty((nnz,), dtype=torch.float32, device=dev)
-        d_user_repr = torch.empty((n_users, d), dtype=torch.float32, device=dev)
-        d_item_repr = torch.zeros((n_items, d), dtype=torch.float32, device=dev)
+        d_user_repr = torch.empty(user_repr.shape, dtype=torch.float32, device=dev)
+        d_item_repr = torch.zeros((n_items, dp), dtype=torch.float32, device=dev)
         d_ub = torch.empty((n_users,), dtype=torch.float32, device=dev) if self.model.biased else None
         d_ib = torch.zeros((n_items,), dtype=torch.float32, device=dev) if self.model.biased else None
-        rc = lib.trk_wmrb_step(_p(repr_u), _p(repr_i), 1 if self.bf16 else 0, _p(ub), _p(ib), _p(inter.indptr),
-                               _p(inter.col), _p(inter.val), _p(weight_sum), _p(samples), n_users, n_items, d,
-                               int(samples.shape[1]), _p(loss), _p(pred), _p(coef), _p(d_user_repr), _p(d_ub),
-                               _p(d_item_repr), _p(d_ib), _stream())
-        _lib.check(rc, 'trk_wmrb_step')
+        if _plain(form):
+            rc = lib.trk_wmrb_step(_p(repr_u), _p(repr_i), 1 if self.bf16 else 0, _p(ub), _p(ib), _p(inter.indptr),
+                                   _p(inter.col), _p(inter.val), _p(weight_sum), _p(samples), n_users, n_items, dp,
+                                   int(samples.shape[1]), _p(loss), _p(pred), _p(coef), _p(d_user_repr), _p(d_ub),
+                                   _p(d_item_repr), _p(d_ib), _stream())
+            _lib.check(rc, 'trk_wmrb_step')
+        else:
+            rc = lib.trk_wmrb_step_tastes(_p(repr_u), _p(repr_i), 1 if self.bf16 else 0, form.n_tastes,
+                                          1 if form.attention else 0, 1 if form.pair == 'euclidean' else 0, _p(ub),
+                                          _p(ib), _p(inter.indptr), _p(inter.col), _p(inter.val), _p(weight_sum),
+                                          _p(samples), n_users, n_items, dp, int(samples.shape[1]), _p(loss), _p(pred),
+                                          _p(coef), _p(d_user_repr), _p(d_ub), _p(d_item_repr), _p(d_ib), _stream())
+            _lib.check(rc, 'trk_wmrb_step_tastes')
         self._mark('wmrb_step')
 
-        # backward through the sparse x dense products: K1 on the transposed CSR
-        grads = {'linear_weights_user_0': kernels.gather_reduce(ucsr_t, d_user_repr, want_f32=True)[0],
-                 'linear_weights_item': kernels.gather_reduce(icsr_t, d_item_repr, want_f32=True)[0]}
+        # backward through the normalisations, then through the sparse x dense products: K1 on the transposed CSR
+        def weight_grad(csr_t, raw, n_norm, d_rows):
+            if raw is not None:
+                _lib.check(lib.trk_l2_normalize_rows_step_f32(_p(raw), raw.shape[0], dp, n_norm, None, _p(d_rows),
+                                                              _stream()), 'trk_l2_normalize_rows_step_f32')
+            g = kernels.gather_reduce(csr_t, d_rows, want_f32=True)[0]
+            return g if dp == d else g[:, :d].contiguous()
+
+        grads = {'linear_weights_item': weight_grad(icsr_t, item_raw, form.normalize_item, d_item_repr)}
+        for r, (name, n_norm) in enumerate(user_ops):
+            grads[name] = weight_grad(ucsr_t, user_raw[r], n_norm, d_user_repr[r])
         if self.model.biased:
             grads['feature_biases_user'] = kernels.project_biases(ucsr_t, d_ub)
             grads['feature_biases_item'] = kernels.project_biases(icsr_t, d_ib)
