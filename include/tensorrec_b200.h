@@ -530,6 +530,19 @@ int trk_topk_merge_dedup_pair(const float* a_score, const int32_t* a_item, int64
  *                    d_item_repr receives one red.global.add per pair, summed over the operand rows.  Constraints:
  *                    d % 4 == 0 (pad with zero columns), d <= 512 for one taste and <= 128 for several, n_tastes <= 8
  *                    (<= 4 and >= 2 with attention), n_sampled <= 2048; others return TRK_ERR_UNSUPPORTED.
+ * trk_serial_loss_step
+ *                    the training step of the serial losses (DESIGN §3.11): loss_kind 0 is RMSELossGraph,
+ *                    L = sqrt(mean_n (y_n - p_n)^2) (tensorrec/loss_graphs.py:53-59), 1 is SeparationLossGraph,
+ *                    L = 1 - Phi(-(mu_Q - mu_P) / sqrt(v_Q + v_P)) over the predictions of P = {y > 0} and
+ *                    Q = {y <= 0} (mean and biased variance, loss_graphs.py:75-98), over all nnz stored interactions
+ *                    (explicit zeros and duplicates included).  Operands, forms and constraints as trk_wmrb_step_tastes,
+ *                    without samples.  Three launches on `stream`: pred_serial [nnz] (as trk_wmrb_step_tastes computes
+ *                    it); the statistics, which write the scalar loss [1] and a loss state into `workspace`
+ *                    (trk_serial_loss_workspace_bytes(nnz) bytes, 8-byte aligned); then the gradients of L: d_user_rows
+ *                    and d_user_bias written, d_item_repr and d_item_bias ADDED to (zero them first).  nnz == 0
+ *                    launches no kernel: loss = NaN, d_user_rows = d_user_bias = 0, and pred_serial, inter_item,
+ *                    inter_val and workspace may be null.  An empty group or L = 0 gives NaN, as the losses' own
+ *                    gradients do.  nnz < 2^31.
  * trk_l2_normalize_rows_step_f32
  *                    row L2-normalisation N(x) = x rsqrt(max(|x|^2, 1e-12)), n_normalize (1 or 2) times, of raw rows
  *                    x [rows, d <= 512]: out (if non-null) receives N^n(x); grad (if non-null) holds d loss / d N^n(x) and
@@ -553,6 +566,13 @@ int trk_wmrb_step_tastes(const void* user_rows, const void* item_repr, int32_t r
                          const float* item_weight_sum, const int32_t* samples, int64_t n_users, int64_t n_items,
                          int32_t d, int32_t n_sampled, float* loss, float* pred_serial, float* coef, float* d_user_rows,
                          float* d_user_bias, float* d_item_repr, float* d_item_bias, void* stream);
+size_t trk_serial_loss_workspace_bytes(int64_t nnz);
+int trk_serial_loss_step(int32_t loss_kind, const void* user_rows, const void* item_repr, int32_t repr_is_bf16,
+                         int32_t n_tastes, int32_t attention, int32_t euclidean, const float* user_bias,
+                         const float* item_bias, const int32_t* inter_indptr, const int32_t* inter_item,
+                         const float* inter_val, int64_t n_users, int64_t n_items, int32_t d, int64_t nnz, float* loss,
+                         float* pred_serial, float* d_user_rows, float* d_user_bias, float* d_item_repr,
+                         float* d_item_bias, void* workspace, size_t workspace_bytes, void* stream);
 int trk_l2_normalize_rows_step_f32(const float* x, int64_t rows, int32_t d, int32_t n_normalize, float* out,
                                    float* grad, void* stream);
 int trk_f32_to_bf16(const float* x, int64_t n, void* out, void* stream);

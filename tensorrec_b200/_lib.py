@@ -108,6 +108,10 @@ SIGNATURES = {
     'trk_wmrb_step_tastes': (ctypes.c_int, [_c_p, _c_p, _c_i32, _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p,
                                             _c_p, _c_p, _c_i64, _c_i64, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p,
                                             _c_p, _c_p, _c_p]),
+    'trk_serial_loss_workspace_bytes': (_c_sz, [_c_i64]),
+    'trk_serial_loss_step': (ctypes.c_int, [_c_i32, _c_p, _c_p, _c_i32, _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p,
+                                            _c_p, _c_i64, _c_i64, _c_i32, _c_i64, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p, _c_p,
+                                            _c_sz, _c_p]),
     'trk_l2_normalize_rows_step_f32': (ctypes.c_int, [_c_p, _c_i64, _c_i32, _c_i32, _c_p, _c_p, _c_p]),
     'trk_f32_to_bf16': (ctypes.c_int, [_c_p, _c_i64, _c_p, _c_p]),
     'trk_adam_step_f32': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_i64, ctypes.c_float, ctypes.c_float, ctypes.c_float,

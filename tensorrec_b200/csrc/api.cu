@@ -145,6 +145,10 @@ int wmrb_step(const void*, const void*, int32_t, const float*, const float*, con
 int wmrb_step_tastes(const void*, const void*, int32_t, int32_t, int32_t, int32_t, const float*, const float*,
                      const int32_t*, const int32_t*, const float*, const float*, const int32_t*, int64_t, int64_t, int32_t,
                      int32_t, float*, float*, float*, float*, float*, float*, float*, cudaStream_t);
+size_t serial_loss_workspace_bytes(int64_t);
+int serial_loss_step(int32_t, const void*, const void*, int32_t, int32_t, int32_t, int32_t, const float*, const float*,
+                     const int32_t*, const int32_t*, const float*, int64_t, int64_t, int32_t, int64_t, float*, float*,
+                     float*, float*, float*, float*, void*, size_t, cudaStream_t);
 int l2_normalize_rows_step(const float*, int64_t, int32_t, int32_t, float*, float*, cudaStream_t);
 int f32_to_bf16(const float*, int64_t, void*, cudaStream_t);
 int adam_step(float*, const float*, float*, float*, int64_t, float, float, float, float, float, cudaStream_t);
@@ -594,6 +598,20 @@ int trk_wmrb_step_tastes(const void* user_rows, const void* item_repr, int32_t r
                                inter_indptr, inter_item, inter_val, item_weight_sum, samples, n_users, n_items, d,
                                n_sampled, loss, pred_serial, coef, d_user_rows, d_user_bias, d_item_repr, d_item_bias,
                                trk::as_stream(stream));
+}
+
+size_t trk_serial_loss_workspace_bytes(int64_t nnz) { return trk::serial_loss_workspace_bytes(nnz); }
+
+int trk_serial_loss_step(int32_t loss_kind, const void* user_rows, const void* item_repr, int32_t repr_is_bf16,
+                         int32_t n_tastes, int32_t attention, int32_t euclidean, const float* user_bias,
+                         const float* item_bias, const int32_t* inter_indptr, const int32_t* inter_item,
+                         const float* inter_val, int64_t n_users, int64_t n_items, int32_t d, int64_t nnz, float* loss,
+                         float* pred_serial, float* d_user_rows, float* d_user_bias, float* d_item_repr,
+                         float* d_item_bias, void* workspace, size_t workspace_bytes, void* stream) {
+  return trk::serial_loss_step(loss_kind, user_rows, item_repr, repr_is_bf16, n_tastes, attention, euclidean, user_bias,
+                               item_bias, inter_indptr, inter_item, inter_val, n_users, n_items, d, nnz, loss,
+                               pred_serial, d_user_rows, d_user_bias, d_item_repr, d_item_bias, workspace,
+                               workspace_bytes, trk::as_stream(stream));
 }
 
 int trk_l2_normalize_rows_step_f32(const float* x, int64_t rows, int32_t d, int32_t n_normalize, float* out,

@@ -18,6 +18,9 @@
 //                         The same kernel, templated on the pair form, the collapse and the taste count, trains cosine,
 //                         Euclidean, mixture-of-tastes and attention models (trk_wmrb_step_tastes; DESIGN §3.10), with
 //                         l2_normalize_rows_step_kernel normalising operands forward and backward;
+//   serial losses         RMSELossGraph / SeparationLossGraph (loss_graphs.py:53-59, 75-98; trk_serial_loss_step,
+//                         DESIGN §3.11): the same kernel's forward mode, serial_stats_kernel + serial_finish_kernel
+//                         (the loss and the state its gradient needs), then the kernel's backward mode;
 //   adam_step_kernel      tf.train.AdamOptimizer.minimize(basic_loss + alpha * sum l2_loss(w)) (tensorrec.py:487-489):
 //                         L2 term, moment updates and the parameter step in one pass over every weight.
 //
@@ -26,6 +29,7 @@
 // (user, interaction or sample) pair, twice (the second time from L2).
 #include <cuda_bf16.h>
 
+#include <algorithm>
 #include <type_traits>
 
 #include "common.cuh"
@@ -149,9 +153,32 @@ struct WmrbParams {
   float* d_user_bias;           // [n_users] or null
   float* d_item_repr;           // [n_items, d], zeroed by the caller: added to with red.global.add
   float* d_item_bias;           // [n_items] or null, zeroed by the caller
+  const void* serial_state;     // serial backward: the SerialLossState serial_finish_kernel wrote
+  int32_t serial_loss;          // serial backward: kSerialRmse | kSerialSeparation
 };
 
 constexpr int kWmrbWarps = 4;
+
+// What one launch of wmrb_step_kernel does: the fused WMRB step (forward, loss and backward in one pass), or one half
+// of a serial-loss step (trk_serial_loss_step; DESIGN §3.11), whose global statistics need a launch in between:
+//   kModeSerialForward   writes pred_serial of every interaction and nothing else;
+//   kModeSerialBackward  reads pred_serial back, forms d loss / d prediction from the loss state, and runs the backward.
+constexpr int kModeWmrb = 0, kModeSerialForward = 1, kModeSerialBackward = 2;
+constexpr int kSerialRmse = 0, kSerialSeparation = 1;
+
+// The gradient of a serial loss with respect to one prediction p of value y is g = a_k + b_k (p - mu_k), k the group of
+// y (0: y > 0, 1: y <= 0) for Separation; RMSE has g = b_0 (p - y).
+struct SerialLossState {
+  float a[2], b[2], mu[2];
+};
+
+__device__ __forceinline__ float serial_grad(const WmrbParams& p, int n) {
+  const SerialLossState* st = static_cast<const SerialLossState*>(p.serial_state);
+  const float pr = p.pred_serial[n], y = __ldg(p.inter_val + n);
+  if (p.serial_loss == kSerialRmse) return (pr - y) * st->b[0];
+  const int k = y > 0.0f ? 0 : 1;
+  return st->a[k] + st->b[k] * (pr - st->mu[k]);
+}
 
 // The forms of the step (trk_wmrb_step_tastes; trk_wmrb_step is the dot / single-taste form):
 //   pair      the scalar function of a pair's operand rows, evaluated as a "row form" f per (pair, operand row):
@@ -259,8 +286,9 @@ __device__ __forceinline__ void taste_coefs(const float (&f)[NF], float g, float
 // NT tastes; the user operand is NR = NT (or 2 NT with attention: the attention rows follow the taste rows) planes
 // [n_users, d], plane r at user_repr + r * n_users * d, and so is d_user_repr.  The dot / single-taste form (kPlain) is
 // the step of trk_wmrb_step; the other forms recompute a pair's row forms in the backward pass (from the item row
-// gathered there anyway) instead of keeping NT values per sample.
-template <typename T, int CH, int kPair = kPairDot, int kCollapse = kCollapseSingle, int NT = 1>
+// gathered there anyway) instead of keeping NT values per sample.  kMode selects the WMRB step or one half of a serial
+// step; the serial modes touch neither the samples nor shared memory.
+template <typename T, int CH, int kPair = kPairDot, int kCollapse = kCollapseSingle, int NT = 1, int kMode = kModeWmrb>
 __global__ void __launch_bounds__(kWmrbWarps * 32)
 wmrb_step_kernel(const WmrbParams p) {
   constexpr bool kPlain = kPair == kPairDot && kCollapse == kCollapseSingle;
@@ -345,179 +373,324 @@ wmrb_step_kernel(const WmrbParams p) {
     using PairRows = std::integral_constant<int, NR>;
 
     // ---- forward 1: the sampled items ----
-    for (int j0 = 0; j0 < S; j0 += 4) {
-      int32_t ids[4];
-      const int nv = min(4, S - j0);
+    if constexpr (kMode == kModeWmrb) {
+      for (int j0 = 0; j0 < S; j0 += 4) {
+        int32_t ids[4];
+        const int nv = min(4, S - j0);
 #pragma unroll
-      for (int q = 0; q < 4; ++q) ids[q] = q < nv ? __ldg(srow + j0 + q) : 0;
-      float s[4];
-      predict4(SampleRows{}, ids, nv, s);
-      if (lane < nv) {
-        sp[j0 + lane] = s[lane == 0 ? 0 : lane == 1 ? 1 : lane == 2 ? 2 : 3];
-        gs[j0 + lane] = 0.0f;
+        for (int q = 0; q < 4; ++q) ids[q] = q < nv ? __ldg(srow + j0 + q) : 0;
+        float s[4];
+        predict4(SampleRows{}, ids, nv, s);
+        if (lane < nv) {
+          sp[j0 + lane] = s[lane == 0 ? 0 : lane == 1 ? 1 : lane == 2 ? 2 : 3];
+          gs[j0 + lane] = 0.0f;
+        }
       }
+      __syncwarp();
     }
-    __syncwarp();
 
     // ---- forward 2 + loss: the user's interactions ----
-    for (int n0 = a; n0 < b; n0 += 4) {
-      int32_t ids[4];
-      const int nv = min(4, b - n0);
+    if constexpr (kMode != kModeSerialBackward) {
+      for (int n0 = a; n0 < b; n0 += 4) {
+        int32_t ids[4];
+        const int nv = min(4, b - n0);
 #pragma unroll
-      for (int q = 0; q < 4; ++q) ids[q] = q < nv ? __ldg(p.inter_item + n0 + q) : 0;
-      float pr[4];
-      predict4(PairRows{}, ids, nv, pr);
-      for (int q = 0; q < nv; ++q) {      // warp-uniform
-        const float val = __ldg(p.inter_val + n0 + q);
-        float loss = 0.0f, coef = 0.0f;
-        if (val > 0.0f) {                 // loss_graphs.py:155 positive_interaction_mask
-          const float base = 1.0f - pr[q];
-          float sum = 0.0f;
-          for (int j = lane; j < S; j += 32) sum += fmaxf(base + sp[j], 0.0f);       // :171-174
-          sum = warp_sum(sum);
-          float smr = p.rank_scale * sum, w = p.rank_scale;                          // :177
-          if (p.item_weight_sum != nullptr) {                                        // :221-223, left to right
-            const float gsum = __ldg(p.item_weight_sum + ids[q]);
-            smr = smr * val / gsum;
-            w = w * val / gsum;
-          }
-          loss = logf(smr + 1.0f);                                                   // :179
-          const float dsum = w / (smr + 1.0f);      // d loss / d sum
-          int active = 0;
-          for (int j = lane; j < S; j += 32) {
-            if (base + sp[j] >= 0.0f) {             // tf.maximum passes the gradient to its first argument on ties
-              gs[j] += dsum;
-              active += 1;
+        for (int q = 0; q < 4; ++q) ids[q] = q < nv ? __ldg(p.inter_item + n0 + q) : 0;
+        float pr[4];
+        predict4(PairRows{}, ids, nv, pr);
+        if constexpr (kMode == kModeSerialForward) {
+          float mine = pr[0];               // lane q stores pr[q]: selects, not a local-memory array
+#pragma unroll
+          for (int q = 1; q < 4; ++q) mine = lane == q ? pr[q] : mine;
+          if (lane < nv) p.pred_serial[n0 + lane] = mine;
+        } else {
+          for (int q = 0; q < nv; ++q) {      // warp-uniform
+            const float val = __ldg(p.inter_val + n0 + q);
+            float loss = 0.0f, coef = 0.0f;
+            if (val > 0.0f) {                 // loss_graphs.py:155 positive_interaction_mask
+              const float base = 1.0f - pr[q];
+              float sum = 0.0f;
+              for (int j = lane; j < S; j += 32) sum += fmaxf(base + sp[j], 0.0f);       // :171-174
+              sum = warp_sum(sum);
+              float smr = p.rank_scale * sum, w = p.rank_scale;                          // :177
+              if (p.item_weight_sum != nullptr) {                                        // :221-223, left to right
+                const float gsum = __ldg(p.item_weight_sum + ids[q]);
+                smr = smr * val / gsum;
+                w = w * val / gsum;
+              }
+              loss = logf(smr + 1.0f);                                                   // :179
+              const float dsum = w / (smr + 1.0f);      // d loss / d sum
+              int active = 0;
+              for (int j = lane; j < S; j += 32) {
+                if (base + sp[j] >= 0.0f) {             // tf.maximum passes the gradient to its first argument on ties
+                  gs[j] += dsum;
+                  active += 1;
+                }
+              }
+#pragma unroll
+              for (int o = 16; o > 0; o >>= 1) active += __shfl_xor_sync(0xffffffffu, active, o);
+              coef = -dsum * static_cast<float>(active);
+            }
+            if (lane == 0) {
+              p.loss[n0 + q] = loss;
+              p.pred_serial[n0 + q] = pr[q];
+              p.coef[n0 + q] = coef;
             }
           }
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) active += __shfl_xor_sync(0xffffffffu, active, o);
-          coef = -dsum * static_cast<float>(active);
-        }
-        if (lane == 0) {
-          p.loss[n0 + q] = loss;
-          p.pred_serial[n0 + q] = pr[q];
-          p.coef[n0 + q] = coef;
         }
       }
+      __syncwarp();
     }
-    __syncwarp();
 
     // ---- backward: d/d user rows in registers, d/d item rows by red.global.add ----
-    float du[NR][CH][4];
+    if constexpr (kMode != kModeSerialForward) {
+      float du[NR][CH][4];
 #pragma unroll
-    for (int r = 0; r < NR; ++r)
+      for (int r = 0; r < NR; ++r)
 #pragma unroll
-      for (int c = 0; c < CH; ++c) du[r][c][0] = du[r][c][1] = du[r][c][2] = du[r][c][3] = 0.0f;
-    float dub = 0.0f;
-    float csum[NR];                   // euclid: sum over the pairs of c_r, the coefficient of -u_r in d u_r
+        for (int c = 0; c < CH; ++c) du[r][c][0] = du[r][c][1] = du[r][c][2] = du[r][c][3] = 0.0f;
+      float dub = 0.0f;
+      float csum[NR];                   // euclid: sum over the pairs of c_r, the coefficient of -u_r in d u_r
 #pragma unroll
-    for (int r = 0; r < NR; ++r) csum[r] = 0.0f;
-    // four pairs at a time: the item rows of all of them are requested before the first FMA (they were read by the
-    // forward pass a moment ago: L1 / L2 hits); a pair whose coefficient is zero (inactive hinge) contributes exact
-    // zeros and is skipped (warp-uniform).  Each pair's item gradient, summed over the operand rows, is one red.add.
-    auto backward4 = [&](auto nu, const int32_t (&ids)[4], const float (&g)[4]) {
-      constexpr int NU = decltype(nu)::value;
-      float iv[4][CH][4];
+      for (int r = 0; r < NR; ++r) csum[r] = 0.0f;
+      // four pairs at a time: the item rows of all of them are requested before the first FMA (they were read by the
+      // forward pass a moment ago: L1 / L2 hits); a pair whose coefficient is zero (inactive hinge) contributes exact
+      // zeros and is skipped (warp-uniform).  Each pair's item gradient, summed over the operand rows, is one red.add.
+      auto backward4 = [&](auto nu, const int32_t (&ids)[4], const float (&g)[4]) {
+        constexpr int NU = decltype(nu)::value;
+        float iv[4][CH][4];
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        if (g[q] == 0.0f) continue;
+        for (int q = 0; q < 4; ++q) {
+          if (g[q] == 0.0f) continue;
 #pragma unroll
-        for (int c = 0; c < CH; ++c) {
-          const int e = 4 * (lane + 32 * c);
-          if (e < d) load4<T>(item_repr + static_cast<int64_t>(ids[q]) * d + e, iv[q][c]);
+          for (int c = 0; c < CH; ++c) {
+            const int e = 4 * (lane + 32 * c);
+            if (e < d) load4<T>(item_repr + static_cast<int64_t>(ids[q]) * d + e, iv[q][c]);
+          }
+        }
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          if (g[q] == 0.0f) continue;
+          dub += g[q];
+          float cr[NU];
+          if constexpr (kPlain) {
+            cr[0] = g[q];
+          } else {
+            float part[NU];
+#pragma unroll
+            for (int r = 0; r < NU; ++r) part[r] = 0.0f;
+#pragma unroll
+            for (int c = 0; c < CH; ++c)
+              if (4 * (lane + 32 * c) < d) row_part(nu, c, iv[q][c], part);
+            float f[NU];
+#pragma unroll
+            for (int r = 0; r < NU; ++r) f[r] = warp_sum(part[r]);
+            taste_coefs<kPair, kCollapse, NT, NU == NT && NR != NT>(f, g[q], cr);
+          }
+          float cs = 0.0f;
+#pragma unroll
+          for (int r = 0; r < NU; ++r) cs += cr[r];
+#pragma unroll
+          for (int c = 0; c < CH; ++c) {
+            const int e = 4 * (lane + 32 * c);
+            if (e < d) {
+#pragma unroll
+              for (int r = 0; r < NU; ++r)
+#pragma unroll
+                for (int w = 0; w < 4; ++w) du[r][c][w] = fmaf(cr[r], iv[q][c][w], du[r][c][w]);
+              float gi[4];
+#pragma unroll
+              for (int w = 0; w < 4; ++w) {
+                if constexpr (kPair == kPairEuclid) gi[w] = -cs * iv[q][c][w];
+                else gi[w] = cr[0] * uv[0][c][w];
+#pragma unroll
+                for (int r = kPair == kPairEuclid ? 0 : 1; r < NU; ++r) gi[w] = fmaf(cr[r], uv[r][c][w], gi[w]);
+              }
+              red_add_v4(p.d_item_repr + static_cast<int64_t>(ids[q]) * d + e, gi[0], gi[1], gi[2], gi[3]);
+            }
+          }
+          if constexpr (kPair == kPairEuclid) {
+#pragma unroll
+            for (int r = 0; r < NU; ++r) csum[r] += cr[r];
+          }
+          if (lane == 0 && p.d_item_bias != nullptr) atomicAdd(p.d_item_bias + ids[q], g[q]);
+        }
+      };
+      if constexpr (kMode == kModeWmrb) {
+        for (int j0 = 0; j0 < S; j0 += 4) {
+          int32_t ids[4];
+          float g[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const bool ok = j0 + q < S;
+            ids[q] = ok ? __ldg(srow + j0 + q) : 0;
+            g[q] = ok ? gs[j0 + q] : 0.0f;
+          }
+          backward4(SampleRows{}, ids, g);
         }
       }
+      for (int n0 = a; n0 < b; n0 += 4) {
+        int32_t ids[4];
+        float g[4];
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        if (g[q] == 0.0f) continue;
-        dub += g[q];
-        float cr[NU];
-        if constexpr (kPlain) {
-          cr[0] = g[q];
-        } else {
-          float part[NU];
-#pragma unroll
-          for (int r = 0; r < NU; ++r) part[r] = 0.0f;
-#pragma unroll
-          for (int c = 0; c < CH; ++c)
-            if (4 * (lane + 32 * c) < d) row_part(nu, c, iv[q][c], part);
-          float f[NU];
-#pragma unroll
-          for (int r = 0; r < NU; ++r) f[r] = warp_sum(part[r]);
-          taste_coefs<kPair, kCollapse, NT, NU == NT && NR != NT>(f, g[q], cr);
+        for (int q = 0; q < 4; ++q) {
+          const bool ok = n0 + q < b;
+          ids[q] = ok ? __ldg(p.inter_item + n0 + q) : 0;
+          if constexpr (kMode == kModeSerialBackward) {
+            g[q] = ok ? serial_grad(p, n0 + q) : 0.0f;    // every lane reads the same words: warp-uniform
+          } else {
+            // coef was written by lane 0 of this warp: that lane reads it back and broadcasts
+            const float mine = (ok && lane == 0) ? p.coef[n0 + q] : 0.0f;
+            g[q] = __shfl_sync(0xffffffffu, mine, 0);
+          }
         }
-        float cs = 0.0f;
+        backward4(PairRows{}, ids, g);
+      }
 #pragma unroll
-        for (int r = 0; r < NU; ++r) cs += cr[r];
+      for (int r = 0; r < NR; ++r) {
 #pragma unroll
         for (int c = 0; c < CH; ++c) {
           const int e = 4 * (lane + 32 * c);
           if (e < d) {
+            if constexpr (kPair == kPairEuclid) {
 #pragma unroll
-            for (int r = 0; r < NU; ++r)
-#pragma unroll
-              for (int w = 0; w < 4; ++w) du[r][c][w] = fmaf(cr[r], iv[q][c][w], du[r][c][w]);
-            float gi[4];
-#pragma unroll
-            for (int w = 0; w < 4; ++w) {
-              if constexpr (kPair == kPairEuclid) gi[w] = -cs * iv[q][c][w];
-              else gi[w] = cr[0] * uv[0][c][w];
-#pragma unroll
-              for (int r = kPair == kPairEuclid ? 0 : 1; r < NU; ++r) gi[w] = fmaf(cr[r], uv[r][c][w], gi[w]);
+              for (int w = 0; w < 4; ++w) du[r][c][w] = fmaf(-csum[r], uv[r][c][w], du[r][c][w]);
             }
-            red_add_v4(p.d_item_repr + static_cast<int64_t>(ids[q]) * d + e, gi[0], gi[1], gi[2], gi[3]);
+            *reinterpret_cast<float4*>(p.d_user_repr + r * plane + u * d + e) =
+                make_float4(du[r][c][0], du[r][c][1], du[r][c][2], du[r][c][3]);
           }
         }
-        if constexpr (kPair == kPairEuclid) {
-#pragma unroll
-          for (int r = 0; r < NU; ++r) csum[r] += cr[r];
-        }
-        if (lane == 0 && p.d_item_bias != nullptr) atomicAdd(p.d_item_bias + ids[q], g[q]);
       }
-    };
-    for (int j0 = 0; j0 < S; j0 += 4) {
-      int32_t ids[4];
-      float g[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const bool ok = j0 + q < S;
-        ids[q] = ok ? __ldg(srow + j0 + q) : 0;
-        g[q] = ok ? gs[j0 + q] : 0.0f;
-      }
-      backward4(SampleRows{}, ids, g);
+      if (lane == 0 && p.d_user_bias != nullptr) p.d_user_bias[u] = dub;
     }
-    for (int n0 = a; n0 < b; n0 += 4) {
-      int32_t ids[4];
-      float g[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const bool ok = n0 + q < b;
-        ids[q] = ok ? __ldg(p.inter_item + n0 + q) : 0;
-        // coef was written by lane 0 of this warp: that lane reads it back and broadcasts
-        const float mine = (ok && lane == 0) ? p.coef[n0 + q] : 0.0f;
-        g[q] = __shfl_sync(0xffffffffu, mine, 0);
-      }
-      backward4(PairRows{}, ids, g);
-    }
-#pragma unroll
-    for (int r = 0; r < NR; ++r) {
-#pragma unroll
-      for (int c = 0; c < CH; ++c) {
-        const int e = 4 * (lane + 32 * c);
-        if (e < d) {
-          if constexpr (kPair == kPairEuclid) {
-#pragma unroll
-            for (int w = 0; w < 4; ++w) du[r][c][w] = fmaf(-csum[r], uv[r][c][w], du[r][c][w]);
-          }
-          *reinterpret_cast<float4*>(p.d_user_repr + r * plane + u * d + e) =
-              make_float4(du[r][c][0], du[r][c][1], du[r][c][2], du[r][c][3]);
-        }
-      }
-    }
-    if (lane == 0 && p.d_user_bias != nullptr) p.d_user_bias[u] = dub;
     __syncwarp();
   }
+}
+
+// The statistics of a serial loss over the nnz predictions, between the forward and the backward launch:
+// serial_stats_kernel (a grid fixed by serial_stats_grid) writes one SerialMoments per block, serial_finish_kernel (one
+// block) merges exactly that many in a fixed order and writes the loss and the SerialLossState.  Double throughout:
+//   RMSE        group 0 holds the count and the sum of (y - p)^2 (in m2);
+//   Separation  per group (0: y > 0, 1: y <= 0) the count, mean and sum of squared deviations, merged pairwise (Chan et
+//               al.), so the biased variance m2 / n does not cancel.
+struct SerialMoments {
+  double n[2], mean[2], m2[2];
+};
+constexpr int kStatsThreads = 256;
+constexpr int kStatsMaxBlocks = 1024;
+constexpr int kStatsPerThread = 8;
+
+__device__ __forceinline__ void merge_moments(double& n, double& mean, double& m2, double nb, double meanb,
+                                              double m2b) {
+  if (nb == 0.0) return;
+  if (n == 0.0) {
+    n = nb; mean = meanb; m2 = m2b;
+    return;
+  }
+  const double nn = n + nb, delta = meanb - mean;
+  mean += delta * (nb / nn);
+  m2 += m2b + delta * delta * (n * nb / nn);
+  n = nn;
+}
+
+// Welford's update of one group's moments by x
+__device__ __forceinline__ void welford(double& n, double& mean, double& m2, double x) {
+  n += 1.0;
+  const double delta = x - mean;
+  mean += delta / n;
+  m2 = fma(delta, x - mean, m2);
+}
+
+// merges s[0, kStatsThreads) into s[0] in a fixed tree order (every thread of the block calls it)
+template <int kLoss>
+__device__ __forceinline__ void block_merge(SerialMoments* s) {
+  const int t = threadIdx.x;
+  for (int half = kStatsThreads / 2; half > 0; half /= 2) {
+    __syncthreads();
+    if (t < half) {
+      for (int k = 0; k < 2; ++k) {
+        if constexpr (kLoss == kSerialRmse) {
+          s[t].n[k] += s[t + half].n[k];
+          s[t].m2[k] += s[t + half].m2[k];
+        } else {
+          merge_moments(s[t].n[k], s[t].mean[k], s[t].m2[k], s[t + half].n[k], s[t + half].mean[k], s[t + half].m2[k]);
+        }
+      }
+    }
+  }
+  __syncthreads();
+}
+
+template <int kLoss>
+__global__ void __launch_bounds__(kStatsThreads)
+serial_stats_kernel(const float* __restrict__ pred, const float* __restrict__ val, int64_t nnz,
+                    SerialMoments* __restrict__ partial) {
+  __shared__ SerialMoments s[kStatsThreads];
+  SerialMoments m = {};
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * kStatsThreads + threadIdx.x; i < nnz;
+       i += static_cast<int64_t>(gridDim.x) * kStatsThreads) {
+    const float p = pred[i], y = val[i];
+    if constexpr (kLoss == kSerialRmse) {
+      const double e = static_cast<double>(y) - static_cast<double>(p);
+      m.n[0] += 1.0;
+      m.m2[0] = fma(e, e, m.m2[0]);
+    } else if (y > 0.0f) {
+      welford(m.n[0], m.mean[0], m.m2[0], p);
+    } else {
+      welford(m.n[1], m.mean[1], m.m2[1], p);
+    }
+  }
+  s[threadIdx.x] = m;
+  block_merge<kLoss>(s);
+  if (threadIdx.x == 0) partial[blockIdx.x] = s[0];
+}
+
+template <int kLoss>
+__global__ void __launch_bounds__(kStatsThreads)
+serial_finish_kernel(const SerialMoments* __restrict__ partial, int n_partial, float* __restrict__ loss,
+                     SerialLossState* __restrict__ state) {
+  __shared__ SerialMoments s[kStatsThreads];
+  SerialMoments m = {};
+  for (int j = threadIdx.x; j < n_partial; j += kStatsThreads) {
+    for (int k = 0; k < 2; ++k) {
+      if constexpr (kLoss == kSerialRmse) {
+        m.n[k] += partial[j].n[k];
+        m.m2[k] += partial[j].m2[k];
+      } else {
+        merge_moments(m.n[k], m.mean[k], m.m2[k], partial[j].n[k], partial[j].mean[k], partial[j].m2[k]);
+      }
+    }
+  }
+  s[threadIdx.x] = m;
+  block_merge<kLoss>(s);
+  if (threadIdx.x != 0) return;
+  SerialLossState st = {};
+  double l;
+  if constexpr (kLoss == kSerialRmse) {
+    // L = sqrt(sum (y - p)^2 / N), dL / dp_n = (p_n - y_n) / (N L)
+    const double n = s[0].n[0];
+    l = sqrt(s[0].m2[0] / n);
+    st.b[0] = static_cast<float>(1.0 / (n * l));
+  } else {
+    // L = 1 - Phi(-loc / sigma), loc = mu_Q - mu_P, sigma = sqrt(v_Q + v_P), with phi the normal density at -loc / sigma:
+    //   n in P: dL / dp_n = -(phi / (sigma |P|)) (1 + loc (p_n - mu_P) / sigma^2)
+    //   n in Q: dL / dp_n =  (phi / (sigma |Q|)) (1 - loc (p_n - mu_Q) / sigma^2)
+    const double np = s[0].n[0], nq = s[0].n[1];
+    const double mp = np > 0.0 ? s[0].mean[0] : nan(""), mq = nq > 0.0 ? s[0].mean[1] : nan("");
+    const double loc = mq - mp, var = s[0].m2[1] / nq + s[0].m2[0] / np, sigma = sqrt(var);
+    const double z = -loc / sigma;
+    l = 1.0 - 0.5 * (1.0 + erf(z * 0.70710678118654752440));
+    const double phi = exp(-0.5 * z * z) * 0.39894228040143267794;
+    const double ap = -phi / (sigma * np), aq = phi / (sigma * nq);
+    st.a[0] = static_cast<float>(ap);
+    st.b[0] = static_cast<float>(ap * loc / var);
+    st.mu[0] = static_cast<float>(mp);
+    st.a[1] = static_cast<float>(aq);
+    st.b[1] = static_cast<float>(-aq * loc / var);
+    st.mu[1] = static_cast<float>(mq);
+  }
+  *state = st;
+  *loss = static_cast<float>(l);
 }
 
 // Row L2-normalisation of an operand of the step, forward and backward, from its raw rows x (K1's output, d <= 512):
@@ -636,14 +809,15 @@ int sample_items(int64_t n_users, int64_t n_items, int32_t n_sampled, int32_t re
   return TRK_OK;
 }
 
-template <typename T, int kPair = kPairDot, int kCollapse = kCollapseSingle, int NT = 1>
+template <typename T, int kPair = kPairDot, int kCollapse = kCollapseSingle, int NT = 1, int kMode = kModeWmrb>
 static int launch_wmrb(const WmrbParams& p, cudaStream_t stream) {
   const int ch = static_cast<int>(ceil_div(p.d, 128));
-  const size_t smem = static_cast<size_t>(kWmrbWarps) * 2 * p.n_sampled * sizeof(float);
+  // the serial modes keep nothing per sample
+  const size_t smem = kMode == kModeWmrb ? static_cast<size_t>(kWmrbWarps) * 2 * p.n_sampled * sizeof(float) : 0;
   const int grid = capped_grid(ceil_div(p.n_users, kWmrbWarps), 16);
 #define TRK_WMRB_LAUNCH(CH)                                                                                             \
   do {                                                                                                                  \
-    auto* kernel = wmrb_step_kernel<T, CH, kPair, kCollapse, NT>;                                                       \
+    auto* kernel = wmrb_step_kernel<T, CH, kPair, kCollapse, NT, kMode>;                                                \
     if (smem > 48 * 1024)                                                                                               \
       TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem))); \
     kernel<<<grid, kWmrbWarps * 32, smem, stream>>>(p);                                                                 \
@@ -661,24 +835,24 @@ static int launch_wmrb(const WmrbParams& p, cudaStream_t stream) {
 }
 
 // the instantiation of (pair form, n_tastes, attention); the caller has checked the limits
-template <typename T, int kPair>
+template <typename T, int kPair, int kMode = kModeWmrb>
 static int launch_wmrb_form(const WmrbParams& p, int n_tastes, bool attention, cudaStream_t stream) {
-  if (n_tastes == 1) return launch_wmrb<T, kPair, kCollapseSingle, 1>(p, stream);
+  if (n_tastes == 1) return launch_wmrb<T, kPair, kCollapseSingle, 1, kMode>(p, stream);
   if (attention) {
     switch (n_tastes) {
-      case 2: return launch_wmrb<T, kPair, kCollapseAttention, 2>(p, stream);
-      case 3: return launch_wmrb<T, kPair, kCollapseAttention, 3>(p, stream);
-      default: return launch_wmrb<T, kPair, kCollapseAttention, 4>(p, stream);
+      case 2: return launch_wmrb<T, kPair, kCollapseAttention, 2, kMode>(p, stream);
+      case 3: return launch_wmrb<T, kPair, kCollapseAttention, 3, kMode>(p, stream);
+      default: return launch_wmrb<T, kPair, kCollapseAttention, 4, kMode>(p, stream);
     }
   }
   switch (n_tastes) {
-    case 2: return launch_wmrb<T, kPair, kCollapseMax, 2>(p, stream);
-    case 3: return launch_wmrb<T, kPair, kCollapseMax, 3>(p, stream);
-    case 4: return launch_wmrb<T, kPair, kCollapseMax, 4>(p, stream);
-    case 5: return launch_wmrb<T, kPair, kCollapseMax, 5>(p, stream);
-    case 6: return launch_wmrb<T, kPair, kCollapseMax, 6>(p, stream);
-    case 7: return launch_wmrb<T, kPair, kCollapseMax, 7>(p, stream);
-    default: return launch_wmrb<T, kPair, kCollapseMax, 8>(p, stream);
+    case 2: return launch_wmrb<T, kPair, kCollapseMax, 2, kMode>(p, stream);
+    case 3: return launch_wmrb<T, kPair, kCollapseMax, 3, kMode>(p, stream);
+    case 4: return launch_wmrb<T, kPair, kCollapseMax, 4, kMode>(p, stream);
+    case 5: return launch_wmrb<T, kPair, kCollapseMax, 5, kMode>(p, stream);
+    case 6: return launch_wmrb<T, kPair, kCollapseMax, 6, kMode>(p, stream);
+    case 7: return launch_wmrb<T, kPair, kCollapseMax, 7, kMode>(p, stream);
+    default: return launch_wmrb<T, kPair, kCollapseMax, 8, kMode>(p, stream);
   }
 }
 
@@ -782,6 +956,116 @@ int wmrb_step_tastes(const void* user_rows, const void* item_repr, int32_t repr_
                      : launch_wmrb_form<__nv_bfloat16, kPairDot>(p, n_tastes, att, stream);
   return euclidean ? launch_wmrb_form<float, kPairEuclid>(p, n_tastes, att, stream)
                    : launch_wmrb_form<float, kPairDot>(p, n_tastes, att, stream);
+}
+
+// The statistics grid of nnz predictions: fixed by nnz alone, so the workspace size and the finish kernel's partial
+// count both come from here.
+static int serial_stats_grid(int64_t nnz) {
+  return static_cast<int>(std::min<int64_t>(ceil_div(nnz, int64_t{kStatsThreads} * kStatsPerThread), kStatsMaxBlocks));
+}
+static constexpr size_t kSerialStateBytes = 64;     // SerialLossState, then the partials at an 8-byte boundary
+static_assert(sizeof(SerialLossState) <= kSerialStateBytes, "loss state outgrows its slot");
+
+size_t serial_loss_workspace_bytes(int64_t nnz) {
+  return kSerialStateBytes + static_cast<size_t>(serial_stats_grid(std::max<int64_t>(nnz, 0))) * sizeof(SerialMoments);
+}
+
+template <int kLoss>
+static int launch_serial_stats(const float* pred, const float* val, int64_t nnz, void* workspace, float* loss,
+                               cudaStream_t stream) {
+  const int grid = serial_stats_grid(nnz);
+  auto* state = static_cast<SerialLossState*>(workspace);
+  auto* partial = reinterpret_cast<SerialMoments*>(static_cast<char*>(workspace) + kSerialStateBytes);
+  serial_stats_kernel<kLoss><<<grid, kStatsThreads, 0, stream>>>(pred, val, nnz, partial);
+  TRK_CHECK_LAUNCH();
+  serial_finish_kernel<kLoss><<<1, kStatsThreads, 0, stream>>>(partial, grid, loss, state);
+  TRK_CHECK_LAUNCH();
+  return TRK_OK;
+}
+
+template <int kMode>
+static int launch_serial_form(const WmrbParams& p, bool bf16, bool euclidean, int n_tastes, bool attention,
+                              cudaStream_t stream) {
+  if (bf16)
+    return euclidean ? launch_wmrb_form<__nv_bfloat16, kPairEuclid, kMode>(p, n_tastes, attention, stream)
+                     : launch_wmrb_form<__nv_bfloat16, kPairDot, kMode>(p, n_tastes, attention, stream);
+  return euclidean ? launch_wmrb_form<float, kPairEuclid, kMode>(p, n_tastes, attention, stream)
+                   : launch_wmrb_form<float, kPairDot, kMode>(p, n_tastes, attention, stream);
+}
+
+int serial_loss_step(int32_t loss_kind, const void* user_rows, const void* item_repr, int32_t repr_is_bf16,
+                     int32_t n_tastes, int32_t attention, int32_t euclidean, const float* user_bias,
+                     const float* item_bias, const int32_t* inter_indptr, const int32_t* inter_item,
+                     const float* inter_val, int64_t n_users, int64_t n_items, int32_t d, int64_t nnz, float* loss,
+                     float* pred_serial, float* d_user_rows, float* d_user_bias, float* d_item_repr,
+                     float* d_item_bias, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  TRK_CHECK_ARG(loss_kind == kSerialRmse || loss_kind == kSerialSeparation, "serial_loss_step: unknown loss %d",
+                loss_kind);
+  TRK_CHECK_ARG((attention == 0 || attention == 1) && (euclidean == 0 || euclidean == 1),
+                "serial_loss_step: attention and euclidean are flags");
+  TRK_CHECK_ARG(n_users >= 0 && n_items >= 1 && n_items < (1ll << 31) && n_tastes >= 1 && nnz >= 0 &&
+                    nnz < (1ll << 31) && (nnz == 0 || n_users >= 1),
+                "serial_loss_step: bad sizes");
+  TRK_CHECK_ARG(item_repr && d_item_repr && loss && inter_indptr,
+                "serial_loss_step: null item operand, loss or indptr");
+  TRK_CHECK_ARG(n_users == 0 || (user_rows && d_user_rows), "serial_loss_step: null user operand");
+  TRK_CHECK_ARG(nnz == 0 || (inter_item && inter_val && pred_serial && workspace),
+                "serial_loss_step: null interaction, prediction or workspace buffer");
+  TRK_CHECK_ARG(workspace_bytes >= serial_loss_workspace_bytes(nnz) && reinterpret_cast<uintptr_t>(workspace) % 8 == 0,
+                "serial_loss_step: workspace of %zu bytes (8-byte aligned) below the %zu needed", workspace_bytes,
+                serial_loss_workspace_bytes(nnz));
+  TRK_CHECK_ARG((user_bias == nullptr) == (item_bias == nullptr), "serial_loss_step: biases must be given together");
+  TRK_CHECK_ARG((user_bias == nullptr) == (d_user_bias == nullptr) && (item_bias == nullptr) == (d_item_bias == nullptr),
+                "serial_loss_step: bias gradients must match the biases");
+  const int max_d = n_tastes == 1 ? 512 : 128;
+  const int max_tastes = attention ? 4 : 8;
+  if (d < 4 || d % 4 != 0 || d > max_d || n_tastes > max_tastes || (attention && n_tastes == 1)) {
+    set_error("serial_loss_step: n_components=%d (multiple of 4, <= 512 for one taste, <= 128 for several) / "
+              "n_tastes=%d (<= 8, <= 4 with attention, attention needs >= 2) outside the fused kernel", d, n_tastes);
+    return TRK_ERR_UNSUPPORTED;
+  }
+  TRK_CHECK_ARG(reinterpret_cast<uintptr_t>(user_rows) % 16 == 0 && reinterpret_cast<uintptr_t>(item_repr) % 16 == 0 &&
+                    reinterpret_cast<uintptr_t>(d_user_rows) % 16 == 0 && reinterpret_cast<uintptr_t>(d_item_repr) % 16 == 0,
+                "serial_loss_step: rows must be 16-byte aligned");
+  if (nnz == 0) {
+    // no interaction: the mean of nothing is NaN and no prediction reaches a representation (launches nothing)
+    TRK_CHECK_CUDA(cudaMemsetAsync(loss, 0xFF, sizeof(float), stream));        // all ones: a quiet NaN
+    const int64_t n_rows = attention ? 2 * n_tastes : n_tastes;
+    if (n_users > 0) {
+      TRK_CHECK_CUDA(cudaMemsetAsync(d_user_rows, 0, static_cast<size_t>(n_rows * n_users * d) * sizeof(float),
+                                     stream));
+      if (d_user_bias)
+        TRK_CHECK_CUDA(cudaMemsetAsync(d_user_bias, 0, static_cast<size_t>(n_users) * sizeof(float), stream));
+    }
+    return TRK_OK;
+  }
+  WmrbParams p = {};
+  p.user_repr = user_rows;
+  p.item_repr = item_repr;
+  p.user_bias = user_bias;
+  p.item_bias = item_bias;
+  p.inter_indptr = inter_indptr;
+  p.inter_item = inter_item;
+  p.inter_val = inter_val;
+  p.n_users = n_users;
+  p.n_items = static_cast<int32_t>(n_items);
+  p.d = d;
+  p.n_sampled = 0;
+  p.pred_serial = pred_serial;
+  p.d_user_repr = d_user_rows;
+  p.d_user_bias = d_user_bias;
+  p.d_item_repr = d_item_repr;
+  p.d_item_bias = d_item_bias;
+  p.serial_state = workspace;
+  p.serial_loss = loss_kind;
+  const bool bf16 = repr_is_bf16 != 0, euclid = euclidean != 0, att = attention != 0;
+  int rc = launch_serial_form<kModeSerialForward>(p, bf16, euclid, n_tastes, att, stream);
+  if (rc != TRK_OK) return rc;
+  rc = loss_kind == kSerialRmse ? launch_serial_stats<kSerialRmse>(pred_serial, inter_val, nnz, workspace, loss, stream)
+                                : launch_serial_stats<kSerialSeparation>(pred_serial, inter_val, nnz, workspace, loss,
+                                                                        stream);
+  if (rc != TRK_OK) return rc;
+  return launch_serial_form<kModeSerialBackward>(p, bf16, euclid, n_tastes, att, stream);
 }
 
 int l2_normalize_rows_step(const float* x, int64_t rows, int32_t d, int32_t n_normalize, float* out, float* grad,

@@ -19,6 +19,11 @@ any n_components (zero-padded to a multiple of 4 inside the step).  There the us
 attention planes) stacked for trk_wmrb_step_tastes, normalised rows come from trk_l2_normalize_rows_step_f32 forward
 and backward, and every weight gets its own K1^T and Adam pass.
 
+RMSELossGraph and SeparationLossGraph models of those forms (serial_loss_plan; DESIGN §3.11) train on the same
+representations, K1^T and Adam, with trk_serial_loss_step in place of the sampler and trk_wmrb_step[_tastes]: a
+forward launch writes the serial predictions, a statistics launch reduces them to the scalar loss and a loss state on
+the device, and a backward launch turns each prediction into its gradient from that state.
+
 Every other model family trains through the torch-autograd mirror of the reference's graph functions
 (TensorRec._training_losses); TENSORREC_B200_TRAIN_PATH=torch forces that path."""
 import collections
@@ -94,8 +99,10 @@ MAX_TASTES_ATTENTION = 4           # n_tastes with attention
 # The form of the fused step that trains a model: pair 'dot' (dot and cosine) or 'euclidean'; how many times the user,
 # attention and item rows are L2-normalised (NormalizedLinearRepresentationGraph once, cosine once more); d_pad the
 # operand width (n_components rounded up to a multiple of 4).
+# loss: 'wmrb' (WMRB / BalancedWMRB on trk_wmrb_step[_tastes]), or 'rmse' / 'separation' (trk_serial_loss_step).
 StepForm = collections.namedtuple('StepForm', ['pair', 'n_tastes', 'attention', 'normalize_user', 'normalize_attn',
-                                               'normalize_item', 'd_pad'])
+                                               'normalize_item', 'd_pad', 'loss'], defaults=('wmrb',))
+SERIAL_LOSS_KIND = {'rmse': 0, 'separation': 1}          # trk_serial_loss_step's loss_kind
 
 
 def step_plan(model, n_sampled_items=None):
@@ -104,11 +111,28 @@ def step_plan(model, n_sampled_items=None):
     (or no attention); n_components <= 512 for one taste, <= 128 with n_tastes <= 8 (<= 4 with attention);
     n_sampled_items <= 2048."""
     from .loss_graphs import WMRBLossGraph, BalancedWMRBLossGraph
+    if TRAIN_PATH == 'torch' or type(model.loss_graph_factory) not in (WMRBLossGraph, BalancedWMRBLossGraph):
+        return None
+    if n_sampled_items is not None and n_sampled_items > MAX_SAMPLED:
+        return None
+    return _form(model, 'wmrb')
+
+
+def serial_loss_plan(model):
+    """The StepForm (loss 'rmse' or 'separation') of the serial-loss training step for this model, or None: an
+    RMSELossGraph / SeparationLossGraph with the prediction, representation and taste forms step_plan() accepts.
+    Nothing is sampled, so there is no n_sampled_items limit."""
+    from .loss_graphs import RMSELossGraph, SeparationLossGraph
+    loss = {RMSELossGraph: 'rmse', SeparationLossGraph: 'separation'}.get(type(model.loss_graph_factory))
+    if TRAIN_PATH == 'torch' or loss is None:
+        return None
+    return _form(model, loss)
+
+
+def _form(model, loss):
     from .prediction_graphs import (CosineSimilarityPredictionGraph, DotProductPredictionGraph,
                                     EuclideanSimilarityPredictionGraph)
     from .representation_graphs import LinearRepresentationGraph, NormalizedLinearRepresentationGraph
-    if TRAIN_PATH == 'torch' or type(model.loss_graph_factory) not in (WMRBLossGraph, BalancedWMRBLossGraph):
-        return None
     pred = type(model.prediction_graph_factory)
     if pred not in (DotProductPredictionGraph, CosineSimilarityPredictionGraph, EuclideanSimilarityPredictionGraph):
         return None
@@ -119,8 +143,6 @@ def step_plan(model, n_sampled_items=None):
     if attention and type(model.attention_graph_factory) not in linear:
         return None
     d, nt = int(model.n_components), int(model.n_tastes)
-    if n_sampled_items is not None and n_sampled_items > MAX_SAMPLED:
-        return None
     if nt == 1:
         if attention or not 1 <= d <= MAX_D_ONE_TASTE:
             return None
@@ -134,7 +156,7 @@ def step_plan(model, n_sampled_items=None):
     return StepForm(pair='euclidean' if pred is EuclideanSimilarityPredictionGraph else 'dot', n_tastes=nt,
                     attention=attention, normalize_user=n_norm(model.user_repr_graph_factory),
                     normalize_attn=n_norm(model.attention_graph_factory) if attention else 0,
-                    normalize_item=n_norm(model.item_repr_graph_factory), d_pad=(d + 3) // 4 * 4)
+                    normalize_item=n_norm(model.item_repr_graph_factory), d_pad=(d + 3) // 4 * 4, loss=loss)
 
 
 def _plain(form):
@@ -222,18 +244,27 @@ class WmrbStep(object):
     def step(self, interactions_in, user_in, item_in, n_sampled_items, learning_rate, l2, samples=None):
         """One Adam step on sum(WMRB loss) + l2 * sum_w 0.5 |w|^2.  `l2` is the coefficient of the L2 term in the
         SUMMED loss (the reference adds alpha * reg to every element of its loss vector, tensorrec.py:488, so it is
-        n_positive_interactions * batched_alpha).  Returns the device tensors of the step (loss, pred_serial)."""
+        n_positive_interactions * batched_alpha).  Returns the device tensors of the step (loss, pred_serial).
+
+        For an RMSE / Separation model (serial_loss_plan) the loss is a scalar: `l2` is batched_alpha itself, the
+        returned loss is a 1-element tensor, and n_sampled_items and samples are not used."""
         lib = kernels.require_cuda()
         from .loss_graphs import BalancedWMRBLossGraph
-        form = step_plan(self.model)
+        form = step_plan(self.model) or serial_loss_plan(self.model)
         if form is None:
-            raise ValueError('the fused training step does not cover this model (train_kernels.step_plan)')
+            raise ValueError('the fused training step does not cover this model (train_kernels.step_plan, '
+                             'serial_loss_plan)')
+        serial = form.loss != 'wmrb'
+        if serial:
+            samples = None
         dev, d, dp = self.device, self.model.n_components, form.d_pad
         n_users, n_items = user_in.shape[0], item_in.shape[0]
         check_step_inputs(interactions_in.shape, n_users, n_items, n_sampled_items, samples)
         ucsr, icsr = user_in.device_csr(dev), item_in.device_csr(dev)
         ucsr_t, icsr_t = user_in.device_csr_t(dev), item_in.device_csr_t(dev)
         inter = interactions_in.device_csr(dev)
+        if serial and inter.nnz >= 2 ** 31:
+            raise ValueError('{} interactions exceed the step\'s int32 indexing'.format(inter.nnz))
         names, ws = self._weights(user_in.shape[1], item_in.shape[1])
         # the user operand: taste planes, then attention planes, [n_rows, n_users, d_pad]
         user_ops = [('linear_weights_user_{}'.format(t), form.normalize_user) for t in range(form.n_tastes)]
@@ -271,36 +302,41 @@ class WmrbStep(object):
             _lib.check(lib.trk_f32_to_bf16(_p(item_repr), item_repr.numel(), _p(repr_i), _stream()), 'trk_f32_to_bf16')
 
         self._mark('representations')
-        if samples is None:
-            samples = sample_items_device(n_items, n_users, n_sampled_items,
-                                          self.model.loss_graph_factory.is_sampled_with_replacement, self.seed, self.t, dev)
-        weight_sum = None
-        if type(self.model.loss_graph_factory) is BalancedWMRBLossGraph:
-            weight_sum = interactions_in.positive_item_sums(dev)
-
-        self._mark('sampler')
-        nnz = inter.nnz
-        loss = torch.empty((nnz,), dtype=torch.float32, device=dev)
-        pred = torch.empty((nnz,), dtype=torch.float32, device=dev)
-        coef = torch.empty((nnz,), dtype=torch.float32, device=dev)
-        d_user_repr = torch.empty(user_repr.shape, dtype=torch.float32, device=dev)
-        d_item_repr = torch.zeros((n_items, dp), dtype=torch.float32, device=dev)
-        d_ub = torch.empty((n_users,), dtype=torch.float32, device=dev) if self.model.biased else None
-        d_ib = torch.zeros((n_items,), dtype=torch.float32, device=dev) if self.model.biased else None
-        if _plain(form):
-            rc = lib.trk_wmrb_step(_p(repr_u), _p(repr_i), 1 if self.bf16 else 0, _p(ub), _p(ib), _p(inter.indptr),
-                                   _p(inter.col), _p(inter.val), _p(weight_sum), _p(samples), n_users, n_items, dp,
-                                   int(samples.shape[1]), _p(loss), _p(pred), _p(coef), _p(d_user_repr), _p(d_ub),
-                                   _p(d_item_repr), _p(d_ib), _stream())
-            _lib.check(rc, 'trk_wmrb_step')
+        if serial:
+            loss, pred, d_user_repr, d_ub, d_item_repr, d_ib = self._serial_loss(lib, form, repr_u, repr_i, ub, ib,
+                                                                                 inter, user_repr.shape)
         else:
-            rc = lib.trk_wmrb_step_tastes(_p(repr_u), _p(repr_i), 1 if self.bf16 else 0, form.n_tastes,
-                                          1 if form.attention else 0, 1 if form.pair == 'euclidean' else 0, _p(ub),
-                                          _p(ib), _p(inter.indptr), _p(inter.col), _p(inter.val), _p(weight_sum),
-                                          _p(samples), n_users, n_items, dp, int(samples.shape[1]), _p(loss), _p(pred),
-                                          _p(coef), _p(d_user_repr), _p(d_ub), _p(d_item_repr), _p(d_ib), _stream())
-            _lib.check(rc, 'trk_wmrb_step_tastes')
-        self._mark('wmrb_step')
+            if samples is None:
+                samples = sample_items_device(n_items, n_users, n_sampled_items,
+                                              self.model.loss_graph_factory.is_sampled_with_replacement, self.seed,
+                                              self.t, dev)
+            weight_sum = None
+            if type(self.model.loss_graph_factory) is BalancedWMRBLossGraph:
+                weight_sum = interactions_in.positive_item_sums(dev)
+
+            self._mark('sampler')
+            nnz = inter.nnz
+            loss = torch.empty((nnz,), dtype=torch.float32, device=dev)
+            pred = torch.empty((nnz,), dtype=torch.float32, device=dev)
+            coef = torch.empty((nnz,), dtype=torch.float32, device=dev)
+            d_user_repr = torch.empty(user_repr.shape, dtype=torch.float32, device=dev)
+            d_item_repr = torch.zeros((n_items, dp), dtype=torch.float32, device=dev)
+            d_ub = torch.empty((n_users,), dtype=torch.float32, device=dev) if self.model.biased else None
+            d_ib = torch.zeros((n_items,), dtype=torch.float32, device=dev) if self.model.biased else None
+            if _plain(form):
+                rc = lib.trk_wmrb_step(_p(repr_u), _p(repr_i), 1 if self.bf16 else 0, _p(ub), _p(ib), _p(inter.indptr),
+                                       _p(inter.col), _p(inter.val), _p(weight_sum), _p(samples), n_users, n_items, dp,
+                                       int(samples.shape[1]), _p(loss), _p(pred), _p(coef), _p(d_user_repr), _p(d_ub),
+                                       _p(d_item_repr), _p(d_ib), _stream())
+                _lib.check(rc, 'trk_wmrb_step')
+            else:
+                rc = lib.trk_wmrb_step_tastes(_p(repr_u), _p(repr_i), 1 if self.bf16 else 0, form.n_tastes,
+                                              1 if form.attention else 0, 1 if form.pair == 'euclidean' else 0, _p(ub),
+                                              _p(ib), _p(inter.indptr), _p(inter.col), _p(inter.val), _p(weight_sum),
+                                              _p(samples), n_users, n_items, dp, int(samples.shape[1]), _p(loss), _p(pred),
+                                              _p(coef), _p(d_user_repr), _p(d_ub), _p(d_item_repr), _p(d_ib), _stream())
+                _lib.check(rc, 'trk_wmrb_step_tastes')
+            self._mark('wmrb_step')
 
         # backward through the normalisations, then through the sparse x dense products: K1 on the transposed CSR
         def weight_grad(csr_t, raw, n_norm, d_rows):
@@ -335,6 +371,27 @@ class WmrbStep(object):
             _lib.check(rc, 'trk_adam_step_f32')
         self._mark('adam')
         return loss, pred
+
+    def _serial_loss(self, lib, form, repr_u, repr_i, ub, ib, inter, user_shape):
+        """trk_serial_loss_step: the scalar loss [1], pred_serial and the operand gradients of an RMSE / Separation
+        step.  An interaction-free batch launches no kernel (loss NaN, zero gradients), as the mean of nothing gives."""
+        dev, dp, n_users, n_items, nnz = self.device, form.d_pad, user_shape[1], repr_i.shape[0], inter.nnz
+        loss = torch.empty((1,), dtype=torch.float32, device=dev)
+        pred = torch.empty((nnz,), dtype=torch.float32, device=dev)
+        d_user_repr = torch.empty(user_shape, dtype=torch.float32, device=dev)
+        d_item_repr = torch.zeros((n_items, dp), dtype=torch.float32, device=dev)
+        d_ub = torch.empty((n_users,), dtype=torch.float32, device=dev) if self.model.biased else None
+        d_ib = torch.zeros((n_items,), dtype=torch.float32, device=dev) if self.model.biased else None
+        ws_bytes = int(lib.trk_serial_loss_workspace_bytes(nnz))
+        workspace = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+        rc = lib.trk_serial_loss_step(SERIAL_LOSS_KIND[form.loss], _p(repr_u), _p(repr_i), 1 if self.bf16 else 0,
+                                      form.n_tastes, 1 if form.attention else 0, 1 if form.pair == 'euclidean' else 0,
+                                      _p(ub), _p(ib), _p(inter.indptr), _p(inter.col), _p(inter.val), n_users, n_items,
+                                      dp, nnz, _p(loss), _p(pred), _p(d_user_repr), _p(d_ub), _p(d_item_repr), _p(d_ib),
+                                      _p(workspace), ws_bytes, _stream())
+        _lib.check(rc, 'trk_serial_loss_step')
+        self._mark('serial_loss_step')
+        return loss, pred, d_user_repr, d_ub, d_item_repr, d_ib
 
 
 def positive_item_sums(matrix, n_items):
