@@ -519,8 +519,10 @@ int trk_topk_merge_dedup_pair(const float* a_score, const int32_t* a_item, int64
  *                      first; the order of the floating-point additions is not fixed, as in tf.gather's GPU gradient).
  *                    Representations are fp32 or bf16 (repr_is_bf16; BASELINE config #4 allows bf16), arithmetic and
  *                    gradients fp32.  coef [nnz] is scratch.  Constraints: d % 4 == 0, d <= 512, n_sampled <= 2048.
+ *                    It is the one-taste dot shorthand of trk_wmrb_step_tastes (n_tastes = 1, attention = 0,
+ *                    euclidean = 0), and checks its arguments as that does.
  * trk_wmrb_step_tastes
- *                    the same step for every other form the fused path trains (DESIGN §3.10): n_tastes taste rows per user,
+ *                    the general WMRB step, every form the fused path trains (DESIGN §3.10): n_tastes taste rows per user,
  *                    with n_tastes attention rows after them when attention = 1, stacked as planes [n_rows, n_users, d]
  *                    in user_rows (and d_user_rows, written); euclidean = 1 scores a pair -sqrt(max(|u - i|^2, 1e-16)),
  *                    0 scores it u . i (cosine: the caller passes L2-normalised rows).  The prediction collapses the

@@ -139,12 +139,9 @@ int select_wide_topk(const void*, const float*, const void*, const float*, const
                      int64_t, int32_t, int32_t, int32_t, int32_t, float*, int32_t*, int64_t, int32_t*, cudaStream_t);
 
 int sample_items(int64_t, int64_t, int32_t, int32_t, uint64_t, uint32_t, int32_t*, cudaStream_t);
-int wmrb_step(const void*, const void*, int32_t, const float*, const float*, const int32_t*, const int32_t*, const float*,
-              const float*, const int32_t*, int64_t, int64_t, int32_t, int32_t, float*, float*, float*, float*, float*,
-              float*, float*, cudaStream_t);
-int wmrb_step_tastes(const void*, const void*, int32_t, int32_t, int32_t, int32_t, const float*, const float*,
-                     const int32_t*, const int32_t*, const float*, const float*, const int32_t*, int64_t, int64_t, int32_t,
-                     int32_t, float*, float*, float*, float*, float*, float*, float*, cudaStream_t);
+int wmrb_step_tastes(const char*, const void*, const void*, int32_t, int32_t, int32_t, int32_t, const float*,
+                     const float*, const int32_t*, const int32_t*, const float*, const float*, const int32_t*, int64_t,
+                     int64_t, int32_t, int32_t, float*, float*, float*, float*, float*, float*, float*, cudaStream_t);
 size_t serial_loss_workspace_bytes(int64_t);
 int serial_loss_step(int32_t, const void*, const void*, int32_t, int32_t, int32_t, int32_t, const float*, const float*,
                      const int32_t*, const int32_t*, const float*, int64_t, int64_t, int32_t, int64_t, float*, float*,
@@ -583,9 +580,11 @@ int trk_wmrb_step(const void* user_repr, const void* item_repr, int32_t repr_is_
                   const float* inter_val, const float* item_weight_sum, const int32_t* samples, int64_t n_users,
                   int64_t n_items, int32_t d, int32_t n_sampled, float* loss, float* pred_serial, float* coef,
                   float* d_user_repr, float* d_user_bias, float* d_item_repr, float* d_item_bias, void* stream) {
-  return trk::wmrb_step(user_repr, item_repr, repr_is_bf16, user_bias, item_bias, inter_indptr, inter_item, inter_val,
-                        item_weight_sum, samples, n_users, n_items, d, n_sampled, loss, pred_serial, coef, d_user_repr,
-                        d_user_bias, d_item_repr, d_item_bias, trk::as_stream(stream));
+  // the one-taste dot form of trk_wmrb_step_tastes
+  return trk::wmrb_step_tastes("wmrb_step", user_repr, item_repr, repr_is_bf16, 1, 0, 0, user_bias, item_bias,
+                               inter_indptr, inter_item, inter_val, item_weight_sum, samples, n_users, n_items, d,
+                               n_sampled, loss, pred_serial, coef, d_user_repr, d_user_bias, d_item_repr, d_item_bias,
+                               trk::as_stream(stream));
 }
 
 int trk_wmrb_step_tastes(const void* user_rows, const void* item_repr, int32_t repr_is_bf16, int32_t n_tastes,
@@ -594,10 +593,10 @@ int trk_wmrb_step_tastes(const void* user_rows, const void* item_repr, int32_t r
                          const float* item_weight_sum, const int32_t* samples, int64_t n_users, int64_t n_items,
                          int32_t d, int32_t n_sampled, float* loss, float* pred_serial, float* coef, float* d_user_rows,
                          float* d_user_bias, float* d_item_repr, float* d_item_bias, void* stream) {
-  return trk::wmrb_step_tastes(user_rows, item_repr, repr_is_bf16, n_tastes, attention, euclidean, user_bias, item_bias,
-                               inter_indptr, inter_item, inter_val, item_weight_sum, samples, n_users, n_items, d,
-                               n_sampled, loss, pred_serial, coef, d_user_rows, d_user_bias, d_item_repr, d_item_bias,
-                               trk::as_stream(stream));
+  return trk::wmrb_step_tastes("wmrb_step_tastes", user_rows, item_repr, repr_is_bf16, n_tastes, attention, euclidean,
+                               user_bias, item_bias, inter_indptr, inter_item, inter_val, item_weight_sum, samples,
+                               n_users, n_items, d, n_sampled, loss, pred_serial, coef, d_user_rows, d_user_bias,
+                               d_item_repr, d_item_bias, trk::as_stream(stream));
 }
 
 size_t trk_serial_loss_workspace_bytes(int64_t nnz) { return trk::serial_loss_workspace_bytes(nnz); }

@@ -197,6 +197,40 @@ __device__ __forceinline__ float pair_score(float f) {
   else return f;
 }
 
+// the max collapse: max_t score_t
+template <int kPair, int NT, int NF>
+__device__ __forceinline__ float max_score(const float (&f)[NF]) {
+  float m = pair_score<kPair>(f[0]);
+#pragma unroll
+  for (int t = 1; t < NT; ++t) m = fmaxf(m, pair_score<kPair>(f[t]));
+  return m;
+}
+
+// the attention collapse: the scores s_t, the softmax weights w_t of the attention scores a_t (a sample's are its own
+// scores) and the prediction sum_t w_t s_t
+template <int kPair, int NT, bool kSample, int NF>
+__device__ __forceinline__ float softmax_collapse(const float (&f)[NF], float (&s)[NT], float (&w)[NT]) {
+  float a[NT];
+#pragma unroll
+  for (int t = 0; t < NT; ++t) {
+    s[t] = pair_score<kPair>(f[t]);
+    a[t] = kSample ? s[t] : pair_score<kPair>(f[NT + t]);
+  }
+  float m = a[0];
+#pragma unroll
+  for (int t = 1; t < NT; ++t) m = fmaxf(m, a[t]);
+  float z = 0.0f;
+#pragma unroll
+  for (int t = 0; t < NT; ++t) z += expf(a[t] - m);
+  float pred = 0.0f;
+#pragma unroll
+  for (int t = 0; t < NT; ++t) {
+    w[t] = expf(a[t] - m) / z;
+    pred += w[t] * s[t];
+  }
+  return pred;
+}
+
 // the prediction (without biases) of one pair from its row forms f[0, NT) (tastes) and f[NT, 2 NT) (attention rows of
 // an interaction; a sample has none)
 template <int kPair, int kCollapse, int NT, bool kSample, int NF>
@@ -204,27 +238,10 @@ __device__ __forceinline__ float collapse_tastes(const float (&f)[NF]) {
   if constexpr (kCollapse == kCollapseSingle) {
     return pair_score<kPair>(f[0]);
   } else if constexpr (kCollapse == kCollapseMax) {
-    float m = pair_score<kPair>(f[0]);
-#pragma unroll
-    for (int t = 1; t < NT; ++t) m = fmaxf(m, pair_score<kPair>(f[t]));
-    return m;
+    return max_score<kPair, NT>(f);
   } else {
-    float s[NT], a[NT];
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-      s[t] = pair_score<kPair>(f[t]);
-      a[t] = kSample ? s[t] : pair_score<kPair>(f[NT + t]);
-    }
-    float m = a[0];
-#pragma unroll
-    for (int t = 1; t < NT; ++t) m = fmaxf(m, a[t]);
-    float z = 0.0f;
-#pragma unroll
-    for (int t = 0; t < NT; ++t) z += expf(a[t] - m);
-    float out = 0.0f;
-#pragma unroll
-    for (int t = 0; t < NT; ++t) out += (expf(a[t] - m) / z) * s[t];
-    return out;
+    float s[NT], w[NT];
+    return softmax_collapse<kPair, NT, kSample>(f, s, w);
   }
 }
 
@@ -239,9 +256,7 @@ __device__ __forceinline__ void taste_coefs(const float (&f)[NF], float g, float
   if constexpr (kCollapse == kCollapseSingle) {
     ds[0] = g;
   } else if constexpr (kCollapse == kCollapseMax) {
-    float m = pair_score<kPair>(f[0]);
-#pragma unroll
-    for (int t = 1; t < NT; ++t) m = fmaxf(m, pair_score<kPair>(f[t]));
+    const float m = max_score<kPair, NT>(f);
     float n_max = 0.0f;
 #pragma unroll
     for (int t = 0; t < NT; ++t) n_max += pair_score<kPair>(f[t]) == m ? 1.0f : 0.0f;
@@ -249,24 +264,8 @@ __device__ __forceinline__ void taste_coefs(const float (&f)[NF], float g, float
 #pragma unroll
     for (int t = 0; t < NT; ++t) ds[t] = pair_score<kPair>(f[t]) == m ? share : 0.0f;
   } else {
-    float s[NT], a[NT], w[NT];
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-      s[t] = pair_score<kPair>(f[t]);
-      a[t] = kSample ? s[t] : pair_score<kPair>(f[NT + t]);
-    }
-    float m = a[0];
-#pragma unroll
-    for (int t = 1; t < NT; ++t) m = fmaxf(m, a[t]);
-    float z = 0.0f;
-#pragma unroll
-    for (int t = 0; t < NT; ++t) z += expf(a[t] - m);
-    float pred = 0.0f;
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-      w[t] = expf(a[t] - m) / z;
-      pred += w[t] * s[t];
-    }
+    float s[NT], w[NT];
+    const float pred = softmax_collapse<kPair, NT, kSample>(f, s, w);
 #pragma unroll
     for (int t = 0; t < NT; ++t) {
       const float da = g * w[t] * (s[t] - pred);    // d pred / d a_t = w_t (s_t - pred)
@@ -601,22 +600,26 @@ __device__ __forceinline__ void welford(double& n, double& mean, double& m2, dou
   m2 = fma(delta, x - mean, m2);
 }
 
+// merges b into m: RMSE adds the counts and the sums, Separation merges each group's moments
+template <int kLoss>
+__device__ __forceinline__ void merge(SerialMoments& m, const SerialMoments& b) {
+  for (int k = 0; k < 2; ++k) {
+    if constexpr (kLoss == kSerialRmse) {
+      m.n[k] += b.n[k];
+      m.m2[k] += b.m2[k];
+    } else {
+      merge_moments(m.n[k], m.mean[k], m.m2[k], b.n[k], b.mean[k], b.m2[k]);
+    }
+  }
+}
+
 // merges s[0, kStatsThreads) into s[0] in a fixed tree order (every thread of the block calls it)
 template <int kLoss>
 __device__ __forceinline__ void block_merge(SerialMoments* s) {
   const int t = threadIdx.x;
   for (int half = kStatsThreads / 2; half > 0; half /= 2) {
     __syncthreads();
-    if (t < half) {
-      for (int k = 0; k < 2; ++k) {
-        if constexpr (kLoss == kSerialRmse) {
-          s[t].n[k] += s[t + half].n[k];
-          s[t].m2[k] += s[t + half].m2[k];
-        } else {
-          merge_moments(s[t].n[k], s[t].mean[k], s[t].m2[k], s[t + half].n[k], s[t + half].mean[k], s[t + half].m2[k]);
-        }
-      }
-    }
+    if (t < half) merge<kLoss>(s[t], s[t + half]);
   }
   __syncthreads();
 }
@@ -651,16 +654,7 @@ serial_finish_kernel(const SerialMoments* __restrict__ partial, int n_partial, f
                      SerialLossState* __restrict__ state) {
   __shared__ SerialMoments s[kStatsThreads];
   SerialMoments m = {};
-  for (int j = threadIdx.x; j < n_partial; j += kStatsThreads) {
-    for (int k = 0; k < 2; ++k) {
-      if constexpr (kLoss == kSerialRmse) {
-        m.n[k] += partial[j].n[k];
-        m.m2[k] += partial[j].m2[k];
-      } else {
-        merge_moments(m.n[k], m.mean[k], m.m2[k], partial[j].n[k], partial[j].mean[k], partial[j].m2[k]);
-      }
-    }
-  }
+  for (int j = threadIdx.x; j < n_partial; j += kStatsThreads) merge<kLoss>(m, partial[j]);
   s[threadIdx.x] = m;
   block_merge<kLoss>(s);
   if (threadIdx.x != 0) return;
@@ -809,7 +803,7 @@ int sample_items(int64_t n_users, int64_t n_items, int32_t n_sampled, int32_t re
   return TRK_OK;
 }
 
-template <typename T, int kPair = kPairDot, int kCollapse = kCollapseSingle, int NT = 1, int kMode = kModeWmrb>
+template <typename T, int kPair, int kCollapse, int NT, int kMode>
 static int launch_wmrb(const WmrbParams& p, cudaStream_t stream) {
   const int ch = static_cast<int>(ceil_div(p.d, 128));
   // the serial modes keep nothing per sample
@@ -835,7 +829,7 @@ static int launch_wmrb(const WmrbParams& p, cudaStream_t stream) {
 }
 
 // the instantiation of (pair form, n_tastes, attention); the caller has checked the limits
-template <typename T, int kPair, int kMode = kModeWmrb>
+template <typename T, int kPair, int kMode>
 static int launch_wmrb_form(const WmrbParams& p, int n_tastes, bool attention, cudaStream_t stream) {
   if (n_tastes == 1) return launch_wmrb<T, kPair, kCollapseSingle, 1, kMode>(p, stream);
   if (attention) {
@@ -856,79 +850,50 @@ static int launch_wmrb_form(const WmrbParams& p, int n_tastes, bool attention, c
   }
 }
 
-int wmrb_step(const void* user_repr, const void* item_repr, int32_t repr_is_bf16, const float* user_bias,
-              const float* item_bias, const int32_t* inter_indptr, const int32_t* inter_item, const float* inter_val,
-              const float* item_weight_sum, const int32_t* samples, int64_t n_users, int64_t n_items, int32_t d,
-              int32_t n_sampled, float* loss, float* pred_serial, float* coef, float* d_user_repr, float* d_user_bias,
-              float* d_item_repr, float* d_item_bias, cudaStream_t stream) {
-  TRK_CHECK_ARG(user_repr && item_repr && inter_indptr && samples, "wmrb_step: null input");
-  TRK_CHECK_ARG(loss && pred_serial && coef && d_user_repr && d_item_repr, "wmrb_step: null output");
-  TRK_CHECK_ARG((user_bias == nullptr) == (item_bias == nullptr), "wmrb_step: biases must be given together");
-  TRK_CHECK_ARG((user_bias == nullptr) == (d_user_bias == nullptr) && (item_bias == nullptr) == (d_item_bias == nullptr),
-                "wmrb_step: bias gradients must match the biases");
-  TRK_CHECK_ARG(n_users >= 0 && n_items >= 1 && n_items < (1ll << 31) && n_sampled >= 1, "wmrb_step: bad sizes");
-  if (d < 4 || d % 4 != 0 || d > 512 || n_sampled > 2048) {
-    set_error("wmrb_step: n_components=%d (multiple of 4, <= 512) / n_sampled=%d (<= 2048) outside the fused kernel", d,
-              n_sampled);
-    return TRK_ERR_UNSUPPORTED;
-  }
-  TRK_CHECK_ARG(reinterpret_cast<uintptr_t>(user_repr) % 16 == 0 && reinterpret_cast<uintptr_t>(item_repr) % 16 == 0 &&
-                    reinterpret_cast<uintptr_t>(d_user_repr) % 16 == 0 && reinterpret_cast<uintptr_t>(d_item_repr) % 16 == 0,
-                "wmrb_step: rows must be 16-byte aligned");
-  if (n_users == 0) return TRK_OK;
-  WmrbParams p;
-  p.user_repr = user_repr;
-  p.item_repr = item_repr;
-  p.user_bias = user_bias;
-  p.item_bias = item_bias;
-  p.inter_indptr = inter_indptr;
-  p.inter_item = inter_item;
-  p.inter_val = inter_val;
-  p.item_weight_sum = item_weight_sum;
-  p.samples = samples;
-  p.n_users = n_users;
-  p.n_items = static_cast<int32_t>(n_items);
-  p.d = d;
-  p.n_sampled = n_sampled;
-  p.rank_scale = static_cast<float>(n_items) / static_cast<float>(n_sampled);
-  p.loss = loss;
-  p.pred_serial = pred_serial;
-  p.coef = coef;
-  p.d_user_repr = d_user_repr;
-  p.d_user_bias = d_user_bias;
-  p.d_item_repr = d_item_repr;
-  p.d_item_bias = d_item_bias;
-  return repr_is_bf16 ? launch_wmrb<__nv_bfloat16>(p, stream) : launch_wmrb<float>(p, stream);
+// one launch of the step in mode kMode for the storage type and the form
+template <int kMode>
+static int launch_step(const WmrbParams& p, bool bf16, bool euclidean, int n_tastes, bool attention,
+                       cudaStream_t stream) {
+  if (bf16)
+    return euclidean ? launch_wmrb_form<__nv_bfloat16, kPairEuclid, kMode>(p, n_tastes, attention, stream)
+                     : launch_wmrb_form<__nv_bfloat16, kPairDot, kMode>(p, n_tastes, attention, stream);
+  return euclidean ? launch_wmrb_form<float, kPairEuclid, kMode>(p, n_tastes, attention, stream)
+                   : launch_wmrb_form<float, kPairDot, kMode>(p, n_tastes, attention, stream);
 }
 
-int wmrb_step_tastes(const void* user_rows, const void* item_repr, int32_t repr_is_bf16, int32_t n_tastes,
-                     int32_t attention, int32_t euclidean, const float* user_bias, const float* item_bias,
-                     const int32_t* inter_indptr, const int32_t* inter_item, const float* inter_val,
-                     const float* item_weight_sum, const int32_t* samples, int64_t n_users, int64_t n_items, int32_t d,
-                     int32_t n_sampled, float* loss, float* pred_serial, float* coef, float* d_user_rows,
-                     float* d_user_bias, float* d_item_repr, float* d_item_bias, cudaStream_t stream) {
-  TRK_CHECK_ARG(user_rows && item_repr && inter_indptr && samples, "wmrb_step_tastes: null input");
-  TRK_CHECK_ARG(loss && pred_serial && coef && d_user_rows && d_item_repr, "wmrb_step_tastes: null output");
-  TRK_CHECK_ARG((user_bias == nullptr) == (item_bias == nullptr), "wmrb_step_tastes: biases must be given together");
+// The checks of the operands and the form that the WMRB and the serial step share, after each entry point has checked
+// its own buffers and sizes; `who` (the entry point) prefixes every message.  n_sampled is 0 for the serial step,
+// which samples nothing.  The form limits return TRK_ERR_UNSUPPORTED, everything else TRK_ERR_ARG.
+static int check_step(const char* who, const void* user_rows, const void* item_repr, int32_t n_tastes,
+                      int32_t attention, int32_t euclidean, const float* user_bias, const float* item_bias,
+                      int64_t n_users, int64_t n_items, int32_t d, int32_t n_sampled, const float* d_user_rows,
+                      const float* d_user_bias, const float* d_item_repr, const float* d_item_bias) {
+  TRK_CHECK_ARG((user_bias == nullptr) == (item_bias == nullptr), "%s: biases must be given together", who);
   TRK_CHECK_ARG((user_bias == nullptr) == (d_user_bias == nullptr) && (item_bias == nullptr) == (d_item_bias == nullptr),
-                "wmrb_step_tastes: bias gradients must match the biases");
-  TRK_CHECK_ARG(n_users >= 0 && n_items >= 1 && n_items < (1ll << 31) && n_sampled >= 1 && n_tastes >= 1,
-                "wmrb_step_tastes: bad sizes");
+                "%s: bias gradients must match the biases", who);
   TRK_CHECK_ARG((attention == 0 || attention == 1) && (euclidean == 0 || euclidean == 1),
-                "wmrb_step_tastes: attention and euclidean are flags");
+                "%s: attention and euclidean are flags", who);
+  TRK_CHECK_ARG(n_users >= 0 && n_items >= 1 && n_items < (1ll << 31) && n_tastes >= 1, "%s: bad sizes", who);
   const int max_d = n_tastes == 1 ? 512 : 128;
   const int max_tastes = attention ? 4 : 8;
   if (d < 4 || d % 4 != 0 || d > max_d || n_sampled > 2048 || n_tastes > max_tastes || (attention && n_tastes == 1)) {
-    set_error("wmrb_step_tastes: n_components=%d (multiple of 4, <= 512 for one taste, <= 128 for several) / "
-              "n_tastes=%d (<= 8, <= 4 with attention, attention needs >= 2) / n_sampled=%d (<= 2048) outside the fused "
-              "kernel", d, n_tastes, n_sampled);
+    set_error("%s: n_components=%d (multiple of 4, <= 512 for one taste, <= 128 for several) / n_tastes=%d (<= 8, <= 4 "
+              "with attention, attention needs >= 2) / n_sampled=%d (<= 2048) outside the fused kernel", who, d,
+              n_tastes, n_sampled);
     return TRK_ERR_UNSUPPORTED;
   }
   TRK_CHECK_ARG(reinterpret_cast<uintptr_t>(user_rows) % 16 == 0 && reinterpret_cast<uintptr_t>(item_repr) % 16 == 0 &&
                     reinterpret_cast<uintptr_t>(d_user_rows) % 16 == 0 && reinterpret_cast<uintptr_t>(d_item_repr) % 16 == 0,
-                "wmrb_step_tastes: rows must be 16-byte aligned");
-  if (n_users == 0) return TRK_OK;
-  WmrbParams p;
+                "%s: rows must be 16-byte aligned", who);
+  return TRK_OK;
+}
+
+// the WmrbParams fields of every mode; the WMRB step adds its samples and loss outputs, the serial step its loss state
+static WmrbParams step_params(const void* user_rows, const void* item_repr, const float* user_bias,
+                              const float* item_bias, const int32_t* inter_indptr, const int32_t* inter_item,
+                              const float* inter_val, int64_t n_users, int64_t n_items, int32_t d, float* pred_serial,
+                              float* d_user_rows, float* d_user_bias, float* d_item_repr, float* d_item_bias) {
+  WmrbParams p = {};
   p.user_repr = user_rows;
   p.item_repr = item_repr;
   p.user_bias = user_bias;
@@ -936,26 +901,41 @@ int wmrb_step_tastes(const void* user_rows, const void* item_repr, int32_t repr_
   p.inter_indptr = inter_indptr;
   p.inter_item = inter_item;
   p.inter_val = inter_val;
-  p.item_weight_sum = item_weight_sum;
-  p.samples = samples;
   p.n_users = n_users;
   p.n_items = static_cast<int32_t>(n_items);
   p.d = d;
-  p.n_sampled = n_sampled;
-  p.rank_scale = static_cast<float>(n_items) / static_cast<float>(n_sampled);
-  p.loss = loss;
   p.pred_serial = pred_serial;
-  p.coef = coef;
   p.d_user_repr = d_user_rows;
   p.d_user_bias = d_user_bias;
   p.d_item_repr = d_item_repr;
   p.d_item_bias = d_item_bias;
-  const bool att = attention != 0;
-  if (repr_is_bf16)
-    return euclidean ? launch_wmrb_form<__nv_bfloat16, kPairEuclid>(p, n_tastes, att, stream)
-                     : launch_wmrb_form<__nv_bfloat16, kPairDot>(p, n_tastes, att, stream);
-  return euclidean ? launch_wmrb_form<float, kPairEuclid>(p, n_tastes, att, stream)
-                   : launch_wmrb_form<float, kPairDot>(p, n_tastes, att, stream);
+  return p;
+}
+
+// trk_wmrb_step_tastes, and trk_wmrb_step as its one-taste dot form (who = the entry point, for the messages)
+int wmrb_step_tastes(const char* who, const void* user_rows, const void* item_repr, int32_t repr_is_bf16,
+                     int32_t n_tastes, int32_t attention, int32_t euclidean, const float* user_bias,
+                     const float* item_bias, const int32_t* inter_indptr, const int32_t* inter_item,
+                     const float* inter_val, const float* item_weight_sum, const int32_t* samples, int64_t n_users,
+                     int64_t n_items, int32_t d, int32_t n_sampled, float* loss, float* pred_serial, float* coef,
+                     float* d_user_rows, float* d_user_bias, float* d_item_repr, float* d_item_bias,
+                     cudaStream_t stream) {
+  TRK_CHECK_ARG(user_rows && item_repr && inter_indptr && samples, "%s: null input", who);
+  TRK_CHECK_ARG(loss && pred_serial && coef && d_user_rows && d_item_repr, "%s: null output", who);
+  TRK_CHECK_ARG(n_sampled >= 1, "%s: bad sizes", who);
+  const int rc = check_step(who, user_rows, item_repr, n_tastes, attention, euclidean, user_bias, item_bias, n_users,
+                            n_items, d, n_sampled, d_user_rows, d_user_bias, d_item_repr, d_item_bias);
+  if (rc != TRK_OK) return rc;
+  if (n_users == 0) return TRK_OK;
+  WmrbParams p = step_params(user_rows, item_repr, user_bias, item_bias, inter_indptr, inter_item, inter_val, n_users,
+                             n_items, d, pred_serial, d_user_rows, d_user_bias, d_item_repr, d_item_bias);
+  p.item_weight_sum = item_weight_sum;
+  p.samples = samples;
+  p.n_sampled = n_sampled;
+  p.rank_scale = static_cast<float>(n_items) / static_cast<float>(n_sampled);
+  p.loss = loss;
+  p.coef = coef;
+  return launch_step<kModeWmrb>(p, repr_is_bf16 != 0, euclidean != 0, n_tastes, attention != 0, stream);
 }
 
 // The statistics grid of nnz predictions: fixed by nnz alone, so the workspace size and the finish kernel's partial
@@ -983,16 +963,6 @@ static int launch_serial_stats(const float* pred, const float* val, int64_t nnz,
   return TRK_OK;
 }
 
-template <int kMode>
-static int launch_serial_form(const WmrbParams& p, bool bf16, bool euclidean, int n_tastes, bool attention,
-                              cudaStream_t stream) {
-  if (bf16)
-    return euclidean ? launch_wmrb_form<__nv_bfloat16, kPairEuclid, kMode>(p, n_tastes, attention, stream)
-                     : launch_wmrb_form<__nv_bfloat16, kPairDot, kMode>(p, n_tastes, attention, stream);
-  return euclidean ? launch_wmrb_form<float, kPairEuclid, kMode>(p, n_tastes, attention, stream)
-                   : launch_wmrb_form<float, kPairDot, kMode>(p, n_tastes, attention, stream);
-}
-
 int serial_loss_step(int32_t loss_kind, const void* user_rows, const void* item_repr, int32_t repr_is_bf16,
                      int32_t n_tastes, int32_t attention, int32_t euclidean, const float* user_bias,
                      const float* item_bias, const int32_t* inter_indptr, const int32_t* inter_item,
@@ -1001,11 +971,7 @@ int serial_loss_step(int32_t loss_kind, const void* user_rows, const void* item_
                      float* d_item_bias, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
   TRK_CHECK_ARG(loss_kind == kSerialRmse || loss_kind == kSerialSeparation, "serial_loss_step: unknown loss %d",
                 loss_kind);
-  TRK_CHECK_ARG((attention == 0 || attention == 1) && (euclidean == 0 || euclidean == 1),
-                "serial_loss_step: attention and euclidean are flags");
-  TRK_CHECK_ARG(n_users >= 0 && n_items >= 1 && n_items < (1ll << 31) && n_tastes >= 1 && nnz >= 0 &&
-                    nnz < (1ll << 31) && (nnz == 0 || n_users >= 1),
-                "serial_loss_step: bad sizes");
+  TRK_CHECK_ARG(nnz >= 0 && nnz < (1ll << 31) && (nnz == 0 || n_users >= 1), "serial_loss_step: bad sizes");
   TRK_CHECK_ARG(item_repr && d_item_repr && loss && inter_indptr,
                 "serial_loss_step: null item operand, loss or indptr");
   TRK_CHECK_ARG(n_users == 0 || (user_rows && d_user_rows), "serial_loss_step: null user operand");
@@ -1014,19 +980,9 @@ int serial_loss_step(int32_t loss_kind, const void* user_rows, const void* item_
   TRK_CHECK_ARG(workspace_bytes >= serial_loss_workspace_bytes(nnz) && reinterpret_cast<uintptr_t>(workspace) % 8 == 0,
                 "serial_loss_step: workspace of %zu bytes (8-byte aligned) below the %zu needed", workspace_bytes,
                 serial_loss_workspace_bytes(nnz));
-  TRK_CHECK_ARG((user_bias == nullptr) == (item_bias == nullptr), "serial_loss_step: biases must be given together");
-  TRK_CHECK_ARG((user_bias == nullptr) == (d_user_bias == nullptr) && (item_bias == nullptr) == (d_item_bias == nullptr),
-                "serial_loss_step: bias gradients must match the biases");
-  const int max_d = n_tastes == 1 ? 512 : 128;
-  const int max_tastes = attention ? 4 : 8;
-  if (d < 4 || d % 4 != 0 || d > max_d || n_tastes > max_tastes || (attention && n_tastes == 1)) {
-    set_error("serial_loss_step: n_components=%d (multiple of 4, <= 512 for one taste, <= 128 for several) / "
-              "n_tastes=%d (<= 8, <= 4 with attention, attention needs >= 2) outside the fused kernel", d, n_tastes);
-    return TRK_ERR_UNSUPPORTED;
-  }
-  TRK_CHECK_ARG(reinterpret_cast<uintptr_t>(user_rows) % 16 == 0 && reinterpret_cast<uintptr_t>(item_repr) % 16 == 0 &&
-                    reinterpret_cast<uintptr_t>(d_user_rows) % 16 == 0 && reinterpret_cast<uintptr_t>(d_item_repr) % 16 == 0,
-                "serial_loss_step: rows must be 16-byte aligned");
+  int rc = check_step("serial_loss_step", user_rows, item_repr, n_tastes, attention, euclidean, user_bias, item_bias,
+                      n_users, n_items, d, 0, d_user_rows, d_user_bias, d_item_repr, d_item_bias);
+  if (rc != TRK_OK) return rc;
   if (nnz == 0) {
     // no interaction: the mean of nothing is NaN and no prediction reaches a representation (launches nothing)
     TRK_CHECK_CUDA(cudaMemsetAsync(loss, 0xFF, sizeof(float), stream));        // all ones: a quiet NaN
@@ -1039,33 +995,18 @@ int serial_loss_step(int32_t loss_kind, const void* user_rows, const void* item_
     }
     return TRK_OK;
   }
-  WmrbParams p = {};
-  p.user_repr = user_rows;
-  p.item_repr = item_repr;
-  p.user_bias = user_bias;
-  p.item_bias = item_bias;
-  p.inter_indptr = inter_indptr;
-  p.inter_item = inter_item;
-  p.inter_val = inter_val;
-  p.n_users = n_users;
-  p.n_items = static_cast<int32_t>(n_items);
-  p.d = d;
-  p.n_sampled = 0;
-  p.pred_serial = pred_serial;
-  p.d_user_repr = d_user_rows;
-  p.d_user_bias = d_user_bias;
-  p.d_item_repr = d_item_repr;
-  p.d_item_bias = d_item_bias;
+  WmrbParams p = step_params(user_rows, item_repr, user_bias, item_bias, inter_indptr, inter_item, inter_val, n_users,
+                             n_items, d, pred_serial, d_user_rows, d_user_bias, d_item_repr, d_item_bias);
   p.serial_state = workspace;
   p.serial_loss = loss_kind;
   const bool bf16 = repr_is_bf16 != 0, euclid = euclidean != 0, att = attention != 0;
-  int rc = launch_serial_form<kModeSerialForward>(p, bf16, euclid, n_tastes, att, stream);
+  rc = launch_step<kModeSerialForward>(p, bf16, euclid, n_tastes, att, stream);
   if (rc != TRK_OK) return rc;
   rc = loss_kind == kSerialRmse ? launch_serial_stats<kSerialRmse>(pred_serial, inter_val, nnz, workspace, loss, stream)
                                 : launch_serial_stats<kSerialSeparation>(pred_serial, inter_val, nnz, workspace, loss,
                                                                         stream);
   if (rc != TRK_OK) return rc;
-  return launch_serial_form<kModeSerialBackward>(p, bf16, euclid, n_tastes, att, stream);
+  return launch_step<kModeSerialBackward>(p, bf16, euclid, n_tastes, att, stream);
 }
 
 int l2_normalize_rows_step(const float* x, int64_t rows, int32_t d, int32_t n_normalize, float* out, float* grad,

@@ -505,27 +505,26 @@ class TensorRec(object):
 
     def _fit_epochs(self, batches, epochs, learning_rate, alpha, batched_alpha, verbose, n_sampled_items, device):
         from . import train_kernels
-        on_kernels = device.type == 'cuda' and train_kernels.step_plan(self, n_sampled_items) is not None
-        # RMSE / Separation: the serial-loss step on the same kernels (train_kernels.serial_loss_plan; DESIGN §3.11)
-        on_serial = (device.type == 'cuda' and not on_kernels
-                     and train_kernels.serial_loss_plan(self) is not None)
+        # the training step on hand-written kernels (train_kernels.step_plan; DESIGN §3.10, §3.11), or the torch path
+        plan = train_kernels.step_plan(self, n_sampled_items) if device.type == 'cuda' else None
+        serial = plan is not None and plan.loss != 'wmrb'         # RMSE / Separation: a scalar loss
         for epoch in range(epochs):
             for batch, (int_in, uf_in, if_in) in enumerate(batches):
                 if uf_in.shape[1] != self.n_user_features or if_in.shape[1] != self.n_item_features:
                     raise ValueError('feature matrices have {} / {} columns but the model was built for {} / {}'.format(
                         uf_in.shape[1], if_in.shape[1], self.n_user_features, self.n_item_features))
-                if on_kernels or on_serial:
+                if plan is not None:
                     # the training step on hand-written kernels (train_kernels.py; SURVEY 8 f1)
                     if getattr(self, '_wmrb_step', None) is None or self._wmrb_step.device != device:
                         self._wmrb_step = train_kernels.WmrbStep(self, device)
                     n_pos = int_in.n_positive
                     # WMRB adds alpha * reg to each positive interaction's loss; a scalar loss adds it once
-                    l2 = batched_alpha if on_serial else n_pos * batched_alpha
+                    l2 = batched_alpha if serial else n_pos * batched_alpha
                     loss_vec, serial_predictions = self._wmrb_step.step(
                         int_in, uf_in, if_in, n_sampled_items, learning_rate, l2=l2)
                     self._stepped = True
                     if verbose:
-                        mean_loss = float(loss_vec[0]) if on_serial else float(loss_vec.sum()) / max(n_pos, 1)
+                        mean_loss = float(loss_vec[0]) if serial else float(loss_vec.sum()) / max(n_pos, 1)
                         mean_pred = float(torch.mean(serial_predictions))
                         wr = sum(0.5 * float(torch.sum(w.detach() * w.detach())) for w in self._variables.values())
                         logging.info('EPOCH {} BATCH {} loss = {}, weight_reg_l2_loss = {}, mean_pred = {}'.format(

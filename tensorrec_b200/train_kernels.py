@@ -7,7 +7,7 @@ WMRBLossGraph or BalancedWMRBLossGraph, one taste, no attention -- one Adam step
         trk_csr_project_biases_f32     projected biases                        (tensorrec/recommendation_graphs.py:4-19)
         trk_f32_to_bf16                [bf16 form] representations rounded once, halving the gather traffic of the step
         trk_sample_items               n_sampled_items item ids per user       (tensorrec/util.py:12-21)
-        trk_wmrb_step                  serial predictions of the interactions and of the samples, WMRB loss, and the
+        trk_wmrb_step_tastes           serial predictions of the interactions and of the samples, WMRB loss, and the
                                        gradient with respect to representations and projected biases, fused
     K1^T trk_csr_gather_reduce_f32     on the transposed CSR: weight gradients (the gradient of sparse_tensor_dense_matmul)
         trk_csr_project_biases_f32     on the transposed CSR: feature-bias gradients
@@ -19,10 +19,10 @@ any n_components (zero-padded to a multiple of 4 inside the step).  There the us
 attention planes) stacked for trk_wmrb_step_tastes, normalised rows come from trk_l2_normalize_rows_step_f32 forward
 and backward, and every weight gets its own K1^T and Adam pass.
 
-RMSELossGraph and SeparationLossGraph models of those forms (serial_loss_plan; DESIGN §3.11) train on the same
-representations, K1^T and Adam, with trk_serial_loss_step in place of the sampler and trk_wmrb_step[_tastes]: a
-forward launch writes the serial predictions, a statistics launch reduces them to the scalar loss and a loss state on
-the device, and a backward launch turns each prediction into its gradient from that state.
+RMSELossGraph and SeparationLossGraph models of those forms (step_plan's loss 'rmse' / 'separation'; DESIGN §3.11)
+train on the same representations, K1^T and Adam, with trk_serial_loss_step in place of the sampler and
+trk_wmrb_step_tastes: a forward launch writes the serial predictions, a statistics launch reduces them to the scalar
+loss and a loss state on the device, and a backward launch turns each prediction into its gradient from that state.
 
 Every other model family trains through the torch-autograd mirror of the reference's graph functions
 (TensorRec._training_losses); TENSORREC_B200_TRAIN_PATH=torch forces that path."""
@@ -76,20 +76,6 @@ def sample_items_host(n_items, n_users, n_sampled_items, replace, seed, step):
     return out
 
 
-def eligible(model):
-    """Does the kernel training step cover this model?"""
-    from .loss_graphs import WMRBLossGraph, BalancedWMRBLossGraph
-    from .prediction_graphs import DotProductPredictionGraph
-    from .representation_graphs import LinearRepresentationGraph
-    return (TRAIN_PATH != 'torch'
-            and type(model.user_repr_graph_factory) is LinearRepresentationGraph
-            and type(model.item_repr_graph_factory) is LinearRepresentationGraph
-            and type(model.prediction_graph_factory) is DotProductPredictionGraph
-            and type(model.loss_graph_factory) in (WMRBLossGraph, BalancedWMRBLossGraph)
-            and model.n_tastes == 1 and model.attention_graph_factory is None
-            and model.n_components % 4 == 0 and 4 <= model.n_components <= 512)
-
-
 MAX_SAMPLED = 2048                 # n_sampled_items the fused step covers
 MAX_D_ONE_TASTE = 512              # n_components with one taste
 MAX_D_TASTES = 128                 # n_components with several tastes
@@ -99,40 +85,28 @@ MAX_TASTES_ATTENTION = 4           # n_tastes with attention
 # The form of the fused step that trains a model: pair 'dot' (dot and cosine) or 'euclidean'; how many times the user,
 # attention and item rows are L2-normalised (NormalizedLinearRepresentationGraph once, cosine once more); d_pad the
 # operand width (n_components rounded up to a multiple of 4).
-# loss: 'wmrb' (WMRB / BalancedWMRB on trk_wmrb_step[_tastes]), or 'rmse' / 'separation' (trk_serial_loss_step).
+# loss: 'wmrb' (WMRB / BalancedWMRB on trk_wmrb_step_tastes), or 'rmse' / 'separation' (trk_serial_loss_step).
 StepForm = collections.namedtuple('StepForm', ['pair', 'n_tastes', 'attention', 'normalize_user', 'normalize_attn',
-                                               'normalize_item', 'd_pad', 'loss'], defaults=('wmrb',))
+                                               'normalize_item', 'd_pad', 'loss'])
 SERIAL_LOSS_KIND = {'rmse': 0, 'separation': 1}          # trk_serial_loss_step's loss_kind
 
 
 def step_plan(model, n_sampled_items=None):
-    """The StepForm of the fused training step for this model, or None when it trains on the torch path: a WMRB /
-    BalancedWMRB loss; dot, cosine or Euclidean prediction; Linear or NormalizedLinear user, item and attention graphs
-    (or no attention); n_components <= 512 for one taste, <= 128 with n_tastes <= 8 (<= 4 with attention);
-    n_sampled_items <= 2048."""
-    from .loss_graphs import WMRBLossGraph, BalancedWMRBLossGraph
-    if TRAIN_PATH == 'torch' or type(model.loss_graph_factory) not in (WMRBLossGraph, BalancedWMRBLossGraph):
-        return None
-    if n_sampled_items is not None and n_sampled_items > MAX_SAMPLED:
-        return None
-    return _form(model, 'wmrb')
-
-
-def serial_loss_plan(model):
-    """The StepForm (loss 'rmse' or 'separation') of the serial-loss training step for this model, or None: an
-    RMSELossGraph / SeparationLossGraph with the prediction, representation and taste forms step_plan() accepts.
-    Nothing is sampled, so there is no n_sampled_items limit."""
-    from .loss_graphs import RMSELossGraph, SeparationLossGraph
-    loss = {RMSELossGraph: 'rmse', SeparationLossGraph: 'separation'}.get(type(model.loss_graph_factory))
-    if TRAIN_PATH == 'torch' or loss is None:
-        return None
-    return _form(model, loss)
-
-
-def _form(model, loss):
+    """The StepForm of the fused training step for this model, or None when it trains on the torch path: loss 'wmrb'
+    for a WMRB / BalancedWMRB loss with n_sampled_items <= 2048, 'rmse' / 'separation' for an RMSELossGraph /
+    SeparationLossGraph (nothing sampled: no n_sampled_items limit); dot, cosine or Euclidean prediction; Linear or
+    NormalizedLinear user, item and attention graphs (or no attention); n_components <= 512 for one taste, <= 128 with
+    n_tastes <= 8 (<= 4 with attention)."""
+    from .loss_graphs import BalancedWMRBLossGraph, RMSELossGraph, SeparationLossGraph, WMRBLossGraph
     from .prediction_graphs import (CosineSimilarityPredictionGraph, DotProductPredictionGraph,
                                     EuclideanSimilarityPredictionGraph)
     from .representation_graphs import LinearRepresentationGraph, NormalizedLinearRepresentationGraph
+    loss = {WMRBLossGraph: 'wmrb', BalancedWMRBLossGraph: 'wmrb', RMSELossGraph: 'rmse',
+            SeparationLossGraph: 'separation'}.get(type(model.loss_graph_factory))
+    if TRAIN_PATH == 'torch' or loss is None:
+        return None
+    if loss == 'wmrb' and n_sampled_items is not None and n_sampled_items > MAX_SAMPLED:
+        return None
     pred = type(model.prediction_graph_factory)
     if pred not in (DotProductPredictionGraph, CosineSimilarityPredictionGraph, EuclideanSimilarityPredictionGraph):
         return None
@@ -157,11 +131,6 @@ def _form(model, loss):
                     attention=attention, normalize_user=n_norm(model.user_repr_graph_factory),
                     normalize_attn=n_norm(model.attention_graph_factory) if attention else 0,
                     normalize_item=n_norm(model.item_repr_graph_factory), d_pad=(d + 3) // 4 * 4, loss=loss)
-
-
-def _plain(form):
-    """The dot / one-taste / unnormalised / unpadded form: trk_wmrb_step."""
-    return (form.pair == 'dot' and form.n_tastes == 1 and form.normalize_user == 0 and form.normalize_item == 0)
 
 
 def check_step_inputs(interactions_shape, n_users, n_items, n_sampled_items, samples=None):
@@ -246,16 +215,14 @@ class WmrbStep(object):
         SUMMED loss (the reference adds alpha * reg to every element of its loss vector, tensorrec.py:488, so it is
         n_positive_interactions * batched_alpha).  Returns the device tensors of the step (loss, pred_serial).
 
-        For an RMSE / Separation model (serial_loss_plan) the loss is a scalar: `l2` is batched_alpha itself, the
-        returned loss is a 1-element tensor, and n_sampled_items and samples are not used."""
+        For an RMSE / Separation model (step_plan's loss 'rmse' / 'separation') the loss is a scalar: `l2` is
+        batched_alpha itself, the returned loss is a 1-element tensor, and n_sampled_items and samples are not used."""
         lib = kernels.require_cuda()
-        from .loss_graphs import BalancedWMRBLossGraph
-        form = step_plan(self.model) or serial_loss_plan(self.model)
+        form = step_plan(self.model)
         if form is None:
-            raise ValueError('the fused training step does not cover this model (train_kernels.step_plan, '
-                             'serial_loss_plan)')
-        serial = form.loss != 'wmrb'
-        if serial:
+            raise ValueError('the fused training step does not cover this model (train_kernels.step_plan)')
+        wmrb = form.loss == 'wmrb'
+        if not wmrb:
             samples = None
         dev, d, dp = self.device, self.model.n_components, form.d_pad
         n_users, n_items = user_in.shape[0], item_in.shape[0]
@@ -263,7 +230,7 @@ class WmrbStep(object):
         ucsr, icsr = user_in.device_csr(dev), item_in.device_csr(dev)
         ucsr_t, icsr_t = user_in.device_csr_t(dev), item_in.device_csr_t(dev)
         inter = interactions_in.device_csr(dev)
-        if serial and inter.nnz >= 2 ** 31:
+        if not wmrb and inter.nnz >= 2 ** 31:
             raise ValueError('{} interactions exceed the step\'s int32 indexing'.format(inter.nnz))
         names, ws = self._weights(user_in.shape[1], item_in.shape[1])
         # the user operand: taste planes, then attention planes, [n_rows, n_users, d_pad]
@@ -302,41 +269,13 @@ class WmrbStep(object):
             _lib.check(lib.trk_f32_to_bf16(_p(item_repr), item_repr.numel(), _p(repr_i), _stream()), 'trk_f32_to_bf16')
 
         self._mark('representations')
-        if serial:
-            loss, pred, d_user_repr, d_ub, d_item_repr, d_ib = self._serial_loss(lib, form, repr_u, repr_i, ub, ib,
-                                                                                 inter, user_repr.shape)
+        # the loss and the gradient with respect to the operands
+        if wmrb:
+            samples, loss, pred, (d_user_repr, d_item_repr, d_ub, d_ib) = self._wmrb_loss(
+                lib, form, interactions_in, inter, repr_u, repr_i, ub, ib, n_sampled_items, samples)
         else:
-            if samples is None:
-                samples = sample_items_device(n_items, n_users, n_sampled_items,
-                                              self.model.loss_graph_factory.is_sampled_with_replacement, self.seed,
-                                              self.t, dev)
-            weight_sum = None
-            if type(self.model.loss_graph_factory) is BalancedWMRBLossGraph:
-                weight_sum = interactions_in.positive_item_sums(dev)
-
-            self._mark('sampler')
-            nnz = inter.nnz
-            loss = torch.empty((nnz,), dtype=torch.float32, device=dev)
-            pred = torch.empty((nnz,), dtype=torch.float32, device=dev)
-            coef = torch.empty((nnz,), dtype=torch.float32, device=dev)
-            d_user_repr = torch.empty(user_repr.shape, dtype=torch.float32, device=dev)
-            d_item_repr = torch.zeros((n_items, dp), dtype=torch.float32, device=dev)
-            d_ub = torch.empty((n_users,), dtype=torch.float32, device=dev) if self.model.biased else None
-            d_ib = torch.zeros((n_items,), dtype=torch.float32, device=dev) if self.model.biased else None
-            if _plain(form):
-                rc = lib.trk_wmrb_step(_p(repr_u), _p(repr_i), 1 if self.bf16 else 0, _p(ub), _p(ib), _p(inter.indptr),
-                                       _p(inter.col), _p(inter.val), _p(weight_sum), _p(samples), n_users, n_items, dp,
-                                       int(samples.shape[1]), _p(loss), _p(pred), _p(coef), _p(d_user_repr), _p(d_ub),
-                                       _p(d_item_repr), _p(d_ib), _stream())
-                _lib.check(rc, 'trk_wmrb_step')
-            else:
-                rc = lib.trk_wmrb_step_tastes(_p(repr_u), _p(repr_i), 1 if self.bf16 else 0, form.n_tastes,
-                                              1 if form.attention else 0, 1 if form.pair == 'euclidean' else 0, _p(ub),
-                                              _p(ib), _p(inter.indptr), _p(inter.col), _p(inter.val), _p(weight_sum),
-                                              _p(samples), n_users, n_items, dp, int(samples.shape[1]), _p(loss), _p(pred),
-                                              _p(coef), _p(d_user_repr), _p(d_ub), _p(d_item_repr), _p(d_ib), _stream())
-                _lib.check(rc, 'trk_wmrb_step_tastes')
-            self._mark('wmrb_step')
+            loss, pred, (d_user_repr, d_item_repr, d_ub, d_ib) = self._serial_loss(lib, form, inter, repr_u, repr_i,
+                                                                                   ub, ib)
 
         # backward through the normalisations, then through the sparse x dense products: K1 on the transposed CSR
         def weight_grad(csr_t, raw, n_norm, d_rows):
@@ -372,26 +311,60 @@ class WmrbStep(object):
         self._mark('adam')
         return loss, pred
 
-    def _serial_loss(self, lib, form, repr_u, repr_i, ub, ib, inter, user_shape):
+    def _operand_grads(self, repr_u, repr_i):
+        """(d user rows, d item rows, d user biases, d item biases) for the loss kernels: the user side is written,
+        the item side added to (zeroed here)."""
+        dev, biased, n_users, n_items = self.device, self.model.biased, repr_u.shape[1], repr_i.shape[0]
+        return (torch.empty(repr_u.shape, dtype=torch.float32, device=dev),
+                torch.zeros(repr_i.shape, dtype=torch.float32, device=dev),
+                torch.empty((n_users,), dtype=torch.float32, device=dev) if biased else None,
+                torch.zeros((n_items,), dtype=torch.float32, device=dev) if biased else None)
+
+    def _wmrb_loss(self, lib, form, interactions_in, inter, repr_u, repr_i, ub, ib, n_sampled_items, samples):
+        """trk_sample_items (unless the caller gives the samples) and trk_wmrb_step_tastes: the samples, the loss
+        [nnz] (0 for the non-positive interactions), pred_serial and the operand gradients of a WMRB / BalancedWMRB
+        step."""
+        from .loss_graphs import BalancedWMRBLossGraph
+        dev, n_users, n_items, nnz = self.device, repr_u.shape[1], repr_i.shape[0], inter.nnz
+        if samples is None:
+            samples = sample_items_device(n_items, n_users, n_sampled_items,
+                                          self.model.loss_graph_factory.is_sampled_with_replacement, self.seed, self.t,
+                                          dev)
+        weight_sum = None
+        if type(self.model.loss_graph_factory) is BalancedWMRBLossGraph:
+            weight_sum = interactions_in.positive_item_sums(dev)
+
+        self._mark('sampler')
+        loss = torch.empty((nnz,), dtype=torch.float32, device=dev)
+        pred = torch.empty((nnz,), dtype=torch.float32, device=dev)
+        coef = torch.empty((nnz,), dtype=torch.float32, device=dev)
+        grads = d_user_repr, d_item_repr, d_ub, d_ib = self._operand_grads(repr_u, repr_i)
+        rc = lib.trk_wmrb_step_tastes(_p(repr_u), _p(repr_i), 1 if self.bf16 else 0, form.n_tastes,
+                                      1 if form.attention else 0, 1 if form.pair == 'euclidean' else 0, _p(ub), _p(ib),
+                                      _p(inter.indptr), _p(inter.col), _p(inter.val), _p(weight_sum), _p(samples),
+                                      n_users, n_items, form.d_pad, int(samples.shape[1]), _p(loss), _p(pred), _p(coef),
+                                      _p(d_user_repr), _p(d_ub), _p(d_item_repr), _p(d_ib), _stream())
+        _lib.check(rc, 'trk_wmrb_step_tastes')
+        self._mark('wmrb_step')
+        return samples, loss, pred, grads
+
+    def _serial_loss(self, lib, form, inter, repr_u, repr_i, ub, ib):
         """trk_serial_loss_step: the scalar loss [1], pred_serial and the operand gradients of an RMSE / Separation
         step.  An interaction-free batch launches no kernel (loss NaN, zero gradients), as the mean of nothing gives."""
-        dev, dp, n_users, n_items, nnz = self.device, form.d_pad, user_shape[1], repr_i.shape[0], inter.nnz
+        dev, n_users, n_items, nnz = self.device, repr_u.shape[1], repr_i.shape[0], inter.nnz
         loss = torch.empty((1,), dtype=torch.float32, device=dev)
         pred = torch.empty((nnz,), dtype=torch.float32, device=dev)
-        d_user_repr = torch.empty(user_shape, dtype=torch.float32, device=dev)
-        d_item_repr = torch.zeros((n_items, dp), dtype=torch.float32, device=dev)
-        d_ub = torch.empty((n_users,), dtype=torch.float32, device=dev) if self.model.biased else None
-        d_ib = torch.zeros((n_items,), dtype=torch.float32, device=dev) if self.model.biased else None
+        grads = d_user_repr, d_item_repr, d_ub, d_ib = self._operand_grads(repr_u, repr_i)
         ws_bytes = int(lib.trk_serial_loss_workspace_bytes(nnz))
         workspace = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
         rc = lib.trk_serial_loss_step(SERIAL_LOSS_KIND[form.loss], _p(repr_u), _p(repr_i), 1 if self.bf16 else 0,
                                       form.n_tastes, 1 if form.attention else 0, 1 if form.pair == 'euclidean' else 0,
                                       _p(ub), _p(ib), _p(inter.indptr), _p(inter.col), _p(inter.val), n_users, n_items,
-                                      dp, nnz, _p(loss), _p(pred), _p(d_user_repr), _p(d_ub), _p(d_item_repr), _p(d_ib),
-                                      _p(workspace), ws_bytes, _stream())
+                                      form.d_pad, nnz, _p(loss), _p(pred), _p(d_user_repr), _p(d_ub), _p(d_item_repr),
+                                      _p(d_ib), _p(workspace), ws_bytes, _stream())
         _lib.check(rc, 'trk_serial_loss_step')
         self._mark('serial_loss_step')
-        return loss, pred, d_user_repr, d_ub, d_item_repr, d_ib
+        return loss, pred, grads
 
 
 def positive_item_sums(matrix, n_items):

@@ -40,19 +40,23 @@ def test_user_blocks_cover_every_row_once_in_order():
     assert rows % 128 == 0 and rows * n_items * 4 <= model.PREDICT_BLOCK_BYTES < (rows + 128) * n_items * 4
 
 
-def test_kernel_training_step_covers_exactly_the_linear_dot_wmrb_models(monkeypatch):
+def test_step_plan_gives_each_model_its_form(monkeypatch):
     monkeypatch.setattr(train_kernels, 'TRAIN_PATH', 'kernel')
-    assert train_kernels.eligible(TensorRec(n_components=8, loss_graph=WMRBLossGraph()))
-    assert train_kernels.eligible(TensorRec(n_components=128, loss_graph=BalancedWMRBLossGraph()))
-    assert not train_kernels.eligible(TensorRec(n_components=8, loss_graph=RMSELossGraph()))
-    assert not train_kernels.eligible(TensorRec(n_components=10, loss_graph=WMRBLossGraph()))     # not a multiple of 4
-    assert not train_kernels.eligible(TensorRec(n_components=8, n_tastes=2, loss_graph=WMRBLossGraph()))
-    assert not train_kernels.eligible(TensorRec(n_components=8, loss_graph=WMRBLossGraph(),
-                                                prediction_graph=CosineSimilarityPredictionGraph()))
-    assert not train_kernels.eligible(TensorRec(n_components=8, loss_graph=WMRBLossGraph(),
-                                                item_repr_graph=NormalizedLinearRepresentationGraph()))
+    plan = train_kernels.step_plan
+    dot = train_kernels.StepForm(pair='dot', n_tastes=1, attention=False, normalize_user=0, normalize_attn=0,
+                                 normalize_item=0, d_pad=8, loss='wmrb')          # Linear x dot x WMRB, one taste
+    assert plan(TensorRec(n_components=8, loss_graph=WMRBLossGraph())) == dot
+    assert plan(TensorRec(n_components=128, loss_graph=BalancedWMRBLossGraph())) == dot._replace(d_pad=128)
+    assert plan(TensorRec(n_components=8, loss_graph=RMSELossGraph())) == dot._replace(loss='rmse')
+    assert plan(TensorRec(n_components=10, loss_graph=WMRBLossGraph())) == dot._replace(d_pad=12)    # zero-padded
+    assert plan(TensorRec(n_components=8, n_tastes=2, loss_graph=WMRBLossGraph())) == dot._replace(n_tastes=2)
+    assert plan(TensorRec(n_components=8, loss_graph=WMRBLossGraph(),
+                          prediction_graph=CosineSimilarityPredictionGraph())) == dot._replace(normalize_user=1,
+                                                                                                normalize_item=1)
+    assert plan(TensorRec(n_components=8, loss_graph=WMRBLossGraph(),
+                          item_repr_graph=NormalizedLinearRepresentationGraph())) == dot._replace(normalize_item=1)
     monkeypatch.setattr(train_kernels, 'TRAIN_PATH', 'torch')
-    assert not train_kernels.eligible(TensorRec(n_components=8, loss_graph=WMRBLossGraph()))
+    assert plan(TensorRec(n_components=8, loss_graph=WMRBLossGraph())) is None
 
 
 def test_positive_item_sums_and_positive_count():

@@ -1,5 +1,5 @@
 """CPU tests of the fused training step's forms (DESIGN §3.10): the general step oracle
-(tests/train_forms_oracle.sampled_rank_step_reference) equals torch autograd over the host mirror of the reference's
+(tests/train_step_oracle.sampled_rank_step_reference) equals torch autograd over the host mirror of the reference's
 graph functions for every factor the step covers, splits tied tastes evenly, the routing predicate covers exactly the
 stated models, and the step's input check rejects malformed inputs before any launch."""
 import itertools
@@ -9,10 +9,11 @@ import pytest
 import torch
 
 from oracle import loss_ops
-from tests.train_forms_oracle import sampled_rank_step_reference
+from tests.helpers import make_model, make_weights, reference_example_models
+from tests.train_step_oracle import sampled_rank_step_reference
 import tensorrec_b200 as T
 from tensorrec_b200 import train_kernels, util
-from tensorrec_b200.loss_graphs import BalancedWMRBLossGraph, RMSELossGraph, WMRBLossGraph
+from tensorrec_b200.loss_graphs import RMSELossGraph, WMRBLossGraph
 from tensorrec_b200.prediction_graphs import (CosineSimilarityPredictionGraph, DotProductPredictionGraph,
                                               EuclideanSimilarityPredictionGraph)
 from tensorrec_b200.representation_graphs import (LinearRepresentationGraph, NormalizedLinearRepresentationGraph,
@@ -28,28 +29,6 @@ def cpu_session():
     sm.set_session(sm.Session('cpu'))
     yield
     sm.set_session(None)
-
-
-def make_weights(uf, itf, d, n_tastes, attention, biased, seed):
-    rng = np.random.default_rng(seed)
-    w = {'linear_weights_item': (0.3 * rng.standard_normal((itf.shape[1], d))).astype(np.float32)}
-    for t in range(n_tastes):
-        w['linear_weights_user_{}'.format(t)] = (0.3 * rng.standard_normal((uf.shape[1], d))).astype(np.float32)
-        if attention:
-            w['linear_weights_attn_{}'.format(t)] = (0.3 * rng.standard_normal((uf.shape[1], d))).astype(np.float32)
-    if biased:
-        w['feature_biases_user'] = (0.2 * rng.standard_normal((uf.shape[1], 1))).astype(np.float32)
-        w['feature_biases_item'] = (0.2 * rng.standard_normal((itf.shape[1], 1))).astype(np.float32)
-    return w
-
-
-def make_model(prediction, user_norm, item_norm, n_tastes, attention, balanced, biased, d):
-    repr_graph = lambda norm: NormalizedLinearRepresentationGraph() if norm else LinearRepresentationGraph()  # noqa
-    return T.TensorRec(n_components=d, n_tastes=n_tastes, user_repr_graph=repr_graph(user_norm),
-                       item_repr_graph=repr_graph(item_norm),
-                       attention_graph=LinearRepresentationGraph() if attention else None,
-                       prediction_graph=PREDICTIONS[prediction](),
-                       loss_graph=BalancedWMRBLossGraph() if balanced else WMRBLossGraph(), biased=biased)
 
 
 def autograd_of_the_mirror(monkeypatch, model, weights, interactions, uf, itf, samples):
@@ -85,8 +64,7 @@ def test_step_oracle_equals_autograd_of_the_host_mirror(monkeypatch, cpu_session
     samples = np.stack([np.random.default_rng(u).choice(itf.shape[0], 7, replace=False) for u in range(uf.shape[0])])
     normalize = [side for side, on in (('user', user_norm), ('item', item_norm)) if on]
     ref = sampled_rank_step_reference(uf, itf, interactions, weights, samples, prediction=prediction,
-                                               normalize=normalize, n_tastes=n_tastes, attention=attention,
-                                               balanced=balanced)
+                                      normalize=normalize, n_tastes=n_tastes, attention=attention, balanced=balanced)
     model = make_model(prediction, user_norm, item_norm, n_tastes, attention, balanced, biased, d)
     loss, pred, grads = autograd_of_the_mirror(monkeypatch, model, weights, interactions, uf, itf, samples)
     assert np.allclose(loss, ref['loss'], rtol=2e-5, atol=2e-6)
@@ -130,22 +108,7 @@ def test_identical_tastes_share_the_gradient_equally(prediction):
 
 
 # ---- routing -------------------------------------------------------------------------------------------------
-def reference_example_models():
-    """The WMRB configurations of the reference's examples (getting_started.py:98, check_movielens_losses.py:45-58,
-    attention_example.py:27-41)."""
-    yield T.TensorRec(n_components=5, loss_graph=WMRBLossGraph())
-    nl = NormalizedLinearRepresentationGraph
-    for pred in (DotProductPredictionGraph, CosineSimilarityPredictionGraph, EuclideanSimilarityPredictionGraph):
-        for nt in (1, 3):
-            for lg in (WMRBLossGraph, BalancedWMRBLossGraph):
-                yield T.TensorRec(n_components=10, n_tastes=nt, user_repr_graph=nl(), prediction_graph=pred(),
-                                  loss_graph=lg())
-    for att in (None, LinearRepresentationGraph()):
-        yield T.TensorRec(n_components=10, n_tastes=3, user_repr_graph=nl(), attention_graph=att,
-                          loss_graph=BalancedWMRBLossGraph())
-
-
-def test_step_plan_covers_the_reference_examples_and_the_stated_limits(monkeypatch):
+def test_step_plan_gives_the_wmrb_models_their_form_within_the_stated_limits(monkeypatch):
     monkeypatch.setattr(train_kernels, 'TRAIN_PATH', 'auto')
     for model in reference_example_models():
         form = train_kernels.step_plan(model, n_sampled_items=100)
@@ -171,7 +134,7 @@ def test_step_plan_covers_the_reference_examples_and_the_stated_limits(monkeypat
     assert not ok(n_components=8, n_tastes=5, attention_graph=lin())
     assert not ok(n_components=8, item_repr_graph=ReLURepresentationGraph())
     assert not ok(n_components=8, attention_graph=ReLURepresentationGraph(), n_tastes=2)
-    assert train_kernels.step_plan(T.TensorRec(n_components=8, loss_graph=RMSELossGraph())) is None
+    assert train_kernels.step_plan(T.TensorRec(n_components=8, loss_graph=RMSELossGraph())).loss == 'rmse'
     assert train_kernels.step_plan(T.TensorRec(n_components=8, loss_graph=WMRBLossGraph()), 2049) is None
     monkeypatch.setattr(train_kernels, 'TRAIN_PATH', 'torch')
     for model in reference_example_models():

@@ -1,5 +1,5 @@
 """GPU tests of the fused training step's forms (DESIGN §3.10) against the general step oracle
-(tests/train_forms_oracle.sampled_rank_step_reference, pinned on the CPU against torch autograd over the host mirror:
+(tests/train_step_oracle.sampled_rank_step_reference, pinned on the CPU against torch autograd over the host mirror:
 tests/test_train_forms_cpu.py): cosine / Euclidean prediction, NormalizedLinear sides, mixtures of tastes with max or
 attention collapse, padded n_components, bf16 representations, Adam over every weight, and fit() on the WMRB
 configurations of the reference's examples."""
@@ -8,8 +8,8 @@ import pytest
 import scipy.sparse as sp
 
 from oracle import loss_ops
-from tests.train_forms_oracle import sampled_rank_step_reference
-from tests.test_train_forms_cpu import make_model, make_weights, reference_example_models
+from tests.helpers import csr_order, kernel_step, make_model, make_weights, reference_example_models
+from tests.train_step_oracle import sampled_rank_step_reference
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
@@ -32,22 +32,6 @@ def make_case(seed, d, n_tastes, attention, biased, n_users=260, n_items=230):
                                                      num_user_features=40, num_item_features=30,
                                                      n_features_per_user=6, n_features_per_item=5, seed=seed)
     return sp.csr_matrix(interactions), uf, itf, make_weights(uf, itf, d, n_tastes, attention, biased, seed + 100)
-
-
-def kernel_step(model, weights, interactions, uf, itf, samples, bf16=False, lr=0.05, l2=0.0):
-    import torch
-    from tensorrec_b200 import train_kernels as TK
-    from tensorrec_b200.input_utils import SparseInput
-    model.set_weights(weights)
-    stepper = TK.WmrbStep(model, torch.device('cuda', 0), seed=3, bf16=bf16)
-    st = torch.from_numpy(np.ascontiguousarray(samples, dtype=np.int32)).cuda()
-    loss, pred = stepper.step(SparseInput(interactions), SparseInput(uf), SparseInput(itf), samples.shape[1], lr, l2,
-                              samples=st)
-    return stepper, loss.cpu().numpy(), pred.cpu().numpy()
-
-
-def csr_order(interactions):
-    return np.argsort(sp.coo_matrix(interactions).row, kind='stable')
 
 
 CASES = [  # prediction, user_norm, item_norm, n_tastes, attention, balanced, biased, d, n_sampled
@@ -77,8 +61,7 @@ def test_kernel_step_matches_the_oracle_fp32(T, prediction, user_norm, item_norm
     samples = np.stack([rng.choice(itf.shape[0], n_sampled, replace=False) for _ in range(uf.shape[0])])
     normalize = [side for side, on in (('user', user_norm), ('item', item_norm)) if on]
     ref = sampled_rank_step_reference(uf, itf, interactions, weights, samples, prediction=prediction,
-                                               normalize=normalize, n_tastes=n_tastes, attention=attention,
-                                               balanced=balanced)
+                                      normalize=normalize, n_tastes=n_tastes, attention=attention, balanced=balanced)
     model = make_model(prediction, user_norm, item_norm, n_tastes, attention, balanced, biased, d)
     stepper, loss, pred = kernel_step(model, weights, interactions, uf, itf, samples)
     order = csr_order(interactions)
@@ -100,8 +83,8 @@ def test_kernel_step_bf16_representations(T, prediction, n_tastes, attention):
     rng = np.random.default_rng(6)
     samples = np.stack([rng.choice(itf.shape[0], 20, replace=False) for _ in range(uf.shape[0])])
     kw = dict(prediction=prediction, normalize=['user'], n_tastes=n_tastes, attention=attention)
-    ref = sampled_rank_step_reference(uf, itf, interactions, weights, samples,
-                                               round_repr=loss_ops.round_to_bfloat16, **kw)
+    ref = sampled_rank_step_reference(uf, itf, interactions, weights, samples, round_repr=loss_ops.round_to_bfloat16,
+                                      **kw)
     model = make_model(prediction, True, False, n_tastes, attention, False, True, 128)
     stepper, loss, pred = kernel_step(model, weights, interactions, uf, itf, samples, bf16=True)
     order = csr_order(interactions)

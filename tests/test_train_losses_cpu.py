@@ -1,13 +1,12 @@
 """CPU tests of the serial-loss training step (RMSELossGraph, SeparationLossGraph; DESIGN §3.11): the step oracle
-(tests/serial_loss_oracle.serial_loss_step_reference) equals torch autograd over the host mirror of the reference's
+(tests/train_step_oracle.serial_loss_step_reference) equals torch autograd over the host mirror of the reference's
 graph functions for every form the step covers, on interactions with explicit zeros, duplicates and negative values;
-the routing covers exactly the stated models and leaves step_plan / eligible as they were; the L2 coefficient of a
-scalar loss is batched_alpha."""
+step_plan gives exactly the stated models a serial loss and the WMRB models the answers they had; the L2 coefficient
+of a scalar loss is batched_alpha."""
 import itertools
 
 import numpy as np
 import pytest
-import scipy.sparse as sp
 import torch
 
 import tensorrec_b200 as T
@@ -18,8 +17,8 @@ from tensorrec_b200.prediction_graphs import (CosineSimilarityPredictionGraph, D
                                               EuclideanSimilarityPredictionGraph)
 from tensorrec_b200.representation_graphs import (LinearRepresentationGraph, NormalizedLinearRepresentationGraph,
                                                   ReLURepresentationGraph)
-from tests.serial_loss_oracle import serial_loss_coefficients, serial_loss_step_reference
-from tests.test_train_forms_cpu import make_weights
+from tests.helpers import make_serial_model, make_weights, rough_interactions
+from tests.train_step_oracle import serial_loss_coefficients, serial_loss_step_reference
 
 PREDICTIONS = {'dot': DotProductPredictionGraph, 'cosine': CosineSimilarityPredictionGraph,
                'euclidean': EuclideanSimilarityPredictionGraph}
@@ -32,34 +31,6 @@ def cpu_session():
     sm.set_session(sm.Session('cpu'))
     yield
     sm.set_session(None)
-
-
-def make_serial_model(loss, prediction, user_norm, item_norm, n_tastes, attention, biased, d):
-    repr_graph = lambda norm: NormalizedLinearRepresentationGraph() if norm else LinearRepresentationGraph()  # noqa
-    return T.TensorRec(n_components=d, n_tastes=n_tastes, user_repr_graph=repr_graph(user_norm),
-                       item_repr_graph=repr_graph(item_norm),
-                       attention_graph=LinearRepresentationGraph() if attention else None,
-                       prediction_graph=PREDICTIONS[prediction](), loss_graph=LOSSES[loss](), biased=biased)
-
-
-def rough_interactions(n_users, n_items, seed, density=0.15):
-    """Dummy interactions with explicit zeros, negative values and duplicate (user, item) entries, as COO in a mixed
-    order: every stored entry is one interaction of the serial losses."""
-    interactions, uf, itf = util.generate_dummy_data(num_users=n_users, num_items=n_items, interaction_density=density,
-                                                     num_user_features=20, num_item_features=18,
-                                                     n_features_per_user=5, n_features_per_item=4, seed=seed)
-    coo = sp.coo_matrix(interactions)
-    rng = np.random.default_rng(seed)
-    val = coo.data.astype(np.float32).copy()
-    val[rng.random(val.shape[0]) < 0.15] = 0.0
-    neg = rng.random(val.shape[0]) < 0.15
-    val[neg] = -np.abs(val[neg]) - 0.5
-    dup = rng.choice(val.shape[0], max(1, val.shape[0] // 10), replace=False)
-    row = np.concatenate([coo.row, coo.row[dup]])
-    col = np.concatenate([coo.col, coo.col[dup]])
-    val = np.concatenate([val, 2.0 * val[dup] + 0.25]).astype(np.float32)
-    order = rng.permutation(row.shape[0])
-    return sp.coo_matrix((val[order], (row[order], col[order])), shape=coo.shape), uf, itf
 
 
 def autograd_of_the_mirror(model, weights, interactions, uf, itf):
@@ -143,14 +114,15 @@ def getting_started_models():
                       prediction_graph=CosineSimilarityPredictionGraph(), loss_graph=SeparationLossGraph())
 
 
-def test_serial_plan_covers_the_stated_forms_and_nothing_else(monkeypatch):
+def test_step_plan_gives_exactly_the_serial_loss_models_a_serial_form(monkeypatch):
     monkeypatch.setattr(train_kernels, 'TRAIN_PATH', 'auto')
     for model in getting_started_models():
-        form = train_kernels.serial_loss_plan(model)
+        form = train_kernels.step_plan(model)
         assert form is not None and form.loss in ('rmse', 'separation')
         assert form.d_pad == (model.n_components + 3) // 4 * 4
-        assert train_kernels.step_plan(model) is None and train_kernels.step_plan(model, 10) is None
-    assert train_kernels.serial_loss_plan(T.TensorRec()).loss == 'rmse'
+        # nothing is sampled: n_sampled_items, even beyond the WMRB step's limit, changes nothing
+        assert train_kernels.step_plan(model, 10) == form and train_kernels.step_plan(model, 4096) == form
+    assert train_kernels.step_plan(T.TensorRec()).loss == 'rmse'
     nl, lin = NormalizedLinearRepresentationGraph, LinearRepresentationGraph
     for loss, pred, un, inn, att, nt, d in itertools.product(LOSSES, PREDICTIONS.values(), (lin, nl), (lin, nl),
                                                              (None, lin, nl), (1, 2, 4), (1, 7, 128)):
@@ -158,14 +130,14 @@ def test_serial_plan_covers_the_stated_forms_and_nothing_else(monkeypatch):
             continue
         model = T.TensorRec(n_components=d, n_tastes=nt, user_repr_graph=un(), item_repr_graph=inn(),
                             attention_graph=att() if att else None, prediction_graph=pred(), loss_graph=LOSSES[loss]())
-        form = train_kernels.serial_loss_plan(model)
+        form = train_kernels.step_plan(model)
         assert form is not None and form.loss == loss
         wmrb = train_kernels.step_plan(T.TensorRec(n_components=d, n_tastes=nt, user_repr_graph=un(),
                                                    item_repr_graph=inn(), attention_graph=att() if att else None,
                                                    prediction_graph=pred(), loss_graph=WMRBLossGraph()))
         assert form == wmrb._replace(loss=loss)            # the same operand layout as the WMRB step's
     for lg in (RMSELossGraph, SeparationLossGraph):
-        ok = lambda **kw: train_kernels.serial_loss_plan(T.TensorRec(loss_graph=lg(), **kw)) is not None  # noqa
+        ok = lambda **kw: train_kernels.step_plan(T.TensorRec(loss_graph=lg(), **kw)) is not None  # noqa
         assert ok(n_components=512) and not ok(n_components=513)
         assert ok(n_components=128, n_tastes=8) and not ok(n_components=129, n_tastes=2)
         assert not ok(n_components=8, n_tastes=9)
@@ -173,17 +145,18 @@ def test_serial_plan_covers_the_stated_forms_and_nothing_else(monkeypatch):
         assert not ok(n_components=8, n_tastes=5, attention_graph=lin())
         assert not ok(n_components=8, user_repr_graph=ReLURepresentationGraph())
         assert not ok(n_components=8, attention_graph=ReLURepresentationGraph(), n_tastes=2)
-    for lg in (WMRBLossGraph, BalancedWMRBLossGraph, RMSEDenseLossGraph, SeparationDenseLossGraph):
-        assert train_kernels.serial_loss_plan(T.TensorRec(n_components=8, loss_graph=lg())) is None
-    # the sampled-rank routing keeps every answer
-    assert train_kernels.step_plan(T.TensorRec(n_components=8, loss_graph=RMSELossGraph())) is None
+    for lg in (WMRBLossGraph, BalancedWMRBLossGraph):
+        assert train_kernels.step_plan(T.TensorRec(n_components=8, loss_graph=lg())).loss == 'wmrb'
+    for lg in (RMSEDenseLossGraph, SeparationDenseLossGraph):
+        assert train_kernels.step_plan(T.TensorRec(n_components=8, loss_graph=lg())) is None
+    # the sampled-rank routing keeps every answer: the serial losses never reach the WMRB step
+    assert train_kernels.step_plan(T.TensorRec(n_components=8, loss_graph=RMSELossGraph())).loss == 'rmse'
+    assert train_kernels.step_plan(T.TensorRec(n_components=8, loss_graph=SeparationLossGraph())).loss == 'separation'
     assert train_kernels.step_plan(T.TensorRec(n_components=8, loss_graph=WMRBLossGraph()), 64).loss == 'wmrb'
-    assert not train_kernels.eligible(T.TensorRec(n_components=8, loss_graph=RMSELossGraph()))
-    assert not train_kernels.eligible(T.TensorRec(n_components=8, loss_graph=SeparationLossGraph()))
-    assert train_kernels.eligible(T.TensorRec(n_components=8, loss_graph=WMRBLossGraph()))
+    assert train_kernels.step_plan(T.TensorRec(n_components=8, loss_graph=WMRBLossGraph()), 2049) is None
     monkeypatch.setattr(train_kernels, 'TRAIN_PATH', 'torch')
     for model in getting_started_models():
-        assert train_kernels.serial_loss_plan(model) is None
+        assert train_kernels.step_plan(model) is None
 
 
 def test_the_serial_step_adds_the_l2_term_once(monkeypatch, cpu_session):

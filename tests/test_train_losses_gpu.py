@@ -1,5 +1,5 @@
 """GPU tests of the serial-loss training step (RMSELossGraph, SeparationLossGraph; DESIGN §3.11) against the step
-oracle (tests/serial_loss_oracle.serial_loss_step_reference, pinned on the CPU against torch autograd over the host
+oracle (tests/train_step_oracle.serial_loss_step_reference, pinned on the CPU against torch autograd over the host
 mirror: tests/test_train_losses_cpu.py): every prediction, representation and taste form, bf16 representations, Adam
 over every weight, fit() on TensorRec()'s default model and the reference's examples, and degenerate batches
 (interaction-free, one-sided, empty) with the torch path's finite / NaN pattern."""
@@ -8,9 +8,8 @@ import pytest
 import scipy.sparse as sp
 
 from oracle import loss_ops
-from tests.serial_loss_oracle import serial_loss_step_reference
-from tests.test_train_forms_cpu import make_weights
-from tests.test_train_losses_cpu import make_serial_model, rough_interactions
+from tests.helpers import csr_order, kernel_step, make_serial_model, make_weights, rough_interactions
+from tests.train_step_oracle import serial_loss_step_reference
 
 pytestmark = pytest.mark.gpu
 F32 = np.float32
@@ -25,21 +24,6 @@ def T():
     torch.cuda.set_device(0)
     sm.set_session(None)
     return tensorrec_b200
-
-
-def kernel_step(model, weights, interactions, uf, itf, bf16=False, lr=0.05, l2=0.0):
-    import torch
-    from tensorrec_b200 import train_kernels as TK
-    from tensorrec_b200.input_utils import SparseInput
-    model.set_weights(weights)
-    stepper = TK.WmrbStep(model, torch.device('cuda', 0), seed=3, bf16=bf16)
-    loss, pred = stepper.step(SparseInput(interactions), SparseInput(uf), SparseInput(itf), None, lr, l2)
-    assert tuple(loss.shape) == (1,)
-    return stepper, float(loss.cpu()[0]), pred.cpu().numpy()
-
-
-def csr_order(interactions):
-    return np.argsort(sp.coo_matrix(interactions).row, kind='stable')
 
 
 CASES = [  # loss, prediction, user_norm, item_norm, n_tastes, attention, biased, d
@@ -70,7 +54,9 @@ def test_kernel_step_matches_the_oracle_fp32(T, loss, prediction, user_norm, ite
     ref = serial_loss_step_reference(uf, itf, interactions, weights, loss=loss, prediction=prediction,
                                      normalize=normalize, n_tastes=n_tastes, attention=attention)
     model = make_serial_model(loss, prediction, user_norm, item_norm, n_tastes, attention, biased, d)
-    stepper, value, pred = kernel_step(model, weights, interactions, uf, itf)
+    stepper, out, pred = kernel_step(model, weights, interactions, uf, itf)
+    assert out.shape == (1,)
+    value = float(out[0])
     order = csr_order(interactions)
     assert np.allclose(pred, ref['pred_serial'][order], rtol=2e-5, atol=2e-6)
     assert np.isfinite(value) and np.isclose(value, ref['loss'], rtol=1e-4, atol=1e-6)
@@ -89,7 +75,9 @@ def test_kernel_step_bf16_representations(T, loss, prediction, n_tastes, attenti
     kw = dict(loss=loss, prediction=prediction, normalize=['user'], n_tastes=n_tastes, attention=attention)
     ref = serial_loss_step_reference(uf, itf, interactions, weights, round_repr=loss_ops.round_to_bfloat16, **kw)
     model = make_serial_model(loss, prediction, True, False, n_tastes, attention, True, 128)
-    stepper, value, pred = kernel_step(model, weights, interactions, uf, itf, bf16=True)
+    stepper, out, pred = kernel_step(model, weights, interactions, uf, itf, bf16=True)
+    assert out.shape == (1,)
+    value = float(out[0])
     order = csr_order(interactions)
     err = np.abs(pred - ref['pred_serial'][order])
     assert np.mean(err <= 2e-5 * np.abs(pred) + 2e-6) > 0.9 and err.max() < 0.02
@@ -109,7 +97,8 @@ def test_two_adam_steps_over_every_weight_match_the_oracle(T, loss):
     weights = make_weights(uf, itf, 10, 3, True, True, seed=5)
     lr, l2 = 0.1, 0.3
     model = make_serial_model(loss, 'cosine', True, False, 3, True, True, 10)
-    stepper, _, _ = kernel_step(model, weights, interactions, uf, itf, lr=lr, l2=l2)
+    stepper, out, _ = kernel_step(model, weights, interactions, uf, itf, lr=lr, l2=l2)
+    assert out.shape == (1,)
     w1 = model.get_weights()
     g1 = {k: v.cpu().numpy().reshape(weights[k].shape) for k, v in stepper.last['grads'].items()}
     assert set(w1) == set(weights)
