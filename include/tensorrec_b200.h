@@ -390,6 +390,49 @@ int trk_score_topk_tastes_f16x3(const void* user_split, const float* user_scale,
                                 const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
                                 void* stream);
 
+/* Mixtures of tastes with Euclidean prediction (EuclideanSimilarityPredictionGraph, tensorrec/prediction_graphs.py:84-100,
+ * then collapse_mixture_of_tastes and bias_prediction_dense): every operand row x_j -- taste rows and attention rows
+ * alike -- gives e_j = -sqrtf(max((|x_j|^2 - 2 p_j) + |i|^2, 1e-16)), p_j its 3-pass dot product with i, and the e_j
+ * are collapsed as above (max over the tastes, or the softmax of the attention e_j weighting the taste e_j).  The
+ * arguments of the _tastes_ twins plus the norms: user_half_sqnorm [n_ops, n_users] = -1/2 |x_j|^2 of every operand
+ * row (trk_operand_half_sqnorm of each slice of the stacked operand) and item_half_sqnorm as for
+ * trk_score_dense_euclid_f16x3 (16-byte aligned, padded to whole item tiles); NULL norms return TRK_ERR_ARG.
+ *   trk_score_dense_tastes_euclid_f16x3       as trk_score_dense_tastes_f16x3.
+ *   trk_score_topk_tastes_euclid_f16x3        as trk_score_topk_tastes_f16x3; attention != 0 (a Euclidean mixture of
+ *                                             tastes without attention returns TRK_ERR_UNSUPPORTED: its top k is the
+ *                                             merge of one trk_score_topk_euclid_f16x3 sweep per taste).
+ *   trk_score_topk_wide_tastes_euclid_f16x3   as trk_score_topk_wide_tastes_f16x3; attention != 0 likewise
+ *                                             (trk_score_topk_wide_euclid_f16x3 per taste).
+ *   trk_score_count_tastes_euclid_f16x3       as trk_score_count_tastes_f16x3, attention or not. */
+int trk_score_dense_tastes_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                        int32_t n_tastes, int32_t attention, const void* item_split,
+                                        const float* item_meta, int64_t n_users, int64_t n_items, int32_t d_pad,
+                                        float* out, int64_t out_row_stride, const float* user_half_sqnorm,
+                                        const float* item_half_sqnorm, void* stream);
+int trk_score_topk_tastes_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                       int32_t n_tastes, int32_t attention, const void* item_split,
+                                       const float* item_meta, int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k,
+                                       int32_t n_splits, int32_t item_id_offset, float* cand_score, int32_t* cand_item,
+                                       const int32_t* excl_indptr, const int32_t* excl_ids,
+                                       const int32_t* excl_row_map, const float* user_half_sqnorm,
+                                       const float* item_half_sqnorm, void* stream);
+int trk_score_topk_wide_tastes_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                            int32_t n_tastes, int32_t attention, const void* item_split,
+                                            const float* item_meta, int64_t n_users, int64_t n_items, int32_t d_pad,
+                                            int32_t k, int32_t n_splits, int32_t item_id_offset, float* list_score,
+                                            int32_t* list_item, int32_t* list_count, const int32_t* excl_indptr,
+                                            const int32_t* excl_ids, const int32_t* excl_row_map,
+                                            const float* user_half_sqnorm, const float* item_half_sqnorm,
+                                            void* stream);
+int trk_score_count_tastes_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                        int32_t n_tastes, int32_t attention, const void* item_split,
+                                        const float* item_meta, int64_t n_users, int64_t n_items, int32_t d_pad,
+                                        int32_t n_splits, int32_t item_id_offset, const int32_t* pair_indptr,
+                                        const int32_t* pair_ids, float* pair_score, int32_t* pair_count,
+                                        const int32_t* block_pairs, int32_t pass, const int32_t* excl_indptr,
+                                        const int32_t* excl_ids, const int32_t* excl_row_map,
+                                        const float* user_half_sqnorm, const float* item_half_sqnorm, void* stream);
+
 /* Wide top-k of the Euclidean and attention forms on the exact kernel: 1 <= k <= 1024, every score final and exact
  * (the same epilogue as trk_score_topk_euclid_f16x3 / trk_score_topk_tastes_f16x3), so no certificate, re-scoring or
  * fallback.  Every (user, item split, column half) keeps a list in global memory of

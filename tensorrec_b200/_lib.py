@@ -68,6 +68,17 @@ SIGNATURES = {
     'trk_score_count_tastes_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i32, _c_i32, _c_p, _c_p, _c_i64, _c_i64,
                                                     _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p, _c_i32, _c_p,
                                                     _c_p, _c_p, _c_p]),
+    'trk_score_dense_tastes_euclid_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i32, _c_i32, _c_p, _c_p, _c_i64, _c_i64,
+                                                           _c_i32, _c_p, _c_i64, _c_p, _c_p, _c_p]),
+    'trk_score_topk_tastes_euclid_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i32, _c_i32, _c_p, _c_p, _c_i64, _c_i64,
+                                                          _c_i32, _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p,
+                                                          _c_p, _c_p, _c_p]),
+    'trk_score_topk_wide_tastes_euclid_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i32, _c_i32, _c_p, _c_p, _c_i64,
+                                                               _c_i64, _c_i32, _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p,
+                                                               _c_p, _c_p, _c_p, _c_p, _c_p, _c_p]),
+    'trk_score_count_tastes_euclid_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i32, _c_i32, _c_p, _c_p, _c_i64, _c_i64,
+                                                           _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p, _c_i32,
+                                                           _c_p, _c_p, _c_p, _c_p, _c_p, _c_p]),
     'trk_select_topk_lists': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i64, _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_i64,
                                              _c_p]),
     'trk_topk_merge': (ctypes.c_int, [_c_p, _c_p, _c_i64, _c_i32, _c_i32, _c_i32, _c_i64, _c_i64, _c_p, _c_p, _c_i64,

@@ -292,6 +292,25 @@ int trk_score_dense_tastes_f16x3(const void* user_split, const float* user_scale
   return trk::score_tc(a, trk::as_stream(stream));
 }
 
+int trk_score_dense_tastes_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                        int32_t n_tastes, int32_t attention, const void* item_split,
+                                        const float* item_meta, int64_t n_users, int64_t n_items, int32_t d_pad,
+                                        float* out, int64_t out_row_stride, const float* user_half_sqnorm,
+                                        const float* item_half_sqnorm, void* stream) {
+  TRK_CHECK_ARG(n_tastes >= 1, "score_tastes: n_tastes=%d < 1", n_tastes);
+  TRK_CHECK_ARG(user_half_sqnorm != nullptr && item_half_sqnorm != nullptr,
+                "trk_score_dense_tastes_euclid_f16x3: null squared norms");
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad};
+  a.user_half_sqnorm = user_half_sqnorm;
+  a.item_half_sqnorm = item_half_sqnorm;
+  a.dense = true;
+  a.dense_out = out;
+  a.dense_stride = out_row_stride;
+  a.n_tastes = n_tastes;
+  a.attention = attention;
+  return trk::score_tc(a, trk::as_stream(stream));
+}
+
 int trk_score_topk_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
                                 int32_t n_tastes, int32_t attention, const void* item_split, const float* item_meta,
                                 int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k, int32_t n_splits,
@@ -304,6 +323,24 @@ int trk_score_topk_tastes_f16x3(const void* user_split, const float* user_scale,
   a.excl_indptr = excl_indptr;
   a.excl_ids = excl_ids;
   a.excl_row_map = excl_row_map;
+  a.n_tastes = n_tastes;
+  a.attention = attention;
+  return trk::score_tc(a, trk::as_stream(stream));
+}
+
+int trk_score_topk_tastes_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                       int32_t n_tastes, int32_t attention, const void* item_split,
+                                       const float* item_meta, int64_t n_users, int64_t n_items, int32_t d_pad, int32_t k,
+                                       int32_t n_splits, int32_t item_id_offset, float* cand_score, int32_t* cand_item,
+                                       const int32_t* excl_indptr, const int32_t* excl_ids,
+                                       const int32_t* excl_row_map, const float* user_half_sqnorm,
+                                       const float* item_half_sqnorm, void* stream) {
+  TRK_CHECK_ARG(n_tastes >= 1, "score_tastes: n_tastes=%d < 1", n_tastes);
+  TRK_CHECK_ARG(user_half_sqnorm != nullptr && item_half_sqnorm != nullptr,
+                "trk_score_topk_tastes_euclid_f16x3: null squared norms");
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k, n_splits,
+                        item_id_offset, cand_score, cand_item, nullptr, excl_indptr, excl_ids, excl_row_map,
+                        user_half_sqnorm, item_half_sqnorm};
   a.n_tastes = n_tastes;
   a.attention = attention;
   return trk::score_tc(a, trk::as_stream(stream));
@@ -340,6 +377,27 @@ int trk_score_topk_wide_tastes_f16x3(const void* user_split, const float* user_s
   a.excl_indptr = excl_indptr;
   a.excl_ids = excl_ids;
   a.excl_row_map = excl_row_map;
+  a.n_tastes = n_tastes;
+  a.attention = attention;
+  a.wide = true;
+  a.list_count = list_count;
+  return trk::score_tc(a, trk::as_stream(stream));
+}
+
+int trk_score_topk_wide_tastes_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                            int32_t n_tastes, int32_t attention, const void* item_split,
+                                            const float* item_meta, int64_t n_users, int64_t n_items, int32_t d_pad,
+                                            int32_t k, int32_t n_splits, int32_t item_id_offset, float* list_score,
+                                            int32_t* list_item, int32_t* list_count, const int32_t* excl_indptr,
+                                            const int32_t* excl_ids, const int32_t* excl_row_map,
+                                            const float* user_half_sqnorm, const float* item_half_sqnorm,
+                                            void* stream) {
+  TRK_CHECK_ARG(n_tastes >= 1, "score_tastes: n_tastes=%d < 1", n_tastes);
+  TRK_CHECK_ARG(user_half_sqnorm != nullptr && item_half_sqnorm != nullptr,
+                "trk_score_topk_wide_tastes_euclid_f16x3: null squared norms");
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, k, n_splits,
+                        item_id_offset, list_score, list_item, nullptr, excl_indptr, excl_ids, excl_row_map,
+                        user_half_sqnorm, item_half_sqnorm};
   a.n_tastes = n_tastes;
   a.attention = attention;
   a.wide = true;
@@ -407,6 +465,27 @@ int trk_score_count_tastes_f16x3(const void* user_split, const float* user_scale
   trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, 0, n_splits,
                         item_id_offset};
   set_count(a, pair_indptr, pair_ids, pair_score, pair_count, block_pairs, pass, excl_indptr, excl_ids, excl_row_map);
+  a.n_tastes = n_tastes;
+  a.attention = attention;
+  return trk::score_tc(a, trk::as_stream(stream));
+}
+
+int trk_score_count_tastes_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                        int32_t n_tastes, int32_t attention, const void* item_split,
+                                        const float* item_meta, int64_t n_users, int64_t n_items, int32_t d_pad,
+                                        int32_t n_splits, int32_t item_id_offset, const int32_t* pair_indptr,
+                                        const int32_t* pair_ids, float* pair_score, int32_t* pair_count,
+                                        const int32_t* block_pairs, int32_t pass, const int32_t* excl_indptr,
+                                        const int32_t* excl_ids, const int32_t* excl_row_map,
+                                        const float* user_half_sqnorm, const float* item_half_sqnorm, void* stream) {
+  TRK_CHECK_ARG(n_tastes >= 1, "score_tastes: n_tastes=%d < 1", n_tastes);
+  TRK_CHECK_ARG(user_half_sqnorm != nullptr && item_half_sqnorm != nullptr,
+                "trk_score_count_tastes_euclid_f16x3: null squared norms");
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, item_meta, n_users, n_items, d_pad, 0, n_splits,
+                        item_id_offset};
+  set_count(a, pair_indptr, pair_ids, pair_score, pair_count, block_pairs, pass, excl_indptr, excl_ids, excl_row_map);
+  a.user_half_sqnorm = user_half_sqnorm;
+  a.item_half_sqnorm = item_half_sqnorm;
   a.n_tastes = n_tastes;
   a.attention = attention;
   return trk::score_tc(a, trk::as_stream(stream));

@@ -22,12 +22,13 @@
 //                 compare is strict, so equal scores keep the lower item id first -- tf.nn.top_k's order.
 //
 // Score forms (ScoreForm, one template parameter; DESIGN.md §3.7): dot / cosine as above, Euclidean similarity (§3.4),
-// and mixtures of tastes collapsed by a max or by attention (§3.5).  Modes (TcMode): the dense matrix, the top-k above
+// and mixtures of tastes collapsed by a max or by attention (§3.5), of dot products or of Euclidean similarities
+// (§3.12).  Modes (TcMode): the dense matrix, the top-k above
 // (k <= 32), or the wide top-k (k <= 1024, DESIGN.md §3.8), where every (row, column half) keeps its list in global
 // memory and a warp compacts a full list to its exact top k, or the counting mode (DESIGN.md §3.9), which captures the
 // scores of listed (user, item) pairs and counts the columns that outrank each of them.  score_tc is the one host
 // entry point behind every trk_score_{topk,dense,count}* function: it validates the arguments and launches one of the
-// 40 instantiations.
+// 56 instantiations.
 #include "common.cuh"
 
 namespace trk {
@@ -86,14 +87,24 @@ enum ScoreForm {
   kFormEuclid,            // Euclidean similarity (score_chunk_euclid, TcEuclid)
   kFormTastesMax,         // pred = max_t u_t . i        (recommendation_graphs.py:107; collapse_chunk, TcTastes)
   kFormTastesAttention,   // pred = sum_t softmax_t(a_t . i) u_t . i   (:96-103)
+  kFormTastesEuclidMax,        // pred = max_t e(u_t, i),  e(x, i) = -|x - i|   (DESIGN.md §3.12)
+  kFormTastesEuclidAttention,  // pred = sum_t softmax_t(e(a_t, i)) e(u_t, i)
 };
-__host__ __device__ constexpr bool is_tastes(ScoreForm f) { return f == kFormTastesMax || f == kFormTastesAttention; }
+__host__ __device__ constexpr bool is_tastes_euclid(ScoreForm f) {
+  return f == kFormTastesEuclidMax || f == kFormTastesEuclidAttention;
+}
+__host__ __device__ constexpr bool is_tastes(ScoreForm f) {
+  return f == kFormTastesMax || f == kFormTastesAttention || is_tastes_euclid(f);
+}
+// the forms that read item norms (TcEuclid)
+__host__ __device__ constexpr bool is_euclid(ScoreForm f) { return f == kFormEuclid || is_tastes_euclid(f); }
 
-// Euclidean similarity (kFormEuclid): -1/2 |row|^2 of every user row [n_users] and item column, as
-// operand_half_sqnorm_kernel (similar_items.cu) computes them from the split operands -- the norms see exactly the values
-// the dot product sees.  The epilogue reads item norms for whole 128-column tiles, so item_half_sqnorm holds
-// n_items_padded256 entries, 0 beyond n_items (finite: the meta's -inf bias still gives those columns -inf).  Also a
-// kernel parameter of its own, for the same reason as TcExcl.
+// Euclidean similarity (kFormEuclid and the Euclidean tastes forms): -1/2 |row|^2 of every user operand row -- [n_users],
+// or [n_ops, n_users] for a mixture of tastes -- and of every item column, as operand_half_sqnorm_kernel
+// (similar_items.cu) computes them from the split operands -- the norms see exactly the values the dot product sees.
+// The epilogue reads item norms for whole 128-column tiles, so item_half_sqnorm holds n_items_padded256 entries, 0
+// beyond n_items (finite: the meta's -inf bias still gives those columns -inf).  Also a kernel parameter of its own,
+// for the same reason as TcExcl.
 struct TcEuclid {
   const float* user_half_sqnorm;
   const float* item_half_sqnorm;
@@ -230,10 +241,20 @@ __device__ __forceinline__ float score_chunk_euclid(uint32_t (&r)[32], const flo
 //   max:        pred = max_t p_t;
 //   attention:  m = max_t a_t,  e_t = expf(a_t - m),  s = sum_t e_t,  pred = sum_t p_t * (e_t / s)  (taste order);
 //   score = (pred + ub) + ib.
-// With attention, e_t is parked in a_t's staging row between the two passes.
+// With attention, e_t is parked in a_t's staging row between the two passes.  The Euclidean tastes forms (DESIGN.md
+// §3.12) give every operand row -- taste rows and attention rows alike, as the reference feeds both through the
+// prediction graph -- its similarity e_j = -sqrt(max(d2_j, 1e-16)), d2_j = (|x_j|^2 - 2 p_j) + |i|^2.  With attention
+// the e_j replace the staged accumulators first and are collapsed as above (operand_value then reads them as they
+// are); the max form takes pred = -sqrt(max(min_t d2_t, 1e-16)), the same value with one root instead of T.
 template <ScoreForm kForm>
-__device__ __forceinline__ void collapse_chunk(float* stage, int wt, int c, const float2* meta, const TcParams& p,
-                                               const TcTastes z, int64_t u0) {
+__device__ __forceinline__ float operand_value(float staged, float scales) {
+  if constexpr (is_tastes_euclid(kForm)) return staged;
+  else return __fmul_rn(staged, scales);
+}
+
+template <ScoreForm kForm>
+__device__ __forceinline__ void collapse_chunk(float* stage, int wt, int c, const float2* meta, const float* ihsq,
+                                               const TcParams& p, const TcEuclid& ev, const TcTastes z, int64_t u0) {
   const int lane = wt % 32;
   const int n_tastes = z.n_tastes;
   for (int e = wt / 32; e < 2 * z.per_wg; e += kConsumerThreads / 32) {   // warp-uniform: one (half, user) per warp
@@ -245,17 +266,32 @@ __device__ __forceinline__ void collapse_chunk(float* stage, int wt, int c, cons
     float* col = stage + (h * kWgRows + q) * kStageStride + lane;   // operand j at col[j * per_wg * kStageStride]
     const int64_t op_stride = z.per_wg * kStageStride;
     float pred;
+    if constexpr (is_tastes_euclid(kForm)) {
+      // |x_j|^2 = -2 (-1/2 |x_j|^2), |i|^2 and 2 p_j are exact; every sum is rounded on its own; sqrtf is correctly
+      // rounded, so -sqrtf(max(., 1e-16)) is non-increasing and the largest e_t is the root of the smallest d2_t
+      const float isq = -2.0f * __ldg(ihsq + h * 64 + c * 32 + lane);
+      float d2_min = __int_as_float(0x7f800000);
+      for (int j = 0; j < z.n_ops; ++j) {
+        const float sj = u_ok ? __ldg(p.user_scale + j * p.n_users + u) : 0.0f;
+        const float xsq = u_ok ? -2.0f * __ldg(ev.user_half_sqnorm + j * p.n_users + u) : 0.0f;
+        const float pj = __fmul_rn(col[j * op_stride], m.x * sj);
+        const float d2 = __fadd_rn(__fsub_rn(xsq, __fmul_rn(2.0f, pj)), isq);
+        if constexpr (kForm == kFormTastesEuclidMax) d2_min = fminf(d2_min, d2);
+        else col[j * op_stride] = -sqrtf(fmaxf(d2, 1e-16f));
+      }
+      if constexpr (kForm == kFormTastesEuclidMax) pred = -sqrtf(fmaxf(d2_min, 1e-16f));
+    }
     if constexpr (kForm == kFormTastesMax) {
       pred = -__int_as_float(0x7f800000);
       for (int t = 0; t < n_tastes; ++t) {
         const float su = u_ok ? __ldg(p.user_scale + t * p.n_users + u) : 0.0f;
-        pred = fmaxf(pred, __fmul_rn(col[t * op_stride], m.x * su));
+        pred = fmaxf(pred, operand_value<kForm>(col[t * op_stride], m.x * su));
       }
-    } else {
+    } else if constexpr (kForm != kFormTastesEuclidMax) {
       float amax = -__int_as_float(0x7f800000);
       for (int t = 0; t < n_tastes; ++t) {
         const float sa = u_ok ? __ldg(p.user_scale + (n_tastes + t) * p.n_users + u) : 0.0f;
-        const float a = __fmul_rn(col[(n_tastes + t) * op_stride], m.x * sa);
+        const float a = operand_value<kForm>(col[(n_tastes + t) * op_stride], m.x * sa);
         col[(n_tastes + t) * op_stride] = a;
         amax = fmaxf(amax, a);
       }
@@ -268,7 +304,7 @@ __device__ __forceinline__ void collapse_chunk(float* stage, int wt, int c, cons
       pred = 0.0f;
       for (int t = 0; t < n_tastes; ++t) {
         const float su = u_ok ? __ldg(p.user_scale + t * p.n_users + u) : 0.0f;
-        const float pt = __fmul_rn(col[t * op_stride], m.x * su);
+        const float pt = operand_value<kForm>(col[t * op_stride], m.x * su);
         const float w = __fdiv_rn(col[(n_tastes + t) * op_stride], sum);
         pred = t == 0 ? __fmul_rn(pt, w) : __fadd_rn(pred, __fmul_rn(pt, w));
       }
@@ -823,7 +859,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
         // ---- epilogue: two rounds, each stages columns [32 c, 32 c + 32) of both 64-column halves ----
         const int32_t id0 = p.item_id_offset + t * kBlockN;
         const float2* meta = p.item_meta + static_cast<int64_t>(t) * kBlockN;
-        const float* ihsq = kForm == kFormEuclid ? e.item_half_sqnorm + static_cast<int64_t>(t) * kBlockN : nullptr;
+        const float* ihsq = is_euclid(kForm) ? e.item_half_sqnorm + static_cast<int64_t>(t) * kBlockN : nullptr;
 #pragma unroll
         for (int c = 0; c < 2; ++c) {
           named_barrier_sync(1 + g, kConsumerThreads);   // the previous round's rows have been read
@@ -836,7 +872,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
           }
           named_barrier_sync(1 + g, kConsumerThreads);
           if constexpr (is_tastes(kForm)) {   // row q of each half now holds user q's final scores
-            collapse_chunk<kForm>(acc_stage, wt, c, meta, p, z, u0);
+            collapse_chunk<kForm>(acc_stage, wt, c, meta, ihsq, p, e, z, u0);
             named_barrier_sync(1 + g, kConsumerThreads);
           }
           uint32_t r[32];
@@ -1002,7 +1038,7 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
     // (one operand row per user is the plain kernel: per_wg would exceed the 32 rows of a dense store tile)
     TRK_CHECK_ARG(a.n_tastes >= 2 || (a.n_tastes == 1 && a.attention),
                   "score_tastes: n_tastes=%d needs n_tastes >= 2 or attention", a.n_tastes);
-    TRK_CHECK_ARG(!euclid && a.n_users_live == nullptr, "score_tastes: no Euclidean form and no live-row count");
+    TRK_CHECK_ARG(a.n_users_live == nullptr, "score_tastes: no live-row count");
     const int n_ops = a.n_tastes <= 64 ? (a.attention ? 2 : 1) * a.n_tastes : 65;
     if (n_ops > kWgRows) {
       set_error("score_tastes: %d operand rows per user (n_tastes=%d%s) exceed %d", n_ops, a.n_tastes,
@@ -1011,25 +1047,39 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
     }
     z = {n_ops, a.n_tastes, kWgRows / n_ops};
   }
-  const ScoreForm form = tastes ? (a.attention ? kFormTastesAttention : kFormTastesMax)
+  const ScoreForm form = tastes ? (euclid ? (a.attention ? kFormTastesEuclidAttention : kFormTastesEuclidMax)
+                                          : (a.attention ? kFormTastesAttention : kFormTastesMax))
                                 : (euclid ? kFormEuclid : kFormDot);
   // every instantiation: [dense | top-k | top-k with exclusion | wide | wide with exclusion | count][form][d_pad / 64 - 1]
-  // (the wide mode exists for the forms without a wide filter: Euclidean similarity and attention; the counting mode
-  // takes its exclusion lists at run time)
-  static constexpr const TcKernelFn* kKernels[6][4] = {
+  // (the wide mode exists for the forms without a wide filter: Euclidean similarity and attention; a Euclidean mixture
+  // of tastes without attention ranks its top k per taste, so its max form has no top-k or wide instantiation; the
+  // counting mode takes its exclusion lists at run time)
+  static constexpr const TcKernelFn* kKernels[6][6] = {
       {TcKernel<kModeDense, false, kFormDot>::fn, TcKernel<kModeDense, false, kFormEuclid>::fn,
-       TcKernel<kModeDense, false, kFormTastesMax>::fn, TcKernel<kModeDense, false, kFormTastesAttention>::fn},
+       TcKernel<kModeDense, false, kFormTastesMax>::fn, TcKernel<kModeDense, false, kFormTastesAttention>::fn,
+       TcKernel<kModeDense, false, kFormTastesEuclidMax>::fn,
+       TcKernel<kModeDense, false, kFormTastesEuclidAttention>::fn},
       {TcKernel<kModeTopk, false, kFormDot>::fn, TcKernel<kModeTopk, false, kFormEuclid>::fn,
-       TcKernel<kModeTopk, false, kFormTastesMax>::fn, TcKernel<kModeTopk, false, kFormTastesAttention>::fn},
+       TcKernel<kModeTopk, false, kFormTastesMax>::fn, TcKernel<kModeTopk, false, kFormTastesAttention>::fn, nullptr,
+       TcKernel<kModeTopk, false, kFormTastesEuclidAttention>::fn},
       {TcKernel<kModeTopk, true, kFormDot>::fn, TcKernel<kModeTopk, true, kFormEuclid>::fn,
-       TcKernel<kModeTopk, true, kFormTastesMax>::fn, TcKernel<kModeTopk, true, kFormTastesAttention>::fn},
-      {nullptr, TcKernel<kModeWide, false, kFormEuclid>::fn, nullptr, TcKernel<kModeWide, false, kFormTastesAttention>::fn},
-      {nullptr, TcKernel<kModeWide, true, kFormEuclid>::fn, nullptr, TcKernel<kModeWide, true, kFormTastesAttention>::fn},
+       TcKernel<kModeTopk, true, kFormTastesMax>::fn, TcKernel<kModeTopk, true, kFormTastesAttention>::fn, nullptr,
+       TcKernel<kModeTopk, true, kFormTastesEuclidAttention>::fn},
+      {nullptr, TcKernel<kModeWide, false, kFormEuclid>::fn, nullptr, TcKernel<kModeWide, false, kFormTastesAttention>::fn,
+       nullptr, TcKernel<kModeWide, false, kFormTastesEuclidAttention>::fn},
+      {nullptr, TcKernel<kModeWide, true, kFormEuclid>::fn, nullptr, TcKernel<kModeWide, true, kFormTastesAttention>::fn,
+       nullptr, TcKernel<kModeWide, true, kFormTastesEuclidAttention>::fn},
       {TcKernel<kModeCount, true, kFormDot>::fn, TcKernel<kModeCount, true, kFormEuclid>::fn,
-       TcKernel<kModeCount, true, kFormTastesMax>::fn, TcKernel<kModeCount, true, kFormTastesAttention>::fn}};
+       TcKernel<kModeCount, true, kFormTastesMax>::fn, TcKernel<kModeCount, true, kFormTastesAttention>::fn,
+       TcKernel<kModeCount, true, kFormTastesEuclidMax>::fn,
+       TcKernel<kModeCount, true, kFormTastesEuclidAttention>::fn}};
   const int mode_row = a.count ? 5 : a.dense ? 0 : (a.wide ? 3 : 1) + (a.excl_indptr != nullptr ? 1 : 0);
   if (kKernels[mode_row][form] == nullptr) {
-    set_error("score_topk_wide: the wide mode serves the Euclidean and attention forms only");
+    if (form == kFormTastesEuclidMax)
+      set_error("score_topk: a Euclidean mixture of tastes without attention has no one-sweep top-k: rank each taste "
+                "on trk_score_topk%s_euclid_f16x3 and merge the lists", a.wide ? "_wide" : "");
+    else
+      set_error("score_topk_wide: the wide mode serves the Euclidean and attention forms only");
     return TRK_ERR_UNSUPPORTED;
   }
 

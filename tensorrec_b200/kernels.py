@@ -351,10 +351,20 @@ def tastes_plan(n_tastes, attention):
     return per_wg, 2 * per_wg, n_ops * per_wg
 
 
+def _tastes_entry(name, users, item_hsq):
+    """The entry point of a mixture of tastes (name: trk_score_<mode>_tastes) and its trailing norm arguments: the
+    Euclidean form (..._tastes_euclid_f16x3, users.hsq and item_hsq) when item_hsq is given."""
+    if item_hsq is None:
+        return name + '_f16x3', ()
+    if users.hsq is None:
+        raise ValueError('a Euclidean mixture of tastes needs the operand norms (SideOperands.hsq)')
+    return name + '_euclid_f16x3', (_p(users.hsq), _p(item_hsq))
+
+
 def score_topk_tastes(users, items, meta, n_tastes, attention, k, n_splits=None, item_id_offset=0, excl=None,
-                      excl_row_map=None):
-    """The fused top-k of a mixture of tastes (users: stacked SideOperands).  Returns (cand_score, cand_item)
-    [U, n_splits, k]."""
+                      excl_row_map=None, item_hsq=None):
+    """The fused top-k of a mixture of tastes (users: stacked SideOperands).  item_hsq (item_half_sqnorm(items)):
+    Euclidean prediction, with the operand norms users.hsq.  Returns (cand_score, cand_item) [U, n_splits, k]."""
     lib = require_cuda()
     n_users = users.n_rows
     if n_splits is None:
@@ -363,31 +373,34 @@ def score_topk_tastes(users, items, meta, n_tastes, attention, k, n_splits=None,
     cand_score = torch.empty((n_users, n_splits, k), dtype=torch.float32, device=dev)
     cand_item = torch.empty((n_users, n_splits, k), dtype=torch.int32, device=dev)
     ex = (None, None, None) if excl is None else (_p(excl.indptr), _p(excl.ids), _p(excl_row_map))
-    rc = lib.trk_score_topk_tastes_f16x3(_p(users.split), _p(users.scale), _p(users.bias), int(n_tastes),
-                                         1 if attention else 0, _p(items.split), _p(meta), n_users, items.n_rows,
-                                         int(users.d_pad), int(k), int(n_splits), int(item_id_offset), _p(cand_score),
-                                         _p(cand_item), *ex, _stream())
-    _lib.check(rc, 'trk_score_topk_tastes_f16x3')
+    name, norms = _tastes_entry('trk_score_topk_tastes', users, item_hsq)
+    rc = getattr(lib, name)(_p(users.split), _p(users.scale), _p(users.bias), int(n_tastes), 1 if attention else 0,
+                            _p(items.split), _p(meta), n_users, items.n_rows, int(users.d_pad), int(k), int(n_splits),
+                            int(item_id_offset), _p(cand_score), _p(cand_item), *ex, *norms, _stream())
+    _lib.check(rc, name)
     return cand_score, cand_item
 
 
-def topk_tastes(users, items, n_tastes, attention, k, n_splits=None, item_id_offset=0, excl=None, out=None):
-    """Fused top-k of a mixture of tastes + merge -> PackedTopK [U, k]."""
+def topk_tastes(users, items, n_tastes, attention, k, n_splits=None, item_id_offset=0, excl=None, out=None,
+                item_hsq=None):
+    """Fused top-k of a mixture of tastes + merge -> PackedTopK [U, k].  item_hsq: as for score_topk_tastes."""
     meta = pack_item_meta(items.scale, items.bias, items.n_rows)
     cs, ci = score_topk_tastes(users, items, meta, n_tastes, attention, k, n_splits=n_splits,
-                               item_id_offset=item_id_offset, excl=excl)
+                               item_id_offset=item_id_offset, excl=excl, item_hsq=item_hsq)
     return topk_merge(cs, ci, k, out=out)
 
 
-def score_dense_tastes(users, item_split, item_meta, n_items, n_tastes, attention, out=None):
-    """Dense scores [U, n_items] of a mixture of tastes (users: stacked SideOperands)."""
+def score_dense_tastes(users, item_split, item_meta, n_items, n_tastes, attention, out=None, item_hsq=None):
+    """Dense scores [U, n_items] of a mixture of tastes (users: stacked SideOperands).  item_hsq: as for
+    score_topk_tastes."""
     lib = require_cuda()
     if out is None:
         out = torch.empty((users.n_rows, n_items), dtype=torch.float32, device=users.split.device)
-    rc = lib.trk_score_dense_tastes_f16x3(_p(users.split), _p(users.scale), _p(users.bias), int(n_tastes),
-                                          1 if attention else 0, _p(item_split), _p(item_meta), users.n_rows, n_items,
-                                          int(users.d_pad), _p(out), out.stride(0), _stream())
-    _lib.check(rc, 'trk_score_dense_tastes_f16x3')
+    name, norms = _tastes_entry('trk_score_dense_tastes', users, item_hsq)
+    rc = getattr(lib, name)(_p(users.split), _p(users.scale), _p(users.bias), int(n_tastes), 1 if attention else 0,
+                            _p(item_split), _p(item_meta), users.n_rows, n_items, int(users.d_pad), _p(out),
+                            out.stride(0), *norms, _stream())
+    _lib.check(rc, name)
     return out
 
 
@@ -679,12 +692,13 @@ def to_host(*tensors):
 
 class SideOperands(object):
     """Everything the score kernels need from one side (users or items), all resident on the device.
-    norm: row norms (users, filter path); stats: float32[3] max norm / max scale / max |bias| (items, filter path)."""
+    norm: row norms (users, filter path); stats: float32[3] max norm / max scale / max |bias| (items, filter path);
+    hsq: -1/2 |x|^2 of every operand row of a stacked operand, [n_ops, U] (a Euclidean mixture of tastes)."""
 
-    def __init__(self, repr_f32, split, scale, bias, n_rows, d, d_pad, norm=None, stats=None):
+    def __init__(self, repr_f32, split, scale, bias, n_rows, d, d_pad, norm=None, stats=None, hsq=None):
         self.repr_f32, self.split, self.scale, self.bias = repr_f32, split, scale, bias
         self.n_rows, self.d, self.d_pad = n_rows, d, d_pad
-        self.norm, self.stats = norm, stats
+        self.norm, self.stats, self.hsq = norm, stats, hsq
 
     def rows(self, r0, r1):
         """The operands of rows [r0, r1) (views)."""
@@ -1031,9 +1045,11 @@ def topk_exact_wide(users, items, k, n_splits=None, item_id_offset=0, out=None, 
     return select_topk_lists(list_s, list_i, count, k, out=out)
 
 
-def topk_tastes_wide(users, items, n_tastes, attention, k, n_splits=None, item_id_offset=0, excl=None, out=None):
+def topk_tastes_wide(users, items, n_tastes, attention, k, n_splits=None, item_id_offset=0, excl=None, out=None,
+                     item_hsq=None):
     """topk_tastes for any 1 <= k <= 1024 on the exact kernel's wide mode (attention only: a mixture of tastes without
-    attention takes the wide filter) -> PackedTopK [U, k]."""
+    attention takes the wide filter, or one Euclidean sweep per taste) -> PackedTopK [U, k].  item_hsq: as for
+    score_topk_tastes."""
     lib = require_cuda()
     n_users = users.n_rows
     if n_splits is None:
@@ -1041,11 +1057,11 @@ def topk_tastes_wide(users, items, n_tastes, attention, k, n_splits=None, item_i
     meta = pack_item_meta(items.scale, items.bias, items.n_rows)
     list_s, list_i, count = _exact_wide_lists(n_users, n_splits, k, users.split.device)
     ex = (None, None, None) if excl is None else (_p(excl.indptr), _p(excl.ids), None)
-    rc = lib.trk_score_topk_wide_tastes_f16x3(_p(users.split), _p(users.scale), _p(users.bias), int(n_tastes),
-                                              1 if attention else 0, _p(items.split), _p(meta), n_users, items.n_rows,
-                                              int(users.d_pad), int(k), int(n_splits), int(item_id_offset), _p(list_s),
-                                              _p(list_i), _p(count), *ex, _stream())
-    _lib.check(rc, 'trk_score_topk_wide_tastes_f16x3')
+    name, norms = _tastes_entry('trk_score_topk_wide_tastes', users, item_hsq)
+    rc = getattr(lib, name)(_p(users.split), _p(users.scale), _p(users.bias), int(n_tastes), 1 if attention else 0,
+                            _p(items.split), _p(meta), n_users, items.n_rows, int(users.d_pad), int(k), int(n_splits),
+                            int(item_id_offset), _p(list_s), _p(list_i), _p(count), *ex, *norms, _stream())
+    _lib.check(rc, name)
     return select_topk_lists(list_s, list_i, count, k, out=out)
 
 
@@ -1167,7 +1183,8 @@ def count_listed_pairs(users, items, meta, indptr, ids, block_rows, excl=None, i
     """Counting mode of the exact kernel over the users of `users` (SideOperands; a mixture of tastes: the stacked
     operand and tastes = (n_tastes, attention)).  indptr / ids: host int32 CSR of the listed pairs, ids LOCAL and
     ascending per row; block_rows: the kernel's user block (128, or 2P for a mixture of tastes); excl: DeviceExclusion
-    of the same rows or None; item_hsq: item_half_sqnorm(items) for a Euclidean model.  Returns (int32 counts [nnz] on
+    of the same rows or None; item_hsq: item_half_sqnorm(items) for a Euclidean model (a Euclidean mixture of tastes:
+    with the operand norms users.hsq).  Returns (int32 counts [nnz] on
     the device in the order of ids -- rank = 1 + count --, passes)."""
     lib = require_cuda()
     dev = users.split.device
@@ -1182,15 +1199,17 @@ def count_listed_pairs(users, items, meta, indptr, ids, block_rows, excl=None, i
     up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev, non_blocking=True)   # noqa: E731
     d_indptr, d_ids, d_block_max = up(indptr), up(ids), up(block_max)
     ex = (None, None, None) if excl is None else (_p(excl.indptr), _p(excl.ids), None)
-    user_hsq = None if item_hsq is None else operand_half_sqnorm(users.split, users.scale, users.d_pad)
+    user_hsq = None
+    if item_hsq is not None and tastes is None:
+        user_hsq = operand_half_sqnorm(users.split, users.scale, users.d_pad)
 
     def launch(pair_ids, pair_score, pair_count, pass_):
         head = (_p(users.split), _p(users.scale), _p(users.bias))
         lists = (_p(d_indptr), _p(pair_ids), _p(pair_score), _p(pair_count), _p(d_block_max), int(pass_)) + ex
         shape = (n_users, n_items, int(users.d_pad), int(n_splits), 0)
         if tastes is not None:
-            name = 'trk_score_count_tastes_f16x3'
-            args = head + (int(tastes[0]), 1 if tastes[1] else 0, _p(items.split), _p(meta)) + shape + lists
+            name, norms = _tastes_entry('trk_score_count_tastes', users, item_hsq)
+            args = head + (int(tastes[0]), 1 if tastes[1] else 0, _p(items.split), _p(meta)) + shape + lists + norms
         elif item_hsq is not None:
             name = 'trk_score_count_euclid_f16x3'
             args = head + (_p(items.split), _p(meta)) + shape + lists + (_p(user_hsq), _p(item_hsq))

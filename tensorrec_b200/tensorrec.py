@@ -73,13 +73,19 @@ EXACT_WIDE_MIN_ITEMS = 4096
 # RANK_AT_MIN_ITEMS items; below that, dense scoring and ranking of the user blocks (see README, "Ranks of listed
 # pairs").
 RANK_AT_MIN_ITEMS = 2048
+# Euclidean mixtures of tastes with attention count from RANK_AT_EUCLID_ATTENTION_MIN_ITEMS items: the capture and the
+# counting sweep each pay 2T roots and the softmax per pair, which costs more than one dense sweep and the sort on smaller
+# catalogues (see README, "Euclidean mixtures of tastes").
+RANK_AT_EUCLID_ATTENTION_MIN_ITEMS = 16384
 
 
-def rank_at_route(n_items, tensor_scored):
+def rank_at_route(n_items, tensor_scored, euclid_attention=False):
     """The route of a predict_rank_at call: 'exact3_count' when predict() scores the model on the exact tensor-core
     kernel (tensor_scored: TensorRec._tensor_score_form() is not None) and the catalogue has at least RANK_AT_MIN_ITEMS
-    items, 'dense+rank' otherwise."""
-    return 'exact3_count' if tensor_scored and n_items >= RANK_AT_MIN_ITEMS else 'dense+rank'
+    items (RANK_AT_EUCLID_ATTENTION_MIN_ITEMS for a Euclidean mixture of tastes with attention), 'dense+rank'
+    otherwise."""
+    floor = RANK_AT_EUCLID_ATTENTION_MIN_ITEMS if euclid_attention else RANK_AT_MIN_ITEMS
+    return 'exact3_count' if tensor_scored and n_items >= floor else 'dense+rank'
 
 
 def rank_at_blocks(indptr, unit, max_rows, max_pairs):
@@ -113,7 +119,7 @@ def topk_route(k, n_items, model_ok, single_taste, filter_max_k, exact_max_k, sh
     goes to dense+rank.  euclidean: a Euclidean user x item model (model_ok from _euclidean_tensor_ok), which has no
     filter or wide form: 'exact3' for k <= exact_max_k on catalogues of at least EUCLIDEAN_MIN_ITEMS items (any shard
     size in a sharded call), 'dense+rank' otherwise.  attention: a mixture of tastes with an attention graph (model_ok
-    from _tastes_tensor_ok), whose softmax has no filter or wide form either: the same rule with ATTENTION_MIN_ITEMS.
+    from _tastes_tensor_ok, or _euclid_tastes_tensor_ok for Euclidean prediction), whose softmax has no filter or wide form either: the same rule with ATTENTION_MIN_ITEMS.
     merge_max_k does not apply to either.  exact_wide_max_k: the largest k of the exact kernel's wide mode (0: none,
     WIDE_MAX_K: trk_score_topk_wide_*); Euclidean and attention models with exact_max_k < k <= exact_wide_max_k take
     'exact3_wide' on catalogues of at least EXACT_WIDE_MIN_ITEMS items (any shard size in a sharded call), with one
@@ -669,10 +675,20 @@ class TensorRec(object):
                 and kernels.tastes_plan(self.n_tastes, self.attention_graph_factory is not None) is not None
                 and kernels.d_pad_for(self.n_components) <= 128)
 
+    def _euclid_tastes_tensor_ok(self):
+        """Can the taste-collapsing tensor-core kernels evaluate this Euclidean mixture of tastes (DESIGN §3.12)?  The
+        built-in Euclidean graph, n_tastes >= 2 within the kernel's operand rows (T <= 64, T <= 32 with attention), any
+        attention graph or none, d_pad <= 128."""
+        return (SCORE_PATH != 'exact' and type(self.prediction_graph_factory) is EuclideanSimilarityPredictionGraph
+                and self.n_tastes >= 2
+                and kernels.tastes_plan(self.n_tastes, self.attention_graph_factory is not None) is not None
+                and kernels.d_pad_for(self.n_components) <= 128)
+
     def _taste_operands(self, block_in, device):
         """The users of a mixture of tastes as kernels.SideOperands whose split is the stacked operand [n_ops, U,
         2 d_pad] (u_0 .. u_{T-1}, then a_0 .. a_{T-1} with attention) and scale [n_ops, U]; K1 writes every operand
-        straight into its slice, normalised as the CUDA-core path normalises it."""
+        straight into its slice, normalised as the CUDA-core path normalises it.  With Euclidean prediction, hsq holds
+        the half squared norms of every slice [n_ops, U] (one operand_half_sqnorm launch over the stacked rows)."""
         extra = 1 if type(self.prediction_graph_factory) is CosineSimilarityPredictionGraph else 0
         d_pad = kernels.d_pad_for(self.n_components)
         rows = block_in.shape[0]
@@ -685,7 +701,11 @@ class TensorRec(object):
             self._represent(graph, block_in, self.n_user_features, name, device, extra, want_f32=False,
                             split_d_pad=d_pad, split_out=(split[j], scale[j]))
         bias = self._projected_biases(block_in, 'feature_biases_user', device) if self.biased else None
-        return kernels.SideOperands(None, split, scale, bias, rows, self.n_components, d_pad)
+        hsq = None
+        if type(self.prediction_graph_factory) is EuclideanSimilarityPredictionGraph:
+            hsq = kernels.operand_half_sqnorm(split.view(len(ops) * rows, 2 * d_pad), scale.view(-1), d_pad)
+            hsq = hsq.view(len(ops), rows)
+        return kernels.SideOperands(None, split, scale, bias, rows, self.n_components, d_pad, hsq=hsq)
 
     def _side_operands(self, side, sparse_in, device, for_filter=False, taste=0):
         """One side ('user' or 'item') as kernels.SideOperands: split-fp16 operand + scale, projected biases and -- for
@@ -714,9 +734,11 @@ class TensorRec(object):
 
     def _tensor_score_form(self):
         """How _score_plan scores this model on the exact tensor-core kernel: 'tastes' (the taste-collapsing form),
-        'euclidean' or 'dot' (dot / cosine); None when it scores it otherwise."""
+        'tastes_euclid' (its Euclidean form), 'euclidean' or 'dot' (dot / cosine); None when it scores it otherwise."""
         if self._tastes_tensor_ok():      # (checked first: SCORE_PATH='tensor' accepts these models)
             return 'tastes'
+        if self._euclid_tastes_tensor_ok():
+            return 'tastes_euclid'
         if self.n_tastes == 1 and self._euclidean_tensor_ok():
             return 'euclidean'
         return 'dot' if self._tensor_path_ok() else None
@@ -728,14 +750,15 @@ class TensorRec(object):
         otherwise."""
         n_items = item_in.shape[0]
         form = self._tensor_score_form()
-        if form == 'tastes':
+        if form in ('tastes', 'tastes_euclid'):
             items = self._side_operands('item', item_in, device)
             meta = kernels.pack_item_meta(items.scale, items.bias, n_items)
+            item_hsq = kernels.item_half_sqnorm(items) if form == 'tastes_euclid' else None
             attention = self.attention_graph_factory is not None
 
             def score(block_in, out=None):
                 return kernels.score_dense_tastes(self._taste_operands(block_in, device), items.split, meta, n_items,
-                                                  self.n_tastes, attention, out=out)
+                                                  self.n_tastes, attention, out=out, item_hsq=item_hsq)
             return score
         euclidean = form == 'euclidean'
         if form is not None:
@@ -957,7 +980,8 @@ class TensorRec(object):
         self._check_features(item_in, self.n_item_features, 'item')
         indptr, ids = kernels.exclusion_host_csr(pairs, 0, n_items)   # the listing rule is the exclusion rule
         form = self._tensor_score_form()
-        path = rank_at_route(n_items, form is not None)
+        attention = self.attention_graph_factory is not None
+        path = rank_at_route(n_items, form is not None, euclid_attention=form == 'tastes_euclid' and attention)
         self.last_rank_info = {'path': path, 'passes': 0}
         ranks = np.zeros(ids.shape[0], dtype=np.int32)
         result = lambda: sp.csr_matrix((ranks, ids, indptr), shape=(n_users, n_items))   # noqa: E731
@@ -965,11 +989,13 @@ class TensorRec(object):
             return result()
         device = self._cuda_device()
 
-        attention = self.attention_graph_factory is not None
-        unit = kernels.tastes_plan(self.n_tastes, attention)[1] if form == 'tastes' else kernels.TILE_USERS
+        tastes_form = form in ('tastes', 'tastes_euclid')
+        unit = kernels.tastes_plan(self.n_tastes, attention)[1] if tastes_form else kernels.TILE_USERS
         if path == 'exact3_count':
-            n_ops = kernels.tastes_n_ops(self.n_tastes, attention) if form == 'tastes' else 1
-            per_row = n_ops * (4 * kernels.d_pad_for(self.n_components) + 8) + 16
+            n_ops = kernels.tastes_n_ops(self.n_tastes, attention) if tastes_form else 1
+            # (tastes_euclid: 4 more bytes per operand row for its half squared norm)
+            per_op = 4 * kernels.d_pad_for(self.n_components) + 8 + (4 if form == 'tastes_euclid' else 0)
+            per_row = n_ops * per_op + 16
         else:
             per_row = kernels.DENSE_RANK_BYTES_PER_PAIR * n_items
         max_rows = self.PREDICT_BLOCK_BYTES // per_row if user_batch_size is None else int(user_batch_size)
@@ -980,7 +1006,7 @@ class TensorRec(object):
         if path == 'exact3_count':
             items = self._side_operands('item', item_in, device)
             meta = kernels.pack_item_meta(items.scale, items.bias, n_items)
-            item_hsq = kernels.item_half_sqnorm(items) if form == 'euclidean' else None
+            item_hsq = kernels.item_half_sqnorm(items) if form in ('euclidean', 'tastes_euclid') else None
         else:
             score = self._score_plan(item_in, device)
         parts = []
@@ -993,7 +1019,7 @@ class TensorRec(object):
             excl = None if exclude is None else kernels.DeviceExclusion.upload(
                 *kernels.exclusion_host_csr(exclude, 0, n_items, u0, u1), device=device)
             if path == 'exact3_count':
-                if form == 'tastes':
+                if tastes_form:
                     users, tastes = self._taste_operands(block_in, device), (self.n_tastes, attention)
                 else:
                     users, tastes = self._side_operands('user', block_in, device), None
@@ -1029,7 +1055,7 @@ class TensorRec(object):
         result by a de-duplicating merge (last_topk_info['fallback_rows'] sums the tastes' fallback rows).  Euclidean
         models run k <= 32 on the exact kernel
         (catalogues of at least EUCLIDEAN_MIN_ITEMS items); so do mixtures of tastes with an attention graph
-        (ATTENTION_MIN_ITEMS), on the taste-collapsing kernel.  Both run 32 < k <= WIDE_MAX_K on the exact kernel's wide
+        (ATTENTION_MIN_ITEMS), on the taste-collapsing kernel, Euclidean prediction included.  Both run 32 < k <= WIDE_MAX_K on the exact kernel's wide
         mode on catalogues of at least EXACT_WIDE_MIN_ITEMS items (a Euclidean mixture of tastes: one sweep per taste,
         folded as on the wide route), and otherwise on dense+rank with tensor-core scoring.
         last_topk_info['path'] names the route (topk_route).
@@ -1066,8 +1092,9 @@ class TensorRec(object):
 
         attention = self.attention_graph_factory is not None
         euclidean = self._euclidean_tensor_ok()      # (checked first: SCORE_PATH='tensor' accepts these models)
+        euclid_attention = attention and self._euclid_tastes_tensor_ok()
         if attention:
-            model_ok = self._tastes_tensor_ok()
+            model_ok = self._tastes_tensor_ok() or euclid_attention
         else:
             model_ok = euclidean or self._tensor_path_ok(allow_tastes=True)
         path = self._topk_path(k, n_items, model_ok, self.n_tastes == 1,
@@ -1079,7 +1106,7 @@ class TensorRec(object):
             items = self._side_operands('item', item_in, device, for_filter=one_pass)
             if one_pass:
                 fitems = kernels.FilterItems(items)
-            if euclidean:
+            if euclidean or euclid_attention:
                 item_hsq = kernels.item_half_sqnorm(items)
 
         if user_batch_size is None:
@@ -1093,7 +1120,8 @@ class TensorRec(object):
                 # the softmax mixes the tastes: one sweep of the taste-collapsing kernel, no device-side fallback
                 users = self._taste_operands(block_in, device)
                 topk = kernels.topk_tastes_wide if route == 'exact3_wide' else kernels.topk_tastes
-                return topk(users, items, self.n_tastes, True, k, item_id_offset=item_id_offset, excl=excl), [(None, 0)]
+                return topk(users, items, self.n_tastes, True, k, item_id_offset=item_id_offset, excl=excl,
+                            item_hsq=item_hsq), [(None, 0)]
             # mixture of tastes (no attention): prediction = max over tastes (recommendation_graphs.py:107), so the top-k
             # lies in the union of the per-taste top-k lists: one fused sweep per taste, then a de-duplicating merge.
             # The wide routes (the wide filter, and the exact kernel's wide mode for Euclidean models) fold each taste's
