@@ -512,6 +512,49 @@ int trk_score_count_tastes_f16x3(const void* user_split, const float* user_scale
                                  const int32_t* excl_indptr, const int32_t* excl_ids, const int32_t* excl_row_map,
                                  void* stream);
 
+/* Pairs mode of the exact kernel: the scores of listed (user, item) pairs, each bit for bit the score
+ * trk_score_dense_{f16x3, euclid_f16x3, tastes_f16x3, tastes_euclid_f16x3} writes for the same users at the same rows
+ * (user row u of the call at accumulator row u mod 128, or u mod 2 floor(64 / n_ops) for a mixture of tastes), from
+ * item tiles gathered out of each user block's listed items (DESIGN.md §3.13):
+ *   tile_items [n_tiles, 128]  the item of every slot of every gathered tile; item i sits at column i mod 128 (its
+ *                              column in the dense sweep), -1 marks an empty slot;
+ *   work [n_work, 3]           (user block, first tile, end tile) of every work item: the block's rows are multiplied
+ *                              against the gathered tiles [first, end);
+ *   pair_indptr [n_users + 1], pair_cols  the pairs of user row u as VIRTUAL columns tile * 128 + column, ascending per
+ *                              row, every one inside a tile of a work item of u's block;
+ *   slot_meta [n_tiles * 128, 2]  {scale, bias} of every slot (trk_pack_item_meta's entries gathered by tile_items);
+ *   pair_score[pair]           the pair's score.
+ *   trk_score_pairs_f16x3                operands as trk_score_count_f16x3 (dot / cosine).
+ *   trk_score_pairs_euclid_f16x3         plus user_half_sqnorm and slot_half_sqnorm [n_tiles * 128], the item norms
+ *                                        gathered as slot_meta (Euclidean similarity).
+ *   trk_score_pairs_tastes_f16x3         operands as trk_score_count_tastes_f16x3 (mixtures of tastes).
+ *   trk_score_pairs_tastes_euclid_f16x3  as trk_score_pairs_tastes_f16x3 plus the operand norms [n_ops, n_users] and
+ *                                        slot_half_sqnorm (Euclidean mixtures of tastes, attention or not).
+ * Constraints: d_pad in {64, 128}; 1 <= n_tiles <= 2^24; n_work >= 1; slot_meta and slot_half_sqnorm 16-byte aligned. */
+int trk_score_pairs_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                          const void* item_split, const float* slot_meta, int64_t n_users, int64_t n_items,
+                          int32_t d_pad, const int32_t* pair_indptr, const int32_t* pair_cols, float* pair_score,
+                          const int32_t* tile_items, int32_t n_tiles, const int32_t* work, int32_t n_work,
+                          void* stream);
+int trk_score_pairs_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                 const void* item_split, const float* slot_meta, int64_t n_users, int64_t n_items,
+                                 int32_t d_pad, const int32_t* pair_indptr, const int32_t* pair_cols,
+                                 float* pair_score, const int32_t* tile_items, int32_t n_tiles, const int32_t* work,
+                                 int32_t n_work, const float* user_half_sqnorm, const float* slot_half_sqnorm,
+                                 void* stream);
+int trk_score_pairs_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                 int32_t n_tastes, int32_t attention, const void* item_split, const float* slot_meta,
+                                 int64_t n_users, int64_t n_items, int32_t d_pad, const int32_t* pair_indptr,
+                                 const int32_t* pair_cols, float* pair_score, const int32_t* tile_items,
+                                 int32_t n_tiles, const int32_t* work, int32_t n_work, void* stream);
+int trk_score_pairs_tastes_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                        int32_t n_tastes, int32_t attention, const void* item_split,
+                                        const float* slot_meta, int64_t n_users, int64_t n_items, int32_t d_pad,
+                                        const int32_t* pair_indptr, const int32_t* pair_cols, float* pair_score,
+                                        const int32_t* tile_items, int32_t n_tiles, const int32_t* work,
+                                        int32_t n_work, const float* user_half_sqnorm, const float* slot_half_sqnorm,
+                                        void* stream);
+
 /* Merges n_lists candidate lists per user (each sorted by (score desc, id asc), k_in entries) into the global
  * top k_out per user, same order.  Lists are the n_splits of one GPU and/or the shards received from the other GPUs
  * (item-axis sharding; the exchange itself is one NCCL all-to-all done by the host layer, SURVEY 8e).

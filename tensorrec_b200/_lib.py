@@ -79,6 +79,15 @@ SIGNATURES = {
     'trk_score_count_tastes_euclid_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i32, _c_i32, _c_p, _c_p, _c_i64, _c_i64,
                                                            _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_p, _c_p, _c_p, _c_i32,
                                                            _c_p, _c_p, _c_p, _c_p, _c_p, _c_p]),
+    'trk_score_pairs_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_p, _c_i64, _c_i64, _c_i32, _c_p, _c_p, _c_p,
+                                             _c_p, _c_i32, _c_p, _c_i32, _c_p]),
+    'trk_score_pairs_euclid_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_p, _c_i64, _c_i64, _c_i32, _c_p, _c_p,
+                                                    _c_p, _c_p, _c_i32, _c_p, _c_i32, _c_p, _c_p, _c_p]),
+    'trk_score_pairs_tastes_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i32, _c_i32, _c_p, _c_p, _c_i64, _c_i64,
+                                                    _c_i32, _c_p, _c_p, _c_p, _c_p, _c_i32, _c_p, _c_i32, _c_p]),
+    'trk_score_pairs_tastes_euclid_f16x3': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i32, _c_i32, _c_p, _c_p, _c_i64, _c_i64,
+                                                           _c_i32, _c_p, _c_p, _c_p, _c_p, _c_i32, _c_p, _c_i32, _c_p,
+                                                           _c_p, _c_p]),
     'trk_select_topk_lists': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i64, _c_i32, _c_i32, _c_i32, _c_p, _c_p, _c_i64,
                                              _c_p]),
     'trk_topk_merge': (ctypes.c_int, [_c_p, _c_p, _c_i64, _c_i32, _c_i32, _c_i32, _c_i64, _c_i64, _c_p, _c_p, _c_i64,

@@ -491,6 +491,80 @@ int trk_score_count_tastes_euclid_f16x3(const void* user_split, const float* use
   return trk::score_tc(a, trk::as_stream(stream));
 }
 
+namespace {
+
+// the pairs-mode fields of score_tc's arguments
+void set_pairs(trk::ScoreTcArgs& a, const int32_t* pair_indptr, const int32_t* pair_cols, float* pair_score,
+               const int32_t* tile_items, int32_t n_tiles, const int32_t* work, int32_t n_work) {
+  a.pairs = true;
+  a.pair_indptr = pair_indptr;
+  a.pair_ids = pair_cols;
+  a.pair_score = pair_score;
+  a.tile_items = tile_items;
+  a.n_tiles = n_tiles;
+  a.work = work;
+  a.n_work = n_work;
+}
+
+}  // namespace
+
+int trk_score_pairs_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                          const void* item_split, const float* slot_meta, int64_t n_users, int64_t n_items,
+                          int32_t d_pad, const int32_t* pair_indptr, const int32_t* pair_cols, float* pair_score,
+                          const int32_t* tile_items, int32_t n_tiles, const int32_t* work, int32_t n_work,
+                          void* stream) {
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, slot_meta, n_users, n_items, d_pad};
+  set_pairs(a, pair_indptr, pair_cols, pair_score, tile_items, n_tiles, work, n_work);
+  return trk::score_tc(a, trk::as_stream(stream));
+}
+
+int trk_score_pairs_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                 const void* item_split, const float* slot_meta, int64_t n_users, int64_t n_items,
+                                 int32_t d_pad, const int32_t* pair_indptr, const int32_t* pair_cols,
+                                 float* pair_score, const int32_t* tile_items, int32_t n_tiles, const int32_t* work,
+                                 int32_t n_work, const float* user_half_sqnorm, const float* slot_half_sqnorm,
+                                 void* stream) {
+  TRK_CHECK_ARG(user_half_sqnorm != nullptr && slot_half_sqnorm != nullptr,
+                "trk_score_pairs_euclid_f16x3: null squared norms");
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, slot_meta, n_users, n_items, d_pad};
+  set_pairs(a, pair_indptr, pair_cols, pair_score, tile_items, n_tiles, work, n_work);
+  a.user_half_sqnorm = user_half_sqnorm;
+  a.item_half_sqnorm = slot_half_sqnorm;
+  return trk::score_tc(a, trk::as_stream(stream));
+}
+
+int trk_score_pairs_tastes_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                 int32_t n_tastes, int32_t attention, const void* item_split, const float* slot_meta,
+                                 int64_t n_users, int64_t n_items, int32_t d_pad, const int32_t* pair_indptr,
+                                 const int32_t* pair_cols, float* pair_score, const int32_t* tile_items,
+                                 int32_t n_tiles, const int32_t* work, int32_t n_work, void* stream) {
+  TRK_CHECK_ARG(n_tastes >= 1, "score_tastes: n_tastes=%d < 1", n_tastes);
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, slot_meta, n_users, n_items, d_pad};
+  set_pairs(a, pair_indptr, pair_cols, pair_score, tile_items, n_tiles, work, n_work);
+  a.n_tastes = n_tastes;
+  a.attention = attention;
+  return trk::score_tc(a, trk::as_stream(stream));
+}
+
+int trk_score_pairs_tastes_euclid_f16x3(const void* user_split, const float* user_scale, const float* user_bias,
+                                        int32_t n_tastes, int32_t attention, const void* item_split,
+                                        const float* slot_meta, int64_t n_users, int64_t n_items, int32_t d_pad,
+                                        const int32_t* pair_indptr, const int32_t* pair_cols, float* pair_score,
+                                        const int32_t* tile_items, int32_t n_tiles, const int32_t* work,
+                                        int32_t n_work, const float* user_half_sqnorm, const float* slot_half_sqnorm,
+                                        void* stream) {
+  TRK_CHECK_ARG(n_tastes >= 1, "score_tastes: n_tastes=%d < 1", n_tastes);
+  TRK_CHECK_ARG(user_half_sqnorm != nullptr && slot_half_sqnorm != nullptr,
+                "trk_score_pairs_tastes_euclid_f16x3: null squared norms");
+  trk::ScoreTcArgs a = {user_split, user_scale, user_bias, item_split, slot_meta, n_users, n_items, d_pad};
+  set_pairs(a, pair_indptr, pair_cols, pair_score, tile_items, n_tiles, work, n_work);
+  a.user_half_sqnorm = user_half_sqnorm;
+  a.item_half_sqnorm = slot_half_sqnorm;
+  a.n_tastes = n_tastes;
+  a.attention = attention;
+  return trk::score_tc(a, trk::as_stream(stream));
+}
+
 int trk_select_topk_lists(const float* list_score, const int32_t* list_item, const int32_t* list_count,
                           int64_t n_rows, int32_t n_lists, int32_t list_width, int32_t k, float* out_score,
                           int32_t* out_item, int64_t out_row_stride, void* stream) {

@@ -96,6 +96,11 @@ struct ScoreTcArgs {
   int32_t* pair_count = nullptr;
   const int32_t* block_pairs = nullptr;
   int32_t pass = 0;
+  bool pairs = false;                 // pairs mode: the listed pairs' scores over gathered item tiles (pair_indptr,
+  const int32_t* tile_items = nullptr;   // pair_ids = virtual columns, pair_score; item_meta / item_half_sqnorm per slot)
+  int32_t n_tiles = 0;
+  const int32_t* work = nullptr;
+  int32_t n_work = 0;
 };
 int score_tc(const ScoreTcArgs& a, cudaStream_t stream);
 

@@ -26,9 +26,10 @@
 // (§3.12).  Modes (TcMode): the dense matrix, the top-k above
 // (k <= 32), or the wide top-k (k <= 1024, DESIGN.md §3.8), where every (row, column half) keeps its list in global
 // memory and a warp compacts a full list to its exact top k, or the counting mode (DESIGN.md §3.9), which captures the
-// scores of listed (user, item) pairs and counts the columns that outrank each of them.  score_tc is the one host
-// entry point behind every trk_score_{topk,dense,count}* function: it validates the arguments and launches one of the
-// 56 instantiations.
+// scores of listed (user, item) pairs and counts the columns that outrank each of them, or the pairs mode (DESIGN.md
+// §3.13), which captures the scores of listed pairs from item tiles gathered out of each user block's own listed items.
+// score_tc is the one host entry point behind every trk_score_{topk,dense,count,pairs}* function: it validates the
+// arguments and launches one of the 68 instantiations.
 #include "common.cuh"
 
 namespace trk {
@@ -41,7 +42,7 @@ constexpr int kExactWideMaxK = 1024;   // wide mode
 
 // What the kernel makes of the scores: the dense matrix, a sorted top-k list per (row, column half) in shared memory
 // (k <= kMaxK), or an unsorted list per (row, column half) in global memory (k <= kExactWideMaxK).
-enum TcMode { kModeDense, kModeTopk, kModeWide, kModeCount };
+enum TcMode { kModeDense, kModeTopk, kModeWide, kModeCount, kModePairs };
 
 // Wide mode: a list keeps at most k entries between compactions and holds exact_wide_cap(k) = 2 keep, keep = k rounded
 // up to 32, so a compacted list always has room for one whole chunk of 32 columns (DESIGN.md §3.8).
@@ -134,6 +135,11 @@ struct TcWide {
 // score in that order -- and pass p adds to count[pair] how many columns outrank pair 32 p + j of the row (j < 32).
 // block_pairs [n_user_blocks]: the most pairs of a row of the block; user blocks with at most 32 max(p, 0) are
 // skipped.  A kernel parameter of its own, for the same reason as TcExcl.
+// The pairs mode (kModePairs, DESIGN.md §3.13) is a capture (pass = -1) over gathered item tiles: ids are VIRTUAL
+// columns tile * 128 + c, ascending per row; tile_items [tiles, 128] = the item of every slot (-1: empty, a zero row);
+// work [n_work, 3] = (user block, first tile, end tile) of every work item; item_split = the item operand rows the
+// producer gathers.  TcParams.item_meta and TcEuclid.item_half_sqnorm hold one entry per slot.  (The fields follow
+// `pass`, so the counting mode's instantiations see the layout they always had.)
 struct TcCount {
   const int32_t* indptr;
   const int32_t* ids;
@@ -141,6 +147,10 @@ struct TcCount {
   int32_t* count;
   const int32_t* block_pairs;
   int32_t pass;
+  int32_t n_work;
+  const int32_t* tile_items;
+  const int32_t* work;
+  const uint8_t* item_split;
 };
 constexpr int kCountTargets = 32;   // targets of a row per counting pass
 
@@ -595,15 +605,15 @@ __device__ __forceinline__ void count_chunk(const uint32_t (&r)[32], int32_t id0
 
 // One 32-column chunk of one user row in counting mode: final scores, then the capture of the row's pairs (pass < 0)
 // or the row's excluded columns masked (kExclude, excl rows set) and the columns counted, unless the chunk's maximum
-// lies below the lowest target.
-template <bool kExclude, ScoreForm kForm>
+// lies below the lowest target.  kCapture (the pairs mode): always the capture, t a virtual tile.
+template <bool kExclude, ScoreForm kForm, bool kCapture = false>
 __device__ __forceinline__ void count_process_chunk(uint32_t (&r)[32], int c, int t, int32_t id0, const float2* meta,
                                                     const float* ihsq, float su, float usq, float ubias, const TcExcl x,
                                                     ExclCursor<kExclude>& xc, const TcCount cn, CountCursor<true>& cc,
                                                     const float* ts, const int32_t* ti, int32_t* h) {
   float cmax = score_chunk_as<kForm>(r, meta + c * 32, ihsq + c * 32, su, usq, ubias);
   const int32_t base = t * kBlockN + c * 32;
-  if (cn.pass < 0) {
+  if (kCapture || cn.pass < 0) {
     if (cc.next < base + 32) capture_chunk(r, cn, cc, base);
     return;
   }
@@ -638,7 +648,45 @@ __device__ __forceinline__ void store_chunk_tma(const uint32_t (&r)[32], uint32_
   }
 }
 
-// kMode: dense, top-k, wide or count (TcMode).  kNKB = d_pad / 64 k-blocks per operand half.  kExclude (top-k modes): columns named in the row's exclusion list are
+// Pairs mode, producer: one B stage (k-block kb2 of a gathered tile, slots = its 128 items) written by the whole
+// producer warp.  Lane l copies 16-byte chunk l % 8 of rows l / 8 + 4 j (8 lanes read one 128-byte row segment) to the
+// address the 128B swizzle gives it -- the layout a TMA box of the same rows writes -- and an empty slot (-1) is
+// zero-filled.  Every lane then
+// arrives on the stage's full barrier (initialised to 32 arrivals) once its copies have landed.
+template <int kNKB>
+__device__ __forceinline__ void gather_b_stage(uint32_t dst, uint64_t* full, const int32_t* slots,
+                                               const uint8_t* item_split, int kb2, int lane) {
+  constexpr int64_t kRowBytes = 4 * kKBlock * kNKB;   // 2 d_pad fp16 per operand row
+  const int c16 = lane % 8;
+#pragma unroll 4
+  for (int j = 0; j < 32; ++j) {
+    const int r = lane / 8 + 4 * j;
+    const int32_t item = __ldg(slots + r);
+    const uint32_t d = dst + r * 128 + ((c16 ^ (r % 8)) << 4);
+    const uint8_t* src = item_split + max(item, 0) * kRowBytes + kb2 * 128 + c16 * 16;
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d), "l"(src), "r"(item >= 0 ? 16 : 0)
+                 : "memory");
+  }
+  asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(full)) : "memory");
+}
+
+// Work item w: (user block, item split, tiles [t0, t1)); the pairs mode reads it from its work list (split 0).
+struct WorkItem {
+  int ub, sp, t0, t1;
+};
+template <bool kPairs>
+__device__ __forceinline__ WorkItem work_item(int64_t w, const TcParams& p, const TcCount& cn) {
+  if constexpr (kPairs) {
+    return {__ldg(cn.work + 3 * w), 0, __ldg(cn.work + 3 * w + 1), __ldg(cn.work + 3 * w + 2)};
+  } else {
+    const int ub = static_cast<int>(w / p.n_splits);
+    const int sp = static_cast<int>(w % p.n_splits);
+    const int t0 = sp * p.tiles_per_split;
+    return {ub, sp, t0, min(t0 + p.tiles_per_split, p.n_tiles)};
+  }
+}
+
+// kMode: dense, top-k, wide, count or pairs (TcMode).  kNKB = d_pad / 64 k-blocks per operand half.  kExclude (top-k modes): columns named in the row's exclusion list are
 // left out of the top-k (excl_mask_scores); the counting mode is always instantiated with it and excludes nothing when
 // x.indptr is null.  kForm: the score form, in every mode.  The tastes forms collapse a
 // mixture of tastes per (user, item) (collapse_chunk); map_users is then the 3-D map of the stacked operand, a user
@@ -651,6 +699,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
   constexpr bool kDense = kMode == kModeDense;
   constexpr bool kWide = kMode == kModeWide;
   constexpr bool kCount = kMode == kModeCount;
+  constexpr bool kPairs = kMode == kModePairs;
   uint8_t* smem = smem_base_1024();
   // (the counting mode stages its targets and buckets in the list region of k = kMaxK)
   const SmemLayout L = make_layout(p.n_kblocks, p.n_stages, kMode == kModeTopk ? p.k : (kCount ? kMaxK : 0),
@@ -667,7 +716,8 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
   // work item w = (user block w / n_splits, item split w % n_splits): the splits of ONE user block go to consecutive
   // CTAs, so a handful of live user blocks (the device-side fallback: ~100 rows of a million) still spreads over the
   // whole machine -- with the block index minor, one live block of 8 x 132 items landed on a quarter of the CTAs
-  const int64_t n_work = static_cast<int64_t>(p.n_user_blocks) * p.n_splits;
+  // (the pairs mode: the work list's items)
+  const int64_t n_work = kPairs ? cn.n_work : static_cast<int64_t>(p.n_user_blocks) * p.n_splits;
   // user blocks at or beyond this one hold no rows (every role skips them: the same test in both loops)
   const int live_blocks = p.n_users_live != nullptr
                               ? static_cast<int>(min(static_cast<int64_t>(p.n_user_blocks),
@@ -682,7 +732,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
     mbar_init(a_full, 1);
     mbar_init(a_empty, 2 * kConsumerThreads / 32);
     for (int i = 0; i < p.n_stages; ++i) {
-      mbar_init(b_full + i, 1);
+      mbar_init(b_full + i, kPairs ? 32 : 1);   // (the pairs mode: every producer lane's gathered copies)
       mbar_init(b_empty + i, 2 * kConsumerThreads / 32);
     }
     fence_mbar_init();
@@ -696,11 +746,9 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
       uint32_t stage_phase = 0;
       uint32_t witer = 0;  // non-empty work items so far
       for (int64_t w = blockIdx.x; w < n_work; w += gridDim.x) {
-        const int ub = static_cast<int>(w / p.n_splits);
-        const int sp = static_cast<int>(w % p.n_splits);
-        const int t0 = sp * p.tiles_per_split;
-        const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
-        if (t1 <= t0 || ub >= live_blocks || (kCount && !count_block_live(cn, ub))) continue;
+        const WorkItem wi = work_item<kPairs>(w, p, cn);
+        const int ub = wi.ub, t0 = wi.t0, t1 = wi.t1;
+        if (t1 <= t0|| ub >= live_blocks || (kCount && !count_block_live(cn, ub))) continue;
         mbar_wait(a_empty, (witer & 1) ^ 1);  // the MMAs of the previous work item no longer read A
         if constexpr (is_tastes(kForm)) {
           // one box of n_ops x per_wg rows per warpgroup half and k-block; a half without users is not loaded
@@ -725,12 +773,17 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
 #pragma unroll
           for (int kb = 0; kb < n_kb2; ++kb) {
             mbar_wait(b_empty + stage, stage_phase ^ 1);
-            if (elect_one()) {
-              mbar_arrive_expect_tx(b_full + stage, kBTileBytes);
-              tma_load_2d(smem + L.b_off + stage * kBTileBytes, &map_items, b_full + stage, kb * kKBlock, t * kBlockN,
-                          kEvictLast);  // the item operand is re-read by every user block: keep it in L2
+            if constexpr (kPairs) {
+              gather_b_stage<kNKB>(smem_u32(smem + L.b_off + stage * kBTileBytes), b_full + stage,
+                                   cn.tile_items + static_cast<int64_t>(t) * kBlockN, cn.item_split, kb, lane);
+            } else {
+              if (elect_one()) {
+                mbar_arrive_expect_tx(b_full + stage, kBTileBytes);
+                tma_load_2d(smem + L.b_off + stage * kBTileBytes, &map_items, b_full + stage, kb * kKBlock,
+                            t * kBlockN, kEvictLast);  // the item operand is re-read by every user block: keep it in L2
+              }
+              __syncwarp();
             }
-            __syncwarp();
             if (++stage == p.n_stages) {   // ring position advances incrementally: no div/mod on the issue path
               stage = 0;
               stage_phase ^= 1;
@@ -738,6 +791,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
           }
         }
       }
+      if constexpr (kPairs) asm volatile("cp.async.wait_all;" ::: "memory");
     }
   } else if (warp >= 4) {
     // ================================ consumers: wgmma + epilogue ================================
@@ -758,10 +812,8 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
     float acc[64];
 
     for (int64_t w = blockIdx.x; w < n_work; w += gridDim.x) {
-      const int ub = static_cast<int>(w / p.n_splits);
-      const int sp = static_cast<int>(w % p.n_splits);
-      const int t0 = sp * p.tiles_per_split;
-      const int t1 = min(t0 + p.tiles_per_split, p.n_tiles);
+      const WorkItem wi = work_item<kPairs>(w, p, cn);
+      const int ub = wi.ub, sp = wi.sp, t0 = wi.t0, t1 = wi.t1;
       if (ub >= live_blocks || (kCount && !count_block_live(cn, ub)))
         continue;   // (an empty split still emits its sentinel candidates)
       // tastes: this warpgroup's users start at u0; the thread of row q < per_wg owns user u0 + q, later rows own none
@@ -793,11 +845,11 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
       const float* cts = reinterpret_cast<const float*>(smem + L.list_score_off) + row;
       const int32_t* cti = reinterpret_cast<const int32_t*>(smem + L.list_score_off + kCountTargets * kBlockM * 4) + row;
       int32_t* ch = reinterpret_cast<int32_t*>(smem + L.list_item_off) + half * kCountTargets * kBlockM + row;
-      CountCursor<kCount> cc;
-      if constexpr (kCount) {
+      CountCursor<kCount || kPairs> cc;
+      if constexpr (kCount || kPairs) {
         const int32_t lo = u_ok ? __ldg(cn.indptr + u) : 0;
         const int32_t hi = u_ok ? __ldg(cn.indptr + u + 1) : 0;
-        if (cn.pass < 0) {
+        if (kPairs || cn.pass < 0) {
           cc.lo = lo;
           cc.hi = hi;
           if (t1 > t0 && hi > lo) cc.next = excl_next_at(cn.indptr, cn.ids, u, t0 * kBlockN);
@@ -836,6 +888,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
 #pragma unroll
         for (int kb2 = 0; kb2 < n_kb2; ++kb2) {
           mbar_wait(b_full + stage, stage_phase);
+          if constexpr (kPairs) fence_proxy_async();   // the gathered stage was written through the generic proxy
           const uint64_t db = wgmma_desc_k_major_sw128(b_base + stage * kBTileBytes);
           const bool b_is_hi = kb2 < kNKB;
           const int kb = b_is_hi ? kb2 : kb2 - kNKB;
@@ -896,10 +949,10 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
           } else if constexpr (kWide) {   // every lane: the compactions are warp-cooperative
             wide_chunk<kExclude, kForm>(r, chunk, t, id0, meta, ihsq, su, usq, ubias, thr, ls, li, wc.cnt, p.k, u_ok, x,
                                         xc, lane, wide_hist(smem + L.list_score_off, warp));
-          } else if constexpr (kCount) {
+          } else if constexpr (kCount || kPairs) {
             if (!is_tastes(kForm) || wt % kWgRows < z.per_wg)
-              count_process_chunk<kExclude, kForm>(r, chunk, t, id0, meta, ihsq, su, usq, ubias, x, xc, cn, cc, cts,
-                                                   cti, ch);
+              count_process_chunk<kExclude, kForm, kPairs>(r, chunk, t, id0, meta, ihsq, su, usq, ubias, x, xc, cn, cc,
+                                                           cts, cti, ch);
           } else if (!is_tastes(kForm) || wt % kWgRows < z.per_wg) {
             process_chunk<kDense, kExclude, kForm>(r, chunk, t, id0, meta, ihsq, su, usq, ubias, thr, ls, li, p, u,
                                                    u_ok, x, xc);
@@ -925,7 +978,7 @@ score_tc_kernel(const __grid_constant__ CUtensorMap map_users, const __grid_cons
             if (acc_count != 0) atomicAdd(cn.count + cc.lo + j, acc_count);
           }
         }
-      } else if constexpr (!kDense) {
+      } else if constexpr (!kDense && !kPairs) {
         // both halves have finished the item range: merge the two lists of each row and emit the candidates
         named_barrier_sync(1 + g, kConsumerThreads);
         if (half == 0 && u_ok) {
@@ -1011,7 +1064,12 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
                     reinterpret_cast<uintptr_t>(a.item_split) % 16 == 0 &&
                     reinterpret_cast<uintptr_t>(a.item_meta) % 16 == 0,
                 "score_tc: operands must be 16-byte aligned");
-  if (a.count) {
+  if (a.pairs) {
+    TRK_CHECK_ARG(a.pair_indptr && a.pair_ids && a.pair_score && a.tile_items && a.work, "score_pairs: null pair plan");
+    TRK_CHECK_ARG(a.n_tiles >= 1 && a.n_work >= 1, "score_pairs: n_tiles=%d and n_work=%d must be positive", a.n_tiles,
+                  a.n_work);
+    TRK_CHECK_ARG(a.n_tiles <= (1 << 24), "score_pairs: n_tiles=%d exceeds int32 virtual columns", a.n_tiles);
+  } else if (a.count) {
     TRK_CHECK_ARG(a.pair_indptr && a.pair_ids && a.pair_score && a.block_pairs, "score_count: null pair list");
     TRK_CHECK_ARG(a.pass >= -1, "score_count: pass=%d < -1", a.pass);
     TRK_CHECK_ARG(a.pass < 0 || a.pair_count, "score_count: null pair_count");
@@ -1050,11 +1108,12 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
   const ScoreForm form = tastes ? (euclid ? (a.attention ? kFormTastesEuclidAttention : kFormTastesEuclidMax)
                                           : (a.attention ? kFormTastesAttention : kFormTastesMax))
                                 : (euclid ? kFormEuclid : kFormDot);
-  // every instantiation: [dense | top-k | top-k with exclusion | wide | wide with exclusion | count][form][d_pad / 64 - 1]
+  // every instantiation:
+  //   [dense | top-k | top-k with exclusion | wide | wide with exclusion | count | pairs][form][d_pad / 64 - 1]
   // (the wide mode exists for the forms without a wide filter: Euclidean similarity and attention; a Euclidean mixture
   // of tastes without attention ranks its top k per taste, so its max form has no top-k or wide instantiation; the
-  // counting mode takes its exclusion lists at run time)
-  static constexpr const TcKernelFn* kKernels[6][6] = {
+  // counting mode takes its exclusion lists at run time; the pairs mode excludes nothing, as dense scores do not)
+  static constexpr const TcKernelFn* kKernels[7][6] = {
       {TcKernel<kModeDense, false, kFormDot>::fn, TcKernel<kModeDense, false, kFormEuclid>::fn,
        TcKernel<kModeDense, false, kFormTastesMax>::fn, TcKernel<kModeDense, false, kFormTastesAttention>::fn,
        TcKernel<kModeDense, false, kFormTastesEuclidMax>::fn,
@@ -1072,8 +1131,12 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
       {TcKernel<kModeCount, true, kFormDot>::fn, TcKernel<kModeCount, true, kFormEuclid>::fn,
        TcKernel<kModeCount, true, kFormTastesMax>::fn, TcKernel<kModeCount, true, kFormTastesAttention>::fn,
        TcKernel<kModeCount, true, kFormTastesEuclidMax>::fn,
-       TcKernel<kModeCount, true, kFormTastesEuclidAttention>::fn}};
-  const int mode_row = a.count ? 5 : a.dense ? 0 : (a.wide ? 3 : 1) + (a.excl_indptr != nullptr ? 1 : 0);
+       TcKernel<kModeCount, true, kFormTastesEuclidAttention>::fn},
+      {TcKernel<kModePairs, false, kFormDot>::fn, TcKernel<kModePairs, false, kFormEuclid>::fn,
+       TcKernel<kModePairs, false, kFormTastesMax>::fn, TcKernel<kModePairs, false, kFormTastesAttention>::fn,
+       TcKernel<kModePairs, false, kFormTastesEuclidMax>::fn,
+       TcKernel<kModePairs, false, kFormTastesEuclidAttention>::fn}};
+  const int mode_row = a.pairs ? 6 : a.count ? 5 : a.dense ? 0 : (a.wide ? 3 : 1) + (a.excl_indptr != nullptr ? 1 : 0);
   if (kKernels[mode_row][form] == nullptr) {
     if (form == kFormTastesEuclidMax)
       set_error("score_topk: a Euclidean mixture of tastes without attention has no one-sweep top-k: rank each taste "
@@ -1093,7 +1156,7 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
   p.k = a.dense ? 0 : a.k;
   p.n_tiles = static_cast<int32_t>(ceil_div(a.n_items, kBlockN));
   p.n_user_blocks = static_cast<int32_t>(ceil_div(a.n_users, tastes ? 2 * z.per_wg : kBlockM));
-  p.n_splits = a.dense ? dense_splits(p.n_user_blocks, a.n_items) : a.n_splits;
+  p.n_splits = a.dense ? dense_splits(p.n_user_blocks, a.n_items) : a.pairs ? 1 : a.n_splits;
   p.tiles_per_split = static_cast<int32_t>(ceil_div(p.n_tiles, p.n_splits));
   p.item_id_offset = a.item_id_offset;
   p.cand_score = a.cand_score;
@@ -1133,9 +1196,10 @@ int score_tc(const ScoreTcArgs& a, cudaStream_t stream) {
       make_layout(p.n_kblocks, p.n_stages, list_k, p.tma_store != 0, a.wide).total + kSmemAlignSlack;
   const TcKernelFn kernel = kKernels[mode_row][form][p.n_kblocks - 1];
   TRK_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-  const int grid = capped_grid(static_cast<int64_t>(p.n_user_blocks) * p.n_splits, 1);
+  const int grid = capped_grid(a.pairs ? a.n_work : static_cast<int64_t>(p.n_user_blocks) * p.n_splits, 1);
   const TcWide wl = {a.list_count};
-  const TcCount cn = {a.pair_indptr, a.pair_ids, a.pair_score, a.pair_count, a.block_pairs, a.pass};
+  const TcCount cn = {a.pair_indptr, a.pair_ids, a.pair_score, a.pair_count, a.block_pairs, a.pairs ? -1 : a.pass,
+                      a.n_work, a.tile_items, a.work, static_cast<const uint8_t*>(a.item_split)};
   kernel<<<grid, kTcThreads, smem_bytes, stream>>>(map_users, map_items, map_out, p, x, e, z, wl, cn);
   TRK_CHECK_LAUNCH();
   return TRK_OK;

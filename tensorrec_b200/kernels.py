@@ -1,5 +1,6 @@
 """Host-side launch layer: torch supplies device memory and streams, every computation is a call through the C ABI
 (libtensorrec_b200.so).  No function here has a CPU path; all of them raise without a CUDA device."""
+import collections
 import ctypes
 
 import numpy as np
@@ -1255,4 +1256,104 @@ def rank_listed_from_scores(scores, pair_row, pair_col, excl=None, block_bytes=4
         t = target[p0:p1, None]
         ahead = (row > t).sum(dim=1) + ((row == t) & (cols[None, :] < pair_col[p0:p1, None])).sum(dim=1)
         out[p0:p1] = (1 + ahead).to(torch.int32)
+    return out
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# pairs mode of the exact kernel: the scores of listed (user, item) pairs, bit for bit predict()'s, from item tiles
+# gathered out of each user block's own listed items (DESIGN §3.13)
+# ---------------------------------------------------------------------------------------------------------------
+PAIR_TILE = 128             # columns of a gathered tile: item i sits at column i % PAIR_TILE, its dense-sweep column
+PAIRS_TILES_PER_WORK = 16   # gathered tiles per work item: a block with many tiles is spread over several CTAs
+# device bytes per listed pair at most: its virtual column, score and permutation, and -- when every tile holds a single
+# listed item -- a whole tile of slots (item id, {scale, bias}, half squared norm)
+PREDICT_AT_BYTES_PER_PAIR = 24 + PAIR_TILE * 16
+
+PairsPlan = collections.namedtuple('PairsPlan', 'tile_items block_tiles work cols order')
+
+
+def pairs_plan(indptr, ids, n_rows, block_rows, max_tiles=PAIRS_TILES_PER_WORK):
+    """Host plan of a pairs-mode launch over n_rows user rows whose listed pairs are the CSR (indptr, ids: LOCAL item
+    ids, ascending per row); block_rows = the kernel's user block (128, or 2P for a mixture of tastes).
+
+    Every user block takes its distinct listed items (an item listed by several of its rows takes one slot), groups
+    them by residue c = i % 128 and puts the j-th item (ascending) of residue c at column c of the block's tile j, so a
+    block gets as many tiles as its largest residue class.  Returns a PairsPlan of numpy arrays:
+      tile_items  int32 [T, 128], -1 = an empty slot;
+      block_tiles int64 [n_blocks + 1]: block b owns tiles [block_tiles[b], block_tiles[b + 1]);
+      work        int32 [W, 3]: (block, first tile, end tile), at most max_tiles tiles each, every tile in one item;
+      cols        int32 [nnz]: the pairs' virtual columns tile * 128 + i % 128, ascending within each row;
+      order       int64 [nnz]: pair k of the kernel's order (cols) is pair order[k] of the listing (ids)."""
+    indptr = np.asarray(indptr, dtype=np.int64)
+    ids = np.asarray(ids, dtype=np.int64)
+    n_blocks = -(-int(n_rows) // int(block_rows))
+    row = np.repeat(np.arange(n_rows, dtype=np.int64), np.diff(indptr))
+    res, quo = ids % PAIR_TILE, ids // PAIR_TILE
+    span = int(quo.max()) + 1 if ids.size else 1
+    # one int64 key per pair whose order is (block, residue, item); its distinct values are the block's slots
+    slots, inv = np.unique(((row // block_rows) * PAIR_TILE + res) * span + quo, return_inverse=True)
+    group = slots // span                              # block * 128 + residue
+    n = slots.size
+    first = np.flatnonzero(np.r_[True, group[1:] != group[:-1]]) if n else np.zeros(0, np.int64)
+    rank = np.arange(n) - np.repeat(first, np.diff(np.r_[first, n]))   # j: rank of the item in its residue class
+    blk = group // PAIR_TILE
+    block_tiles = np.zeros(n_blocks + 1, dtype=np.int64)
+    if n:
+        b_first = np.flatnonzero(np.r_[True, blk[1:] != blk[:-1]])
+        block_tiles[blk[b_first] + 1] = np.maximum.reduceat(rank + 1, b_first)
+    np.cumsum(block_tiles, out=block_tiles)
+    n_tiles = int(block_tiles[-1])
+    if n_tiles > 1 << 24:
+        raise ValueError('%d gathered tiles exceed the int32 virtual columns of one launch' % n_tiles)
+    tile = block_tiles[blk] + rank
+    tile_items = np.full((n_tiles, PAIR_TILE), -1, dtype=np.int32)
+    tile_items[tile, group % PAIR_TILE] = (slots % span) * PAIR_TILE + group % PAIR_TILE
+    col = (tile * PAIR_TILE + group % PAIR_TILE)[inv.reshape(-1)]
+    order = np.argsort(row * (n_tiles * PAIR_TILE) + col, kind='stable')
+    per_block = np.diff(block_tiles)
+    chunks = -(-per_block // max_tiles)
+    w_blk = np.repeat(np.arange(n_blocks, dtype=np.int64), chunks)
+    w_k = np.arange(w_blk.size) - np.repeat(np.cumsum(chunks) - chunks, chunks)
+    t0 = block_tiles[w_blk] + w_k * max_tiles
+    work = np.stack([w_blk, t0, np.minimum(t0 + max_tiles, block_tiles[w_blk + 1])], axis=1).astype(np.int32)
+    return PairsPlan(tile_items, block_tiles, work, col[order].astype(np.int32), order)
+
+
+def score_listed_pairs(users, items, meta, indptr, plan, item_hsq=None, tastes=None):
+    """Pairs mode of the exact kernel over the users of `users` (SideOperands; a mixture of tastes: the stacked operand
+    and tastes = (n_tastes, attention)); meta = pack_item_meta(items ...), item_hsq = item_half_sqnorm(items) for a
+    Euclidean model; indptr / plan: the host pair CSR and its pairs_plan.  Returns float32 scores on the device in the
+    order of the listing."""
+    lib = require_cuda()
+    dev = users.split.device
+    nnz = int(indptr[-1])
+    up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev, non_blocking=True)   # noqa: E731
+    d_indptr, d_cols, d_tiles, d_work = up(indptr), up(plan.cols), up(plan.tile_items), up(plan.work)
+    slot = d_tiles.view(-1).long()
+    empty = slot < 0
+    slot = slot.clamp(min=0)
+    slot_meta = meta[slot]
+    slot_meta[empty] = torch.tensor([0.0, float('-inf')], device=dev)   # an empty slot scores as a padding column
+    slot_hsq = None
+    if item_hsq is not None:
+        slot_hsq = item_hsq[slot]
+        slot_hsq[empty] = 0.0
+    score = torch.empty((nnz,), dtype=torch.float32, device=dev)
+    n_tiles, n_work = int(plan.tile_items.shape[0]), int(plan.work.shape[0])
+    head = (_p(users.split), _p(users.scale), _p(users.bias))
+    shape = (users.n_rows, items.n_rows, int(users.d_pad))
+    lists = (_p(d_indptr), _p(d_cols), _p(score), _p(d_tiles), n_tiles, _p(d_work), n_work)
+    if tastes is not None:
+        name, norms = _tastes_entry('trk_score_pairs_tastes', users, slot_hsq)
+        args = head + (int(tastes[0]), 1 if tastes[1] else 0, _p(items.split), _p(slot_meta)) + shape + lists + norms
+    elif item_hsq is not None:
+        name = 'trk_score_pairs_euclid_f16x3'
+        user_hsq = operand_half_sqnorm(users.split, users.scale, users.d_pad)
+        args = head + (_p(items.split), _p(slot_meta)) + shape + lists + (_p(user_hsq), _p(slot_hsq))
+    else:
+        name = 'trk_score_pairs_f16x3'
+        args = head + (_p(items.split), _p(slot_meta)) + shape + lists
+    _lib.check(getattr(lib, name)(*args, _stream()), name)
+    out = torch.empty_like(score)
+    out[up(plan.order)] = score
     return out

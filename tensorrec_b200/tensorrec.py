@@ -77,6 +77,10 @@ RANK_AT_MIN_ITEMS = 2048
 # counting sweep each pay 2T roots and the softmax per pair, which costs more than one dense sweep and the sort on smaller
 # catalogues (see README, "Euclidean mixtures of tastes").
 RANK_AT_EUCLID_ATTENTION_MIN_ITEMS = 16384
+# predict_at scores on the exact kernel's pairs mode (route 'exact3_pairs') on catalogues of at least
+# PREDICT_AT_MIN_ITEMS items; below that, dense scoring of the user blocks gathered at the pairs is faster, as the pairs
+# mode pays its host planner per pair (see README, "Scores of listed pairs").
+PREDICT_AT_MIN_ITEMS = 1 << 20
 
 
 def rank_at_route(n_items, tensor_scored, euclid_attention=False):
@@ -86,6 +90,14 @@ def rank_at_route(n_items, tensor_scored, euclid_attention=False):
     otherwise."""
     floor = RANK_AT_EUCLID_ATTENTION_MIN_ITEMS if euclid_attention else RANK_AT_MIN_ITEMS
     return 'exact3_count' if tensor_scored and n_items >= floor else 'dense+rank'
+
+
+def predict_at_route(n_items, tensor_scored):
+    """The route of a predict_at call: 'exact3_pairs', the exact kernel's pairs mode, when predict() scores the model
+    on the exact tensor-core kernel (tensor_scored: TensorRec._tensor_score_form() is not None) and the catalogue has at
+    least PREDICT_AT_MIN_ITEMS items, 'dense+gather' (dense scores of the user blocks, gathered at the pairs)
+    otherwise."""
+    return 'exact3_pairs' if tensor_scored and n_items >= PREDICT_AT_MIN_ITEMS else 'dense+gather'
 
 
 def rank_at_blocks(indptr, unit, max_rows, max_pairs):
@@ -1034,6 +1046,87 @@ class TensorRec(object):
                 parts.append(kernels.rank_listed_from_scores(score(block_in), rows, cols, excl=excl,
                                                              block_bytes=self.PREDICT_BLOCK_BYTES))
         ranks = (torch.cat(parts) if len(parts) > 1 else parts[0]).cpu().numpy()
+        return result()
+
+    def predict_at(self, user_features, item_features, pairs, user_batch_size=None):
+        """The scores of listed (user, item) pairs, without the [n_users, n_items] score matrix: held-out ratings,
+        the candidates of a re-ranking stage, the items a user was shown.
+
+        pairs: a scipy sparse matrix [n_users, n_items]; the pair (u, i) is listed when pairs[u, i] != 0 after
+        duplicates are summed (explicit zeros list nothing), as for predict_rank_at.  Returns a scipy.sparse.csr_matrix
+        of float32 [n_users, n_items] with sorted indices and one stored entry per listed pair (a score of 0.0 is
+        stored too): predict(user_features, item_features)[u, i], bit for bit.
+
+        Users go in blocks that start at multiples of the kernel's user block (128 rows, or 2P for a mixture of
+        tastes: DESIGN §3.5), so user_batch_size is rounded down to a positive multiple of it.
+        last_predict_at_info['path'] names the route (predict_at_route): 'exact3_pairs', the exact kernel's pairs
+        mode (catalogues of at least PREDICT_AT_MIN_ITEMS items), or 'dense+gather', predict()'s scores of each block
+        gathered at the pairs; last_predict_at_info['tiles'] = the item tiles the pairs mode gathered (0 on
+        dense+gather)."""
+        if self.tf_prediction is None:
+            raise ModelNotFitException(method='predict_at')
+        user_in = self._single_input(user_features, 'user_features')
+        item_in = self._single_input(item_features, 'item_features')
+        n_users, n_items = user_in.shape[0], item_in.shape[0]
+        if not sp.issparse(pairs):
+            raise ValueError('pairs must be a scipy sparse matrix with one row per user and one column per item')
+        if tuple(pairs.shape) != (n_users, n_items):
+            raise ValueError('pairs has shape %s but there are %d users and %d items'
+                             % (tuple(pairs.shape), n_users, n_items))
+        self._check_features(user_in, self.n_user_features, 'user')
+        self._check_features(item_in, self.n_item_features, 'item')
+        indptr, ids = kernels.exclusion_host_csr(pairs, 0, n_items)   # the listing rule is the exclusion rule
+        form = self._tensor_score_form()
+        path = predict_at_route(n_items, form is not None)
+        self.last_predict_at_info = {'path': path, 'tiles': 0}
+        scores = np.zeros(ids.shape[0], dtype=np.float32)
+        result = lambda: sp.csr_matrix((scores, ids, indptr), shape=(n_users, n_items))   # noqa: E731
+        if ids.size == 0:
+            return result()
+        device = self._cuda_device()
+
+        attention = self.attention_graph_factory is not None
+        tastes_form = form in ('tastes', 'tastes_euclid')
+        unit = kernels.tastes_plan(self.n_tastes, attention)[1] if tastes_form else kernels.TILE_USERS
+        if path == 'exact3_pairs':
+            n_ops = kernels.tastes_n_ops(self.n_tastes, attention) if tastes_form else 1
+            # (tastes_euclid: 4 more bytes per operand row for its half squared norm)
+            per_row = n_ops * (4 * kernels.d_pad_for(self.n_components) + 8 + (4 if form == 'tastes_euclid' else 0)) + 8
+        else:
+            per_row = 4 * n_items
+        max_rows = self.PREDICT_BLOCK_BYTES // per_row if user_batch_size is None else int(user_batch_size)
+        max_rows = max(unit, max_rows // unit * unit)
+        blocks = rank_at_blocks(indptr, unit, max_rows, self.PREDICT_BLOCK_BYTES // kernels.PREDICT_AT_BYTES_PER_PAIR)
+        csr = user_in.matrix if isinstance(user_in.matrix, sp.csr_matrix) else sp.csr_matrix(user_in.matrix)
+
+        if path == 'exact3_pairs':
+            items = self._side_operands('item', item_in, device)
+            meta = kernels.pack_item_meta(items.scale, items.bias, n_items)
+            item_hsq = kernels.item_half_sqnorm(items) if form in ('euclidean', 'tastes_euclid') else None
+        else:
+            score = self._score_plan(item_in, device)
+        parts = []
+        for u0, u1 in blocks:
+            p0, p1 = int(indptr[u0]), int(indptr[u1])
+            if p1 == p0:
+                continue
+            block_in = user_in if (u0, u1) == (0, n_users) else SparseInput(csr[u0:u1])
+            b_indptr, b_ids = (indptr[u0:u1 + 1] - p0).astype(np.int32), ids[p0:p1]
+            if path == 'exact3_pairs':
+                if tastes_form:
+                    users, tastes = self._taste_operands(block_in, device), (self.n_tastes, attention)
+                else:
+                    users, tastes = self._side_operands('user', block_in, device), None
+                plan = kernels.pairs_plan(b_indptr, b_ids, u1 - u0, unit)
+                self.last_predict_at_info['tiles'] += int(plan.tile_items.shape[0])
+                parts.append(kernels.score_listed_pairs(users, items, meta, b_indptr, plan, item_hsq=item_hsq,
+                                                        tastes=tastes))
+                del users
+            else:
+                rows = torch.from_numpy(np.repeat(np.arange(u1 - u0), np.diff(b_indptr))).to(device)
+                cols = torch.from_numpy(b_ids.astype(np.int64)).to(device)
+                parts.append(score(block_in)[rows, cols])
+        scores = (torch.cat(parts) if len(parts) > 1 else parts[0]).cpu().numpy()
         return result()
 
     def predict_top_k(self, user_features, item_features, k, item_id_offset=0, gather_group=None, to_host=True,
