@@ -639,6 +639,17 @@ int trk_topk_merge_dedup_pair(const float* a_score, const int32_t* a_item, int64
  * trk_adam_step_f32  tf.train.AdamOptimizer on (grad + l2 * w) (tensorrec/tensorrec.py:487-489):
  *                      m = b1 m + (1 - b1) g;  v = b2 v + (1 - b2) g^2;  w -= lr_t m / (sqrt(v) + epsilon),
  *                    lr_t = lr sqrt(1 - b2^t) / (1 - b1^t) formed by the caller.
+ * trk_relu_layer_forward_f32
+ *                    the hidden layer of ReLURepresentationGraph (DESIGN §3.14): out [rows, d] = relu(pre + bias) . w2 for
+ *                    pre [rows, hidden] (the K1 product X . W1), bias [hidden], w2 [hidden, d], as 3xTF32 products on
+ *                    the tensor cores (fp32-grade).  hidden % 8 == 0 and <= 2048, d % 4 == 0 and <= 512 (pad hidden with
+ *                    zero W1 columns, bias and w2 rows, d with zero w2 columns); pre, bias, w2 and out 16-byte aligned.
+ * trk_relu_layer_backward_f32
+ *                    its gradients for d_out = d loss / d out [rows, d]: pre is REPLACED by d loss / d pre =
+ *                    (d_out . w2^T) * [pre + bias > 0] (an exact 0 passes no gradient, tf.nn.relu's rule); d_bias
+ *                    [hidden] and d_w2 [hidden, d] are written.  Deterministic: per-CTA partials in `workspace`
+ *                    (trk_relu_layer_workspace_bytes(rows, hidden, d) bytes, 16-byte aligned), summed in a fixed order;
+ *                    no atomics.  Constraints as the forward; d_out 16-byte aligned.
  * ---------------------------------------------------------------------------------------------------- */
 int trk_sample_items(int64_t n_users, int64_t n_items, int32_t n_sampled, int32_t replace, uint64_t seed,
                      uint32_t step, int32_t* out, void* stream);
@@ -666,6 +677,12 @@ int trk_l2_normalize_rows_step_f32(const float* x, int64_t rows, int32_t d, int3
 int trk_f32_to_bf16(const float* x, int64_t n, void* out, void* stream);
 int trk_adam_step_f32(float* w, const float* grad, float* m, float* v, int64_t n, float lr_t, float beta1, float beta2,
                       float epsilon, float l2, void* stream);
+size_t trk_relu_layer_workspace_bytes(int64_t rows, int32_t hidden, int32_t d);
+int trk_relu_layer_forward_f32(const float* pre, const float* bias, const float* w2, int64_t rows, int32_t hidden,
+                               int32_t d, float* out, void* stream);
+int trk_relu_layer_backward_f32(float* pre, const float* bias, const float* w2, const float* d_out, int64_t rows,
+                                int32_t hidden, int32_t d, float* d_bias, float* d_w2, void* workspace,
+                                size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

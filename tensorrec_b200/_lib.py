@@ -136,6 +136,10 @@ SIGNATURES = {
     'trk_f32_to_bf16': (ctypes.c_int, [_c_p, _c_i64, _c_p, _c_p]),
     'trk_adam_step_f32': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_i64, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                          ctypes.c_float, ctypes.c_float, _c_p]),
+    'trk_relu_layer_workspace_bytes': (_c_sz, [_c_i64, _c_i32, _c_i32]),
+    'trk_relu_layer_forward_f32': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_i64, _c_i32, _c_i32, _c_p, _c_p]),
+    'trk_relu_layer_backward_f32': (ctypes.c_int, [_c_p, _c_p, _c_p, _c_p, _c_i64, _c_i32, _c_i32, _c_p, _c_p, _c_p,
+                                                   _c_sz, _c_p]),
 }
 
 _lib = None

@@ -150,6 +150,10 @@ int l2_normalize_rows_step(const float*, int64_t, int32_t, int32_t, float*, floa
 int f32_to_bf16(const float*, int64_t, void*, cudaStream_t);
 int adam_step(float*, const float*, float*, float*, int64_t, float, float, float, float, float, cudaStream_t);
 uint64_t philox_u64_host(uint64_t, uint32_t, uint32_t, uint32_t);
+size_t relu_layer_workspace_bytes(int64_t, int32_t, int32_t);
+int relu_layer_forward(const float*, const float*, const float*, int64_t, int32_t, int32_t, float*, cudaStream_t);
+int relu_layer_backward(float*, const float*, const float*, const float*, int64_t, int32_t, int32_t, float*, float*,
+                        void*, size_t, cudaStream_t);
 
 static inline cudaStream_t as_stream(void* s) { return static_cast<cudaStream_t>(s); }
 
@@ -778,6 +782,22 @@ int trk_f32_to_bf16(const float* x, int64_t n, void* out, void* stream) {
 int trk_adam_step_f32(float* w, const float* grad, float* m, float* v, int64_t n, float lr_t, float beta1, float beta2,
                       float epsilon, float l2, void* stream) {
   return trk::adam_step(w, grad, m, v, n, lr_t, beta1, beta2, epsilon, l2, trk::as_stream(stream));
+}
+
+size_t trk_relu_layer_workspace_bytes(int64_t rows, int32_t hidden, int32_t d) {
+  return trk::relu_layer_workspace_bytes(rows, hidden, d);
+}
+
+int trk_relu_layer_forward_f32(const float* pre, const float* bias, const float* w2, int64_t rows, int32_t hidden,
+                               int32_t d, float* out, void* stream) {
+  return trk::relu_layer_forward(pre, bias, w2, rows, hidden, d, out, trk::as_stream(stream));
+}
+
+int trk_relu_layer_backward_f32(float* pre, const float* bias, const float* w2, const float* d_out, int64_t rows,
+                                int32_t hidden, int32_t d, float* d_bias, float* d_w2, void* workspace,
+                                size_t workspace_bytes, void* stream) {
+  return trk::relu_layer_backward(pre, bias, w2, d_out, rows, hidden, d, d_bias, d_w2, workspace, workspace_bytes,
+                                  trk::as_stream(stream));
 }
 
 }  // extern "C"

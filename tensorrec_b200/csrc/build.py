@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 SOURCES = ['api.cu', 'csr_gather.cu', 'score_simt.cu', 'rank_full.cu', 'topk_merge.cu', 'score_topk_tc.cu',
            'score_filter_tc.cu', 'score_wide_tc.cu', 'rescore_topk.cu', 'rescore_wide.cu', 'similar_items.cu',
-           'wmrb_step.cu']
+           'wmrb_step.cu', 'relu_layer.cu']
 HEADERS = [os.path.join(HERE, 'common.cuh'), os.path.join(HERE, 'filter_tc.cuh'),
            os.path.join(ROOT, 'include', 'tensorrec_b200.h')]
 LIB_PATH = os.path.join(os.path.dirname(HERE), 'libtensorrec_b200.so')

@@ -523,8 +523,11 @@ class TensorRec(object):
 
     def _fit_epochs(self, batches, epochs, learning_rate, alpha, batched_alpha, verbose, n_sampled_items, device):
         from . import train_kernels
-        # the training step on hand-written kernels (train_kernels.step_plan; DESIGN §3.10, §3.11), or the torch path
-        plan = train_kernels.step_plan(self, n_sampled_items) if device.type == 'cuda' else None
+        # the training step on hand-written kernels (train_kernels.step_plan, relu_step_plan; DESIGN §3.10, §3.11,
+        # §3.14), or the torch path
+        plan = None
+        if device.type == 'cuda':
+            plan = train_kernels.step_plan(self, n_sampled_items) or train_kernels.relu_step_plan(self, n_sampled_items)
         serial = plan is not None and plan.loss != 'wmrb'         # RMSE / Separation: a scalar loss
         for epoch in range(epochs):
             for batch, (int_in, uf_in, if_in) in enumerate(batches):

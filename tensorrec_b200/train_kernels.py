@@ -24,6 +24,10 @@ train on the same representations, K1^T and Adam, with trk_serial_loss_step in p
 trk_wmrb_step_tastes: a forward launch writes the serial predictions, a statistics launch reduces them to the scalar
 loss and a loss state on the device, and a backward launch turns each prediction into its gradient from that state.
 
+ReLURepresentationGraph user, item or attention sides (relu_step_plan; DESIGN §3.14) add a hidden-layer stage: K1 of
+X . W1 into the pre-activations P, trk_relu_layer_forward_f32 (relu(P + b) . W2) into the operand plane, and after the
+loss kernel trk_relu_layer_backward_f32 (dP over P, d relu_biases, d linear_weights) before K1^T of dP and Adam.
+
 Every other model family trains through the torch-autograd mirror of the reference's graph functions
 (TensorRec._training_losses); TENSORREC_B200_TRAIN_PATH=torch forces that path."""
 import collections
@@ -82,12 +86,16 @@ MAX_D_TASTES = 128                 # n_components with several tastes
 MAX_TASTES = 8                     # n_tastes without attention
 MAX_TASTES_ATTENTION = 4           # n_tastes with attention
 
+MAX_HIDDEN = 2048                  # relu_size of a ReLURepresentationGraph (trk_relu_layer_*_f32)
+
 # The form of the fused step that trains a model: pair 'dot' (dot and cosine) or 'euclidean'; how many times the user,
 # attention and item rows are L2-normalised (NormalizedLinearRepresentationGraph once, cosine once more); d_pad the
 # operand width (n_components rounded up to a multiple of 4).
 # loss: 'wmrb' (WMRB / BalancedWMRB on trk_wmrb_step_tastes), or 'rmse' / 'separation' (trk_serial_loss_step).
+# hidden: the hidden layer width of the user, attention and item graphs when they are ReLURepresentationGraph (relu_size
+# rounded up to a multiple of 8), 0 for a Linear / NormalizedLinear graph (relu_step_plan; DESIGN §3.14).
 StepForm = collections.namedtuple('StepForm', ['pair', 'n_tastes', 'attention', 'normalize_user', 'normalize_attn',
-                                               'normalize_item', 'd_pad', 'loss'])
+                                               'normalize_item', 'd_pad', 'loss', 'hidden'], defaults=((0, 0, 0),))
 SERIAL_LOSS_KIND = {'rmse': 0, 'separation': 1}          # trk_serial_loss_step's loss_kind
 
 
@@ -97,10 +105,31 @@ def step_plan(model, n_sampled_items=None):
     SeparationLossGraph (nothing sampled: no n_sampled_items limit); dot, cosine or Euclidean prediction; Linear or
     NormalizedLinear user, item and attention graphs (or no attention); n_components <= 512 for one taste, <= 128 with
     n_tastes <= 8 (<= 4 with attention)."""
+    return _plan(model, n_sampled_items, relu=False)
+
+
+def relu_step_plan(model, n_sampled_items=None):
+    """The StepForm of the fused training step for a model with at least one ReLURepresentationGraph whose other
+    graphs are Linear or NormalizedLinear, or None: step_plan's losses, predictions and limits, and relu_size <= 2048.
+    A ReLU side adds its hidden layer (trk_relu_layer_forward_f32 / _backward_f32) between K1 and the loss kernels;
+    cosine prediction normalises its output once.  step_plan answers None for every model this planner covers."""
+    return _plan(model, n_sampled_items, relu=True)
+
+
+def _relu_hidden(model, graph):
+    """relu_size of a ReLURepresentationGraph (default 4 n_components), 0 for any other graph."""
+    from .representation_graphs import ReLURepresentationGraph
+    if type(graph) is not ReLURepresentationGraph:
+        return 0
+    return 4 * int(model.n_components) if graph.relu_size is None else int(graph.relu_size)
+
+
+def _plan(model, n_sampled_items, relu):
     from .loss_graphs import BalancedWMRBLossGraph, RMSELossGraph, SeparationLossGraph, WMRBLossGraph
     from .prediction_graphs import (CosineSimilarityPredictionGraph, DotProductPredictionGraph,
                                     EuclideanSimilarityPredictionGraph)
-    from .representation_graphs import LinearRepresentationGraph, NormalizedLinearRepresentationGraph
+    from .representation_graphs import (LinearRepresentationGraph, NormalizedLinearRepresentationGraph,
+                                        ReLURepresentationGraph)
     loss = {WMRBLossGraph: 'wmrb', BalancedWMRBLossGraph: 'wmrb', RMSELossGraph: 'rmse',
             SeparationLossGraph: 'separation'}.get(type(model.loss_graph_factory))
     if TRAIN_PATH == 'torch' or loss is None:
@@ -110,11 +139,14 @@ def step_plan(model, n_sampled_items=None):
     pred = type(model.prediction_graph_factory)
     if pred not in (DotProductPredictionGraph, CosineSimilarityPredictionGraph, EuclideanSimilarityPredictionGraph):
         return None
-    linear = (LinearRepresentationGraph, NormalizedLinearRepresentationGraph)
     attention = model.attention_graph_factory is not None
-    if type(model.user_repr_graph_factory) not in linear or type(model.item_repr_graph_factory) not in linear:
+    graphs = [model.user_repr_graph_factory, model.item_repr_graph_factory]
+    if attention:
+        graphs.append(model.attention_graph_factory)
+    kinds = (LinearRepresentationGraph, NormalizedLinearRepresentationGraph) + ((ReLURepresentationGraph,) if relu else ())
+    if any(type(graph) not in kinds for graph in graphs):
         return None
-    if attention and type(model.attention_graph_factory) not in linear:
+    if relu and not any(type(graph) is ReLURepresentationGraph for graph in graphs):
         return None
     d, nt = int(model.n_components), int(model.n_tastes)
     if nt == 1:
@@ -122,15 +154,22 @@ def step_plan(model, n_sampled_items=None):
             return None
     elif d > MAX_D_TASTES or nt > (MAX_TASTES_ATTENTION if attention else MAX_TASTES):
         return None
+    hidden = [_relu_hidden(model, graph) for graph in graphs]
+    if any(type(graph) is ReLURepresentationGraph and not 1 <= h <= MAX_HIDDEN for graph, h in zip(graphs, hidden)):
+        return None
     cos = 1 if pred is CosineSimilarityPredictionGraph else 0
 
     def n_norm(graph):
         return (1 if type(graph) is NormalizedLinearRepresentationGraph else 0) + cos
 
-    return StepForm(pair='euclidean' if pred is EuclideanSimilarityPredictionGraph else 'dot', n_tastes=nt,
+    form = StepForm(pair='euclidean' if pred is EuclideanSimilarityPredictionGraph else 'dot', n_tastes=nt,
                     attention=attention, normalize_user=n_norm(model.user_repr_graph_factory),
                     normalize_attn=n_norm(model.attention_graph_factory) if attention else 0,
                     normalize_item=n_norm(model.item_repr_graph_factory), d_pad=(d + 3) // 4 * 4, loss=loss)
+    if relu:
+        pad8 = [(h + 7) // 8 * 8 for h in hidden]
+        form = form._replace(hidden=(pad8[0], pad8[2] if attention else 0, pad8[1]))
+    return form
 
 
 def check_step_inputs(interactions_shape, n_users, n_items, n_sampled_items, samples=None):
@@ -186,7 +225,11 @@ class WmrbStep(object):
             raise ValueError('weight {!r} has shape {} but the inputs need {}'.format(name, tuple(w.shape), shape))
         return w
 
-    def _weights(self, n_user_features, n_item_features):
+    def _weights(self, n_user_features, n_item_features, form):
+        """The weights in the creation order of the reference's graph: item, then user_<t> (and attn_<t>) per taste,
+        then the feature biases.  A Linear / NormalizedLinear side has linear_weights_<end> [n_features, d]; a ReLU side
+        has relu_weights_<end> [n_features, H], relu_biases_<end> [1, H] and linear_weights_<end> [H, d]
+        (representation_graphs.py: ReLURepresentationGraph), H = relu_size."""
         d = self.model.n_components
 
         def normal_rows(n):       # representation_graphs.py:35-36: random_normal rows, L2-normalised
@@ -195,14 +238,28 @@ class WmrbStep(object):
                 return w * torch.rsqrt(torch.clamp((w * w).sum(dim=1, keepdim=True), min=1e-12))
             return init
 
-        names = ['linear_weights_item']           # creation order of the reference's graph
+        def normal(shape):        # ReLURepresentationGraph: random_normal, stddev .5
+            return lambda: torch.randn(*shape, dtype=torch.float32) * .5
+
+        names, ws = [], {}
+
+        def side(end, graph, n_features):
+            h = _relu_hidden(self.model, graph)
+            if h:
+                specs = [('relu_weights_' + end, (n_features, h), normal((n_features, h))),
+                         ('relu_biases_' + end, (1, h), lambda: torch.zeros(1, h, dtype=torch.float32)),
+                         ('linear_weights_' + end, (h, d), normal((h, d)))]
+            else:
+                specs = [('linear_weights_' + end, (n_features, d), normal_rows(n_features))]
+            for name, shape, init in specs:
+                ws[name] = self._weight(name, shape, init)
+                names.append(name)
+
+        side('item', self.model.item_repr_graph_factory, n_item_features)
         for t in range(self.model.n_tastes):
-            names.append('linear_weights_user_{}'.format(t))
+            side('user_{}'.format(t), self.model.user_repr_graph_factory, n_user_features)
             if self.model.attention_graph_factory is not None:
-                names.append('linear_weights_attn_{}'.format(t))
-        ws = {name: self._weight(name, (n_item_features if name == 'linear_weights_item' else n_user_features, d),
-                                 normal_rows(n_item_features if name == 'linear_weights_item' else n_user_features))
-              for name in names}
+                side('attn_{}'.format(t), self.model.attention_graph_factory, n_user_features)
         if self.model.biased:         # recommendation_graphs.py:11: zeros
             for name, n in (('feature_biases_user', n_user_features), ('feature_biases_item', n_item_features)):
                 ws[name] = self._weight(name, (n, 1), lambda n=n: torch.zeros(n, 1, dtype=torch.float32))
@@ -218,9 +275,10 @@ class WmrbStep(object):
         For an RMSE / Separation model (step_plan's loss 'rmse' / 'separation') the loss is a scalar: `l2` is
         batched_alpha itself, the returned loss is a 1-element tensor, and n_sampled_items and samples are not used."""
         lib = kernels.require_cuda()
-        form = step_plan(self.model)
+        form = step_plan(self.model) or relu_step_plan(self.model)
         if form is None:
-            raise ValueError('the fused training step does not cover this model (train_kernels.step_plan)')
+            raise ValueError('the fused training step does not cover this model (train_kernels.step_plan, '
+                             'relu_step_plan)')
         wmrb = form.loss == 'wmrb'
         if not wmrb:
             samples = None
@@ -232,15 +290,28 @@ class WmrbStep(object):
         inter = interactions_in.device_csr(dev)
         if not wmrb and inter.nnz >= 2 ** 31:
             raise ValueError('{} interactions exceed the step\'s int32 indexing'.format(inter.nnz))
-        names, ws = self._weights(user_in.shape[1], item_in.shape[1])
-        # the user operand: taste planes, then attention planes, [n_rows, n_users, d_pad]
-        user_ops = [('linear_weights_user_{}'.format(t), form.normalize_user) for t in range(form.n_tastes)]
+        names, ws = self._weights(user_in.shape[1], item_in.shape[1], form)
+        # the user operand: taste planes, then attention planes, [n_rows, n_users, d_pad]; (end, normalisations, H)
+        user_ops = [('user_{}'.format(t), form.normalize_user, form.hidden[0]) for t in range(form.n_tastes)]
         if form.attention:
-            user_ops += [('linear_weights_attn_{}'.format(t), form.normalize_attn) for t in range(form.n_tastes)]
+            user_ops += [('attn_{}'.format(t), form.normalize_attn, form.hidden[1]) for t in range(form.n_tastes)]
+        relu_sides = {}              # end -> (pre-activations P [rows, H_pad], b, W2 padded) of a ReLU side
 
-        def operand(csr, name, n_norm, out):
-            """K1 of one weight into `out` (normalised rows: K1's raw rows are kept for the backward pass)."""
-            w = ws[name].detach()
+        def operand(csr, end, n_norm, hp, out):
+            """K1 of one side into `out`, or for a ReLU side into its pre-activations P (the layer runs after every
+            K1).  Returns K1's raw rows when they are normalised (kept for the backward pass)."""
+            if hp:
+                h = ws['relu_weights_' + end].shape[1]
+                w1 = ws['relu_weights_' + end].detach()
+                b = ws['relu_biases_' + end].detach().reshape(-1)
+                w2 = ws['linear_weights_' + end].detach()
+                if hp != h or dp != d:     # zero units and columns change no prediction, norm or gradient
+                    w1 = torch.nn.functional.pad(w1, (0, hp - h))
+                    b = torch.nn.functional.pad(b, (0, hp - h))
+                    w2 = torch.nn.functional.pad(w2, (0, dp - d, 0, hp - h))
+                relu_sides[end] = (kernels.gather_reduce(csr, w1, want_f32=True)[0], b, w2)
+                return None
+            w = ws['linear_weights_' + end].detach()
             if dp != d:                # zero columns change no prediction, norm or gradient
                 w = torch.nn.functional.pad(w, (0, dp - d))
             if n_norm == 0:
@@ -251,16 +322,36 @@ class WmrbStep(object):
                        'trk_l2_normalize_rows_step_f32')
             return raw
 
+        def layer(end, n_norm, out):
+            """The hidden layer of a ReLU side into `out` (normalised for cosine: its raw rows are returned)."""
+            pre, b, w2 = relu_sides[end]
+            raw = out if n_norm == 0 else torch.empty(out.shape, dtype=torch.float32, device=dev)
+            _lib.check(lib.trk_relu_layer_forward_f32(_p(pre), _p(b), _p(w2), pre.shape[0], pre.shape[1], dp, _p(raw),
+                                                      _stream()), 'trk_relu_layer_forward_f32')
+            if n_norm == 0:
+                return None
+            _lib.check(lib.trk_l2_normalize_rows_step_f32(_p(raw), raw.shape[0], dp, n_norm, _p(out), None, _stream()),
+                       'trk_l2_normalize_rows_step_f32')
+            return raw
+
         self._mark('start')
         # forward: representations and projected biases (K1)
         user_repr = torch.empty((len(user_ops), n_users, dp), dtype=torch.float32, device=dev)
         item_repr = torch.empty((n_items, dp), dtype=torch.float32, device=dev)
-        item_raw = operand(icsr, 'linear_weights_item', form.normalize_item, item_repr)
-        user_raw = [operand(ucsr, name, n_norm, user_repr[r]) for r, (name, n_norm) in enumerate(user_ops)]
+        item_raw = operand(icsr, 'item', form.normalize_item, form.hidden[2], item_repr)
+        user_raw = [operand(ucsr, end, n_norm, hp, user_repr[r]) for r, (end, n_norm, hp) in enumerate(user_ops)]
         ub = ib = None
         if self.model.biased:
             ub = kernels.project_biases(ucsr, ws['feature_biases_user'].detach().reshape(-1))
             ib = kernels.project_biases(icsr, ws['feature_biases_item'].detach().reshape(-1))
+        if relu_sides:
+            self._mark('representations')
+            # the hidden layers of the ReLU sides (trk_relu_layer_forward_f32), then their normalisation
+            if form.hidden[2]:
+                item_raw = layer('item', form.normalize_item, item_repr)
+            for r, (end, n_norm, hp) in enumerate(user_ops):
+                if hp:
+                    user_raw[r] = layer(end, n_norm, user_repr[r])
         repr_u, repr_i = user_repr, item_repr
         if self.bf16:
             repr_u = torch.empty(user_repr.shape, dtype=torch.bfloat16, device=dev)
@@ -268,7 +359,7 @@ class WmrbStep(object):
             _lib.check(lib.trk_f32_to_bf16(_p(user_repr), user_repr.numel(), _p(repr_u), _stream()), 'trk_f32_to_bf16')
             _lib.check(lib.trk_f32_to_bf16(_p(item_repr), item_repr.numel(), _p(repr_i), _stream()), 'trk_f32_to_bf16')
 
-        self._mark('representations')
+        self._mark('layer_forward' if relu_sides else 'representations')
         # the loss and the gradient with respect to the operands
         if wmrb:
             samples, loss, pred, (d_user_repr, d_item_repr, d_ub, d_ib) = self._wmrb_loss(
@@ -277,17 +368,45 @@ class WmrbStep(object):
             loss, pred, (d_user_repr, d_item_repr, d_ub, d_ib) = self._serial_loss(lib, form, inter, repr_u, repr_i,
                                                                                    ub, ib)
 
-        # backward through the normalisations, then through the sparse x dense products: K1 on the transposed CSR
-        def weight_grad(csr_t, raw, n_norm, d_rows):
+        # backward through the normalisations and the ReLU layers, then through the sparse x dense products: K1 on
+        # the transposed CSR
+        grads = {}
+
+        def layer_grad(end, raw, n_norm, d_rows):
+            """d_rows -> the gradient K1^T takes: through the normalisations, and for a ReLU side through its layer
+            (trk_relu_layer_backward_f32 replaces P by dP and gives the gradients of relu_biases and linear_weights)."""
             if raw is not None:
                 _lib.check(lib.trk_l2_normalize_rows_step_f32(_p(raw), raw.shape[0], dp, n_norm, None, _p(d_rows),
                                                               _stream()), 'trk_l2_normalize_rows_step_f32')
-            g = kernels.gather_reduce(csr_t, d_rows, want_f32=True)[0]
-            return g if dp == d else g[:, :d].contiguous()
+            if end not in relu_sides:
+                return d_rows
+            pre, b, w2 = relu_sides[end]
+            rows, hp = pre.shape
+            h = ws['relu_biases_' + end].shape[1]
+            ws_bytes = int(lib.trk_relu_layer_workspace_bytes(rows, hp, dp))
+            workspace = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+            d_b = torch.empty((hp,), dtype=torch.float32, device=dev)
+            d_w2 = torch.empty((hp, dp), dtype=torch.float32, device=dev)
+            _lib.check(lib.trk_relu_layer_backward_f32(_p(pre), _p(b), _p(w2), _p(d_rows), rows, hp, dp, _p(d_b),
+                                                       _p(d_w2), _p(workspace), ws_bytes, _stream()),
+                       'trk_relu_layer_backward_f32')
+            grads['relu_biases_' + end] = d_b[:h].reshape(1, h).contiguous()
+            grads['linear_weights_' + end] = d_w2 if (hp, dp) == (h, d) else d_w2[:h, :d].contiguous()
+            return pre
 
-        grads = {'linear_weights_item': weight_grad(icsr_t, item_raw, form.normalize_item, d_item_repr)}
-        for r, (name, n_norm) in enumerate(user_ops):
-            grads[name] = weight_grad(ucsr_t, user_raw[r], n_norm, d_user_repr[r])
+        def weight_grad(csr_t, end, d_rows):
+            name = ('relu_weights_' if end in relu_sides else 'linear_weights_') + end
+            g = kernels.gather_reduce(csr_t, d_rows, want_f32=True)[0]
+            width = ws[name].shape[1]
+            grads[name] = g if g.shape[1] == width else g[:, :width].contiguous()
+
+        sides = [(icsr_t, 'item', layer_grad('item', item_raw, form.normalize_item, d_item_repr))]
+        for r, (end, n_norm, _) in enumerate(user_ops):
+            sides.append((ucsr_t, end, layer_grad(end, user_raw[r], n_norm, d_user_repr[r])))
+        if relu_sides:
+            self._mark('layer_backward')
+        for csr_t, end, d_rows in sides:
+            weight_grad(csr_t, end, d_rows)
         if self.model.biased:
             grads['feature_biases_user'] = kernels.project_biases(ucsr_t, d_ub)
             grads['feature_biases_item'] = kernels.project_biases(icsr_t, d_ib)
